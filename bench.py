@@ -20,6 +20,7 @@ At N > 1 rank 0 re-evaluates the full problem on one GPU (vgx_comm_suspend) and 
   python bench.py --gpus 1 --steps 20 --warmup 3
   python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
   python bench.py --impl reference      # restated reference CPU path on the host cores
+  python bench.py ... --dump-outputs DIR  # + cost / gradient / H of the last timed step as DIR/*.npy
 """
 import argparse
 import json
@@ -27,6 +28,7 @@ import os
 import pickle
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -38,6 +40,8 @@ if ROOT not in sys.path:
 
 ALGO_BYTES_PER_RESIDUAL = 84  # SURVEY.md §8(d): 20 B point + 8 corners x (4 B distance + 4 B weight)
 ALGO_BYTES_PER_TSDF_UPDATE = 16
+DUMP_MAX_BYTES = 64 << 20
+H100_HBM_GBS = 3350.0  # NVIDIA H100 SXM data sheet; a denominator, not a measured figure
 _REAL_STDOUT = sys.stdout
 
 WORKLOADS = {
@@ -64,7 +68,16 @@ def parse_args():
     ap.add_argument("--no-stream", action="store_true", help="N = 1: skip the streaming (configs[2]) leg")
     ap.add_argument("--stream-scans", type=int, default=40)
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="CPU baseline budget")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the registration workload's last timed evaluation (cost, gradient, H) as "
+                         "DIR/<name>.npy, at most 64 MB, to compare two builds output for output")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and (args.impl != "b200" or args.workload in ("stream", "rgbd")):
+        ap.error("--dump-outputs applies to the GPU registration workloads (--impl b200, --workload "
+                 "auto|config2|config4)")
+    return args
 
 
 def workload_params(name, args):
@@ -79,13 +92,13 @@ def workload_params(name, args):
 
 # --------------------------------------------------------------------------- workload
 def build_scene(w, rank=0, wait_s=1500.0):
-    """Seeded synthetic scene, cached in /tmp (generation is host-side numpy, forked workers: must
-    run before this process touches CUDA).  Under torchrun only rank 0 generates; the others wait
+    """Seeded synthetic scene, cached in the temporary directory (generation is host-side numpy,
+    forked workers: must run before this process touches CUDA).  Under torchrun only rank 0 generates; the others wait
     for the cache file."""
     from voxgraph_b200 import synth
     key = "vgx_scene_v3_%s_s%d_p%d_k%d_v%g.pkl" % (w["name"], w["submaps"], w["pairs"], w["points"],
                                                    w["voxel_size"])
-    path = os.path.join("/tmp", key)
+    path = os.path.join(tempfile.gettempdir(), key)
 
     def load():
         try:
@@ -132,9 +145,10 @@ def _scan_job(job):
 def build_stream(kind, n_scans, rank=0, wait_s=900.0):
     """Synthetic sensor stream (SURVEY §8d cfg 3 / cfg 5): the sensor moves at 2 m/s through the hall;
     kind = "lidar": 64 x 1024 beams @ 10 Hz; "rgbd": 640 x 480 depth @ 30 Hz (<= 5 m).  Odometry =
-    ground truth + integrated drift.  Host-side numpy ray casting, forked workers, cached in /tmp."""
+    ground truth + integrated drift.  Host-side numpy ray casting, forked workers, cached in the
+    temporary directory."""
     from voxgraph_b200 import synth
-    path = "/tmp/vgx_stream_v3_%s_%d.pkl" % (kind, n_scans)
+    path = os.path.join(tempfile.gettempdir(), "vgx_stream_v3_%s_%d.pkl" % (kind, n_scans))
 
     def load():
         try:
@@ -453,7 +467,7 @@ def run_stream(args):
         raise RuntimeError("bench.py needs a CUDA device (no CPU fallback)")
     ctx = api.Context(0)
     peaks_path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    peak = float(json.load(open(peaks_path))["hbm_gbs"]) if os.path.exists(peaks_path) else 6650.0
+    peak = float(json.load(open(peaks_path))["hbm_gbs"]) if os.path.exists(peaks_path) else H100_HBM_GBS
     r = stream_leg(ctx, api, st, 0.15, 10, peak)
     line = {"metric": "stream_scans_per_s", "value": r["scans_per_s_e2e"], "unit": "scans/s", "n_gpus": 1,
             "steps": args.stream_scans, "warmup": 2, "ms_per_step": 1e3 / r["scans_per_s_e2e"],
@@ -476,7 +490,7 @@ def scene_problem(sc):
 class ClockSampler:
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index):
         self.rows = []
@@ -496,10 +510,10 @@ class ClockSampler:
 
     def stop(self, t0, t1):
         if not self.proc:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
-        sm, smax, reasons = [], None, set()
+        sm, smax, plim, reasons = [], None, None, set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         rows = [r for (t, r) in self.rows if t0 - 0.05 <= t <= t1 + 0.15] or [r for (_, r) in self.rows]
         for r in rows:
@@ -508,10 +522,14 @@ class ClockSampler:
                 sm.append(float(f[0])); smax = float(f[1])
             except Exception:
                 continue
+            try:
+                plim = float(f[7])
+            except Exception:
+                pass
             for k, nm in enumerate(names):
                 if len(f) > 3 + k and f[3 + k].lower().startswith("active"):
                     reasons.add(nm)
-        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": smax,
+        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": smax, "power_limit_w": plim,
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
@@ -619,7 +637,8 @@ def workload_config(w, sc, n_gpus):
             "name": w["name"], "submaps": len(sc.submaps), "pairs": len(sc.pairs),
             "points_per_constraint": w["points"], "voxel_size": w["voxel_size"],
             "registration_point_type": "isosurface", "sampling_ratio": -1,
-            "l2": "inputs (points + reading bricks) exceed the 126 MB L2; no explicit flush in the bracketed region",
+            "l2": "inputs (points + reading bricks) exceed the 50 MB L2 of an H100; no explicit flush in the "
+                  "bracketed region",
             "parallelism": ("constraints sharded x%d; packed H/g blocks summed by a one-shot NVLink "
                             "peer-memory all-gather-reduce (CUDA IPC), NCCL all-reduce as fallback" % n_gpus)
             if n_gpus > 1 else "single GPU"}
@@ -667,7 +686,7 @@ class Problem:
             self.ctx.submap_free(self.id_base + sid)
 
 
-def measure(P, args, torch, dist, world, stream, want_cpu_pose_check=None):
+def measure(P, args, torch, dist, world, stream, dump_dir=None):
     """Device-resident throughput, end-to-end call, roofline split and the pose-graph solve of one
     resident problem.  Every rank takes part (each evaluation contains the exchange)."""
     ctx = P.ctx
@@ -702,6 +721,8 @@ def measure(P, args, torch, dist, world, stream, want_cpu_pose_check=None):
     out["ms_per_step"] = ms_step
     out["value"] = P.r_global / (ms_step * 1e-3)
     out["gpu_launches"] = int(ctx.launch_count - launches0)
+    if dump_dir is not None:
+        dump_eval(ctx, P.n_nodes, dump_dir)
 
     # ---- end to end through the public call with host buffers
     e2e_steps = max(3, min(args.steps, 10))
@@ -770,6 +791,27 @@ def measure(P, args, torch, dist, world, stream, want_cpu_pose_check=None):
         ctx.graph_set_poses(P.pinit)
         out["solve"] = solve
     return out
+
+
+def dump_eval(ctx, n_nodes, dump_dir):
+    """DIR/{cost,gradient,hessian}.npy: what a caller of the timed evaluation receives.  It is evaluated
+    once more at the poses of the timed steps; that equals the last timed step's result bit for bit
+    because the evaluation is deterministic (the constraint sums add their tiles in tile-index order,
+    graph.cu reg_csum_kernel, whatever order the tiles ran in).  A dense H over DUMP_MAX_BYTES is
+    reduced to a fixed, seeded subset of its rows, listed in hessian_rows.npy."""
+    ok, cost, g, H = ctx.graph_eval(n_nodes, want_H=True)
+    if int(os.environ.get("RANK", "0")) != 0:
+        return
+    out = {"cost": np.array([cost]), "gradient": g, "hessian": H}
+    budget = DUMP_MAX_BYTES - 8 * (1 + g.size)
+    if H.nbytes > budget:
+        rows = np.sort(np.random.default_rng(0).choice(H.shape[0], budget // (8 * H.shape[1]) - 1,
+                                                        replace=False))
+        out["hessian"] = H[rows]
+        out["hessian_rows"] = rows
+    os.makedirs(dump_dir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(dump_dir, name + ".npy"), np.ascontiguousarray(a, np.float64))
 
 
 def single_rank_parity(P, torch, dist, world, rank):
@@ -858,7 +900,7 @@ def run_b200(args):
     sampler = ClockSampler(local_rank) if rank == 0 else None
     t_load0 = time.time()
     P = Problem(ctx, api, sc)
-    M = measure(P, args, torch, dist, world, stream)
+    M = measure(P, args, torch, dist, world, stream, dump_dir=args.dump_outputs)
     ms_step = M["ms_per_step"]
 
     parity = None
@@ -883,12 +925,12 @@ def run_b200(args):
     if os.path.exists(peaks_path):
         peak = float(json.load(open(peaks_path))["hbm_gbs"]); peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak = 6650.0; peak_src = "fallback 6.65 TB/s (MEASURED_PEAKS.json absent)"
+        peak = H100_HBM_GBS; peak_src = "H100 SXM data sheet 3.35 TB/s (MEASURED_PEAKS.json absent)"
 
     def roofline_of(Pm, Mm):
         achieved = Pm.r_local * ALGO_BYTES_PER_RESIDUAL / (Mm["kernel_ms"] * 1e-3) / 1e9
         return {"bound": "hbm", "kernel": "reg_reduce_kernel<true>", "achieved": achieved, "peak": peak,
-                "unit": "GB/s", "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
+                "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_residual": ALGO_BYTES_PER_RESIDUAL,
                 "residuals_per_launch": int(Pm.r_local), "kernel_ms": Mm["kernel_ms"],
                 "kernel_share_of_step": Mm["kernel_ms"] / Mm["ms_per_step"] if Mm["ms_per_step"] > 0 else None,
@@ -896,12 +938,6 @@ def run_b200(args):
                 "step_breakdown_us_serialised": Mm.get("step_breakdown_us")}
 
     roofline = roofline_of(P, M)
-    prof_traffic = os.path.join(ROOT, "profiles", "reg_reduce_traffic.json")
-    if os.path.exists(prof_traffic) and wname == "config2":
-        try:
-            roofline["traffic"] = json.load(open(prof_traffic)).get("dram_bytes_per_launch")
-        except Exception:
-            pass
 
     e2e = M["e2e"]
     extras = {}
@@ -1000,6 +1036,7 @@ def run_b200(args):
                 "vs_baseline": None, "dtype": "f32", "data": "synthetic",
                 "config": workload_config(w_main, sc, n_gpus),
                 "residuals_per_step": int(P.r_global), "gpu_launches": M["gpu_launches"],
+                "device": torch.cuda.get_device_name(local_rank),
                 "clocks": clocks, "e2e": e2e, "roofline": roofline,
                 "cpu_baseline": ({k: cpu[k] for k in ("value", "unit", "cores", "kind", "sample",
                                                        "value_4_threads", "value_best", "spread", "note")}

@@ -1,7 +1,7 @@
 /*
- * voxgraph_b200.h — C-ABI of the B200-native voxgraph hot paths.
+ * voxgraph_b200.h — C-ABI of the H100-native voxgraph hot paths.
  *
- * Drop-in boundary for (paths relative to /root/reference/voxgraph/):
+ * Drop-in boundary for (paths relative to voxgraph/ of the reference, ethz-asl/voxgraph):
  *   b1  RegistrationCostFunction::Evaluate
  *         include/voxgraph/backend/constraint/cost_functions/registration_cost_function.h:47-48
  *         src/backend/constraint/cost_functions/registration_cost_function.cpp:58-298

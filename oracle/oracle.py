@@ -32,17 +32,13 @@ _ref_sampler = None
 
 
 def ref_sampler_lib():
-    """oracle/_ref/libvgref_sampler.so: the REFERENCE's own WeightedSampler template compiled from
-    /root/reference (oracle/ref_sampler_shim.cpp + Makefile target `ref`).  Returns None when it has
-    not been built (no /root/reference and no prebuilt file)."""
+    """oracle/_ref/libvgref_sampler.so: the REFERENCE's own WeightedSampler template compiled from a
+    voxgraph checkout (oracle/ref_sampler_shim.cpp + Makefile target `ref`, VOXGRAPH_SRC=<voxgraph/>).
+    Returns None when it has not been built."""
     global _ref_sampler
     if _ref_sampler is None:
         if not os.path.exists(_REF_SAMPLER_PATH):
-            if os.path.isdir("/root/reference/voxgraph/include"):
-                subprocess.run(["make", "-C", _HERE, "ref"], check=False, stdout=subprocess.PIPE,
-                               stderr=subprocess.STDOUT)
-            if not os.path.exists(_REF_SAMPLER_PATH):
-                return None
+            return None
         L = C.CDLL(_REF_SAMPLER_PATH)
         L.vgref_sampler_create.restype = C.c_void_p
         L.vgref_sampler_create.argtypes = [C.POINTER(C.c_float), C.c_int]

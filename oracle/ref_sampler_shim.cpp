@@ -1,9 +1,9 @@
 // oracle/_ref recipe: compiles the REFERENCE's own WeightedSampler template
-// (/root/reference/voxgraph/include/voxgraph/frontend/submap_collection/weighted_sampler.h and
+// (voxgraph/include/voxgraph/frontend/submap_collection/weighted_sampler.h and
 // weighted_sampler_inl.h - header-only, no third-party dependency) behind a C interface, so the
 // oracle's restatement (vgo_sampler_*) and the product's sampling mode can be pinned against the
 // real reference code.  TEST INFRASTRUCTURE ONLY; built into oracle/_ref/ (git-ignored) when
-// /root/reference is present; the reference sources are included from where they lie, never copied.
+// VOXGRAPH_SRC names a voxgraph checkout; its sources are included from where they lie, never copied.
 #include <stdint.h>
 
 #include "voxgraph/frontend/submap_collection/weighted_sampler.h"

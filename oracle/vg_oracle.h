@@ -10,13 +10,13 @@
  * vectors or fixtures, and its arithmetic dependencies (voxblox, cblox, minkindr,
  * Ceres, Eigen) are neither vendored nor installed, so neither the reference nor its
  * dependencies can be compiled here.  The restatement follows the reference sources
- * line by line where they exist under /root/reference (cited per function below) and
+ * line by line where they exist in the reference, ethz-asl/voxgraph (cited per function below) and
  * the published upstream algorithms (SURVEY.md Appendix A) elsewhere; it is pinned
  * by analytic known-answer tests (tests/test_oracle_*.py) and by golden vectors
  * generated from the reference's own sympy derivation
  * (voxgraph/scripts/jacobians_xyz_yaw.py -> tests/golden/).
  *
- * Paths are relative to /root/reference/voxgraph/.
+ * Paths are relative to voxgraph/ of the reference.
  */
 #ifndef VG_ORACLE_H_
 #define VG_ORACLE_H_

@@ -1,7 +1,5 @@
-"""One 64 x 1024 LiDAR scan through both TSDF schedulers and one finishSubmap on the device - the
-command the ncu captures of the HP1 / extraction kernels are taken on (profiles/README.md).
-  ncu --set full --clock-control none -k regex:'tsdf|iso_|relevant|build_view|esdf' -o gpurun_out/r2_tsdf python scripts/profile_tsdf.py
-"""
+"""One 64 x 1024 LiDAR scan through both TSDF schedulers and one finishSubmap on the device - a
+workload to profile the HP1 / extraction kernels on."""
 import os
 import sys
 

@@ -1,26 +1,24 @@
 """Generates tests/golden/pose_jacobians.json from the reference's own symbolic derivation.
 
-Runs /root/reference/voxgraph/scripts/jacobians_xyz_yaw.py (sympy; import-only, prints
+Runs voxgraph/scripts/jacobians_xyz_yaw.py of a voxgraph checkout (sympy; import-only, prints
 disabled), takes its T_eo and pose symbols, and lambdifies d(T_eo * o_r_oi)/d(params) —
-the two 3x4 matrices hard-coded at registration_cost_function.cpp:214-227.
-Run in the build container only (/root/reference does not exist on the GPU box):
-    python tests/golden/make_jacobian_golden.py
+the two 3x4 matrices hard-coded at registration_cost_function.cpp:214-227:
+    python tests/golden/make_jacobian_golden.py <voxgraph checkout>/voxgraph/scripts/jacobians_xyz_yaw.py
 """
 import contextlib
 import io
 import json
 import os
 import runpy
+import sys
 
 import numpy as np
 
-SCRIPT = "/root/reference/voxgraph/scripts/jacobians_xyz_yaw.py"
 
-
-def main():
+def main(script):
     import sympy as sp
     with contextlib.redirect_stdout(io.StringIO()):
-        ns = runpy.run_path(SCRIPT)
+        ns = runpy.run_path(script)
     T_eo = ns["T_eo"]
     so = [ns[k] for k in ("x_o", "y_o", "z_o", "theta_o")]
     se = [ns[k] for k in ("x_e", "y_e", "z_e", "theta_e")]
@@ -47,9 +45,9 @@ def main():
                           dTp_dref=np.asarray(f_o(*args), float).tolist(),
                           dTp_dread=np.asarray(f_e(*args), float).tolist()))
     out = os.path.join(os.path.dirname(os.path.abspath(__file__)), "pose_jacobians.json")
-    json.dump(dict(source=SCRIPT, cases=cases), open(out, "w"), indent=1)
+    json.dump(dict(source="voxgraph/scripts/jacobians_xyz_yaw.py", cases=cases), open(out, "w"), indent=1)
     print("wrote", out, len(cases), "cases; point symbols", [str(s) for s in pt])
 
 
 if __name__ == "__main__":
-    main()
+    main(sys.argv[1])

@@ -1,4 +1,4 @@
-"""In-tree build of libvoxgraph_b200.so (hand-written CUDA for sm_100a + the C-ABI)."""
+"""In-tree build of libvoxgraph_b200.so (hand-written CUDA for sm_90a + the C-ABI)."""
 import os
 import subprocess
 import sys
@@ -8,7 +8,7 @@ CSRC = os.path.join(HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 LIB = os.path.join(HERE, "libvoxgraph_b200.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-I" + INCLUDE, "-I" + CSRC]
 # (source, extra flags). -fmad=false: the reference's float expressions are restated
 # operation by operation (see registration.cuh); graph.cu is double-precision solver code.

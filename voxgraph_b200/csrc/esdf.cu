@@ -6,7 +6,7 @@
 // The ESDF feeds the reference's default registration branch (use_esdf_distance = true,
 // registration_cost_function.h:35; cpp:133-140) and findRelevantVoxelIndices' ESDF distance.
 //
-// B200 form: voxblox pops a bucketed priority queue on one thread; here every observed, non-fixed
+// GPU form: voxblox pops a bucketed priority queue on one thread; here every observed, non-fixed
 // voxel repeatedly PULLS  d <- min(d, d_neighbour + |offset| voxel_size)  over its 26 neighbours
 // (max on the negative side) in place until a sweep changes nothing.  The update is monotone, so
 // any interleaving reaches the same least fixed point = the exact shortest quasi-Euclidean path in

@@ -229,6 +229,8 @@ __device__ __forceinline__ double reg_constraint_sum(const RegSums& R, int c, in
 // Per-constraint sums csum[c][21] from the tile rows: one warp per constraint, a programmatic
 // dependent of the reduce kernel (and the assembly kernel is one of this).  A separate, massively
 // parallel stage: inside the assembly the same loop is a chain of dependent L2 latencies per item.
+// The tiles are added in tile-index order, never in completion order: every evaluation at the same
+// poses is bit-identical, which the parity tests and bench.py --dump-outputs rely on.
 __global__ void __launch_bounds__(128)
 reg_csum_kernel(RegSums R, int n, double* __restrict__ csum, const int* __restrict__ skip) {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");

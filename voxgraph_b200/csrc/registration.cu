@@ -53,7 +53,7 @@ __device__ __forceinline__ void dmma_8x8x4(double& d0, double& d1, double a, dou
 
 #define VGX_STAGE_STRIDE 36  // doubles per component row (32 points + pad: 2-way = optimal for 8 B)
 
-// ---- TMA (1-D bulk copy) + mbarrier primitives, sm_100a PTX
+// ---- TMA (1-D bulk copy) + mbarrier primitives, sm_90a PTX
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
@@ -226,15 +226,8 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
       R.ox = L.ox; R.oy = L.oy; R.oz = L.oz;
       if (R.found) {
         const float4* o = view + 2 * (((size_t)slot_b << vox_shift) + (size_t)L.lin);
-#if VGX_REG_LDG256
-        // the whole 32-byte octet = one sector = ONE 256-bit load (SASS LDG.E.ENL2.256)
-        asm volatile("ld.global.nc.v8.f32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                     : "=f"(R.lo.x), "=f"(R.lo.y), "=f"(R.lo.z), "=f"(R.lo.w), "=f"(R.hi.x), "=f"(R.hi.y),
-                       "=f"(R.hi.z), "=f"(R.hi.w)
-                     : "l"(o));
-#else
+        // the whole 32-byte octet = one sector = two 128-bit loads (sm_90 has no 256-bit LDG)
         R.lo = __ldg(o); R.hi = __ldg(o + 1);
-#endif
       }
     };
     // stage B: consume the octet issued one unit ago
@@ -437,7 +430,7 @@ void vgx_launch_reg_reduce(cudaStream_t st, const RegConstraintDev* cons, const 
 }
 
 int vgx_reg_resident_ctas(int device, int grid_capacity) {
-  int sms = 148, per_sm = 0;
+  int sms = 132, per_sm = 0;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
   const size_t smem = sizeof(uint16_t) * (size_t)grid_capacity;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, reg_reduce_kernel<true>, VGX_REG_THREADS,

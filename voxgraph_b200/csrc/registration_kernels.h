@@ -10,13 +10,11 @@ struct RegPoseConst;
 #define VGX_REG_THREADS 128        // 4 warps per CTA, each with its own TMA ring + software pipeline
 #endif
 #ifndef VGX_REG_MIN_BLOCKS
-#define VGX_REG_MIN_BLOCKS 7       // resident CTAs per SM the register budget is sized for (72 registers)
+#define VGX_REG_MIN_BLOCKS 6       // resident CTAs per SM the register budget is sized for (80 registers;
+                                   // sm_90a spills at the 72 that 7 would allow, for the same step time)
 #endif
 #ifndef VGX_REG_RING
 #define VGX_REG_RING 4             // point-slice ring slots per warp (units in flight = RING - 1)
-#endif
-#ifndef VGX_REG_LDG256
-#define VGX_REG_LDG256 1           // one 256-bit load per octet (LDG.E.ENL2.256) instead of two 128-bit ones
 #endif
 #ifndef VGX_REG_EARLYOUT
 #define VGX_REG_EARLYOUT 1         // a warp whose 32 points all miss the containing block skips the unit
