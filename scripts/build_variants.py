@@ -17,8 +17,6 @@ VARIANTS = {
     "t64_b16": ["-DVGX_REG_THREADS=64", "-DVGX_REG_MIN_BLOCKS=16"],
     # ablations of the final kernel (results are wrong by construction: timing only)
     "x_nogram": ["-DVGX_X_NOGRAM=1"],
-    "x_nomath": ["-DVGX_X_NOMATH=1"],
-    "x_noload": ["-DVGX_X_NOLOAD=1"],
 }
 
 if __name__ == "__main__":

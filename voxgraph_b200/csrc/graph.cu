@@ -70,6 +70,7 @@ struct VgxGraph {
   RegConstraintDev* d_cons = nullptr;
   RegPoseConst* d_poses = nullptr;
   RegTile* d_tiles = nullptr;
+  float4* d_unit_bounds = nullptr;   // bounding sphere per 32-point unit of the tiles (RegTile::unit0)
   int* d_tile_begin = nullptr;
   int* d_cta_tile_begin = nullptr;
   double* d_partials = nullptr;
@@ -107,6 +108,7 @@ struct VgxGraph {
 
 static void free_tables(VgxGraph* g) {
   cudaFree(g->d_cons); cudaFree(g->d_poses); cudaFree(g->d_tiles); cudaFree(g->d_tile_begin); cudaFree(g->d_cta_tile_begin);
+  cudaFree(g->d_unit_bounds); g->d_unit_bounds = nullptr;
   cudaFree(g->d_partials); cudaFree(g->d_csum); cudaFree(g->d_rel); cudaFree(g->d_counters);
   cudaFree(g->d_tile_order); cudaFree(g->d_tile_cost); cudaFree(g->d_block_mask);
   g->d_tile_order = nullptr; g->d_tile_cost = nullptr; g->d_block_mask = nullptr;
@@ -1233,7 +1235,8 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
       const int tile_pts = hw_units * VGX_REG_UNIT;
       for (int s0 = 0; s0 < cons[k].n; s0 += tile_pts) {
         RegTile t;
-        t.constraint = k; t.start = s0; t.count = std::min(tile_pts, cons[k].n - s0);
+        t.constraint = k; t.count = std::min(tile_pts, cons[k].n - s0);
+        t.pts = cons[k].pts + (size_t)(s0 / VGX_REG_UNIT) * VGX_PT_UNIT_FLOATS;
         tiles.push_back(t);
       }
     }
@@ -1255,8 +1258,8 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
         const int64_t take = std::min<int64_t>(uc - u, cta_end(cta) - (ubase + u));
         RegTile t;
         t.constraint = k;
-        t.start = (int)(u * VGX_REG_UNIT);
-        t.count = (int)std::min<int64_t>(take * VGX_REG_UNIT, (int64_t)cons[k].n - t.start);
+        t.count = (int)std::min<int64_t>(take * VGX_REG_UNIT, (int64_t)cons[k].n - u * VGX_REG_UNIT);
+        t.pts = cons[k].pts + (size_t)u * VGX_PT_UNIT_FLOATS;
         tiles.push_back(t);
         u += take;
       }
@@ -1266,10 +1269,12 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
   }
   tile_begin.push_back((int)tiles.size());
   g->n_tiles = (int)tiles.size();
+  int n_units = 0;   // units of all tiles = entries of the unit-bound table
   for (auto& t : tiles) {   // what the CTA needs to start its bulk copies without a dependent load
     const RegConstraintDev& cc = cons[t.constraint];
     const int cells = cc.gd0 * cc.gd1 * cc.gd2;
-    t.pts = cc.pts + (size_t)(t.start / VGX_REG_UNIT) * VGX_PT_UNIT_FLOATS;
+    t.unit0 = n_units;
+    n_units += (t.count + VGX_REG_UNIT - 1) / VGX_REG_UNIT;
     t.grid16 = cc.grid16;
     t.grid_bytes = (cc.grid16 && cells > 0) ? (int)((((size_t)cells + 7) & ~(size_t)7) * sizeof(uint16_t)) : 0;
   }
@@ -1356,6 +1361,12 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
   auto dmalloc = [&](void** p, size_t bytes) {
     if (e == cudaSuccess) e = cudaMalloc(p, std::max<size_t>(bytes, 8));
   };
+  dmalloc((void**)&g->d_unit_bounds, sizeof(float4) * (size_t)n_units);
+  if (e == cudaSuccess && g->n_tiles > 0) {
+    vgx_launch_reg_unit_bounds(st, g->d_tiles, g->n_tiles, g->d_unit_bounds);
+    c->launches++;
+    e = cudaGetLastError();
+  }
   dmalloc((void**)&g->d_poses, sizeof(RegPoseConst) * g->n_local);
   dmalloc((void**)&g->d_partials, sizeof(double) * VGX_REG_NSTRIDE * (size_t)g->n_tiles);
   dmalloc((void**)&g->d_csum, sizeof(double) * VGX_REG_NSTRIDE * (size_t)g->n_local);
@@ -1416,7 +1427,8 @@ static int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_pa
     {
       VgxLaunchScope s(c, 0);
       vgx_launch_reg_reduce(st, g->d_cons, g->d_poses, g->d_tiles, g->n_ctas, g->d_cta_tile_begin,
-                            g->d_tile_order, g->d_tile_cost, g->d_partials, g->grid_capacity, jacobian, skip);
+                            g->d_tile_order, g->d_tile_cost, g->d_partials, g->grid_capacity,
+                            g->d_unit_bounds, jacobian, skip);
     }
     if (g->evals_since_order < 0) g->evals_since_order = -2;   // a cost has been measured now
   }

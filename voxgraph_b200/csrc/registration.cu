@@ -80,7 +80,91 @@ __device__ __forceinline__ void tma_load_1d(uint32_t dst, const void* src, uint3
                ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
-// Registration reduce kernel, v4.  Persistent CTAs; the local residual index space is cut into
+// ---- unit culling
+// A point contributes to the sums only if the block that contains it exists in the reading submap:
+// otherwise its octet is missing (early-out in stage A) or holds NaN, and with
+// no_correspondence_cost == 0 it adds nothing.  A unit none of whose points can reach an existing
+// block is therefore skipped as a whole, before its points are fetched; the sums do not change by a
+// bit (a whole unit of zero contributions leaves every accumulator as it was).  Points of weight 0
+// with finite coordinates and distance, such as the zero padding of the last unit, are left out of
+// the bounds: with the reading submap's distances finite or NaN, such a point adds only +-0.
+__global__ void __launch_bounds__(128)
+reg_unit_bounds_kernel(const RegTile* __restrict__ tiles, float4* __restrict__ bounds) {
+  const RegTile T = tiles[blockIdx.x];
+  const int lane = threadIdx.x & 31;
+  const int n_units = (T.count + VGX_REG_UNIT - 1) / VGX_REG_UNIT;
+  for (int u = threadIdx.x >> 5; u < n_units; u += blockDim.x >> 5) {
+    const float* p = T.pts + (size_t)u * VGX_PT_UNIT_FLOATS + lane;
+    const float x = p[0], y = p[32], z = p[64], d = p[96], w = p[128];
+    const bool finite = isfinite(x) && isfinite(y) && isfinite(z);
+    const bool in = !(w == 0.f && finite && isfinite(d));
+    float lo0 = in ? x : INFINITY, lo1 = in ? y : INFINITY, lo2 = in ? z : INFINITY;
+    float hi0 = in ? x : -INFINITY, hi1 = in ? y : -INFINITY, hi2 = in ? z : -INFINITY;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      lo0 = fminf(lo0, __shfl_xor_sync(0xffffffffu, lo0, off));
+      lo1 = fminf(lo1, __shfl_xor_sync(0xffffffffu, lo1, off));
+      lo2 = fminf(lo2, __shfl_xor_sync(0xffffffffu, lo2, off));
+      hi0 = fmaxf(hi0, __shfl_xor_sync(0xffffffffu, hi0, off));
+      hi1 = fmaxf(hi1, __shfl_xor_sync(0xffffffffu, hi1, off));
+      hi2 = fmaxf(hi2, __shfl_xor_sync(0xffffffffu, hi2, off));
+    }
+    const float c0 = 0.5f * (lo0 + hi0), c1 = 0.5f * (lo1 + hi1), c2 = 0.5f * (lo2 + hi2);
+    // distance to the (rounded) centre in double, radius rounded up to float
+    const double e0 = (double)x - c0, e1 = (double)y - c1, e2 = (double)z - c2;
+    double r2 = in ? e0 * e0 + e1 * e1 + e2 * e2 : 0.0;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) r2 = fmax(r2, __shfl_xor_sync(0xffffffffu, r2, off));
+    const bool never = __any_sync(0xffffffffu, in && !finite) || !__any_sync(0xffffffffu, in);
+    if (lane == 0)
+      bounds[T.unit0 + u] = make_float4(c0, c1, c2, never ? INFINITY : __double2float_ru(__dsqrt_ru(r2)));
+  }
+}
+
+void vgx_launch_reg_unit_bounds(cudaStream_t st, const RegTile* tiles, int n_tiles, float4* bounds) {
+  if (n_tiles > 0) reg_unit_bounds_kernel<<<n_tiles, 128, 0, st>>>(tiles, bounds);
+}
+
+// May a point of the unit with bounding sphere b (reference frame) lie in an existing block?  One
+// lane per unit; false only when the answer is provably no.
+//
+// Why the test is conservative.  Stage A computes, per point x, p = vgx_reg_transform(x) in float and
+// then b = floor(p * block_size_inv + VGX_COORD_EPS) (vgx_block_index).  Every one of those last
+// operations is monotone in p (round-to-nearest and floor are monotone), so if L <= p <= H on an
+// axis, b lies between the block indices of L and H computed by the same expression.  It remains to
+// bound p.  With n = qw^2 + qz^2, the transform is p = M x + t exactly, where M is n times a rotation
+// in x-y (|M| <= 1 + 2|n - 1|) and the identity in z; so |M x + t - (M c + t)| <= (1 + 2|n - 1|) r on
+// every axis.  The float evaluation (six roundings, every intermediate at most 5 (|x| + |t|)) adds
+// under 32 ulp-units of (|x| + |t|) for x and again for the centre c, and S below bounds |x| + |t|
+// and |c| + |t|; the margin S * 2^-16 = 256 u S (u = 2^-24) covers both with the rounding of L and H
+// themselves, and r * 2^-10 covers the rounding of the radius and of |n - 1|.  Non-finite values make
+// the unit live.
+__device__ __forceinline__ bool reg_unit_may_hit(const RegConstraintDev& C, const RegPoseConst& P,
+                                                 const uint16_t* __restrict__ s_grid, const float4 b) {
+  float c0, c1, c2;
+  vgx_reg_transform(P, b.x, b.y, b.z, c0, c1, c2);
+  const float n1 = fabsf(P.qw * P.qw + P.qz * P.qz - 1.0f);
+  const float S = ((fabsf(b.x) + fabsf(b.y)) + (fabsf(b.z) + 3.0f * b.w)) +
+                  ((fabsf(P.tx) + fabsf(P.ty)) + fabsf(P.tz));
+  const float R = b.w + (b.w * (2.0f * n1 + 0x1p-10f) + S * 0x1p-16f);
+  if (!isfinite((c0 + c1) + (c2 + R))) return true;
+  int l0, l1, l2, h0, h1, h2;
+  vgx_block_index(C, c0 - R, c1 - R, c2 - R, l0, l1, l2);
+  vgx_block_index(C, c0 + R, c1 + R, c2 + R, h0, h1, h2);
+  // box of grid cells, clipped to the grid (64-bit: the indices may be saturated)
+  const long long a0 = max((long long)min(l0, h0) - C.gmin0, 0ll), z0 = min((long long)max(l0, h0) - C.gmin0, (long long)C.gd0 - 1);
+  const long long a1 = max((long long)min(l1, h1) - C.gmin1, 0ll), z1 = min((long long)max(l1, h1) - C.gmin1, (long long)C.gd1 - 1);
+  const long long a2 = max((long long)min(l2, h2) - C.gmin2, 0ll), z2 = min((long long)max(l2, h2) - C.gmin2, (long long)C.gd2 - 1);
+  if (a0 > z0 || a1 > z1 || a2 > z2) return false;   // entirely outside the grid
+  if ((z0 - a0 + 1) * (z1 - a1 + 1) * (z2 - a2 + 1) > 27) return true;
+  for (int g2 = (int)a2; g2 <= (int)z2; ++g2)
+    for (int g1 = (int)a1; g1 <= (int)z1; ++g1)
+      for (int g0 = (int)a0; g0 <= (int)z0; ++g0)
+        if (s_grid[(g2 * C.gd1 + g1) * C.gd0 + g0] != 0xFFFF) return true;
+  return false;
+}
+
+// Registration reduce kernel, v5.  Persistent CTAs; the local residual index space is cut into
 // 32-point units that are dealt evenly to the CTAs (a tile = a CTA's run of units inside one
 // residual block).  Inside a tile every warp runs its own software pipeline over the units
 // u = warp, warp + W, ...:
@@ -93,13 +177,16 @@ __device__ __forceinline__ void tma_load_1d(uint32_t dst, const void* src, uint3
 //     u+1 is hidden behind the arithmetic of unit u inside the same warp.
 // The last unit is zero-padded to 32 points (weight 0 -> zero contribution), so the
 // loop carries no "active" predicate.  Warps never synchronise with each other inside a tile.
+// Block-grid tiles without a no-correspondence cost first test every unit's bounding sphere against
+// the block grid (one lane per unit, reg_unit_may_hit); the ring then carries only the units that
+// may hit, in the same order, so the per-warp sums are those of the full walk.
 template <bool kJacobian>
 __global__ void __launch_bounds__(VGX_REG_THREADS, VGX_REG_MIN_BLOCKS)
 reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
                   const RegPoseConst* __restrict__ poses, const RegTile* __restrict__ tiles,
                   const int* __restrict__ cta_tile_begin, const int* __restrict__ tile_order,
                   int* __restrict__ tile_cost, double* __restrict__ partials, int grid_capacity,
-                  const int* __restrict__ skip) {
+                  const float4* __restrict__ unit_bounds, const int* __restrict__ skip) {
   if (skip && *skip) return;   // evaluation enqueued ahead of a solve that has already ended
   constexpr int kWarps = VGX_REG_THREADS / 32;
   constexpr int kRing = VGX_REG_RING;
@@ -144,7 +231,7 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
     const int4 rec0 = __ldg(reinterpret_cast<const int4*>(tiles + tile));
     const ulonglong2 rec1 = __ldg(reinterpret_cast<const ulonglong2*>(tiles + tile) + 1);
     RegTile T;
-    T.constraint = rec0.x; T.start = rec0.y; T.count = rec0.z; T.grid_bytes = rec0.w;
+    T.constraint = rec0.x; T.unit0 = rec0.y; T.count = rec0.z; T.grid_bytes = rec0.w;
     T.pts = reinterpret_cast<const float*>(rec1.x);
     T.grid16 = reinterpret_cast<const uint16_t*>(rec1.y);
     const bool use_grid = T.grid_bytes > 0 && T.grid_bytes <= 2 * grid_capacity;
@@ -166,8 +253,17 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
     if (stage_grid) grid_of = T.constraint;
     const int n_units = (T.count + 31) >> 5;
     const int my_units = warp < n_units ? (n_units - warp + kWarps - 1) / kWarps : 0;
-    // producer (lane 0): bring unit j of this warp into ring slot seq % kRing
-    auto issue = [&](int j, uint32_t seq) {
+    // culling needs the pose block, so a tile that may cull issues its first units after the tile
+    // barrier; lane j tests unit j of this warp
+    const bool may_cull = unit_bounds && use_grid && my_units <= 32;
+    float4 bnd = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (may_cull && lane < my_units) bnd = __ldg(unit_bounds + T.unit0 + warp + lane * kWarps);
+    uint32_t live = 0;   // may_cull: units of this warp not yet issued that may hit (bit j: unit j)
+    int next = 0;        // otherwise: next unit to issue
+    // producer (lane 0): bring the next unit of this warp into ring slot seq % kRing
+    auto issue = [&](uint32_t seq) {
+      int j = next++;
+      if (may_cull) { j = __ffs(live) - 1; live &= live - 1; }
       if (lane == 0) {
         const uint32_t slot = seq % kRing;
         const uint32_t bar = bar0 + 8u * slot, dst = ring0 + 640u * slot;
@@ -175,21 +271,29 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
         tma_load_1d(dst, T.pts + (size_t)(warp + j * kWarps) * VGX_PT_UNIT_FLOATS, 640u, bar);
       }
     };
-    if (my_units > 0) {
+    int n_live = my_units;   // units this warp consumes
+    if (!may_cull) {
 #pragma unroll
       for (int j = 0; j < kRing - 1; ++j)
-        if (j < my_units) issue(j, it + j);
+        if (j < n_live) issue(it + j);
     }
     mbar_wait(tbar, tseq & 1u);   // descriptor, pose block and grid have landed
     const long long clk0 = clock64();
     const RegPoseConst P = s_P;
+    const bool gram_always = s_C.no_corr != 0.0;  // r = w * no_correspondence_cost without a match
+    if (may_cull) {
+      live = __ballot_sync(0xffffffffu, lane < my_units && (gram_always || reg_unit_may_hit(s_C, P, s_grid, bnd)));
+      n_live = __popc(live);
+#pragma unroll
+      for (int j = 0; j < kRing - 1; ++j)
+        if (j < n_live) issue(it + j);
+    }
     double d0 = 0.0, d1 = 0.0;
     const size_t vox_shift = 3 * s_C.vps_shift;
     const float4* view = reinterpret_cast<const float4*>(s_C.view);
 
     // stage A: everything up to the ISSUE of the octet load
     struct Pipe { float4 lo, hi; float ox, oy, oz; bool found; };
-    const bool gram_always = s_C.no_corr != 0.0;  // r = w * no_correspondence_cost without a match
     auto stage_a = [&](uint32_t seq, Pipe& R) {
       const uint32_t slot = seq % kRing;
       mbar_wait(bar0 + 8u * slot, (seq / kRing) & 1u);
@@ -271,20 +375,20 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
       __syncwarp();  // every lane is done with this unit's ring slot and the Gram staging buffer
     };
 
-    if (my_units > 0) {
+    if (n_live > 0) {
       // two register sets alternate (loop unrolled by two): the in-flight octet is never copied
       Pipe Ra, Rb;
       stage_a(it, Ra);
       int j = 0;
-      for (; j + 2 <= my_units; j += 2, it += 2) {
-        if (j + kRing - 1 < my_units) issue(j + kRing - 1, it + kRing - 1);
+      for (; j + 2 <= n_live; j += 2, it += 2) {
+        if (j + kRing - 1 < n_live) issue(it + kRing - 1);
         stage_a(it + 1, Rb);
         stage_b(it, Ra);
-        if (j + kRing < my_units) issue(j + kRing, it + kRing);
-        if (j + 2 < my_units) stage_a(it + 2, Ra);
+        if (j + kRing < n_live) issue(it + kRing);
+        if (j + 2 < n_live) stage_a(it + 2, Ra);
         stage_b(it + 1, Rb);
       }
-      if (j < my_units) {
+      if (j < n_live) {
         stage_b(it, Ra);
         ++it;
       }
@@ -405,7 +509,7 @@ void vgx_launch_reg_pose_setup(cudaStream_t st, const RegConstraintDev* cons, co
 void vgx_launch_reg_reduce(cudaStream_t st, const RegConstraintDev* cons, const RegPoseConst* poses,
                            const RegTile* tiles, int n_ctas, const int* cta_tile_begin,
                            const int* tile_order, int* tile_cost, double* partials, int grid_capacity,
-                           bool jacobian, const int* skip) {
+                           const float4* unit_bounds, bool jacobian, const int* skip) {
   if (n_ctas <= 0) return;
   // launched with programmatic stream serialisation: its CTAs may start while the pose set-up kernel
   // is still running; they block at griddepcontrol.wait before touching the pose blocks
@@ -423,10 +527,10 @@ void vgx_launch_reg_reduce(cudaStream_t st, const RegConstraintDev* cons, const 
   cfg.numAttrs = (no_pdl && no_pdl[0] == '1') ? 0 : 1;
   if (jacobian)
     cudaLaunchKernelEx(&cfg, reg_reduce_kernel<true>, cons, poses, tiles, cta_tile_begin, tile_order, tile_cost,
-                       partials, grid_capacity, skip);
+                       partials, grid_capacity, unit_bounds, skip);
   else
     cudaLaunchKernelEx(&cfg, reg_reduce_kernel<false>, cons, poses, tiles, cta_tile_begin, tile_order, tile_cost,
-                       partials, grid_capacity, skip);
+                       partials, grid_capacity, unit_bounds, skip);
 }
 
 int vgx_reg_resident_ctas(int device, int grid_capacity) {

@@ -34,7 +34,7 @@ struct RegPoseConst;
 
 struct __align__(16) RegTile {   // 32 bytes: everything a CTA needs to start its bulk copies
   int constraint;
-  int start;
+  int unit0;                 // index of the tile's first unit in the unit-bound table
   int count;
   int grid_bytes;            // bytes of the 16-bit block grid to stage (multiple of 16), 0: hash path
   const float* pts;          // first unit of the tile (unit-major points)
@@ -46,11 +46,15 @@ struct __align__(16) RegTile {   // 32 bytes: everything a CTA needs to start it
 void vgx_launch_reg_pose_setup(cudaStream_t st, const RegConstraintDev* cons, const double* x,
                                RegPoseConst* poses, int n, const int* skip = nullptr);
 // One CTA per tile (or persistent CTAs walking their tiles) -> partials[tile][21]; the consumer adds
-// a constraint's tiles in tile order (graph.cu: reg_constraint_sum).
+// a constraint's tiles in tile order (graph.cu: reg_constraint_sum).  unit_bounds (may be null: no
+// culling): the table vgx_launch_reg_unit_bounds fills, indexed by RegTile::unit0 + unit.
 void vgx_launch_reg_reduce(cudaStream_t st, const RegConstraintDev* cons, const RegPoseConst* poses,
                            const RegTile* tiles, int n_ctas, const int* cta_tile_begin,
                            const int* tile_order, int* tile_cost, double* partials, int grid_capacity,
-                           bool jacobian, const int* skip = nullptr);
+                           const float4* unit_bounds, bool jacobian, const int* skip = nullptr);
+// bounds[tile.unit0 + u] <- a sphere (centre xyz, radius w) around the points of unit u of every tile
+// that can contribute (radius +inf: the unit is never culled)
+void vgx_launch_reg_unit_bounds(cudaStream_t st, const RegTile* tiles, int n_tiles, float4* bounds);
 // tile_order <- tiles sorted by measured cost, most expensive first (one-CTA-per-tile mode)
 void vgx_launch_reg_order(cudaStream_t st, const int* tile_cost, int n_tiles, int* tile_order);
 // persistent grid size: SMs x CTAs that are co-resident with `grid_capacity` cells of dynamic smem
