@@ -6,6 +6,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <type_traits>
+
 // ------------------------------------------------------------------ emit mode
 // One thread per registration point; writes the normalised residual and the two 1x4
 // Jacobian rows exactly as Evaluate leaves them for Ceres (cpp:254-291).
@@ -289,64 +291,16 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
         if (j < n_live) issue(it + j);
     }
     double d0 = 0.0, d1 = 0.0;
-    const size_t vox_shift = 3 * s_C.vps_shift;
-    const float4* view = reinterpret_cast<const float4*>(s_C.view);
 
-    // stage A: everything up to the ISSUE of the octet load
-    struct Pipe { float4 lo, hi; float ox, oy, oz; bool found; };
-    auto stage_a = [&](uint32_t seq, Pipe& R) {
-      const uint32_t slot = seq % kRing;
-      mbar_wait(bar0 + 8u * slot, (seq / kRing) & 1u);
-      const float* sp = ringf + 160 * slot + lane;
-      float p0, p1, p2;
-      vgx_reg_transform(P, sp[0], sp[32], sp[64], p0, p1, p2);
-      const float qnan = __int_as_float(0x7fc00000);
-      R.lo = make_float4(qnan, qnan, qnan, qnan);
-      R.hi = R.lo;
-      R.found = false;
-      R.ox = R.oy = R.oz = 0.f;
-      int b0, b1, b2;
-      vgx_block_index(s_C, p0, p1, p2, b0, b1, b2);
-      RegLocate L;
-      int slot_b;
-      if (use_grid) {
-#if VGX_REG_EARLYOUT
-        // getVoxelsAndQVector fails right away when the block that contains pos does not exist;
-        // overlapping submaps share only part of their surface and consecutive points are
-        // spatially coherent: most warps miss with all 32 lanes and skip the rest of the unit
-        const bool hit = vgx_grid_slot(s_C, s_grid, b0, b1, b2) >= 0;
-        if (!__any_sync(0xffffffffu, hit)) return;
-        vgx_locate_in_block<true>(s_C, p0, p1, p2, b0, b1, b2, L, s_grid);
-        slot_b = hit ? L.slot : -1;
-#else
-        vgx_locate_in_block<true>(s_C, p0, p1, p2, b0, b1, b2, L, s_grid);
-        slot_b = L.slot;
-#endif
-      } else {
-        vgx_locate_in_block<false>(s_C, p0, p1, p2, b0, b1, b2, L);
-        slot_b = vgx_resolve(s_C, L);
-      }
-      R.found = slot_b >= 0;
-      R.ox = L.ox; R.oy = L.oy; R.oz = L.oz;
-      if (R.found) {
-        const float4* o = view + 2 * (((size_t)slot_b << vox_shift) + (size_t)L.lin);
-        // the whole 32-byte octet = one sector = two 128-bit loads (sm_90 has no 256-bit LDG)
-        R.lo = __ldg(o); R.hi = __ldg(o + 1);
-      }
-    };
-    // stage B: consume the octet issued one unit ago
+    // a lane without a correspondence carries an all-NaN octet
+    struct Pipe { float4 lo, hi; float ox, oy, oz; };
+    // stage B: consume the octet issued by stage A
     auto stage_b = [&](uint32_t seq, const Pipe& R) {
       const float* sp = ringf + 160 * (seq % kRing) + lane;
       const float d[8] = {R.lo.x, R.lo.y, R.lo.z, R.lo.w, R.hi.x, R.hi.y, R.hi.z, R.hi.w};
-#if VGX_REG_SKIPGRAM
-      bool ok = false;
-      if (__any_sync(0xffffffffu, R.found)) ok = R.found && vgx_octet_ok(d);
-      const bool work = gram_always || __any_sync(0xffffffffu, ok);
-#else
-      const bool ok = R.found && vgx_octet_ok(d);
-      const bool work = true;
-#endif
-      if (work) {
+      // a unit without a single correspondence adds nothing unless a missing one costs something
+      const bool ok = vgx_octet_ok(d);
+      if (gram_always || __any_sync(0xffffffffu, ok)) {
         const float xi = sp[0], yi = sp[32], dist = sp[96], w = sp[128];
         const RegPointResult Q = vgx_reg_math<kJacobian>(s_C, P, xi, yi, dist, w, ok, d, R.ox, R.oy, R.oz);
 #if defined(VGX_X_NOGRAM)
@@ -375,7 +329,49 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
       __syncwarp();  // every lane is done with this unit's ring slot and the Gram staging buffer
     };
 
-    if (n_live > 0) {
+    // The tile's pipeline, instantiated once per lookup path (use_grid is uniform across the CTA):
+    // kGrid, the reading submap's block grid staged in shared memory, or its hash in global memory.
+    auto run_tile = [&](auto path) {
+      constexpr bool kGrid = decltype(path)::value;
+      // stage A: everything up to the ISSUE of the octet load
+      auto stage_a = [&](uint32_t seq, Pipe& R) {
+        const uint32_t slot = seq % kRing;
+        mbar_wait(bar0 + 8u * slot, (seq / kRing) & 1u);
+        const float* sp = ringf + 160 * slot + lane;
+        float p0, p1, p2;
+        vgx_reg_transform(P, sp[0], sp[32], sp[64], p0, p1, p2);
+        const float qnan = __int_as_float(0x7fc00000);
+        R.lo = make_float4(qnan, qnan, qnan, qnan);
+        R.hi = R.lo;
+        R.ox = R.oy = R.oz = 0.f;
+        int b0, b1, b2;
+        vgx_block_index(s_C, p0, p1, p2, b0, b1, b2);
+        RegLocate L;
+        int slot_b;
+        if constexpr (kGrid) {
+          // getVoxelsAndQVector fails right away when the block that contains pos does not exist;
+          // overlapping submaps share only part of their surface and consecutive points are
+          // spatially coherent: most warps miss with all 32 lanes and skip the rest of the unit
+          const int slot_c = vgx_grid_slot(s_C, s_grid, b0, b1, b2);
+          if (!__any_sync(0xffffffffu, slot_c >= 0)) return;
+          vgx_locate_in_block(s_C, p0, p1, p2, b0, b1, b2, L);
+          // the base corner lies in another block only when it moved into a lower neighbour
+          const bool moved = (L.b0 != b0) | (L.b1 != b1) | (L.b2 != b2);
+          const int slot_m = moved ? vgx_grid_slot(s_C, s_grid, L.b0, L.b1, L.b2) : slot_c;
+          slot_b = slot_c >= 0 ? slot_m : -1;
+        } else {
+          vgx_locate_in_block(s_C, p0, p1, p2, b0, b1, b2, L);
+          RegProbe H = vgx_probe_start(s_C, L);
+          slot_b = vgx_resolve(s_C, H);
+        }
+        R.ox = L.ox; R.oy = L.oy; R.oz = L.oz;
+        if (slot_b >= 0) {
+          const float4* o = reinterpret_cast<const float4*>(s_C.view) +
+                            2 * (((size_t)slot_b << (3 * s_C.vps_shift)) + (size_t)L.lin);
+          // the whole 32-byte octet = one sector = two 128-bit loads (sm_90 has no 256-bit LDG)
+          R.lo = __ldg(o); R.hi = __ldg(o + 1);
+        }
+      };
       // two register sets alternate (loop unrolled by two): the in-flight octet is never copied
       Pipe Ra, Rb;
       stage_a(it, Ra);
@@ -388,10 +384,11 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
         if (j + 2 < n_live) stage_a(it + 2, Ra);
         stage_b(it + 1, Rb);
       }
-      if (j < n_live) {
-        stage_b(it, Ra);
-        ++it;
-      }
+      if (j < n_live) stage_b(it++, Ra);
+    };
+    if (n_live > 0) {
+      if (use_grid) run_tile(std::true_type());
+      else run_tile(std::false_type());
     }
     // ---- tile epilogue: warp Gram fragments -> 21 sums -> partials[tile]
     if (kJacobian) {

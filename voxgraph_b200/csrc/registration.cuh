@@ -132,8 +132,9 @@ __device__ __forceinline__ int vgx_floor_idx(float v) { return __float2int_rd(v)
 // getVoxelsAndQVector on the octet view, split into phases so that a thread working on several
 // points can keep their loads in flight together:
 //   locate : base corner voxel (the one whose centre is <= pos on every axis, possibly in the
-//            lower neighbour block) + first hash probe issued
-//   resolve: finish the probe sequence -> brick slot
+//            lower neighbour block) and the q-vector offsets
+//   probe  : hash path only: first hash probe issued (vgx_probe_start), then the probe sequence
+//            finished -> brick slot (vgx_resolve); the block grid path looks the slot up instead
 //   fetch  : the voxel's 2x2x2 octet (two 128-bit loads), NaN test
 // Returns false when the base block is missing or any corner is unobserved / in a missing
 // block (NaN baked into the view).  The reference's first lookup of the block containing pos
@@ -141,11 +142,12 @@ __device__ __forceinline__ int vgx_floor_idx(float v) { return __float2int_rd(v)
 struct RegLocate {
   float ox, oy, oz;   // q-vector offsets
   int lin;            // voxel index inside the brick
+  int b0, b1, b2;     // block of the base corner voxel
+};
+struct RegProbe {
   uint32_t h;         // current hash table index
   uint64_t key;
   int4 e;             // probed entry
-  int slot;           // kGrid: resolved directly from the shared-memory block grid
-  int b0, b1, b2;     // block of the base corner voxel
 };
 
 // step (1) of getVoxelsAndQVector: index of the block that contains pos
@@ -166,60 +168,68 @@ __device__ __forceinline__ int vgx_grid_slot(const RegConstraintDev& C, const ui
   return gs == 0xFFFF ? -1 : gs;
 }
 
-template <bool kGrid>
-__device__ __forceinline__ void vgx_locate_in_block(const RegConstraintDev& C, float p0, float p1,
-                                                    float p2, int b0, int b1, int b2, RegLocate& L,
-                                                    const uint16_t* __restrict__ s_grid = nullptr,
-                                                    bool no_lookup = false) {
+// One axis of the base-corner selection.  In: b = the block that contains p.  Out: v = the voxel of
+// the base corner, b moved to the lower neighbour block when that corner lies in it, o = the q-vector
+// offset from the corner.  The reference moves the voxel index down by one when p lies below the
+// voxel centre and then recomputes the corner's centre from the moved indices; here the moved centre
+// is selected instead, computed from the same float values:
+//   (float)(v - 1) + 0.5f == fv - 0.5f       v is a small integer: both are exact
+//   (float)(b - 1) == fb - 1.0f              b is the floor of a float, so fb == b exactly and both
+//                                            are b - 1 rounded once (a saturated b has no block)
+//   (float)(vps - 1) + 0.5f == vps - 0.5f    exact
+// so every corner coordinate, and with it o, is bit-identical to the reference's.
+__device__ __forceinline__ void vgx_corner_axis(const RegConstraintDev& C, float p, int& b, int& v, float& o) {
   const int vps = C.vps;
-  const float or0 = (float)b0 * C.block_size, or1 = (float)b1 * C.block_size,
-              or2 = (float)b2 * C.block_size;
-  int v0 = vgx_floor_idx((p0 - or0) * C.voxel_size_inv + VGX_COORD_EPS);
-  int v1 = vgx_floor_idx((p1 - or1) * C.voxel_size_inv + VGX_COORD_EPS);
-  int v2 = vgx_floor_idx((p2 - or2) * C.voxel_size_inv + VGX_COORD_EPS);
-  v0 = max(min(v0, vps - 1), 0);
-  v1 = max(min(v1, vps - 1), 0);
-  v2 = max(min(v2, vps - 1), 0);
-  if (p0 - (or0 + ((float)v0 + 0.5f) * C.voxel_size) < 0) {
-    if (--v0 < 0) { --b0; v0 += vps; }
-  }
-  if (p1 - (or1 + ((float)v1 + 0.5f) * C.voxel_size) < 0) {
-    if (--v1 < 0) { --b1; v1 += vps; }
-  }
-  if (p2 - (or2 + ((float)v2 + 0.5f) * C.voxel_size) < 0) {
-    if (--v2 < 0) { --b2; v2 += vps; }
-  }
+  const float fb = (float)b;
+  const float orb = fb * C.block_size;
+  v = vgx_floor_idx((p - orb) * C.voxel_size_inv + VGX_COORD_EPS);
+  v = max(min(v, vps - 1), 0);
+  const float fv = (float)v;
+  const float cv = (fv + 0.5f) * C.voxel_size;
+  const bool down = p - (orb + cv) < 0;   // the corner is the voxel below
+  const bool wrap = down && v == 0;       // ... and it lies in block b - 1
+  const float ob = wrap ? (fb - 1.0f) * C.block_size : orb;
+  const float oc = down ? ((wrap ? (float)vps : fv) - 0.5f) * C.voxel_size : cv;
+  b = wrap ? b - 1 : b;
+  v = down ? (wrap ? vps - 1 : v - 1) : v;
+  o = (p - (ob + oc)) * C.voxel_size_inv;
+}
+
+// b0..b2: the block that contains p (vgx_block_index) -> L (base corner block, voxel, q offsets)
+__device__ __forceinline__ void vgx_locate_in_block(const RegConstraintDev& C, float p0, float p1,
+                                                    float p2, int b0, int b1, int b2, RegLocate& L) {
+  int v0, v1, v2;
+  vgx_corner_axis(C, p0, b0, v0, L.ox);
+  vgx_corner_axis(C, p1, b1, v1, L.oy);
+  vgx_corner_axis(C, p2, b2, v2, L.oz);
   L.b0 = b0; L.b1 = b1; L.b2 = b2;
-  if (kGrid) {
-    L.slot = vgx_grid_slot(C, s_grid, b0, b1, b2);
-  } else if (!no_lookup) {
-    L.key = vgx_pack_key(b0, b1, b2);
-    L.h = vgx_hash_index(b0, b1, b2, C.hash.mask);
-    L.e = __ldg(reinterpret_cast<const int4*>(C.hash.entries + L.h));
-  }
-  // q vector offsets from the base corner (block origin recomputed from the moved index)
-  L.ox = (p0 - ((float)b0 * C.block_size + ((float)v0 + 0.5f) * C.voxel_size)) * C.voxel_size_inv;
-  L.oy = (p1 - ((float)b1 * C.block_size + ((float)v1 + 0.5f) * C.voxel_size)) * C.voxel_size_inv;
-  L.oz = (p2 - ((float)b2 * C.block_size + ((float)v2 + 0.5f) * C.voxel_size)) * C.voxel_size_inv;
   const int sh = C.vps_shift;
   L.lin = v0 + (v1 << sh) + (v2 << (2 * sh));
 }
 
-template <bool kGrid>
 __device__ __forceinline__ void vgx_locate(const RegConstraintDev& C, float p0, float p1, float p2,
-                                           RegLocate& L, const uint16_t* __restrict__ s_grid = nullptr) {
+                                           RegLocate& L) {
   int b0, b1, b2;
   vgx_block_index(C, p0, p1, p2, b0, b1, b2);
-  vgx_locate_in_block<kGrid>(C, p0, p1, p2, b0, b1, b2, L, s_grid);
+  vgx_locate_in_block(C, p0, p1, p2, b0, b1, b2, L);
 }
 
-__device__ __forceinline__ int vgx_resolve(const RegConstraintDev& C, RegLocate& L) {
+// first probe of the base corner's block in the reading submap's hash (load issued)
+__device__ __forceinline__ RegProbe vgx_probe_start(const RegConstraintDev& C, const RegLocate& L) {
+  RegProbe H;
+  H.key = vgx_pack_key(L.b0, L.b1, L.b2);
+  H.h = vgx_hash_index(L.b0, L.b1, L.b2, C.hash.mask);
+  H.e = __ldg(reinterpret_cast<const int4*>(C.hash.entries + H.h));
+  return H;
+}
+
+__device__ __forceinline__ int vgx_resolve(const RegConstraintDev& C, RegProbe& H) {
   for (;;) {
-    const uint64_t k = (uint64_t)(uint32_t)L.e.x | ((uint64_t)(uint32_t)L.e.y << 32);
-    if (k == L.key) return L.e.z;
+    const uint64_t k = (uint64_t)(uint32_t)H.e.x | ((uint64_t)(uint32_t)H.e.y << 32);
+    if (k == H.key) return H.e.z;
     if (k == VGX_EMPTY_KEY) return -1;
-    L.h = (L.h + 1) & C.hash.mask;
-    L.e = __ldg(reinterpret_cast<const int4*>(C.hash.entries + L.h));
+    H.h = (H.h + 1) & C.hash.mask;
+    H.e = __ldg(reinterpret_cast<const int4*>(C.hash.entries + H.h));
   }
 }
 
@@ -234,8 +244,9 @@ __device__ __forceinline__ bool vgx_interp_gather(const RegConstraintDev& C, flo
                                                   float p2, float d[8], float& ox, float& oy,
                                                   float& oz) {
   RegLocate L;
-  vgx_locate<false>(C, p0, p1, p2, L);
-  const int slot = vgx_resolve(C, L);
+  vgx_locate(C, p0, p1, p2, L);
+  RegProbe H = vgx_probe_start(C, L);
+  const int slot = vgx_resolve(C, H);
   if (slot < 0) return false;
   ox = L.ox; oy = L.oy; oz = L.oz;
   const size_t lin = ((size_t)slot << (3 * C.vps_shift)) + L.lin;
@@ -310,62 +321,6 @@ __device__ __forceinline__ RegPointResult vgx_reg_math(const RegConstraintDev& C
     R.je3 = m0 * ae03 + m1 * ae13;
   }
   return R;
-}
-
-// Branch-free form of vgx_reg_math for the fused reduce kernel: everything is computed, the
-// "interpolation impossible" case is selected at the end (NaN octets just flow through), so two
-// points per lane can be scheduled as two independent instruction streams.  Same operations in
-// the same order as vgx_reg_math -> identical values.
-__device__ __forceinline__ void vgx_reg_math_nb(const RegConstraintDev& C, const RegPoseConst& P,
-                                                float xi, float yi, float dist, float w, bool ok,
-                                                const float4& lo, const float4& hi, float ox, float oy,
-                                                float oz, double& r_out, float jr[4], float& je3) {
-  const float d0 = lo.x, d1 = lo.y, d2 = lo.z, d3 = lo.w, d4 = hi.x, d5 = hi.y, d6 = hi.z, d7 = hi.w;
-  const float a0 = d0;
-  const float a1 = -d0 + d4;
-  const float a2 = -d0 + d2;
-  const float a3 = -d0 + d1;
-  const float a4 = d0 - d2 - d4 + d6;
-  const float a5 = d0 - d1 - d2 + d3;
-  const float a6 = d0 - d1 - d4 + d5;
-  const float a7 = -d0 + d1 + d2 - d3 + d4 - d5 - d6 + d7;
-  const float q4 = ox * oy, q5 = oy * oz, q6 = oz * ox, q7 = ox * oy * oz;
-  float interp = 1.0f * a0;
-  interp = interp + ox * a1;
-  interp = interp + oy * a2;
-  interp = interp + oz * a3;
-  interp = interp + q4 * a4;
-  interp = interp + q5 * a5;
-  interp = interp + q6 * a6;
-  interp = interp + q7 * a7;
-  const double r = ((double)dist - (double)interp) * (double)w;  // cpp:158-163
-  const float finv = C.voxel_size_inv;
-  const float iDx = finv * ox, iDy = finv * oy, iDz = finv * oz;
-  const double inv = (double)finv;
-  const double Dx = (double)ox, Dy = (double)oy, Dz = (double)oz;
-  const double iDyd = inv * Dy, iDxd = inv * Dx;
-  const float iDyDz = (float)(iDyd * Dz), iDxDz = (float)(iDxd * Dz), iDxDy = (float)(iDxd * Dy);
-  float g0 = a1 * finv;
-  g0 = g0 + a4 * iDy; g0 = g0 + a6 * iDz; g0 = g0 + a7 * iDyDz;
-  float g1 = a2 * finv;
-  g1 = g1 + a4 * iDx; g1 = g1 + a5 * iDz; g1 = g1 + a7 * iDxDz;
-  float g2 = a3 * finv;
-  g2 = g2 + a5 * iDy; g2 = g2 + a6 * iDx; g2 = g2 + a7 * iDxDy;
-  const float ar03 = xi * P.sin_emo - yi * P.cos_emo;
-  const float ar13 = xi * P.cos_emo + yi * P.sin_emo;
-  const float ae03 = -xi * P.sin_emo + yi * P.cos_emo + P.dxs - P.dyc;
-  const float ae13 = -xi * P.cos_emo - yi * P.sin_emo + P.dxc + P.dys;
-  const float m0 = -w * g0, m1 = -w * g1, m2 = -w * g2;
-  const float j0 = m0 * P.cos_e + m1 * (-P.sin_e);
-  const float j1 = m0 * P.sin_e + m1 * P.cos_e;
-  const float j3 = m0 * ar03 + m1 * ar13;
-  const float j4 = m0 * ae03 + m1 * ae13;
-  r_out = ok ? r : (double)w * C.no_corr;  // cpp:164-166
-  jr[0] = ok ? j0 : 0.f;
-  jr[1] = ok ? j1 : 0.f;
-  jr[2] = ok ? m2 : 0.f;
-  jr[3] = ok ? j3 : 0.f;
-  je3 = ok ? j4 : 0.f;
 }
 
 // cpp:128-129  reading_coordinate = T_reading__reference * reference_coordinate

@@ -10,17 +10,12 @@ struct RegPoseConst;
 #define VGX_REG_THREADS 128        // 4 warps per CTA, each with its own TMA ring + software pipeline
 #endif
 #ifndef VGX_REG_MIN_BLOCKS
-#define VGX_REG_MIN_BLOCKS 6       // resident CTAs per SM the register budget is sized for (80 registers;
-                                   // sm_90a spills at the 72 that 7 would allow, for the same step time)
+#define VGX_REG_MIN_BLOCKS 7       // resident CTAs per SM the register budget is sized for (72 registers).
+                                   // 8 also fits without spills, but the tile size follows the resident CTA
+                                   // count (graph.cu), so config 2's tiles and with them its sums would change
 #endif
 #ifndef VGX_REG_RING
 #define VGX_REG_RING 4             // point-slice ring slots per warp (units in flight = RING - 1)
-#endif
-#ifndef VGX_REG_EARLYOUT
-#define VGX_REG_EARLYOUT 1         // a warp whose 32 points all miss the containing block skips the unit
-#endif
-#ifndef VGX_REG_SKIPGRAM
-#define VGX_REG_SKIPGRAM 1         // no Gram stage for a unit without a single correspondence
 #endif
 #ifndef VGX_REG_HW_TILE_UNITS
 #define VGX_REG_HW_TILE_UNITS 64   // > 0: one CTA per tile of that many units (hardware scheduling); 0: persistent
