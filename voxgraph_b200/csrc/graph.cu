@@ -503,9 +503,12 @@ __device__ __forceinline__ double fast_rsqrt(double d) {
 
 // Blocked right-looking Cholesky of the (n+1) x (n+1) lower-triangular system, one CTA.
 // smem: sD[32][33] diagonal block, sP[(M - 32)][33] panel.
+// A pivot d_k fails when !(d_k > 0); with diag0 (the unfactored diagonal, covariances only) it also
+// fails when d_k <= rank_tol * diag0[k] (see VGX_COV_RANK_TOL).
 #define CH_NB 32
 __global__ void __launch_bounds__(1024) chol_kernel(double* __restrict__ A, int n,
-                                                    LmState* __restrict__ st) {
+                                                    LmState* __restrict__ st,
+                                                    const double* __restrict__ diag0, double rank_tol) {
   extern __shared__ double smem[];
   if (st->done) return;
   double* sD = smem;                 // 32 x 33
@@ -529,7 +532,8 @@ __global__ void __launch_bounds__(1024) chol_kernel(double* __restrict__ A, int 
       const int r = tid;
       for (int k = 0; k < nb; ++k) {
         double d = sD[k * 33 + k];
-        if (!(d > 0.0) || !isfinite(d)) { if (r == 0) s_fail = 1; d = 1.0; }
+        const double floor_k = diag0 ? rank_tol * diag0[j0 + k] : 0.0;
+        if (!(d > floor_k) || !isfinite(d)) { if (r == 0) s_fail = 1; d = 1.0; }
         const double rs = fast_rsqrt(d);
         __syncwarp();
         if (r == k) { sD[k * 33 + k] = d * rs; sDinv[k] = rs; }
@@ -788,8 +792,10 @@ chol_solve_smem_kernel(const double* __restrict__ A, int n, double* __restrict__
 // Multi-CTA variant (cooperative launch, grid-wide barriers): every CTA factors the 32x32
 // diagonal block redundantly in shared memory (deterministic, saves a barrier), the panel rows
 // and the 32x32 trailing tiles are spread over the grid.  Two grid syncs per panel.
+// diag0 / rank_tol: as chol_kernel.
 __global__ void __launch_bounds__(256) chol_coop_kernel(double* __restrict__ A, int n,
-                                                        LmState* __restrict__ st) {
+                                                        LmState* __restrict__ st,
+                                                        const double* __restrict__ diag0, double rank_tol) {
   cg::grid_group grid = cg::this_grid();
   if (st->done) return;   // uniform over the grid
   __shared__ double sD[CH_NB * 33];
@@ -813,7 +819,8 @@ __global__ void __launch_bounds__(256) chol_coop_kernel(double* __restrict__ A, 
       const int r = tid;
       for (int k = 0; k < nb; ++k) {
         double d = sD[k * 33 + k];
-        if (!(d > 0.0) || !isfinite(d)) { if (r == 0) s_fail = 1; d = 1.0; }
+        const double floor_k = diag0 ? rank_tol * diag0[j0 + k] : 0.0;
+        if (!(d > floor_k) || !isfinite(d)) { if (r == 0) s_fail = 1; d = 1.0; }
         const double rs = fast_rsqrt(d);
         __syncwarp();
         if (r == k) { sD[k * 33 + k] = d * rs; sDinv[k] = rs; }
@@ -1731,9 +1738,19 @@ extern "C" int vgx_graph_registration_costs(vgx_ctx* c, double* per_constraint) 
 // poses (no LM damping, no Jacobi scaling, no loss function); constant blocks have zero covariance.
 // Dense reduced H -> Cholesky (the solver's factorisation kernels) -> two triangular solves per
 // requested column.
+//
+// ceres::Covariance::Compute returns false when J^T J is rank deficient.  A plain sign test on the
+// pivots cannot decide that: on a graph without a constant node (a 4-dimensional gauge null space)
+// the null-space pivots come out within ~1e-14 of 0 relative to their diagonal, with either sign,
+// so the result would be the error or finite covariances of ~1e14 depending on rounding.  A pivot
+// d_k <= VGX_COV_RANK_TOL * H_kk is therefore taken as rank deficient.  1e-10 lies 4 orders above
+// that rounding noise and 7 below the smallest relative pivot of anchored chains (4e-3 for
+// 64..250-node chains with condition numbers up to 4e8; tests/test_host_dense_solve.py checks both
+// margins).  It approximates Ceres' rank decision (SPARSE_QR's) rather than restating it.
+#define VGX_COV_RANK_TOL 1e-10
 __global__ void cov_build_kernel(const double* __restrict__ packed, const int* __restrict__ red,
                                  const int* __restrict__ block_nodes, int N, int E, int n,
-                                 double* __restrict__ A) {
+                                 double* __restrict__ A, double* __restrict__ diag0) {
   const int M = n + 1;
   const double* D = packed + PACK_HDR + 4 * (size_t)N;
   const double* O = D + 16 * (size_t)N;
@@ -1743,6 +1760,7 @@ __global__ void cov_build_kernel(const double* __restrict__ packed, const int* _
     const int off = red[node];
     if (off < 0 || r < c) continue;
     A[(size_t)(off + c) * M + off + r] = D[16 * (size_t)node + 4 * r + c];
+    if (r == c) diag0[off + r] = D[16 * (size_t)node + 4 * r + c];
   }
   for (int t = tid; t < E * 16; t += stride) {
     const int b = t >> 4, r = (t >> 2) & 3, c = t & 3;
@@ -1831,12 +1849,21 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
   rc = eval_enqueue(c, g, g->d_x, g->d_packed[0], true, false);
   if (rc != VGX_OK) return rc;
   const size_t M = (size_t)n + 1;
+  // scratch: requested column indices | X (ncols x n) | the unfactored diagonal (n)
+  const size_t ncols = cols.size();
+  const size_t x_off = (sizeof(int) * ncols + 255) & ~(size_t)255;
+  rc = c->ensure_scratch(x_off + sizeof(double) * (ncols + 1) * (size_t)n);
+  if (rc != VGX_OK) return rc;
+  int* d_cols = (int*)c->d_scratch;
+  double* d_X = (double*)((char*)c->d_scratch + x_off);
+  double* d_diag0 = d_X + ncols * (size_t)n;
   VGX_CUDA(c, cudaMemsetAsync(g->d_A, 0, sizeof(double) * M * M, st));
   {
     VgxLaunchScope s(c, 4);
     const int nthreads = 16 * (N + g->E);
     cov_build_kernel<<<std::min(296, (nthreads + 255) / 256), 256, 0, st>>>(g->d_packed[0], g->d_red_offset,
-                                                                          g->d_block_nodes, N, g->E, n, g->d_A);
+                                                                          g->d_block_nodes, N, g->E, n, g->d_A,
+                                                                          d_diag0);
   }
   // factorise with the solver's kernels (the rhs row n of the augmented matrix stays zero)
   VGX_CUDA(c, cudaMemsetAsync(g->d_state, 0, sizeof(LmState), st));
@@ -1858,24 +1885,20 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
       const int tiles = ((n + 1 + CH_NB - 1) / CH_NB) * ((n + CH_NB - 1) / CH_NB);
       coop_grid = std::max(1, std::min(sms * std::min(per_sm, 2), std::max(tiles / 2, (n + 256) / 256)));
     }
+    double tol = VGX_COV_RANK_TOL;
     if (coop_grid > 0) {
       int n_arg = n;
-      void* args[] = {(void*)&g->d_A, (void*)&n_arg, (void*)&g->d_state};
+      void* args[] = {(void*)&g->d_A, (void*)&n_arg, (void*)&g->d_state, (void*)&d_diag0, (void*)&tol};
       VGX_CUDA(c, cudaLaunchCooperativeKernel((void*)chol_coop_kernel, dim3(coop_grid), dim3(256), args, 0, st));
     } else {
       if (chol_smem > 227 * 1024)
         VGX_FAIL(c, VGX_ERR_CAPACITY, "pose graph too large for the single-CTA dense factorisation");
       VGX_CUDA(c, cudaFuncSetAttribute(chol_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)chol_smem));
-      chol_kernel<<<1, 1024, chol_smem, st>>>(g->d_A, n, g->d_state);
+      chol_kernel<<<1, 1024, chol_smem, st>>>(g->d_A, n, g->d_state, d_diag0, tol);
     }
   }
   VGX_CUDA(c, cudaGetLastError());
   // inverse columns
-  const size_t ncols = cols.size();
-  rc = c->ensure_scratch(sizeof(int) * ncols + 256 + sizeof(double) * ncols * (size_t)n);
-  if (rc != VGX_OK) return rc;
-  int* d_cols = (int*)c->d_scratch;
-  double* d_X = (double*)((char*)c->d_scratch + ((sizeof(int) * ncols + 255) & ~(size_t)255));
   VGX_CUDA(c, cudaMemcpyAsync(d_cols, cols.data(), sizeof(int) * ncols, cudaMemcpyHostToDevice, st));
   if (sizeof(double) * (size_t)n > 48 * 1024)
     VGX_CUDA(c, cudaFuncSetAttribute(cov_column_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -1890,7 +1913,7 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
   VGX_CUDA(c, cudaMemcpyAsync(X.data(), d_X, sizeof(double) * X.size(), cudaMemcpyDeviceToHost, st));
   VGX_CUDA(c, cudaMemcpyAsync(&hs, g->d_state, sizeof(hs), cudaMemcpyDeviceToHost, st));
   VGX_CUDA(c, cudaStreamSynchronize(st));
-  if (!hs.step_valid)   // ceres::Covariance::Compute returns false on a rank-deficient Jacobian
+  if (!hs.step_valid)   // a pivot failed the rank rule above (ceres::Covariance::Compute returns false)
     VGX_FAIL(c, VGX_ERR_INVALID, "vgx_graph_edge_covariances: J^T J is not positive definite (rank deficient)");
   for (int k = 0; k < m; ++k) {
     const int a = pr[k].first, b = pr[k].second;
@@ -2022,10 +2045,12 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
                                                                 g->d_block_nodes, N, g->E, d_chol_dbg);
       } else if (coop_grid > 0) {
         int n_arg = n;
-        void* args[] = {(void*)&g->d_A, (void*)&n_arg, (void*)&g->d_state};
+        const double* no_diag = nullptr;   // LM: sign test only (as Eigen's LLT in the reference)
+        double no_tol = 0.0;
+        void* args[] = {(void*)&g->d_A, (void*)&n_arg, (void*)&g->d_state, (void*)&no_diag, (void*)&no_tol};
         VGX_CUDA(c, cudaLaunchCooperativeKernel((void*)chol_coop_kernel, dim3(coop_grid), dim3(256), args, 0, st));
       } else {
-        chol_kernel<<<1, 1024, chol_smem, st>>>(g->d_A, n, g->d_state);
+        chol_kernel<<<1, 1024, chol_smem, st>>>(g->d_A, n, g->d_state, nullptr, 0.0);
       }
       lm_step_kernel<<<1, 1024, sizeof(double) * n, st>>>(g->d_A, n, N, g->d_red_offset, g->d_scale,
                                                          g->d_diag, g->d_gs, g->d_x, g->d_xc, g->d_step,
