@@ -1,7 +1,7 @@
 """Backward-error checks of the dense pose-graph solves (test support; importable without a GPU).
 
 The Levenberg-Marquardt step and the edge covariances go through hand-written Cholesky kernels
-(graph.cu: chol_solve_smem_kernel, chol_coop_kernel + lm_step_kernel, chol_kernel + cov_column_kernel).
+(solve.cu: chol_solve_smem_kernel, chol_coop_kernel + lm_step_kernel, chol_coop_kernel + cov_column_kernel).
 Converged poses cannot pin them: LM corrects a step that is wrong by 1e-6 relative in its next
 iteration.  What a correct float64 Cholesky solve guarantees, whatever the conditioning, is a small
 backward error (Higham, Accuracy and Stability of Numerical Algorithms, Thm 10.4):
@@ -22,16 +22,15 @@ import numpy as np
 
 U = 2.0 ** -53                 # unit roundoff of float64
 SLACK = 8                      # fast_rsqrt (a few ulps) and the restated A (fma on the diagonal)
-RANK_TOL = 1e-10               # graph.cu VGX_COV_RANK_TOL: pivot <= tol * H_kk is rank deficient
+RANK_TOL = 1e-10               # solve.cu VGX_COV_RANK_TOL: pivot <= tol * H_kk is rank deficient
 FRAME_ID = 0x80000000          # api.FRAME_NODE_ID_BASE: reference-frame node 0
 INFO_ODOM = np.diag([1.0, 1.0, 2500.0, 2500.0])
 
-# Dispatch edges of graph.cu (tests/test_host_dense_solve.py derives them from the source):
+# Dispatch edges of solve.cu (tests/test_host_dense_solve.py derives them from the source):
 # the LM factors in shared memory up to n = 232 and on the cooperative grid from 236; the
-# covariances use chol_kernel up to n = 256 and chol_coop_kernel beyond.
+# covariances always use the cooperative grid (252 | 256 | 260 cross one of its panel edges).
 SMEM_MAX_N = 232
 COOP_MIN_N = 236
-COV_SWITCH_N = 256
 LM_SIZES = [4, 8, 12, 28, 32, 36, 124, 128, 132, 228, 232, 236, 252, 256, 260, 796, 1000]
 COV_SIZES = [4, 20, 32, 36, 64, 68, 252, 256, 260, 796]
 

@@ -1,8 +1,8 @@
 """The device's dense solves against a backward-error bound (tests/solve_exact.py).
 
-LM first and second steps at sizes straddling every dispatch edge of graph.cu (shared-memory FP64-MMA
-Cholesky up to n = 232, the cooperative grid from 236), edge covariances on chol_kernel (n <= 256)
-and chol_coop_kernel (beyond), and the rank rule of getEdgeCovarianceMap."""
+LM first and second steps at sizes straddling the dispatch edge of solve.cu (shared-memory FP64-MMA
+Cholesky up to n = 232, the cooperative grid from 236), edge covariances (always on the cooperative
+grid) and the rank rule of getEdgeCovarianceMap."""
 import numpy as np
 import pytest
 
@@ -134,7 +134,7 @@ def _check_covariances(ctx, spec, path):
 
 
 def _cov_path(n):
-    return "covariance chol_kernel" if n <= SX.COV_SWITCH_N else "covariance coop"
+    return "covariance n <= 256" if n <= 256 else "covariance n > 256"
 
 
 @pytest.mark.parametrize("n", SX.COV_SIZES)

@@ -1,5 +1,5 @@
 """The backward-error harness of tests/solve_exact.py, checked on the oracle's plain float64 Cholesky,
-and the dispatch sizes and rank rule it assumes, read from graph.cu."""
+and the dispatch sizes and rank rule it assumes, read from solve.cu."""
 import os
 import re
 
@@ -11,8 +11,8 @@ import solve_exact as SX
 CSRC = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "voxgraph_b200", "csrc")
 
 
-def _graph_src():
-    with open(os.path.join(CSRC, "graph.cu")) as f:
+def _solve_src():
+    with open(os.path.join(CSRC, "solve.cu")) as f:
         return f.read()
 
 
@@ -83,10 +83,15 @@ def test_rank_threshold_separates_gauge_freedom_from_anchored_chains(oracle):
 
 
 def test_dispatch_sizes_follow_the_source():
-    """The GPU size lists straddle graph.cu's dispatch edges: the last LM size solved in shared
-    memory, the first on the cooperative grid, and chol_kernel / chol_coop_kernel for covariances
-    on both sides of their switch.  Moving a limit in graph.cu fails this until the sizes move."""
-    src = _graph_src()
+    """The GPU size lists straddle solve.cu's one dispatch: the last LM size solved in shared memory
+    and the first on the cooperative grid.  The covariances always factor on the cooperative grid;
+    their sizes cross a CH_NB panel edge.  Moving a limit in solve.cu fails this until the sizes move."""
+    src = _solve_src()
+    assert len(re.findall(r"static int chol_dispatch\(", src)) == 1
+    assert len(re.findall(r"cudaOccupancyMaxActiveBlocksPerMultiprocessor\(&per_sm, chol_coop_kernel,", src)) == 1
+    assert len(re.findall(r"cudaLaunchCooperativeKernel\(", src)) == 1
+    assert re.findall(r"chol_dispatch\(c, n, (true|false),", src) == ["false", "true"], \
+        "the covariances (first) must not take the shared-memory solver, the LM (second) may"
     m = re.findall(r"const size_t smem_chol_bytes = sizeof\(double\) \* \(\(size_t\)\(n \+ 1\) \* \(n \+ 2\) / 2 \+ n \+ 2\);", src)
     assert len(m) == 1, "the shared-memory solver's footprint changed"
     m = re.findall(r"const bool use_smem_chol = n > 0 && n <= (\d+) && smem_chol_bytes <= (\d+) \* 1024;", src)
@@ -99,17 +104,17 @@ def test_dispatch_sizes_follow_the_source():
     smem_max = max(n for n in range(4, 4096, 4) if fits(n))
     coop_min = smem_max + 4
     assert not fits(coop_min)
-    m = re.findall(r"if \(n > (\d+) && coop &&", src)
-    assert len(m) == 1, "the covariance factorisation switch changed"
-    cov_switch = int(m[0])
-    assert (smem_max, coop_min, cov_switch) == (SX.SMEM_MAX_N, SX.COOP_MIN_N, SX.COV_SWITCH_N)
+    assert (smem_max, coop_min) == (SX.SMEM_MAX_N, SX.COOP_MIN_N)
     assert smem_max in SX.LM_SIZES and coop_min in SX.LM_SIZES
-    for n in (cov_switch - 4, cov_switch, cov_switch + 4):
+    m = re.findall(r"#define CH_NB (\d+)", src)
+    assert len(m) == 1
+    panel_edge = 8 * int(m[0])   # n = 256: the last unknown closes chol_coop_kernel's 8th panel
+    for n in (panel_edge - 4, panel_edge, panel_edge + 4):
         assert n in SX.COV_SIZES
     assert all(n % 4 == 0 for n in SX.LM_SIZES + SX.COV_SIZES)
 
 
 def test_rank_tolerance_is_the_kernels():
-    src = _graph_src()
+    src = _solve_src()
     m = re.findall(r"#define VGX_COV_RANK_TOL (\S+)", src)
     assert len(m) == 1 and float(m[0]) == SX.RANK_TOL

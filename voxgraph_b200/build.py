@@ -11,7 +11,7 @@ LIB = os.path.join(HERE, "libvoxgraph_b200.so")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "-I" + INCLUDE, "-I" + CSRC]
 # (source, extra flags). -fmad=false: the reference's float expressions are restated
-# operation by operation (see registration.cuh); graph.cu is double-precision solver code.
+# operation by operation (see registration.cuh); graph.cu and solve.cu are double-precision pose-graph code.
 SOURCES = [
     ("submap.cu", ["-fmad=false"]),
     ("registration.cu", ["-fmad=false"]),
@@ -20,6 +20,7 @@ SOURCES = [
     ("overlap.cu", ["-fmad=false"]),
     ("esdf.cu", ["-fmad=false"]),
     ("graph.cu", []),
+    ("solve.cu", []),
     ("p2p.cu", []),
     ("nccl_dyn.cpp", []),
 ]

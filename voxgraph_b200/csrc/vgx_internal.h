@@ -132,7 +132,7 @@ struct VgxRelEdge {
   double t_obs[3], yaw_obs, L[16];
 };
 
-struct VgxGraph;  // defined in graph.cu
+struct VgxGraph;  // defined in graph.h
 
 struct VgxProfileSlot {
   double total_ms = 0;
