@@ -216,10 +216,10 @@ def tile_problem(ctx, oracle, small_scene):
     return pb, ex
 
 
-@pytest.mark.parametrize("tile_units", ["0", "1", "2", "3", "5", "17", "64", "128", "129", "256"])
+@pytest.mark.parametrize("tile_units", ["1", "2", "3", "5", "17", "64", "128", "129", "256"])
 def test_tile_shapes(ctx, tile_problem, monkeypatch, tile_units):
-    """VGX_REG_HW_TILE_UNITS is read at every table build: 0 = persistent CTAs walking several
-    constraints' tiles, small tiles below the ring depth, tiles above 128 units (no culling)."""
+    """VGX_REG_HW_TILE_UNITS is read at every table build: small tiles below the ring depth,
+    tiles above 128 units (no culling)."""
     from voxgraph_b200 import api
     pb, ex = tile_problem
     monkeypatch.setenv("VGX_REG_HW_TILE_UNITS", tile_units)
@@ -232,7 +232,7 @@ def test_tile_shapes(ctx, tile_problem, monkeypatch, tile_units):
     assert pg.registration_blocks == pg0.registration_blocks
     pb.pg = pg
     try:
-        _check_eval(pb, ex, "tile_units=%s" % tile_units, costs=(tile_units in ("0", "1", "129")))
+        _check_eval(pb, ex, "tile_units=%s" % tile_units, costs=(tile_units in ("1", "2", "129")))
     finally:
         pb.pg = pg0
 

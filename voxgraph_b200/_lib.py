@@ -7,7 +7,7 @@ import ctypes as C
 import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("VGX_LIB") or os.path.join(HERE, "libvoxgraph_b200.so")  # VGX_LIB: tuning variants
+LIB_PATH = os.path.join(HERE, "libvoxgraph_b200.so")
 
 VGX_OK = 0
 VGX_ZERO_WEIGHT = 1

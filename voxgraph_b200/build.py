@@ -42,13 +42,11 @@ def needs_build():
     return any(os.path.getmtime(d) > t for d in deps)
 
 
-def build(force=False, verbose=False, defines=None, out=None):
-    """defines/out: build an experimental variant (extra -D flags) into another file."""
-    if defines is None and not force and not needs_build():
+def build(force=False, verbose=False):
+    if not force and not needs_build():
         return LIB
     nvcc = _nvcc()
-    lib = out or LIB
-    objdir = os.path.join(HERE, "build" if out is None else "build_" + os.path.basename(out))
+    objdir = os.path.join(HERE, "build")
     os.makedirs(objdir, exist_ok=True)
     objs = []
     procs = []
@@ -57,7 +55,7 @@ def build(force=False, verbose=False, defines=None, out=None):
         if not os.path.exists(path):
             continue
         obj = os.path.join(objdir, os.path.splitext(src)[0] + ".o")
-        cmd = [nvcc] + ARCH + COMMON + extra + list(defines or []) + ["-c", path, "-o", obj]
+        cmd = [nvcc] + ARCH + COMMON + extra + ["-c", path, "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT)))
@@ -72,9 +70,9 @@ def build(force=False, verbose=False, defines=None, out=None):
             sys.stderr.write(out)
     if failed:
         raise RuntimeError("CUDA build failed")
-    cmd = [nvcc] + ARCH + ["-shared", "-o", lib] + objs + ["-lcudart", "-ldl"]
+    cmd = [nvcc] + ARCH + ["-shared", "-o", LIB] + objs + ["-lcudart", "-ldl"]
     subprocess.run(cmd, check=True)
-    return lib
+    return LIB
 
 
 if __name__ == "__main__":

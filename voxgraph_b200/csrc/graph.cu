@@ -20,7 +20,7 @@
 #include "registration_kernels.h"
 
 static void free_tables(VgxGraph* g) {
-  cudaFree(g->d_cons); cudaFree(g->d_poses); cudaFree(g->d_tiles); cudaFree(g->d_tile_begin); cudaFree(g->d_cta_tile_begin);
+  cudaFree(g->d_cons); cudaFree(g->d_poses); cudaFree(g->d_tiles); cudaFree(g->d_tile_begin);
   cudaFree(g->d_unit_bounds); g->d_unit_bounds = nullptr;
   cudaFree(g->d_partials); cudaFree(g->d_csum); cudaFree(g->d_rel);
   cudaFree(g->d_tile_order); cudaFree(g->d_tile_cost); cudaFree(g->d_block_mask);
@@ -34,7 +34,7 @@ static void free_tables(VgxGraph* g) {
   g->d_sample_pts = nullptr; g->d_sample_idx = nullptr;
   cudaFree(g->d_snap); g->d_snap = nullptr;
   // the pinned host buffers (h_state, h_snap, h_x) outlive the tables: cudaMallocHost costs ~0.2 ms each
-  g->d_cons = nullptr; g->d_poses = nullptr; g->d_tiles = nullptr; g->d_tile_begin = nullptr; g->d_cta_tile_begin = nullptr;
+  g->d_cons = nullptr; g->d_poses = nullptr; g->d_tiles = nullptr; g->d_tile_begin = nullptr;
   g->d_partials = nullptr; g->d_csum = nullptr; g->d_rel = nullptr;
   g->d_csr_begin = nullptr; g->d_csr_items = nullptr; g->d_block_nodes = nullptr;
   g->d_red_offset = nullptr; g->d_x = nullptr; g->d_xc = nullptr;
@@ -423,68 +423,38 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
       VGX_CUDA(c, cudaStreamSynchronize(c->stream));  // g->samples[] are pageable host vectors
     }
   }
-  // Cut the local residual index space into 32-point units and deal them evenly to the resident
-  // CTAs; a tile is the part of one CTA's run of units that lies inside one residual block (tiles
-  // never straddle constraints and start on a unit boundary = 128-byte aligned SoA slices for TMA).
+  // Scheduling of the reduce kernel.  The cost of a unit varies ~4x with the share of its points
+  // that land in the reading submap, so a static equal cut of the units over the resident CTAs
+  // leaves SMs idle while the hit-heavy ones finish (measured: max SM busy time 16 % above the
+  // mean).  Instead each residual block is cut into fixed tiles of hw_units 32-point units, ONE CTA
+  // PER TILE, dealt to the SMs by the hardware block scheduler as resident CTAs retire (dynamic
+  // balancing at no instruction cost; the per-CTA set-up latency hides behind the other resident
+  // CTAs).  Tiles never straddle constraints and start on a unit boundary (128-byte aligned SoA
+  // slices for TMA).
   g->grid_capacity = 0;
   for (const auto& cc : cons)
     if (cc.grid) g->grid_capacity = std::max(g->grid_capacity, (cc.gd0 * cc.gd1 * cc.gd2 + 7) & ~7);  // 16-byte multiple
-  const int n_ctas_max = std::max(vgx_reg_resident_ctas(c->device, g->grid_capacity), 1);
+  const int resident_ctas = std::max(vgx_reg_resident_ctas(c->device, g->grid_capacity), 1);
   int64_t U = 0;  // total units
   for (const auto& cc : cons) U += (cc.n + VGX_REG_UNIT - 1) / VGX_REG_UNIT;
-  g->n_ctas = (int)std::min<int64_t>(n_ctas_max, U);
-  std::vector<int> cta_tile_begin;
-  // Scheduling of the reduce kernel.  The cost of a unit varies ~4x with the share of its points
-  // that land in the reading submap, so a static equal cut leaves SMs idle while the hit-heavy
-  // ones finish (measured: max SM busy time 16 % above the mean).  hw_units > 0: fixed tiles of
-  // that many units, ONE CTA PER TILE, dealt to the SMs by the hardware block scheduler as
-  // resident CTAs retire (dynamic balancing at no instruction cost; the per-CTA set-up latency
-  // hides behind the other resident CTAs).  0: persistent CTAs with an equal static cut.
   // Tile size: at most VGX_REG_HW_TILE_UNITS units, fewer when the problem is small, so that there
   // are at least ~2 tiles per resident CTA slot (a 3-pair streaming graph still fills the machine).
-  int hw_units = VGX_REG_HW_TILE_UNITS;
-  if (hw_units > 0)
-    hw_units = (int)std::min<int64_t>(hw_units, std::max<int64_t>(4, (U + 2 * (int64_t)n_ctas_max - 1) / (2 * (int64_t)n_ctas_max)));
-  if (const char* e = getenv("VGX_REG_HW_TILE_UNITS")) hw_units = atoi(e);
-  g->hw_tiles = false;
+  // The environment variable of the same name forces a size (n >= 1; tests use it for shapes the
+  // formula never produces).
+  int hw_units = (int)std::min<int64_t>(VGX_REG_HW_TILE_UNITS,
+                                        std::max<int64_t>(4, (U + 2 * (int64_t)resident_ctas - 1) / (2 * (int64_t)resident_ctas)));
+  if (const char* env = getenv("VGX_REG_HW_TILE_UNITS"))
+    if (atoi(env) >= 1) hw_units = atoi(env);
   g->evals_since_order = -1;
-  if (hw_units > 0) {
-    for (int k = 0; k < g->n_local; ++k) {
-      tile_begin.push_back((int)tiles.size());
-      const int tile_pts = hw_units * VGX_REG_UNIT;
-      for (int s0 = 0; s0 < cons[k].n; s0 += tile_pts) {
-        RegTile t;
-        t.constraint = k; t.count = std::min(tile_pts, cons[k].n - s0);
-        t.pts = cons[k].pts + (size_t)(s0 / VGX_REG_UNIT) * VGX_PT_UNIT_FLOATS;
-        tiles.push_back(t);
-      }
+  const int tile_pts = hw_units * VGX_REG_UNIT;
+  for (int k = 0; k < g->n_local; ++k) {
+    tile_begin.push_back((int)tiles.size());
+    for (int s0 = 0; s0 < cons[k].n; s0 += tile_pts) {
+      RegTile t;
+      t.constraint = k; t.count = std::min(tile_pts, cons[k].n - s0);
+      t.pts = cons[k].pts + (size_t)(s0 / VGX_REG_UNIT) * VGX_PT_UNIT_FLOATS;
+      tiles.push_back(t);
     }
-    g->n_ctas = (int)tiles.size();
-    g->hw_tiles = true;
-    cta_tile_begin.resize(tiles.size() + 1);
-    for (size_t k = 0; k <= tiles.size(); ++k) cta_tile_begin[k] = (int)k;
-  } else {
-    int64_t ubase = 0;  // unit index of the current constraint's first unit
-    int cta = 0;
-    auto cta_end = [&](int k) { return (int64_t)(((__int128)U * (k + 1)) / std::max(g->n_ctas, 1)); };
-    if (g->n_ctas > 0) cta_tile_begin.push_back(0);
-    for (int k = 0; k < g->n_local; ++k) {
-      tile_begin.push_back((int)tiles.size());
-      const int64_t uc = (cons[k].n + VGX_REG_UNIT - 1) / VGX_REG_UNIT;
-      int64_t u = 0;
-      while (u < uc) {
-        while (cta + 1 < g->n_ctas && ubase + u >= cta_end(cta)) { cta_tile_begin.push_back((int)tiles.size()); ++cta; }
-        const int64_t take = std::min<int64_t>(uc - u, cta_end(cta) - (ubase + u));
-        RegTile t;
-        t.constraint = k;
-        t.count = (int)std::min<int64_t>(take * VGX_REG_UNIT, (int64_t)cons[k].n - u * VGX_REG_UNIT);
-        t.pts = cons[k].pts + (size_t)u * VGX_PT_UNIT_FLOATS;
-        tiles.push_back(t);
-        u += take;
-      }
-      ubase += uc;
-    }
-    while ((int)cta_tile_begin.size() <= g->n_ctas) cta_tile_begin.push_back((int)tiles.size());
   }
   tile_begin.push_back((int)tiles.size());
   g->n_tiles = (int)tiles.size();
@@ -563,11 +533,9 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
   if (e == cudaSuccess) e = upload_vec(&g->d_cons, cons, st);
   if (e == cudaSuccess) e = upload_vec(&g->d_tiles, tiles, st);
   if (e == cudaSuccess) e = upload_vec(&g->d_tile_begin, tile_begin, st);
-  if (e == cudaSuccess) e = upload_vec(&g->d_cta_tile_begin, cta_tile_begin, st);
-  static const char* lpt_env = getenv("VGX_REG_LPT");
-  if (g->hw_tiles && !(lpt_env && lpt_env[0] == '0')) {
+  {
     std::vector<int> ident(tiles.size()), zero(tiles.size(), 0);
-    for (size_t k = 0; k < tiles.size(); ++k) ident[k] = (int)k;
+    std::iota(ident.begin(), ident.end(), 0);
     if (e == cudaSuccess) e = upload_vec(&g->d_tile_order, ident, st);
     if (e == cudaSuccess) e = upload_vec(&g->d_tile_cost, zero, st);
   }
@@ -634,7 +602,7 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
   if (do_reg) {
     // refresh the longest-first tile order from the cost measured by the previous evaluation: before
     // the second evaluation on new tables, then every 32nd (the poses move little inside a solve)
-    if (g->d_tile_order && g->n_tiles > 1 && (g->evals_since_order == -2 || g->evals_since_order >= 32)) {
+    if (g->n_tiles > 1 && (g->evals_since_order == -2 || g->evals_since_order >= 32)) {
       VgxLaunchScope s(c, 5);
       vgx_launch_reg_order(st, g->d_tile_cost, g->n_tiles, g->d_tile_order);
       g->evals_since_order = 0;
@@ -646,9 +614,8 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
     }
     {
       VgxLaunchScope s(c, 0);
-      vgx_launch_reg_reduce(st, g->d_cons, g->d_poses, g->d_tiles, g->n_ctas, g->d_cta_tile_begin,
-                            g->d_tile_order, g->d_tile_cost, g->d_partials, g->grid_capacity,
-                            g->d_unit_bounds, jacobian, skip);
+      vgx_launch_reg_reduce(st, g->d_cons, g->d_poses, g->d_tiles, g->n_tiles, g->d_tile_order,
+                            g->d_tile_cost, g->d_partials, g->grid_capacity, g->d_unit_bounds, jacobian, skip);
     }
     if (g->evals_since_order < 0) g->evals_since_order = -2;   // a cost has been measured now
   }
@@ -662,23 +629,14 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
   push.dst[0] = d_packed;
   // the assembly kernels and the constraint-sum kernel are launched as programmatic dependents of
   // what precedes them on the stream
-  cudaLaunchAttribute pdl[1];
-  pdl[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  pdl[0].val.programmaticStreamSerializationAllowed = 1;
-  static const char* no_pdl = getenv("VGX_NO_PDL");
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.blockDim = dim3(128);
-  cfg.stream = st;
-  cfg.attrs = pdl;
-  cfg.numAttrs = (no_pdl && no_pdl[0] == '1') ? 0 : 1;
+  VgxPdlLaunch L(st, dim3(1), dim3(128));
   const int excl = do_reg ? 0 : 1;
   if (do_reg) {
     RegSums sums;
     sums.partials = g->d_partials; sums.tile_begin = g->d_tile_begin; sums.cons = g->d_cons;
     VgxLaunchScope s(c, 7);
-    cfg.gridDim = dim3((unsigned)((g->n_local + 3) / 4));
-    cudaLaunchKernelEx(&cfg, reg_csum_kernel, sums, g->n_local, g->d_csum, skip);
+    L.cfg.gridDim = dim3((unsigned)((g->n_local + 3) / 4));
+    cudaLaunchKernelEx(&L.cfg, reg_csum_kernel, sums, g->n_local, g->d_csum, skip);
   }
   if (p2p) {
     int rc = vgx_p2p_begin(c, g->packed_len, &push, &gat);
@@ -697,8 +655,8 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
     const int grid = std::min(g->N + g->E + 1, resident);
     {
       VgxLaunchScope s(c, 8);
-      cfg.gridDim = dim3((unsigned)grid);
-      cudaLaunchKernelEx(&cfg, assemble_exchange_kernel, (const double*)g->d_csum, (const VgxRelEdge*)g->d_rel, d_x,
+      L.cfg.gridDim = dim3((unsigned)grid);
+      cudaLaunchKernelEx(&L.cfg, assemble_exchange_kernel, (const double*)g->d_csum, (const VgxRelEdge*)g->d_rel, d_x,
                          (const int*)g->d_csr_begin, (const int4*)g->d_csr_items, push, g->N, g->E, g->n_local,
                          g->n_rel_local, excl, gat, d_packed, (int)g->packed_len, skip,
                          (const unsigned char*)g->d_block_mask);
@@ -708,8 +666,8 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
   }
   {
     VgxLaunchScope s(c, 8);
-    cfg.gridDim = dim3((unsigned)(g->N + g->E + 1));
-    cudaLaunchKernelEx(&cfg, assemble_kernel, (const double*)g->d_csum, (const VgxRelEdge*)g->d_rel, d_x, (const int*)g->d_csr_begin,
+    L.cfg.gridDim = dim3((unsigned)(g->N + g->E + 1));
+    cudaLaunchKernelEx(&L.cfg, assemble_kernel, (const double*)g->d_csum, (const VgxRelEdge*)g->d_rel, d_x, (const int*)g->d_csr_begin,
                        (const int4*)g->d_csr_items, push, g->N, g->E, g->n_local, g->n_rel_local, excl, skip);
   }
   VGX_CUDA(c, cudaGetLastError());

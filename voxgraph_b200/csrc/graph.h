@@ -35,7 +35,7 @@ struct VgxGraph {
   std::vector<int> local;  // global indices of this rank's registration constraints
   std::vector<int> block_nodes;  // E x 2 (host copy)
   std::vector<int> red;    // N: reduced offset or -1 (host copy of d_red_offset)
-  int n_local = 0, n_tiles = 0, n_rel_local = 0, n_ctas = 0, grid_capacity = 0;
+  int n_local = 0, n_tiles = 0, n_rel_local = 0, grid_capacity = 0;
   int E = 0;               // off-diagonal blocks
   int n_free = 0;          // reduced dimension 4 * (non-constant nodes)
   int64_t residuals_local = 0, residuals_global = 0;
@@ -48,14 +48,12 @@ struct VgxGraph {
   RegTile* d_tiles = nullptr;
   float4* d_unit_bounds = nullptr;   // bounding sphere per 32-point unit of the tiles (RegTile::unit0)
   int* d_tile_begin = nullptr;
-  int* d_cta_tile_begin = nullptr;
   double* d_partials = nullptr;
   double* d_csum = nullptr;
   VgxRelEdge* d_rel = nullptr;
   unsigned char* d_block_mask = nullptr;   // per output block: bit r = rank r contributes (peer exchange)
-  int* d_tile_order = nullptr;  // one-CTA-per-tile mode: CTA b runs tile d_tile_order[b] (longest first)
+  int* d_tile_order = nullptr;  // CTA b of the reduce kernel runs tile d_tile_order[b] (longest first)
   int* d_tile_cost = nullptr;   // SM cycles each tile took in the latest evaluation
-  bool hw_tiles = false;
   int evals_since_order = -1;   // -1: no cost measured yet since the tables were built
   int* d_csr_begin = nullptr;   // N + E + 1
   int4* d_csr_items = nullptr;  // (source, role, first tile, end tile)

@@ -3,9 +3,6 @@
 #include "registration.cuh"
 #include "registration_kernels.h"
 
-#include <stdlib.h>
-#include <string.h>
-
 #include <type_traits>
 
 // ------------------------------------------------------------------ emit mode
@@ -166,10 +163,12 @@ __device__ __forceinline__ bool reg_unit_may_hit(const RegConstraintDev& C, cons
   return false;
 }
 
-// Registration reduce kernel, v5.  Persistent CTAs; the local residual index space is cut into
-// 32-point units that are dealt evenly to the CTAs (a tile = a CTA's run of units inside one
-// residual block).  Inside a tile every warp runs its own software pipeline over the units
-// u = warp, warp + W, ...:
+// Registration reduce kernel, v5.  One CTA per tile; a tile is a run of 32-point units inside one
+// residual block (graph.cu cuts them).  CTA b runs tile tile_order[b], the longest-first order
+// from the cost measured by an earlier evaluation: the hardware hands CTAs out in index order, so
+// the expensive tiles start first and the tail of the grid is made of cheap ones.  The CTA writes
+// the tile's 21 sums to partials[tile] and its cost in SM cycles to tile_cost[tile].  Inside the
+// tile every warp runs its own software pipeline over the units u = warp, warp + W, ...:
 //   * the unit's points (640 contiguous bytes of the unit-major AoSoA layout) are brought into a
 //     per-warp 4-slot shared-memory ring by ONE cp.async.bulk (TMA 1-D) completing on an
 //     mbarrier, three units ahead - the point loads never touch the LSU path of the math warps;
@@ -178,7 +177,7 @@ __device__ __forceinline__ bool reg_unit_may_hit(const RegConstraintDev& C, cons
 //     B1 coefficients, residual, Jacobian, Gram staging + 8 DMMA.  The gather latency of unit
 //     u+1 is hidden behind the arithmetic of unit u inside the same warp.
 // The last unit is zero-padded to 32 points (weight 0 -> zero contribution), so the
-// loop carries no "active" predicate.  Warps never synchronise with each other inside a tile.
+// loop carries no "active" predicate.  Warps never synchronise with each other before the epilogue.
 // Block-grid tiles without a no-correspondence cost first test every unit's bounding sphere against
 // the block grid (one lane per unit, reg_unit_may_hit); the ring then carries only the units that
 // may hit, in the same order, so the per-warp sums are those of the full walk.
@@ -186,15 +185,16 @@ template <bool kJacobian>
 __global__ void __launch_bounds__(VGX_REG_THREADS, VGX_REG_MIN_BLOCKS)
 reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
                   const RegPoseConst* __restrict__ poses, const RegTile* __restrict__ tiles,
-                  const int* __restrict__ cta_tile_begin, const int* __restrict__ tile_order,
-                  int* __restrict__ tile_cost, double* __restrict__ partials, int grid_capacity,
-                  const float4* __restrict__ unit_bounds, const int* __restrict__ skip) {
+                  const int* __restrict__ tile_order, int* __restrict__ tile_cost,
+                  double* __restrict__ partials, int grid_capacity, const float4* __restrict__ unit_bounds,
+                  const int* __restrict__ skip) {
   if (skip && *skip) return;   // evaluation enqueued ahead of a solve that has already ended
   constexpr int kWarps = VGX_REG_THREADS / 32;
   constexpr int kRing = VGX_REG_RING;
   __shared__ __align__(128) float s_ring[kWarps][kRing][5][32];
   __shared__ __align__(8) unsigned long long s_bar[kWarps][kRing];
   __shared__ __align__(8) unsigned long long s_tbar;   // tile barrier: descriptor + pose block + grid
+  __shared__ long long s_clk0;   // tile start, SM cycles (thread 0; in a register it spills at 72)
   __shared__ double s_stage[kWarps][6][VGX_STAGE_STRIDE];
   __shared__ double s_gram[kWarps][64];
   __shared__ __align__(16) RegConstraintDev s_C;
@@ -219,212 +219,194 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
   double* stage_w = &s_stage[warp][0][lane];
   const double* stage_r = &s_stage[warp][grp < 6 ? grp : 0][tig];
   uint32_t it = 0;   // units consumed by this warp so far: ring slot = it % kRing, parity = (it / kRing) & 1
-  int grid_of = -1;  // constraint whose block grid is currently staged
 
-  uint32_t tseq = 0;  // tiles staged by this CTA (parity of the tile barrier)
-  // one CTA per tile: CTA b runs tile_order[b] (longest-first order from the measured cost of an earlier
-  // evaluation: the hardware hands CTAs out in index order, so the expensive tiles start first and the
-  // tail of the grid is made of cheap ones); persistent mode: CTA b walks its run of tiles
-  int tile_first, tile_end;
-  if (tile_order) { tile_first = __ldg(tile_order + blockIdx.x); tile_end = tile_first + 1; }
-  else { tile_first = cta_tile_begin[blockIdx.x]; tile_end = cta_tile_begin[blockIdx.x + 1]; }
-  for (int tile = tile_first; tile < tile_end; ++tile, ++tseq) {
-    // the 32-byte tile record is all a thread needs to start the bulk copies
-    const int4 rec0 = __ldg(reinterpret_cast<const int4*>(tiles + tile));
-    const ulonglong2 rec1 = __ldg(reinterpret_cast<const ulonglong2*>(tiles + tile) + 1);
-    RegTile T;
-    T.constraint = rec0.x; T.unit0 = rec0.y; T.count = rec0.z; T.grid_bytes = rec0.w;
-    T.pts = reinterpret_cast<const float*>(rec1.x);
-    T.grid16 = reinterpret_cast<const uint16_t*>(rec1.y);
-    const bool use_grid = T.grid_bytes > 0 && T.grid_bytes <= 2 * grid_capacity;
-    const bool stage_grid = use_grid && grid_of != T.constraint;
-    __syncthreads();  // previous tile: every warp is out of its loop (s_C / s_P / s_grid readers)
-    // ---- descriptor (160 B), pose block (64 B) and the 16-bit block grid: three bulk copies on the
-    //      tile barrier; the warps' first point units follow on their own barriers
-    if (threadIdx.x == 0) {
-      const uint32_t bytes = (uint32_t)sizeof(RegConstraintDev) + (uint32_t)sizeof(RegPoseConst) +
-                             (stage_grid ? (uint32_t)T.grid_bytes : 0u);
-      mbar_expect_tx(tbar, bytes);
-      tma_load_1d(smem_u32(&s_C), constraints + T.constraint, (uint32_t)sizeof(RegConstraintDev), tbar);
-      if (stage_grid) tma_load_1d(smem_u32(s_grid), T.grid16, (uint32_t)T.grid_bytes, tbar);
-      // the pose blocks are the only input the preceding kernel (pose set-up) writes: everything
-      // above was independent of it (programmatic dependent launch)
-      asm volatile("griddepcontrol.wait;" ::: "memory");
-      tma_load_1d(smem_u32(&s_P), poses + T.constraint, (uint32_t)sizeof(RegPoseConst), tbar);
+  const int tile = __ldg(tile_order + blockIdx.x);
+  // the 32-byte tile record is all a thread needs to start the bulk copies
+  const int4 rec0 = __ldg(reinterpret_cast<const int4*>(tiles + tile));
+  const ulonglong2 rec1 = __ldg(reinterpret_cast<const ulonglong2*>(tiles + tile) + 1);
+  RegTile T;
+  T.constraint = rec0.x; T.unit0 = rec0.y; T.count = rec0.z; T.grid_bytes = rec0.w;
+  T.pts = reinterpret_cast<const float*>(rec1.x);
+  T.grid16 = reinterpret_cast<const uint16_t*>(rec1.y);
+  const bool use_grid = T.grid_bytes > 0 && T.grid_bytes <= 2 * grid_capacity;
+  // ---- descriptor (160 B), pose block (64 B) and the 16-bit block grid: three bulk copies on the
+  //      tile barrier; the warps' first point units follow on their own barriers
+  if (threadIdx.x == 0) {
+    const uint32_t bytes = (uint32_t)sizeof(RegConstraintDev) + (uint32_t)sizeof(RegPoseConst) +
+                           (use_grid ? (uint32_t)T.grid_bytes : 0u);
+    mbar_expect_tx(tbar, bytes);
+    tma_load_1d(smem_u32(&s_C), constraints + T.constraint, (uint32_t)sizeof(RegConstraintDev), tbar);
+    if (use_grid) tma_load_1d(smem_u32(s_grid), T.grid16, (uint32_t)T.grid_bytes, tbar);
+    // the pose blocks are the only input the preceding kernel (pose set-up) writes: everything
+    // above was independent of it (programmatic dependent launch)
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    tma_load_1d(smem_u32(&s_P), poses + T.constraint, (uint32_t)sizeof(RegPoseConst), tbar);
+  }
+  const int n_units = (T.count + 31) >> 5;
+  const int my_units = warp < n_units ? (n_units - warp + kWarps - 1) / kWarps : 0;
+  // culling needs the pose block, so a tile that may cull issues its first units after the tile
+  // barrier; lane j tests unit j of this warp
+  const bool may_cull = unit_bounds && use_grid && my_units <= 32;
+  float4 bnd = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (may_cull && lane < my_units) bnd = __ldg(unit_bounds + T.unit0 + warp + lane * kWarps);
+  uint32_t live = 0;   // may_cull: units of this warp not yet issued that may hit (bit j: unit j)
+  int next = 0;        // otherwise: next unit to issue
+  // producer (lane 0): bring the next unit of this warp into ring slot seq % kRing
+  auto issue = [&](uint32_t seq) {
+    int j = next++;
+    if (may_cull) { j = __ffs(live) - 1; live &= live - 1; }
+    if (lane == 0) {
+      const uint32_t slot = seq % kRing;
+      const uint32_t bar = bar0 + 8u * slot, dst = ring0 + 640u * slot;
+      mbar_expect_tx(bar, 640u);
+      tma_load_1d(dst, T.pts + (size_t)(warp + j * kWarps) * VGX_PT_UNIT_FLOATS, 640u, bar);
     }
-    if (stage_grid) grid_of = T.constraint;
-    const int n_units = (T.count + 31) >> 5;
-    const int my_units = warp < n_units ? (n_units - warp + kWarps - 1) / kWarps : 0;
-    // culling needs the pose block, so a tile that may cull issues its first units after the tile
-    // barrier; lane j tests unit j of this warp
-    const bool may_cull = unit_bounds && use_grid && my_units <= 32;
-    float4 bnd = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (may_cull && lane < my_units) bnd = __ldg(unit_bounds + T.unit0 + warp + lane * kWarps);
-    uint32_t live = 0;   // may_cull: units of this warp not yet issued that may hit (bit j: unit j)
-    int next = 0;        // otherwise: next unit to issue
-    // producer (lane 0): bring the next unit of this warp into ring slot seq % kRing
-    auto issue = [&](uint32_t seq) {
-      int j = next++;
-      if (may_cull) { j = __ffs(live) - 1; live &= live - 1; }
-      if (lane == 0) {
-        const uint32_t slot = seq % kRing;
-        const uint32_t bar = bar0 + 8u * slot, dst = ring0 + 640u * slot;
-        mbar_expect_tx(bar, 640u);
-        tma_load_1d(dst, T.pts + (size_t)(warp + j * kWarps) * VGX_PT_UNIT_FLOATS, 640u, bar);
-      }
-    };
-    int n_live = my_units;   // units this warp consumes
-    if (!may_cull) {
+  };
+  int n_live = my_units;   // units this warp consumes
+  if (!may_cull) {
 #pragma unroll
-      for (int j = 0; j < kRing - 1; ++j)
-        if (j < n_live) issue(it + j);
-    }
-    mbar_wait(tbar, tseq & 1u);   // descriptor, pose block and grid have landed
-    const long long clk0 = clock64();
-    const RegPoseConst P = s_P;
-    const bool gram_always = s_C.no_corr != 0.0;  // r = w * no_correspondence_cost without a match
-    if (may_cull) {
-      live = __ballot_sync(0xffffffffu, lane < my_units && (gram_always || reg_unit_may_hit(s_C, P, s_grid, bnd)));
-      n_live = __popc(live);
+    for (int j = 0; j < kRing - 1; ++j)
+      if (j < n_live) issue(it + j);
+  }
+  mbar_wait(tbar, 0);   // descriptor, pose block and grid have landed
+  if (threadIdx.x == 0) s_clk0 = clock64();
+  const RegPoseConst P = s_P;
+  const bool gram_always = s_C.no_corr != 0.0;  // r = w * no_correspondence_cost without a match
+  if (may_cull) {
+    live = __ballot_sync(0xffffffffu, lane < my_units && (gram_always || reg_unit_may_hit(s_C, P, s_grid, bnd)));
+    n_live = __popc(live);
 #pragma unroll
-      for (int j = 0; j < kRing - 1; ++j)
-        if (j < n_live) issue(it + j);
-    }
-    double d0 = 0.0, d1 = 0.0;
+    for (int j = 0; j < kRing - 1; ++j)
+      if (j < n_live) issue(it + j);
+  }
+  double d0 = 0.0, d1 = 0.0;
 
-    // a lane without a correspondence carries an all-NaN octet
-    struct Pipe { float4 lo, hi; float ox, oy, oz; };
-    // stage B: consume the octet issued by stage A
-    auto stage_b = [&](uint32_t seq, const Pipe& R) {
-      const float* sp = ringf + 160 * (seq % kRing) + lane;
-      const float d[8] = {R.lo.x, R.lo.y, R.lo.z, R.lo.w, R.hi.x, R.hi.y, R.hi.z, R.hi.w};
-      // a unit without a single correspondence adds nothing unless a missing one costs something
-      const bool ok = vgx_octet_ok(d);
-      if (gram_always || __any_sync(0xffffffffu, ok)) {
-        const float xi = sp[0], yi = sp[32], dist = sp[96], w = sp[128];
-        const RegPointResult Q = vgx_reg_math<kJacobian>(s_C, P, xi, yi, dist, w, ok, d, R.ox, R.oy, R.oz);
-#if defined(VGX_X_NOGRAM)
-        // timing ablation only (scripts/build_variants.py x_nogram): no staging, no MMA - results are wrong
-        d0 = fma(Q.r, (double)Q.jr[0] + (double)Q.jr[3] + (double)Q.je3, d0);
-        if (false) {
-#else
-        if (kJacobian) {
-#endif
-          stage_w[0 * VGX_STAGE_STRIDE] = (double)Q.jr[0];
-          stage_w[1 * VGX_STAGE_STRIDE] = (double)Q.jr[1];
-          stage_w[2 * VGX_STAGE_STRIDE] = (double)Q.jr[2];
-          stage_w[3 * VGX_STAGE_STRIDE] = (double)Q.jr[3];
-          stage_w[4 * VGX_STAGE_STRIDE] = (double)Q.je3;
-          stage_w[5 * VGX_STAGE_STRIDE] = Q.r;
-          __syncwarp();
-#pragma unroll
-          for (int t4 = 0; t4 < 8; ++t4) {
-            const double a = (grp < 6) ? stage_r[4 * t4] : 0.0;
-            dmma_8x8x4(d0, d1, a, a);
-          }
-        } else {
-          d0 = fma(Q.r, Q.r, d0);
-        }
-      }
-      __syncwarp();  // every lane is done with this unit's ring slot and the Gram staging buffer
-    };
-
-    // The tile's pipeline, instantiated once per lookup path (use_grid is uniform across the CTA):
-    // kGrid, the reading submap's block grid staged in shared memory, or its hash in global memory.
-    auto run_tile = [&](auto path) {
-      constexpr bool kGrid = decltype(path)::value;
-      // stage A: everything up to the ISSUE of the octet load
-      auto stage_a = [&](uint32_t seq, Pipe& R) {
-        const uint32_t slot = seq % kRing;
-        mbar_wait(bar0 + 8u * slot, (seq / kRing) & 1u);
-        const float* sp = ringf + 160 * slot + lane;
-        float p0, p1, p2;
-        vgx_reg_transform(P, sp[0], sp[32], sp[64], p0, p1, p2);
-        const float qnan = __int_as_float(0x7fc00000);
-        R.lo = make_float4(qnan, qnan, qnan, qnan);
-        R.hi = R.lo;
-        R.ox = R.oy = R.oz = 0.f;
-        int b0, b1, b2;
-        vgx_block_index(s_C, p0, p1, p2, b0, b1, b2);
-        RegLocate L;
-        int slot_b;
-        if constexpr (kGrid) {
-          // getVoxelsAndQVector fails right away when the block that contains pos does not exist;
-          // overlapping submaps share only part of their surface and consecutive points are
-          // spatially coherent: most warps miss with all 32 lanes and skip the rest of the unit
-          const int slot_c = vgx_grid_slot(s_C, s_grid, b0, b1, b2);
-          if (!__any_sync(0xffffffffu, slot_c >= 0)) return;
-          vgx_locate_in_block(s_C, p0, p1, p2, b0, b1, b2, L);
-          // the base corner lies in another block only when it moved into a lower neighbour
-          const bool moved = (L.b0 != b0) | (L.b1 != b1) | (L.b2 != b2);
-          const int slot_m = moved ? vgx_grid_slot(s_C, s_grid, L.b0, L.b1, L.b2) : slot_c;
-          slot_b = slot_c >= 0 ? slot_m : -1;
-        } else {
-          vgx_locate_in_block(s_C, p0, p1, p2, b0, b1, b2, L);
-          RegProbe H = vgx_probe_start(s_C, L);
-          slot_b = vgx_resolve(s_C, H);
-        }
-        R.ox = L.ox; R.oy = L.oy; R.oz = L.oz;
-        if (slot_b >= 0) {
-          const float4* o = reinterpret_cast<const float4*>(s_C.view) +
-                            2 * (((size_t)slot_b << (3 * s_C.vps_shift)) + (size_t)L.lin);
-          // the whole 32-byte octet = one sector = two 128-bit loads (sm_90 has no 256-bit LDG)
-          R.lo = __ldg(o); R.hi = __ldg(o + 1);
-        }
-      };
-      // two register sets alternate (loop unrolled by two): the in-flight octet is never copied
-      Pipe Ra, Rb;
-      stage_a(it, Ra);
-      int j = 0;
-      for (; j + 2 <= n_live; j += 2, it += 2) {
-        if (j + kRing - 1 < n_live) issue(it + kRing - 1);
-        stage_a(it + 1, Rb);
-        stage_b(it, Ra);
-        if (j + kRing < n_live) issue(it + kRing);
-        if (j + 2 < n_live) stage_a(it + 2, Ra);
-        stage_b(it + 1, Rb);
-      }
-      if (j < n_live) stage_b(it++, Ra);
-    };
-    if (n_live > 0) {
-      if (use_grid) run_tile(std::true_type());
-      else run_tile(std::false_type());
-    }
-    // ---- tile epilogue: warp Gram fragments -> 21 sums -> partials[tile]
-    if (kJacobian) {
-      s_gram[warp][grp * 8 + 2 * tig] = d0;
-      s_gram[warp][grp * 8 + 2 * tig + 1] = d1;
-    } else {
-#pragma unroll
-      for (int off = 16; off > 0; off >>= 1) d0 += __shfl_xor_sync(0xffffffffu, d0, off);
-      if (lane == 0) s_gram[warp][0] = d0;
-    }
-    __syncthreads();
-    if (threadIdx.x < VGX_REG_NSUM) {
-      // entry e of the 21 sums -> (row, col) of the Gram matrix
-      int row = 5, col = 5;
-      const int e = threadIdx.x;
-      if (e < 15) {
-        int p = 0, rem = e;
-        while (rem >= 5 - p) { rem -= 5 - p; ++p; }
-        row = p; col = p + rem;
-      } else if (e < 20) {
-        row = e - 15; col = 5;
-      }
-      double s = 0;
+  // a lane without a correspondence carries an all-NaN octet
+  struct Pipe { float4 lo, hi; float ox, oy, oz; };
+  // stage B: consume the octet issued by stage A
+  auto stage_b = [&](uint32_t seq, const Pipe& R) {
+    const float* sp = ringf + 160 * (seq % kRing) + lane;
+    const float d[8] = {R.lo.x, R.lo.y, R.lo.z, R.lo.w, R.hi.x, R.hi.y, R.hi.z, R.hi.w};
+    // a unit without a single correspondence adds nothing unless a missing one costs something
+    const bool ok = vgx_octet_ok(d);
+    if (gram_always || __any_sync(0xffffffffu, ok)) {
+      const float xi = sp[0], yi = sp[32], dist = sp[96], w = sp[128];
+      const RegPointResult Q = vgx_reg_math<kJacobian>(s_C, P, xi, yi, dist, w, ok, d, R.ox, R.oy, R.oz);
       if (kJacobian) {
+        stage_w[0 * VGX_STAGE_STRIDE] = (double)Q.jr[0];
+        stage_w[1 * VGX_STAGE_STRIDE] = (double)Q.jr[1];
+        stage_w[2 * VGX_STAGE_STRIDE] = (double)Q.jr[2];
+        stage_w[3 * VGX_STAGE_STRIDE] = (double)Q.jr[3];
+        stage_w[4 * VGX_STAGE_STRIDE] = (double)Q.je3;
+        stage_w[5 * VGX_STAGE_STRIDE] = Q.r;
+        __syncwarp();
 #pragma unroll
-        for (int wv = 0; wv < kWarps; ++wv) s += s_gram[wv][row * 8 + col];
-      } else if (e == 20) {
-#pragma unroll
-        for (int wv = 0; wv < kWarps; ++wv) s += s_gram[wv][0];
+        for (int t4 = 0; t4 < 8; ++t4) {
+          const double a = (grp < 6) ? stage_r[4 * t4] : 0.0;
+          dmma_8x8x4(d0, d1, a, a);
+        }
+      } else {
+        d0 = fma(Q.r, Q.r, d0);
       }
-      // The tile's sums are final here: no ticket, no fence.  The assembly kernel (a programmatic
-      // dependent of this one) adds a constraint's tiles in tile order and applies factor^2
-      // (cpp:274-291) - bit-reproducible whatever order the tiles ran in.
-      partials[(size_t)tile * VGX_REG_NSTRIDE + e] = s;
-      if (e == 0 && tile_cost) tile_cost[tile] = (int)min(clock64() - clk0, (long long)0x3fffffff);
     }
+    __syncwarp();  // every lane is done with this unit's ring slot and the Gram staging buffer
+  };
+
+  // The tile's pipeline, instantiated once per lookup path (use_grid is uniform across the CTA):
+  // kGrid, the reading submap's block grid staged in shared memory, or its hash in global memory.
+  auto run_tile = [&](auto path) {
+    constexpr bool kGrid = decltype(path)::value;
+    // stage A: everything up to the ISSUE of the octet load
+    auto stage_a = [&](uint32_t seq, Pipe& R) {
+      const uint32_t slot = seq % kRing;
+      mbar_wait(bar0 + 8u * slot, (seq / kRing) & 1u);
+      const float* sp = ringf + 160 * slot + lane;
+      float p0, p1, p2;
+      vgx_reg_transform(P, sp[0], sp[32], sp[64], p0, p1, p2);
+      const float qnan = __int_as_float(0x7fc00000);
+      R.lo = make_float4(qnan, qnan, qnan, qnan);
+      R.hi = R.lo;
+      R.ox = R.oy = R.oz = 0.f;
+      int b0, b1, b2;
+      vgx_block_index(s_C, p0, p1, p2, b0, b1, b2);
+      RegLocate L;
+      int slot_b;
+      if constexpr (kGrid) {
+        // getVoxelsAndQVector fails right away when the block that contains pos does not exist;
+        // overlapping submaps share only part of their surface and consecutive points are
+        // spatially coherent: most warps miss with all 32 lanes and skip the rest of the unit
+        const int slot_c = vgx_grid_slot(s_C, s_grid, b0, b1, b2);
+        if (!__any_sync(0xffffffffu, slot_c >= 0)) return;
+        vgx_locate_in_block(s_C, p0, p1, p2, b0, b1, b2, L);
+        // the base corner lies in another block only when it moved into a lower neighbour
+        const bool moved = (L.b0 != b0) | (L.b1 != b1) | (L.b2 != b2);
+        const int slot_m = moved ? vgx_grid_slot(s_C, s_grid, L.b0, L.b1, L.b2) : slot_c;
+        slot_b = slot_c >= 0 ? slot_m : -1;
+      } else {
+        vgx_locate_in_block(s_C, p0, p1, p2, b0, b1, b2, L);
+        RegProbe H = vgx_probe_start(s_C, L);
+        slot_b = vgx_resolve(s_C, H);
+      }
+      R.ox = L.ox; R.oy = L.oy; R.oz = L.oz;
+      if (slot_b >= 0) {
+        const float4* o = reinterpret_cast<const float4*>(s_C.view) +
+                          2 * (((size_t)slot_b << (3 * s_C.vps_shift)) + (size_t)L.lin);
+        // the whole 32-byte octet = one sector = two 128-bit loads (sm_90 has no 256-bit LDG)
+        R.lo = __ldg(o); R.hi = __ldg(o + 1);
+      }
+    };
+    // two register sets alternate (loop unrolled by two): the in-flight octet is never copied
+    Pipe Ra, Rb;
+    stage_a(it, Ra);
+    int j = 0;
+    for (; j + 2 <= n_live; j += 2, it += 2) {
+      if (j + kRing - 1 < n_live) issue(it + kRing - 1);
+      stage_a(it + 1, Rb);
+      stage_b(it, Ra);
+      if (j + kRing < n_live) issue(it + kRing);
+      if (j + 2 < n_live) stage_a(it + 2, Ra);
+      stage_b(it + 1, Rb);
+    }
+    if (j < n_live) stage_b(it++, Ra);
+  };
+  if (n_live > 0) {
+    if (use_grid) run_tile(std::true_type());
+    else run_tile(std::false_type());
+  }
+  // ---- tile epilogue: warp Gram fragments -> 21 sums -> partials[tile]
+  if (kJacobian) {
+    s_gram[warp][grp * 8 + 2 * tig] = d0;
+    s_gram[warp][grp * 8 + 2 * tig + 1] = d1;
+  } else {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) d0 += __shfl_xor_sync(0xffffffffu, d0, off);
+    if (lane == 0) s_gram[warp][0] = d0;
+  }
+  __syncthreads();
+  if (threadIdx.x < VGX_REG_NSUM) {
+    // entry e of the 21 sums -> (row, col) of the Gram matrix
+    int row = 5, col = 5;
+    const int e = threadIdx.x;
+    if (e < 15) {
+      int p = 0, rem = e;
+      while (rem >= 5 - p) { rem -= 5 - p; ++p; }
+      row = p; col = p + rem;
+    } else if (e < 20) {
+      row = e - 15; col = 5;
+    }
+    double s = 0;
+    if (kJacobian) {
+#pragma unroll
+      for (int wv = 0; wv < kWarps; ++wv) s += s_gram[wv][row * 8 + col];
+    } else if (e == 20) {
+#pragma unroll
+      for (int wv = 0; wv < kWarps; ++wv) s += s_gram[wv][0];
+    }
+    // The tile's sums are final here: no ticket, no fence.  The assembly kernel (a programmatic
+    // dependent of this one) adds a constraint's tiles in tile order and applies factor^2
+    // (cpp:274-291) - bit-reproducible whatever order the tiles ran in.
+    partials[(size_t)tile * VGX_REG_NSTRIDE + e] = s;
+    if (e == 0) tile_cost[tile] = (int)min(clock64() - s_clk0, (long long)0x3fffffff);
   }
 }
 
@@ -489,45 +471,24 @@ __global__ void reg_pose_setup_kernel(const RegConstraintDev* __restrict__ const
 void vgx_launch_reg_pose_setup(cudaStream_t st, const RegConstraintDev* cons, const double* x,
                                RegPoseConst* poses, int n, const int* skip) {
   if (n <= 0) return;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)((n + 127) / 128));
-  cfg.blockDim = dim3(128);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  static const char* no_pdl = getenv("VGX_NO_PDL");
-  cfg.attrs = attr;
-  cfg.numAttrs = (no_pdl && no_pdl[0] == '1') ? 0 : 1;
-  cudaLaunchKernelEx(&cfg, reg_pose_setup_kernel, cons, x, poses, n, skip);
+  VgxPdlLaunch L(st, dim3((unsigned)((n + 127) / 128)), dim3(128));
+  cudaLaunchKernelEx(&L.cfg, reg_pose_setup_kernel, cons, x, poses, n, skip);
 }
 
 void vgx_launch_reg_reduce(cudaStream_t st, const RegConstraintDev* cons, const RegPoseConst* poses,
-                           const RegTile* tiles, int n_ctas, const int* cta_tile_begin,
-                           const int* tile_order, int* tile_cost, double* partials, int grid_capacity,
-                           const float4* unit_bounds, bool jacobian, const int* skip) {
-  if (n_ctas <= 0) return;
-  // launched with programmatic stream serialisation: its CTAs may start while the pose set-up kernel
-  // is still running; they block at griddepcontrol.wait before touching the pose blocks
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3((unsigned)n_ctas);
-  cfg.blockDim = dim3(VGX_REG_THREADS);
-  cfg.dynamicSmemBytes = sizeof(uint16_t) * (size_t)grid_capacity;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  static const char* no_pdl = getenv("VGX_NO_PDL");
-  cfg.attrs = attr;
-  cfg.numAttrs = (no_pdl && no_pdl[0] == '1') ? 0 : 1;
+                           const RegTile* tiles, int n_tiles, const int* tile_order, int* tile_cost,
+                           double* partials, int grid_capacity, const float4* unit_bounds, bool jacobian,
+                           const int* skip) {
+  if (n_tiles <= 0) return;
+  // its CTAs may start while the pose set-up kernel is still running; they block at
+  // griddepcontrol.wait before touching the pose blocks
+  VgxPdlLaunch L(st, dim3((unsigned)n_tiles), dim3(VGX_REG_THREADS), sizeof(uint16_t) * (size_t)grid_capacity);
   if (jacobian)
-    cudaLaunchKernelEx(&cfg, reg_reduce_kernel<true>, cons, poses, tiles, cta_tile_begin, tile_order, tile_cost,
-                       partials, grid_capacity, unit_bounds, skip);
+    cudaLaunchKernelEx(&L.cfg, reg_reduce_kernel<true>, cons, poses, tiles, tile_order, tile_cost, partials,
+                       grid_capacity, unit_bounds, skip);
   else
-    cudaLaunchKernelEx(&cfg, reg_reduce_kernel<false>, cons, poses, tiles, cta_tile_begin, tile_order, tile_cost,
-                       partials, grid_capacity, unit_bounds, skip);
+    cudaLaunchKernelEx(&L.cfg, reg_reduce_kernel<false>, cons, poses, tiles, tile_order, tile_cost, partials,
+                       grid_capacity, unit_bounds, skip);
 }
 
 int vgx_reg_resident_ctas(int device, int grid_capacity) {
@@ -537,8 +498,6 @@ int vgx_reg_resident_ctas(int device, int grid_capacity) {
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, reg_reduce_kernel<true>, VGX_REG_THREADS,
                                                     smem) != cudaSuccess || per_sm <= 0)
     per_sm = VGX_REG_MIN_BLOCKS;
-  static const char* env = getenv("VGX_REG_CTAS_PER_SM");  // tuning override
-  if (env && atoi(env) > 0) per_sm = atoi(env);
   return sms * per_sm;
 }
 
