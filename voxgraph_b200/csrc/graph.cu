@@ -131,10 +131,6 @@ __device__ __forceinline__ double reg_tile_sum(const double* __restrict__ partia
   for (; t < t1; ++t, p += VGX_REG_NSTRIDE) s += __ldcg(p);
   return s;
 }
-__device__ __forceinline__ double reg_constraint_sum(const RegSums& R, int c, int e) {
-  const double f = R.cons[c].factor;
-  return reg_tile_sum(R.partials, R.tile_begin[c], R.tile_begin[c + 1], e) * (f * f);
-}
 
 // Per-constraint sums csum[c][21] from the tile rows: one warp per constraint, a programmatic
 // dependent of the reduce kernel (and the assembly kernel is one of this).  A separate, massively
@@ -144,10 +140,22 @@ __device__ __forceinline__ double reg_constraint_sum(const RegSums& R, int c, in
 __global__ void __launch_bounds__(128)
 reg_csum_kernel(RegSums R, int n, double* __restrict__ csum, const int* __restrict__ skip) {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  const int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  const bool active = c < n && lane < VGX_REG_NSUM;
+  // the tile range and factor are tables built with the graph: read before the wait
+  int t0 = 0, t1 = 0;
+  double f = 0.0;
+  if (active) { t0 = __ldg(R.tile_begin + c); t1 = __ldg(R.tile_begin + c + 1); f = __ldg(&R.cons[c].factor); }
   asm volatile("griddepcontrol.wait;" ::: "memory");
   if (skip && *skip) return;
-  const int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (c < n && lane < VGX_REG_NSUM) csum[(size_t)c * VGX_REG_NSTRIDE + lane] = reg_constraint_sum(R, c, lane);
+  if (active) csum[(size_t)c * VGX_REG_NSTRIDE + lane] = reg_tile_sum(R.partials, t0, t1, lane) * (f * f);
+}
+
+// Single-rank assembly: wait for the constraint sums (programmatic dependent of the constraint-sum
+// kernel, itself one of the reduce kernel), then let the next evaluation's pose set-up be scheduled.
+__device__ __forceinline__ void vgx_assemble_wait() {
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 
 // Assembly of the packed normal equations, one 4-warp CTA per output block (N diagonal, E
@@ -166,9 +174,11 @@ __device__ __forceinline__ void assemble_block(int ob, const double* __restrict_
                                                const int* __restrict__ csr_begin,
                                                const int4* __restrict__ items,
                                                const VgxP2PPush& push, int N, int E, int n_reg,
-                                               int n_rel, int exclude_reg, double (*s_part)[20]) {
+                                               int n_rel, int exclude_reg, double (*s_part)[20],
+                                               bool wait) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (ob == N + E) {
+    if (wait) vgx_assemble_wait();
     // cost = 1/2 sum r^2
     double a = 0;
     if (!exclude_reg)
@@ -192,7 +202,13 @@ __device__ __forceinline__ void assemble_block(int ob, const double* __restrict_
     __syncthreads();
     return;
   }
-  const int i0 = csr_begin[ob], i1 = csr_begin[ob + 1];
+  const int i0 = __ldg(csr_begin + ob), i1 = __ldg(csr_begin + ob + 1);
+  // the CSR and its items are tables built with the graph: this warp's first two items are read
+  // before the wait, the next trip's during the current one
+  int4 nA = make_int4(-1, 0, 0, 0), nB = make_int4(-1, 0, 0, 0);
+  if (i0 + warp < i1) nA = __ldg(items + i0 + warp);
+  if (i0 + warp + 4 < i1) nB = __ldg(items + i0 + warp + 4);
+  if (wait) vgx_assemble_wait();
   // peer exchange: a block this rank has nothing for is not pushed (the receivers know from the
   // block's rank mask that this slot holds no value of this epoch)
   if (push.tag != 0 && i0 == i1) return;
@@ -202,8 +218,10 @@ __device__ __forceinline__ void assemble_block(int ob, const double* __restrict_
   // warp w expands items w, w + 4, ... in list order; two items per trip so their loads overlap
   for (int i = i0 + warp; i < i1; i += 8) {
     const bool two = i + 4 < i1;
-    const int4 itA = __ldg(items + i);
-    const int4 itB = two ? __ldg(items + i + 4) : make_int4(-1, 0, 0, 0);
+    const int4 itA = nA;
+    const int4 itB = two ? nB : make_int4(-1, 0, 0, 0);
+    if (i + 8 < i1) nA = __ldg(items + i + 8);
+    if (i + 12 < i1) nB = __ldg(items + i + 12);
     double svA = 0.0, svB = 0.0;
     if (!exclude_reg && lane < VGX_REG_NSUM) {
       if (itA.x >= 0) svA = __ldcg(csum + (size_t)itA.x * VGX_REG_NSTRIDE + lane);
@@ -280,11 +298,9 @@ assemble_kernel(const double* __restrict__ csum, const VgxRelEdge* __restrict__ 
                 int n_rel, int exclude_reg, const int* __restrict__ skip) {
   __shared__ double s_part[4][20];
   if (skip && *skip) return;   // evaluation enqueued ahead of a solve that has already ended
-  // programmatic dependent of the constraint-sum kernel (itself one of the reduce kernel): scheduled
-  // while those grids drain, blocked here until the sums are visible
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");   // next evaluation's pose set-up
-  assemble_block(blockIdx.x, csum, rel, x, csr_begin, items, push, N, E, n_reg, n_rel, exclude_reg, s_part);
+  // scheduled while the constraint-sum grid drains; assemble_block reads this block's CSR range and
+  // first items, then blocks in vgx_assemble_wait until the sums are visible
+  assemble_block(blockIdx.x, csum, rel, x, csr_begin, items, push, N, E, n_reg, n_rel, exclude_reg, s_part, true);
 }
 
 // Fused compute + collective (multi-rank, peer exchange): ONE launch assembles this rank's
@@ -305,7 +321,7 @@ assemble_exchange_kernel(const double* __restrict__ csum, const VgxRelEdge* __re
   asm volatile("griddepcontrol.wait;" ::: "memory");   // see assemble_kernel
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   for (int ob = blockIdx.x; ob <= N + E; ob += gridDim.x)
-    assemble_block(ob, csum, rel, x, csr_begin, items, push, N, E, n_reg, n_rel, exclude_reg, s_part);
+    assemble_block(ob, csum, rel, x, csr_begin, items, push, N, E, n_reg, n_rel, exclude_reg, s_part, false);
   vgx_ll_gather(gat, out, (size_t)count, (size_t)blockIdx.x * blockDim.x + threadIdx.x,
                 (size_t)gridDim.x * blockDim.x, block_mask, N);
 }
@@ -434,15 +450,18 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
   g->grid_capacity = 0;
   for (const auto& cc : cons)
     if (cc.grid) g->grid_capacity = std::max(g->grid_capacity, (cc.gd0 * cc.gd1 * cc.gd2 + 7) & ~7);  // 16-byte multiple
-  const int resident_ctas = std::max(vgx_reg_resident_ctas(c->device, g->grid_capacity), 1);
+  int sms = 132;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
+  const int slots = std::max(sms, 1) * VGX_REG_TILE_SLOTS_PER_SM;
   int64_t U = 0;  // total units
   for (const auto& cc : cons) U += (cc.n + VGX_REG_UNIT - 1) / VGX_REG_UNIT;
   // Tile size: at most VGX_REG_HW_TILE_UNITS units, fewer when the problem is small, so that there
-  // are at least ~2 tiles per resident CTA slot (a 3-pair streaming graph still fills the machine).
+  // are at least ~2 tiles per CTA slot (a 3-pair streaming graph still fills the machine).  The slots
+  // are a fixed count per SM, not the resident CTAs, so that the tiles do not follow the occupancy.
   // The environment variable of the same name forces a size (n >= 1; tests use it for shapes the
   // formula never produces).
   int hw_units = (int)std::min<int64_t>(VGX_REG_HW_TILE_UNITS,
-                                        std::max<int64_t>(4, (U + 2 * (int64_t)resident_ctas - 1) / (2 * (int64_t)resident_ctas)));
+                                        std::max<int64_t>(4, (U + 2 * (int64_t)slots - 1) / (2 * (int64_t)slots)));
   if (const char* env = getenv("VGX_REG_HW_TILE_UNITS"))
     if (atoi(env) >= 1) hw_units = atoi(env);
   g->evals_since_order = -1;

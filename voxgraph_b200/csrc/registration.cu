@@ -449,21 +449,49 @@ void vgx_launch_reg_order(cudaStream_t st, const int* tile_cost, int n_tiles, in
   if (n_tiles > 0) reg_order_kernel<<<1, 1024, 0, st>>>(tile_cost, n_tiles, tile_order);
 }
 
-__global__ void reg_pose_setup_kernel(const RegConstraintDev* __restrict__ constraints,
-                                      const double* __restrict__ x, RegPoseConst* __restrict__ poses,
-                                      int n_constraints, const int* __restrict__ skip) {
+// The pose blocks of one evaluation, one thread per constraint.  The kernel is a programmatic
+// dependent of what precedes it, and the pose arithmetic (eight double sin / cos) is most of its
+// time, so it is done speculatively BEFORE griddepcontrol.wait from the poses as they read then.
+// After the wait the poses are read again (through L2), and the block is recomputed only if one of
+// them differs bit for bit: the block written is always the one of the poses the predecessor left,
+// and when they did not change (consecutive evaluations at the same poses) the arithmetic is off the
+// critical path.  The pose blocks themselves are written after the wait: they were read by the
+// previous evaluation's reduce kernel, which has completed once the assembly (its dependent) has.
+__device__ __forceinline__ void reg_load_pose(const double* x, int node, double* p) {
+  const double2* q = reinterpret_cast<const double2*>(x + 4 * (size_t)node);   // 32-byte aligned rows
+  const double2 a = __ldcg(q), b = __ldcg(q + 1);
+  p[0] = a.x; p[1] = a.y; p[2] = b.x; p[3] = b.y;
+}
+__global__ void reg_pose_setup_kernel(const RegConstraintDev* __restrict__ constraints, const double* x,
+                                      RegPoseConst* __restrict__ poses, int n_constraints,
+                                      const int* __restrict__ skip) {
   // programmatic dependent launch: the reduce kernel may start its prologue (tile records, TMA of the
   // descriptors, block grids and first point units) while the pose blocks are still being computed
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  // ... and this kernel may itself have been scheduled while the previous evaluation's assembly was
-  // still running: the pose blocks it overwrites were read by that evaluation's reduce kernel, which
-  // has completed once the assembly (its dependent) has
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool active = c < n_constraints;
+  int na = 0, nb = 0;
+  double ref[4] = {0, 0, 0, 0}, read[4] = {0, 0, 0, 0};
+  RegPoseConst P;
+  if (active) {
+    na = __ldg(&constraints[c].ref_node);
+    nb = __ldg(&constraints[c].read_node);
+    reg_load_pose(x, na, ref);
+    reg_load_pose(x, nb, read);
+    vgx_reg_pose_setup<TrigDevice>(ref, read, P);
+  }
   asm volatile("griddepcontrol.wait;" ::: "memory");
   if (skip && *skip) return;
-  const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= n_constraints) return;
-  RegPoseConst P;
-  vgx_reg_pose_setup<TrigDevice>(x + 4 * constraints[c].ref_node, x + 4 * constraints[c].read_node, P);
+  if (!active) return;
+  double ref1[4], read1[4];
+  reg_load_pose(x, na, ref1);
+  reg_load_pose(x, nb, read1);
+  bool same = true;
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    same = same && __double_as_longlong(ref1[k]) == __double_as_longlong(ref[k]) &&
+           __double_as_longlong(read1[k]) == __double_as_longlong(read[k]);
+  if (!same) vgx_reg_pose_setup<TrigDevice>(ref1, read1, P);
   poses[c] = P;
 }
 
@@ -489,16 +517,6 @@ void vgx_launch_reg_reduce(cudaStream_t st, const RegConstraintDev* cons, const 
   else
     cudaLaunchKernelEx(&L.cfg, reg_reduce_kernel<false>, cons, poses, tiles, tile_order, tile_cost, partials,
                        grid_capacity, unit_bounds, skip);
-}
-
-int vgx_reg_resident_ctas(int device, int grid_capacity) {
-  int sms = 132, per_sm = 0;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-  const size_t smem = sizeof(uint16_t) * (size_t)grid_capacity;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, reg_reduce_kernel<true>, VGX_REG_THREADS,
-                                                    smem) != cudaSuccess || per_sm <= 0)
-    per_sm = VGX_REG_MIN_BLOCKS;
-  return sms * per_sm;
 }
 
 // cpp:45-55: num_residuals = int(sampling_ratio * size()) (float product) or size()

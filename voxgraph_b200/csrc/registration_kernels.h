@@ -7,9 +7,10 @@ struct RegConstraintDev;
 struct RegPoseConst;
 
 #define VGX_REG_THREADS 128        // 4 warps per CTA, each with its own TMA ring + software pipeline
-#define VGX_REG_MIN_BLOCKS 7       // resident CTAs per SM the register budget is sized for (72 registers).
-                                   // 8 also fits without spills, but the tile size follows the resident CTA
-                                   // count (graph.cu), so config 2's tiles and with them its sums would change
+#define VGX_REG_MIN_BLOCKS 8       // resident CTAs per SM the register budget is sized for (64 registers)
+#define VGX_REG_TILE_SLOTS_PER_SM 7  // CTA slots per SM the tile size is cut for (graph.cu).  A fixed count,
+                                     // not the resident one: the tiles, and with them the last bits of every
+                                     // sum, do not follow the occupancy (7 CTAs per SM when the rule was set)
 #define VGX_REG_RING 4             // point-slice ring slots per warp (units in flight = RING - 1)
 #define VGX_REG_HW_TILE_UNITS 64   // largest tile, in units (graph.cu makes them smaller on small problems)
 #define VGX_REG_UNIT 32            // points per unit = one warp iteration; tiles are cut on unit boundaries
@@ -50,7 +51,7 @@ struct VgxPdlLaunch {
 void vgx_launch_reg_pose_setup(cudaStream_t st, const RegConstraintDev* cons, const double* x,
                                RegPoseConst* poses, int n, const int* skip = nullptr);
 // One CTA per tile, CTA b running tile tile_order[b] -> partials[tile][21] and tile_cost[tile]; the
-// consumer adds a constraint's tiles in tile order (graph.cu: reg_constraint_sum).  unit_bounds (may be
+// consumer adds a constraint's tiles in tile order (graph.cu: reg_csum_kernel).  unit_bounds (may be
 // null: no culling): the table vgx_launch_reg_unit_bounds fills, indexed by RegTile::unit0 + unit.
 void vgx_launch_reg_reduce(cudaStream_t st, const RegConstraintDev* cons, const RegPoseConst* poses,
                            const RegTile* tiles, int n_tiles, const int* tile_order, int* tile_cost,
@@ -61,9 +62,6 @@ void vgx_launch_reg_reduce(cudaStream_t st, const RegConstraintDev* cons, const 
 void vgx_launch_reg_unit_bounds(cudaStream_t st, const RegTile* tiles, int n_tiles, float4* bounds);
 // tile_order <- tiles sorted by measured cost, most expensive first
 void vgx_launch_reg_order(cudaStream_t st, const int* tile_cost, int n_tiles, int* tile_order);
-// SMs x CTAs of the reduce kernel that are co-resident with `grid_capacity` cells of dynamic smem; the
-// tile size follows it (graph.cu), and with the tiles the last bits of every sum
-int vgx_reg_resident_ctas(int device, int grid_capacity);
 // Fills the descriptor of one (reference -> reading) residual block.  Deterministic mode: pts / n /
 // factor describe all registration points.  Sampling mode (*sampled = true): n = int(ratio * K),
 // factor = 1 (all weights forced to 1) and pts is left null for the caller, who draws the
