@@ -298,7 +298,12 @@ typedef struct vgx_tsdf_stats {
 
 void vgx_tsdf_config_default(vgx_tsdf_config* cfg);
 /* integratePointCloud(T_G_C, points_C, colors): T_G_C = [qw qx qy qz tx ty tz];
- * rgba may be NULL. Host buffers; copies are part of the call. */
+ * rgba may be NULL. Host buffers; copies are part of the call.
+ * Index range (both modes): a block with a component outside [VGX_BLOCK_INDEX_MIN,
+ * VGX_BLOCK_INDEX_MAX] (in the submap frame, |coordinate| beyond about 2^20 block sizes) is never
+ * allocated.  Its voxels are skipped: not updated, not counted in voxel_updates, no capacity error;
+ * the ray still counts in rays_valid / rays_cast.  Every downloaded block index is therefore one
+ * vgx_submap_upload accepts. */
 int vgx_tsdf_integrate(vgx_ctx* ctx, uint32_t submap_id, const float T_G_C[7], int n,
                        const float* points_C /* n x 3 */, const uint8_t* rgba /* n x 4 or NULL */,
                        const vgx_tsdf_config* cfg, vgx_tsdf_stats* stats /* may be NULL */);
@@ -327,7 +332,10 @@ int vgx_reg_num_residuals(vgx_ctx* ctx, uint32_t reference_submap_id, const vgx_
 /* Evaluate(parameters, residuals, jacobians): Ceres layout, residuals[K] and two K x 4
  * row-major Jacobian blocks (either may be NULL). Returns VGX_OK, or VGX_ZERO_WEIGHT
  * where Evaluate returns false.  In sampling mode every call draws a fresh sample from the
- * reference submap's generator, exactly as every Evaluate does in the reference. */
+ * reference submap's generator, exactly as every Evaluate does in the reference.
+ * Index range (here and in vgx_graph_eval): no block exists outside [VGX_BLOCK_INDEX_MIN,
+ * VGX_BLOCK_INDEX_MAX], so a point whose block lies outside it has no correspondence, as in the
+ * reference, whose blocks can never be there (uploads and integration refuse them). */
 int vgx_reg_eval_emit(vgx_ctx* ctx, uint32_t reference_submap_id, uint32_t reading_submap_id,
                       const vgx_reg_config* cfg, const double reference_pose[4],
                       const double reading_pose[4], double* residuals, double* jac_reference,

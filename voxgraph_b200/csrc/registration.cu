@@ -343,6 +343,7 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
         const int slot_m = moved ? vgx_grid_slot(s_C, s_grid, L.b0, L.b1, L.b2) : slot_c;
         slot_b = slot_c >= 0 ? slot_m : -1;
       } else {
+        vgx_probe_range(b0, b1, b2);
         vgx_locate_in_block(s_C, p0, p1, p2, b0, b1, b2, L);
         RegProbe H = vgx_probe_start(s_C, L);
         slot_b = vgx_resolve(s_C, H);

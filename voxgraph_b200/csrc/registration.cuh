@@ -214,6 +214,19 @@ __device__ __forceinline__ void vgx_locate(const RegConstraintDev& C, float p0, 
   vgx_locate_in_block(C, p0, p1, p2, b0, b1, b2, L);
 }
 
+// Range rule of the hash path, applied to b0..b2 = the block that CONTAINS pos (vgx_block_index) before
+// the base corner is located.  Outside [VGX_BLOCK_INDEX_MIN, VGX_BLOCK_INDEX_MAX] there is no block
+// (vgx_block_in_range): the reference's first lookup fails and the point has no correspondence, while
+// a probe of the packed key would find the block it aliases, 2^21 away.  Such a block is moved to
+// x = MIN - 1, and the base corner then lies at x = MIN - 1 or MIN - 2: their 21-bit key fields are 0 and
+// 2^21 - 1, which no block in the range packs to, so the probe runs on to an empty slot and misses.
+// Inside the range the base corner lies in [MIN - 1, MAX] on every axis, where vgx_pack_key is
+// injective and MIN - 1 is never inserted: the probe is exact.  (A select, not a branch: the cost-only
+// reduce kernel has no register to keep a predicate live across the locate phase.)
+__device__ __forceinline__ void vgx_probe_range(int& b0, int b1, int b2) {
+  b0 = vgx_block_in_range(b0, b1, b2) ? b0 : VGX_BLOCK_INDEX_MIN - 1;
+}
+
 // first probe of the base corner's block in the reading submap's hash (load issued)
 __device__ __forceinline__ RegProbe vgx_probe_start(const RegConstraintDev& C, const RegLocate& L) {
   RegProbe H;
@@ -243,8 +256,11 @@ __device__ __forceinline__ bool vgx_octet_ok(const float d[8]) {
 __device__ __forceinline__ bool vgx_interp_gather(const RegConstraintDev& C, float p0, float p1,
                                                   float p2, float d[8], float& ox, float& oy,
                                                   float& oz) {
+  int b0, b1, b2;
+  vgx_block_index(C, p0, p1, p2, b0, b1, b2);
+  vgx_probe_range(b0, b1, b2);
   RegLocate L;
-  vgx_locate(C, p0, p1, p2, L);
+  vgx_locate_in_block(C, p0, p1, p2, b0, b1, b2, L);
   RegProbe H = vgx_probe_start(C, L);
   const int slot = vgx_resolve(C, H);
   if (slot < 0) return false;

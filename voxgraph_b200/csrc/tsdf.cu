@@ -214,6 +214,16 @@ __device__ __forceinline__ int tsdf_get_or_alloc(const VgxHash& hash, int32_t* _
   return -1;
 }
 
+// Block of the global voxel index g.  False when a component lies outside [VGX_BLOCK_INDEX_MIN,
+// VGX_BLOCK_INDEX_MAX]: such a block is never allocated and its voxels are skipped (its key would alias
+// a block 2^21 away).  The test is made on the 64-bit index, before the cast to int could wrap it.
+__device__ __forceinline__ bool tsdf_block_of(const long long g[3], int sh, int& b0, int& b1, int& b2) {
+  const long long c0 = g[0] >> sh, c1 = g[1] >> sh, c2 = g[2] >> sh;
+  b0 = (int)c0; b1 = (int)c1; b2 = (int)c2;
+  return c0 >= VGX_BLOCK_INDEX_MIN && c0 <= VGX_BLOCK_INDEX_MAX && c1 >= VGX_BLOCK_INDEX_MIN &&
+         c1 <= VGX_BLOCK_INDEX_MAX && c2 >= VGX_BLOCK_INDEX_MIN && c2 <= VGX_BLOCK_INDEX_MAX;
+}
+
 // ------------------------------------------------------------------ pass 1: allocate
 __global__ void __launch_bounds__(128)
 tsdf_allocate_kernel(TsdfParams P, const float* __restrict__ pts, VgxHash hash,
@@ -224,10 +234,10 @@ tsdf_allocate_kernel(TsdfParams P, const float* __restrict__ pts, VgxHash hash,
   float origin[3], pG[3], weight;
   if (!point_to_ray(P, pts, i, rc, origin, pG, weight)) return;
   long long g[3];
-  int lb0 = INT_MIN, lb1 = 0, lb2 = 0;
+  int lb0 = INT_MIN, lb1 = 0, lb2 = 0;   // INT_MIN: no block (outside the range)
   while (ray_next(rc, g)) {
-    const int b0 = (int)(g[0] >> P.vps_shift), b1 = (int)(g[1] >> P.vps_shift),
-              b2 = (int)(g[2] >> P.vps_shift);
+    int b0, b1, b2;
+    if (!tsdf_block_of(g, P.vps_shift, b0, b1, b2)) { lb0 = INT_MIN; continue; }
     if (b0 == lb0 && b1 == lb1 && b2 == lb2) continue;
     lb0 = b0; lb1 = b1; lb2 = b2;
     tsdf_get_or_alloc<false>(hash, block_idx, counters, capacity, b0, b1, b2);
@@ -326,8 +336,10 @@ tsdf_emit_kernel(TsdfParams P, const float* __restrict__ pts, VgxHash hash,
       int lb0 = INT_MIN, lb1 = 0, lb2 = 0, slot = -1;
       const int vmask = P.vps - 1, sh = P.vps_shift;
       while (ray_next(rc, g)) {
-        const int b0 = (int)(g[0] >> sh), b1 = (int)(g[1] >> sh), b2 = (int)(g[2] >> sh);
-        if (!(b0 == lb0 && b1 == lb1 && b2 == lb2)) {
+        int b0, b1, b2;
+        if (!tsdf_block_of(g, sh, b0, b1, b2)) {
+          lb0 = INT_MIN; slot = -1;            // outside the range: the voxel is skipped
+        } else if (!(b0 == lb0 && b1 == lb1 && b2 == lb2)) {
           lb0 = b0; lb1 = b1; lb2 = b2;
           slot = vgx_hash_find(hash, b0, b1, b2);
         }
@@ -499,12 +511,14 @@ tsdf_integrate_kernel(TsdfParams P, const float* __restrict__ pts, VgxHash hash,
             if (old == h) ++collisions; else collisions = 0;
             if (collisions > P.cfg.max_consecutive_ray_collisions) break;
           }
-          const int b0 = (int)(g[0] >> sh), b1 = (int)(g[1] >> sh), b2 = (int)(g[2] >> sh);
-          if (!(b0 == lb0 && b1 == lb1 && b2 == lb2)) {
+          int b0, b1, b2;
+          if (!tsdf_block_of(g, sh, b0, b1, b2)) {
+            lb0 = INT_MIN; slot = -1;          // outside the range: the voxel is skipped
+          } else if (!(b0 == lb0 && b1 == lb1 && b2 == lb2)) {
             lb0 = b0; lb1 = b1; lb2 = b2;
             slot = tsdf_get_or_alloc<true>(hash, block_idx, counters, capacity, b0, b1, b2);
           }
-          if (slot < 0) continue;  // capacity exhausted (reported by the host)
+          if (slot < 0) continue;  // outside the range, or capacity exhausted (reported by the host)
           const int lin = (int)(g[0] & vmask) + (((int)(g[1] & vmask)) << sh) + (((int)(g[2] & vmask)) << (2 * sh));
           update_tsdf_voxel(P, origin, pG, g, weight, dw + (size_t)slot * vpb + lin);
           ++n_upd;

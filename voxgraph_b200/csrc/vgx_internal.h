@@ -41,6 +41,12 @@ __host__ __device__ __forceinline__ uint64_t vgx_pack_key(int bx, int by, int bz
 __host__ __device__ __forceinline__ bool vgx_block_index_ok(int b) {
   return b >= VGX_BLOCK_INDEX_MIN && b <= VGX_BLOCK_INDEX_MAX;
 }
+// The range rule: no block exists outside [VGX_BLOCK_INDEX_MIN, VGX_BLOCK_INDEX_MAX] on any axis
+// (uploads refuse one, integration never allocates one), so a lookup there is a miss without a probe.
+// Inside the range vgx_pack_key is injective; outside it a key aliases a block 2^21 away.
+__host__ __device__ __forceinline__ bool vgx_block_in_range(int bx, int by, int bz) {
+  return vgx_block_index_ok(bx) && vgx_block_index_ok(by) && vgx_block_index_ok(bz);
+}
 __host__ __device__ __forceinline__ uint32_t vgx_hash_index(int bx, int by, int bz, uint32_t mask) {
   uint64_t h = (uint64_t)(int64_t)bx + (uint64_t)(int64_t)by * 17191ull +
                (uint64_t)(int64_t)bz * (17191ull * 17191ull);
@@ -63,8 +69,10 @@ struct VgxHash {
 #ifdef __CUDACC__
 // Read-only lookup (finished layers / kernels that do not insert concurrently).  At most
 // table-size probes: a completely full table (capacity overflow) ends the search instead of
-// spinning.  Entries with val < 0 (unmapped / overflowed) read as "no block".
+// spinning.  Entries with val < 0 (unmapped / overflowed) read as "no block", and so does an index
+// outside the range (vgx_block_in_range).
 __device__ __forceinline__ int vgx_hash_find(const VgxHash& h, int bx, int by, int bz) {
+  if (!vgx_block_in_range(bx, by, bz)) return -1;
   const uint64_t key = vgx_pack_key(bx, by, bz);
   uint32_t i = vgx_hash_index(bx, by, bz, h.mask);
   for (uint32_t n = 0; n <= h.mask; ++n) {
