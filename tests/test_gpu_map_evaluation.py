@@ -425,7 +425,7 @@ def test_map_evaluate_recovers_offset(ctx, oracle, scene):
     ctx.submap_free(gt)
 
 
-def test_map_evaluate_deterministic_and_api(ctx, scene, tmp_path):
+def test_map_evaluate_deterministic_and_api(ctx, oracle, scene, tmp_path):
     from voxgraph_b200 import api
     map_id, data, lay = scene
     T = _offset_T()[None]
@@ -448,6 +448,8 @@ def test_map_evaluate_deterministic_and_api(ctx, scene, tmp_path):
     Tinv = ev.T_ground_truth__reading
     Tf = np.frombuffer(res[0][2], F32)
     assert Tinv[0] == Tf[0] and Tinv[3] == -Tf[3]
+    # the shared float inverse (minkindr QuatTransformation::inverse), all seven components bit for bit
+    assert np.asarray(Tinv, F32).tobytes() == oracle.T_inverse(Tf).tobytes()
     ctx.submap_free(gt)
 
 

@@ -21,7 +21,7 @@ SOURCES = [
     ("esdf.cu", ["-fmad=false"]),
     ("mesh.cu", ["-fmad=false"]),
     ("project.cu", ["-fmad=false", "-Xcompiler", "-ffp-contract=off"]),
-    ("evaluate.cu", ["-fmad=false"]),
+    ("evaluate.cu", ["-fmad=false", "-Xcompiler", "-ffp-contract=off"]),
     ("collection.cu", []),
     ("graph.cu", []),
     ("solve.cu", []),

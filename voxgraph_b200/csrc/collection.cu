@@ -441,9 +441,14 @@ struct Parser {
     }
     if (!(have[0] && have[1] && have[2])) return fail("SubmapCollectionProto lacks a field");
     if (*num_submaps == 0) return true;   // no layer: the geometry is not used
-    const uint32_t vps = L->vps;
-    if (vps < 2 || vps > 32 || (vps & (vps - 1)) != 0) return fail("voxels_per_side must be a power of two in [2, 32]");
-    if (!(L->voxel_size > 0) || !((float)L->voxel_size > 0) || !isfinite((float)L->voxel_size))
+    return geometry(*L);
+  }
+
+  // the layer geometry of the header, as the upload path accepts it
+  bool geometry(const CollLayout& L) {
+    if (L.vps < 2 || L.vps > 32 || (L.vps & (L.vps - 1)) != 0)
+      return fail("voxels_per_side must be a power of two in [2, 32]");
+    if (!(L.voxel_size > 0) || !((float)L.voxel_size > 0) || !isfinite((float)L.voxel_size))
       return fail("voxel_size must be positive and finite");
     return true;
   }
@@ -555,6 +560,18 @@ struct Parser {
     return true;
   }
 
+  // the next n BlockProtos, appended to L's blocks
+  bool blocks(CollLayout* L, uint32_t n) {
+    for (uint32_t k = 0; k < n; ++k) {
+      CollBlockRef b{};
+      int32_t idx[3];
+      if (!block(*L, &b, idx)) return false;
+      L->blocks.push_back(b);
+      L->block_idx.insert(L->block_idx.end(), idx, idx + 3);
+    }
+    return true;
+  }
+
   // a voxblox layer file (vgx_layer_load): the whole stream is one layer, held as one submap entry
   bool layer_stream(CollLayout* L) {
     uint32_t count = 0;
@@ -584,21 +601,12 @@ struct Parser {
     }
     if (!(have[0] && have[1] && have[2])) return fail("LayerProto lacks a field");
     if (type != "tsdf") return fail("LayerProto.type is not \"tsdf\"");
-    const uint32_t vps = L->vps;
-    if (vps < 2 || vps > 32 || (vps & (vps - 1)) != 0) return fail("voxels_per_side must be a power of two in [2, 32]");
-    if (!(L->voxel_size > 0) || !((float)L->voxel_size > 0) || !isfinite((float)L->voxel_size))
-      return fail("voxel_size must be positive and finite");
+    if (!geometry(*L)) return false;
     CollSubmapRef s{};
     s.n_blocks = count - 1;
     s.first_block = 0;
     if (s.n_blocks > (uint32_t)INT32_MAX) return fail("too many blocks");
-    for (uint32_t k = 0; k < s.n_blocks; ++k) {
-      CollBlockRef b{};
-      int32_t idx[3];
-      if (!block(*L, &b, idx)) return false;
-      L->blocks.push_back(b);
-      L->block_idx.insert(L->block_idx.end(), idx, idx + 3);
-    }
+    if (!blocks(L, s.n_blocks)) return false;
     L->submaps.push_back(s);
     if (c.p != c.end) return fail("trailing bytes after the last block");
     return true;
@@ -613,13 +621,7 @@ struct Parser {
       if (!submap(&s)) return false;
       if (!ids.insert(s.id).second) return fail("submap id " + std::to_string(s.id) + " appears twice");
       s.first_block = L->blocks.size();
-      for (uint32_t k = 0; k < s.n_blocks; ++k) {
-        CollBlockRef b{};
-        int32_t idx[3];
-        if (!block(*L, &b, idx)) return false;
-        L->blocks.push_back(b);
-        L->block_idx.insert(L->block_idx.end(), idx, idx + 3);
-      }
+      if (!blocks(L, s.n_blocks)) return false;
       L->submaps.push_back(s);
     }
     if (c.p != c.end) return fail("trailing bytes after the last block");
@@ -628,24 +630,14 @@ struct Parser {
   }
 };
 
-bool parse_stream(const uint8_t* bytes, uint64_t n, CollLayout* L, std::string* err) {
+// layer: a voxblox layer file (one submap entry) instead of a submap collection
+bool parse_stream(const uint8_t* bytes, uint64_t n, bool layer, CollLayout* L, std::string* err) {
   Parser p{bytes, Cursor{bytes, bytes + n}, std::string()};
   if (!bytes && n) {
     *err = "null stream";
     return false;
   }
-  const bool ok = p.stream(L);
-  if (!ok) *err = p.err;
-  return ok;
-}
-
-bool parse_layer_stream(const uint8_t* bytes, uint64_t n, CollLayout* L, std::string* err) {
-  Parser p{bytes, Cursor{bytes, bytes + n}, std::string()};
-  if (!bytes && n) {
-    *err = "null stream";
-    return false;
-  }
-  const bool ok = p.layer_stream(L);
+  const bool ok = layer ? p.layer_stream(L) : p.stream(L);
   if (!ok) *err = p.err;
   return ok;
 }
@@ -772,7 +764,7 @@ extern "C" int vgx_collection_scan(const uint8_t* bytes, uint64_t n, int max_sub
   *n_submaps = 0;
   CollLayout L;
   std::string err;
-  if (!parse_stream(bytes, n, &L, &err)) return VGX_ERR_INVALID;
+  if (!parse_stream(bytes, n, false, &L, &err)) return VGX_ERR_INVALID;
   if (L.submaps.size() > (size_t)INT32_MAX) return VGX_ERR_INVALID;
   *n_submaps = (int)L.submaps.size();
   if (L.submaps.size() > (size_t)max_submaps) return VGX_ERR_CAPACITY;
@@ -787,27 +779,11 @@ extern "C" int vgx_collection_scan(const uint8_t* bytes, uint64_t n, int max_sub
   return VGX_OK;
 }
 
-extern "C" int vgx_collection_load(vgx_ctx* c, const uint8_t* bytes, uint64_t n, int* n_submaps) {
-  if (!c) return VGX_ERR_INVALID;
-  if (n_submaps) *n_submaps = 0;
-  CollLayout L;
-  std::string err;
-  if (!parse_stream(bytes, n, &L, &err)) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_collection_load: " + err);
-  for (const CollSubmapRef& s : L.submaps)
-    if (c->find(s.id))
-      VGX_FAIL(c, VGX_ERR_INVALID, "vgx_collection_load: submap " + std::to_string(s.id) + " already exists");
+// Decodes a parsed stream into new submaps, one per entry of L.submaps under the entry's id, then runs the
+// upload path (block hash, registration view, block-index rules, grid) on each.  `what` prefixes errors.
+static int decode_layout(vgx_ctx* c, const char* what, const CollLayout& L, const uint8_t* bytes, uint64_t n) {
   VGX_CUDA(c, cudaSetDevice(c->device));
   const int vpb = (int)(L.vps * L.vps * L.vps);
-  const float voxel_size = (float)L.voxel_size;
-  std::vector<uint32_t> created;
-  // every failure past this point removes the submaps this call created
-  auto fail_all = [&](int rc) {
-    const std::string msg = c->error;
-    for (uint32_t id : created)
-      if (c->find(id)) vgx_submap_free(c, id);
-    c->set_error(msg);
-    return rc;
-  };
   const size_t table_bytes = (L.blocks.size() * sizeof(CollBlockRef) + 15) & ~(size_t)15;
   const size_t bytes_off = table_bytes + 16;   // [regions | error word | stream bytes]
   int rc = c->ensure_scratch(bytes_off + (size_t)n);
@@ -816,7 +792,7 @@ extern "C" int vgx_collection_load(vgx_ctx* c, const uint8_t* bytes, uint64_t n,
   CollBlockRef* d_regions = (CollBlockRef*)d;
   int* d_err = (int*)(d + table_bytes);
   {
-    VgxLaunchScope copies(c, 10, 0);
+    VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
     if (!L.blocks.empty())
       VGX_CUDA(c, cudaMemcpyAsync(d_regions, L.blocks.data(), L.blocks.size() * sizeof(CollBlockRef),
                                   cudaMemcpyHostToDevice, c->stream));
@@ -826,22 +802,21 @@ extern "C" int vgx_collection_load(vgx_ctx* c, const uint8_t* bytes, uint64_t n,
   }
   for (const CollSubmapRef& s : L.submaps) {
     VgxSubmap* sm = nullptr;
-    rc = vgx_submap_alloc(c, s.id, voxel_size, (int)L.vps, (int)s.n_blocks, true, &sm);
-    if (rc != VGX_OK) return fail_all(rc);
-    created.push_back(s.id);
+    rc = vgx_submap_alloc(c, s.id, (float)L.voxel_size, (int)L.vps, (int)s.n_blocks, true, &sm);
+    if (rc != VGX_OK) return rc;
     sm->n_blocks = (int)s.n_blocks;
     sm->finished = true;
     if (s.n_blocks == 0) continue;
     {
-      VgxLaunchScope copies(c, 10, 0);
+      VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
       const cudaError_t e = cudaMemcpyAsync(sm->d_block_idx, L.block_idx.data() + 3 * s.first_block,
                                             sizeof(int32_t) * 3 * s.n_blocks, cudaMemcpyHostToDevice, c->stream);
       if (e != cudaSuccess) {
-        c->set_error(std::string("vgx_collection_load: ") + cudaGetErrorString(e));
-        return fail_all(VGX_ERR_CUDA);
+        c->set_error(std::string(what) + ": " + cudaGetErrorString(e));
+        return VGX_ERR_CUDA;
       }
     }
-    VgxLaunchScope scope(c, 9);
+    VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
     collection_decode_kernel<<<s.n_blocks, COLL_THREADS, 0, c->stream>>>(
         d + bytes_off, d_regions + s.first_block, vpb, reinterpret_cast<float*>(sm->d_dw), d_err);
   }
@@ -850,25 +825,45 @@ extern "C" int vgx_collection_load(vgx_ctx* c, const uint8_t* bytes, uint64_t n,
   if (e == cudaSuccess) e = cudaMemcpyAsync(&h_err, d_err, sizeof(int), cudaMemcpyDeviceToHost, c->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
   if (e != cudaSuccess) {
-    c->set_error(std::string("vgx_collection_load: ") + cudaGetErrorString(e));
-    return fail_all(VGX_ERR_CUDA);
+    c->set_error(std::string(what) + ": " + cudaGetErrorString(e));
+    return VGX_ERR_CUDA;
   }
   if (h_err) {
-    c->set_error(std::string("vgx_collection_load: voxel_data: ") +
+    c->set_error(std::string(what) + ": voxel_data: " +
                  ((h_err & COLL_ERR_TAG) ? "unexpected tag; " : "") +
                  ((h_err & COLL_ERR_VARINT) ? "varint longer than 5 bytes, above 32 bits or truncated; " : "") +
                  ((h_err & COLL_ERR_COUNT) ? "not 3 vps^3 values; " : "") +
                  ((h_err & COLL_ERR_LENGTH) ? "packed length does not match the block; " : ""));
-    return fail_all(VGX_ERR_INVALID);
+    return VGX_ERR_INVALID;
   }
-  // the upload path's hash build, view and block-index rules
   for (const CollSubmapRef& s : L.submaps) {
-    VgxLaunchScope scope(c, 11, 0);
-    rc = vgx_submap_upload_finish(c, c->find(s.id), "vgx_collection_load");
-    if (rc != VGX_OK) return fail_all(rc);
+    VgxLaunchScope scope(c, VGX_SLOT_COLL_UPLOAD, 0);
+    rc = vgx_submap_upload_finish(c, c->find(s.id), what);
+    if (rc != VGX_OK) return rc;
   }
-  if (n_submaps) *n_submaps = (int)L.submaps.size();
   return VGX_OK;
+}
+
+// decode_layout for ids none of which exists yet: on failure no submap of L is left
+static int load_layout(vgx_ctx* c, const char* what, const CollLayout& L, const uint8_t* bytes, uint64_t n) {
+  const int rc = decode_layout(c, what, L, bytes, n);
+  if (rc != VGX_OK)
+    for (const CollSubmapRef& s : L.submaps) vgx_submap_drop(c, s.id);
+  return rc;
+}
+
+extern "C" int vgx_collection_load(vgx_ctx* c, const uint8_t* bytes, uint64_t n, int* n_submaps) {
+  if (!c) return VGX_ERR_INVALID;
+  if (n_submaps) *n_submaps = 0;
+  CollLayout L;
+  std::string err;
+  if (!parse_stream(bytes, n, false, &L, &err)) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_collection_load: " + err);
+  for (const CollSubmapRef& s : L.submaps)
+    if (c->find(s.id))
+      VGX_FAIL(c, VGX_ERR_INVALID, "vgx_collection_load: submap " + std::to_string(s.id) + " already exists");
+  const int rc = load_layout(c, "vgx_collection_load", L, bytes, n);
+  if (rc == VGX_OK && n_submaps) *n_submaps = (int)L.submaps.size();
+  return rc;
 }
 
 extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const float* T_M_S, uint8_t* out,
@@ -913,7 +908,7 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
       a.block_idx = s->d_block_idx;
       a.vox_per_block = s->vox_per_block;
       a.out_sizes = d_sizes + first;
-      VgxLaunchScope scope(c, 9);
+      VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
       collection_encode_kernel<false><<<s->n_blocks, COLL_THREADS, 0, c->stream>>>(a);
     }
     first += (size_t)s->n_blocks;
@@ -953,7 +948,7 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
   uint64_t* d_offs = (uint64_t*)((uint8_t*)c->d_scratch + sizes_bytes);
   uint8_t* d_msgs = (uint8_t*)c->d_scratch + sizes_bytes + offs_bytes;
   if (total_blocks) {
-    VgxLaunchScope copies(c, 10, 0);
+    VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
     VGX_CUDA(c, cudaMemcpyAsync(d_sizes, sizes.data(), total_blocks * sizeof(uint32_t), cudaMemcpyHostToDevice,
                                 c->stream));
     VGX_CUDA(c, cudaMemcpyAsync(d_offs, offsets.data(), total_blocks * sizeof(uint64_t), cudaMemcpyHostToDevice,
@@ -970,13 +965,13 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
       a.block_size = s->block_size;
       a.sizes = d_sizes + first;
       a.offsets = d_offs + first;
-      VgxLaunchScope scope(c, 9);
+      VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
       collection_encode_kernel<true><<<s->n_blocks, COLL_THREADS, 0, c->stream>>>(a);
     }
     first += (size_t)s->n_blocks;
   }
   VGX_CUDA(c, cudaGetLastError());
-  VgxLaunchScope copies(c, 10, 0);
+  VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
   uint8_t* o = out;
   uint64_t dev_off = 0;
   memcpy(o, framing[0].data(), framing[0].size());
@@ -998,77 +993,12 @@ extern "C" int vgx_layer_load(vgx_ctx* c, uint32_t id, const uint8_t* bytes, uin
   if (n_blocks) *n_blocks = 0;
   CollLayout L;
   std::string err;
-  if (!parse_layer_stream(bytes, n, &L, &err)) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_layer_load: " + err);
+  if (!parse_stream(bytes, n, true, &L, &err)) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_layer_load: " + err);
   if (c->find(id)) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_layer_load: submap " + std::to_string(id) + " already exists");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  const CollSubmapRef& s = L.submaps[0];
-  const int vpb = (int)(L.vps * L.vps * L.vps);
-  auto drop = [&](int rc) {   // no submap is left behind
-    const std::string msg = c->error;
-    if (c->find(id)) vgx_submap_free(c, id);
-    c->set_error(msg);
-    return rc;
-  };
-  const size_t table_bytes = (L.blocks.size() * sizeof(CollBlockRef) + 15) & ~(size_t)15;
-  const size_t bytes_off = table_bytes + 16;   // [regions | error word | stream bytes]
-  int rc = c->ensure_scratch(bytes_off + (size_t)n);
-  if (rc != VGX_OK) return rc;
-  uint8_t* d = (uint8_t*)c->d_scratch;
-  CollBlockRef* d_regions = (CollBlockRef*)d;
-  int* d_err = (int*)(d + table_bytes);
-  {
-    VgxLaunchScope copies(c, 10, 0);
-    if (!L.blocks.empty())
-      VGX_CUDA(c, cudaMemcpyAsync(d_regions, L.blocks.data(), L.blocks.size() * sizeof(CollBlockRef),
-                                  cudaMemcpyHostToDevice, c->stream));
-    VGX_CUDA(c, cudaMemsetAsync(d_err, 0, sizeof(int), c->stream));
-    rc = copy_h2d_chunked(c, d + bytes_off, bytes, n);
-    if (rc != VGX_OK) return rc;
-  }
-  VgxSubmap* sm = nullptr;
-  rc = vgx_submap_alloc(c, id, (float)L.voxel_size, (int)L.vps, (int)s.n_blocks, true, &sm);
-  if (rc != VGX_OK) return drop(rc);
-  sm->n_blocks = (int)s.n_blocks;
-  sm->finished = true;
-  if (s.n_blocks > 0) {
-    {
-      VgxLaunchScope copies(c, 10, 0);
-      const cudaError_t e = cudaMemcpyAsync(sm->d_block_idx, L.block_idx.data(), sizeof(int32_t) * 3 * s.n_blocks,
-                                            cudaMemcpyHostToDevice, c->stream);
-      if (e != cudaSuccess) {
-        c->set_error(std::string("vgx_layer_load: ") + cudaGetErrorString(e));
-        return drop(VGX_ERR_CUDA);
-      }
-    }
-    {
-      VgxLaunchScope scope(c, 9);
-      collection_decode_kernel<<<s.n_blocks, COLL_THREADS, 0, c->stream>>>(d + bytes_off, d_regions, vpb,
-                                                                           reinterpret_cast<float*>(sm->d_dw), d_err);
-    }
-    int h_err = 0;
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&h_err, d_err, sizeof(int), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    if (e != cudaSuccess) {
-      c->set_error(std::string("vgx_layer_load: ") + cudaGetErrorString(e));
-      return drop(VGX_ERR_CUDA);
-    }
-    if (h_err) {
-      c->set_error(std::string("vgx_layer_load: voxel_data: ") +
-                   ((h_err & COLL_ERR_TAG) ? "unexpected tag; " : "") +
-                   ((h_err & COLL_ERR_VARINT) ? "varint longer than 5 bytes, above 32 bits or truncated; " : "") +
-                   ((h_err & COLL_ERR_COUNT) ? "not 3 vps^3 values; " : "") +
-                   ((h_err & COLL_ERR_LENGTH) ? "packed length does not match the block; " : ""));
-      return drop(VGX_ERR_INVALID);
-    }
-  }
-  {
-    // the upload path's hash build, view and block-index rules; a repeated block index is refused there
-    // (voxblox BlockMergingStrategy::kProhibit) and the submap dropped
-    VgxLaunchScope scope(c, 11, 0);
-    rc = vgx_submap_upload_finish(c, sm, "vgx_layer_load");
-  }
-  if (rc != VGX_OK) return drop(rc);
-  if (n_blocks) *n_blocks = (int)s.n_blocks;
-  return VGX_OK;
+  // the layer is the single submap entry; a repeated block index is refused by the upload path
+  // (voxblox BlockMergingStrategy::kProhibit)
+  L.submaps[0].id = id;
+  const int rc = load_layout(c, "vgx_layer_load", L, bytes, n);
+  if (rc == VGX_OK && n_blocks) *n_blocks = (int)L.submaps[0].n_blocks;
+  return rc;
 }

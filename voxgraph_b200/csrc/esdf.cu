@@ -133,8 +133,7 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
   P.max_distance = dc.max_distance_m; P.default_distance = dc.default_distance_m;
   P.min_distance = dc.min_distance_m; P.min_weight = dc.min_weight;
   P.vps = s->vps;
-  P.sh = 0;
-  while ((1 << P.sh) < s->vps) P.sh++;
+  P.sh = s->sh;
   P.n_blocks = s->n_blocks;
   cudaStream_t st = c->stream;
   VGX_CUDA(c, cudaMalloc((void**)&s->d_esdf, sizeof(float2) * nvox));

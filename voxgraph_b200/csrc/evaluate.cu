@@ -22,9 +22,8 @@
 #include <string>
 #include <vector>
 
-#include "vgx_internal.h"
+#include "layer_access.cuh"
 
-#define VGX_EVAL_SLOT 14   // vgx_profile_get: map evaluation kernels
 #define RMSE_THREADS 256
 
 struct RmsePartial {
@@ -171,12 +170,12 @@ extern "C" int vgx_evaluate_layers_rmse(vgx_ctx* c, uint32_t gt_id, int gt_layer
     cudaStream_t st = c->stream;
     const int threads = std::min(RMSE_THREADS, g->vox_per_block);
     {
-      VgxLaunchScope scope(c, VGX_EVAL_SLOT);
+      VgxLaunchScope scope(c, VGX_SLOT_EVAL);
       rmse_block_kernel<<<(unsigned)n_part, threads, 0, st>>>(G, T, g->vox_per_block, d_part);
     }
     VGX_CUDA(c, cudaGetLastError());
     {
-      VgxLaunchScope scope(c, VGX_EVAL_SLOT);
+      VgxLaunchScope scope(c, VGX_SLOT_EVAL);
       rmse_total_kernel<<<1, RMSE_THREADS, 0, st>>>(d_part, (int)n_part, d_part + n_part);
     }
     VGX_CUDA(c, cudaGetLastError());
@@ -206,19 +205,6 @@ static void eval_exp_xyzyaw(const double pose[4], float T[7]) {
   T[4] = (float)pose[0];
   T[5] = (float)pose[1];
   T[6] = (float)pose[2];
-}
-
-// minkindr QuatTransformation::inverse, float (as proj_T_inverse)
-static void eval_T_inverse(const float T[7], float o[7]) {
-  const float q[4] = {T[0], -T[1], -T[2], -T[3]};
-  const float* v = T + 4;
-  const float w = q[0], x = q[1], y = q[2], z = q[3];
-  float uv0 = y * v[2] - z * v[1], uv1 = z * v[0] - x * v[2], uv2 = x * v[1] - y * v[0];
-  uv0 += uv0; uv1 += uv1; uv2 += uv2;
-  const float c0 = y * uv2 - z * uv1, c1 = z * uv0 - x * uv2, c2 = x * uv1 - y * uv0;
-  const float r[3] = {(v[0] + w * uv0) + c0, (v[1] + w * uv1) + c1, (v[2] + w * uv2) + c2};
-  o[0] = q[0]; o[1] = q[1]; o[2] = q[2]; o[3] = q[3];
-  o[4] = -r[0]; o[5] = -r[1]; o[6] = -r[2];
 }
 
 // the projected map: view, ESDF (defaults), relevant voxels with the reference's registration filter
@@ -277,13 +263,11 @@ static int eval_align(vgx_ctx* c, uint32_t projected, uint32_t gt, double pose[4
       rc = VGX_OK;
     }
   }
-  const std::string msg = c->error;
   vgx_graph_free(c);
   c->graph = saved;
   c->nranks = saved_nranks;
   c->rank = saved_rank;
   vgx_graph_invalidate_registration(c);
-  c->set_error(msg);
   return rc;
 }
 
@@ -307,26 +291,21 @@ extern "C" int vgx_map_evaluate(vgx_ctx* c, uint32_t gt_id, int n, const uint32_
   const uint32_t pid = vgx_scratch_id(c);
   int rc = vgx_project_map(c, n, ids, T_M_S, pid, nullptr);
   if (rc != VGX_OK) return rc;
-  auto drop = [&](int code) {
-    const std::string msg = c->error;
-    if (c->find(pid)) vgx_submap_free(c, pid);
-    c->set_error(msg);
-    return code;
-  };
   // 2.-3. finish both
   rc = eval_finish_projected(c, pid);
   if (rc == VGX_OK) rc = eval_finish_gt(c, gt_id);
-  if (rc != VGX_OK) return drop(rc);
   // 4. align the ground truth (reading, free) to the projected map (reference, constant)
-  rc = eval_align(c, pid, gt_id, out->aligned_pose, &out->summary);
-  if (rc != VGX_OK) return drop(rc);
+  if (rc == VGX_OK) rc = eval_align(c, pid, gt_id, out->aligned_pose, &out->summary);
   // 5. move the ground truth into the map's frame and finish it again
-  eval_exp_xyzyaw(out->aligned_pose, out->T_projected_map__ground_truth);
-  eval_T_inverse(out->T_projected_map__ground_truth, out->T_ground_truth__reading);
-  rc = vgx_submap_transform(c, gt_id, out->T_projected_map__ground_truth);
+  if (rc == VGX_OK) {
+    eval_exp_xyzyaw(out->aligned_pose, out->T_projected_map__ground_truth);
+    ov_inverse(out->T_projected_map__ground_truth, out->T_ground_truth__reading);
+    rc = vgx_submap_transform(c, gt_id, out->T_projected_map__ground_truth);
+  }
   if (rc == VGX_OK) rc = eval_finish_gt(c, gt_id);
   // 6. RMSE of the projected map's ESDF against the ground truth's
   if (rc == VGX_OK) rc = vgx_evaluate_layers_rmse(c, gt_id, VGX_LAYER_ESDF, pid, VGX_LAYER_ESDF, &out->details);
   // 7.
-  return drop(rc);
+  vgx_submap_drop(c, pid);
+  return rc;
 }

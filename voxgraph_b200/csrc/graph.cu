@@ -622,17 +622,17 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
     // refresh the longest-first tile order from the cost measured by the previous evaluation: before
     // the second evaluation on new tables, then every 32nd (the poses move little inside a solve)
     if (g->n_tiles > 1 && (g->evals_since_order == -2 || g->evals_since_order >= 32)) {
-      VgxLaunchScope s(c, 5);
+      VgxLaunchScope s(c, VGX_SLOT_OTHER);
       vgx_launch_reg_order(st, g->d_tile_cost, g->n_tiles, g->d_tile_order);
       g->evals_since_order = 0;
     }
     if (g->evals_since_order >= 0) ++g->evals_since_order;
     {
-      VgxLaunchScope s(c, 6);
+      VgxLaunchScope s(c, VGX_SLOT_REG_POSE_SETUP);
       vgx_launch_reg_pose_setup(st, g->d_cons, d_x, g->d_poses, g->n_local, skip);
     }
     {
-      VgxLaunchScope s(c, 0);
+      VgxLaunchScope s(c, VGX_SLOT_REG_REDUCE);
       vgx_launch_reg_reduce(st, g->d_cons, g->d_poses, g->d_tiles, g->n_tiles, g->d_tile_order,
                             g->d_tile_cost, g->d_partials, g->grid_capacity, g->d_unit_bounds, jacobian, skip);
     }
@@ -653,7 +653,7 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
   if (do_reg) {
     RegSums sums;
     sums.partials = g->d_partials; sums.tile_begin = g->d_tile_begin; sums.cons = g->d_cons;
-    VgxLaunchScope s(c, 7);
+    VgxLaunchScope s(c, VGX_SLOT_REG_SUMS);
     L.cfg.gridDim = dim3((unsigned)((g->n_local + 3) / 4));
     cudaLaunchKernelEx(&L.cfg, reg_csum_kernel, sums, g->n_local, g->d_csum, skip);
   }
@@ -673,7 +673,7 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
     }
     const int grid = std::min(g->N + g->E + 1, resident);
     {
-      VgxLaunchScope s(c, 8);
+      VgxLaunchScope s(c, VGX_SLOT_ASSEMBLY);
       L.cfg.gridDim = dim3((unsigned)grid);
       cudaLaunchKernelEx(&L.cfg, assemble_exchange_kernel, (const double*)g->d_csum, (const VgxRelEdge*)g->d_rel, d_x,
                          (const int*)g->d_csr_begin, (const int4*)g->d_csr_items, push, g->N, g->E, g->n_local,
@@ -684,7 +684,7 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
     return VGX_OK;
   }
   {
-    VgxLaunchScope s(c, 8);
+    VgxLaunchScope s(c, VGX_SLOT_ASSEMBLY);
     L.cfg.gridDim = dim3((unsigned)(g->N + g->E + 1));
     cudaLaunchKernelEx(&L.cfg, assemble_kernel, (const double*)g->d_csum, (const VgxRelEdge*)g->d_rel, d_x, (const int*)g->d_csr_begin,
                        (const int4*)g->d_csr_items, push, g->N, g->E, g->n_local, g->n_rel_local, excl, skip);

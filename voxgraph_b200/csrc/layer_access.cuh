@@ -1,7 +1,7 @@
 // Device access to a resident block layer shared by the kernels that sweep marching cubes over it
 // (extract.cu: isosurface vertices, mesh.cu: submap meshes), the trilinear interpolator shared by
-// extract.cu and project.cu, and the minkindr float transform shared by overlap.cu, mesh.cu and
-// project.cu.  Compiled with -fmad=false by every includer.
+// extract.cu and project.cu, and the minkindr float transform and its inverse shared by overlap.cu,
+// mesh.cu, project.cu and evaluate.cu.  Compiled with -fmad=false by every includer.
 #pragma once
 
 #include "vgx_internal.h"
@@ -22,8 +22,7 @@ static inline LayerDev layer_of(const VgxSubmap* s) {
   L.voxel_size = s->voxel_size; L.voxel_size_inv = s->voxel_size_inv;
   L.block_size = s->block_size; L.block_size_inv = s->block_size_inv;
   L.vps = s->vps;
-  L.sh = 0;
-  while ((1 << L.sh) < s->vps) L.sh++;
+  L.sh = s->sh;
   L.n_blocks = s->n_blocks;
   return L;
 }
@@ -159,4 +158,12 @@ __host__ __device__ inline void ov_transform(const float T[7], const float p[3],
   float r[3];
   ov_rotate(T, p, r);
   o[0] = r[0] + T[4]; o[1] = r[1] + T[5]; o[2] = r[2] + T[6];
+}
+// minkindr QuatTransformation::inverse, float (oracle vgo_T_inverse)
+__host__ __device__ inline void ov_inverse(const float T[7], float o[7]) {
+  const float qi[4] = {T[0], -T[1], -T[2], -T[3]};
+  float r[3];
+  ov_rotate(qi, T + 4, r);
+  o[0] = qi[0]; o[1] = qi[1]; o[2] = qi[2]; o[3] = qi[3];
+  o[4] = -r[0]; o[5] = -r[1]; o[6] = -r[2];
 }

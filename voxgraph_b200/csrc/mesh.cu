@@ -34,7 +34,6 @@
 #include "layer_access.cuh"
 
 #define VGX_MESH_BATCH_VOXELS ((size_t)1 << 27)   // 16 B of scratch per voxel: 2 GiB per batch
-#define VGX_MESH_SLOT 12                          // vgx_profile_get: mesh kernels
 
 static __constant__ uint8_t c_mesh_ntri[256];
 static __constant__ uint8_t c_mesh_tri[256][15];   // up to 5 triangles of 3 cube edges
@@ -411,7 +410,6 @@ static int grow_keep(vgx_ctx* c, void** p, size_t* cap, size_t need, size_t used
   return VGX_OK;
 }
 
-static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 extern "C" void vgx_mesh_config_default(vgx_mesh_config* cfg) {
   if (!cfg) return;
@@ -441,27 +439,27 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
   VGX_CUDA(c, cudaMemsetAsync(d_flag, 0, n_vox * sizeof(unsigned), st));
   const unsigned g128 = (unsigned)((n_vox + 127) / 128), g256 = (unsigned)((n_vox + 255) / 256);
   {
-    VgxLaunchScope scope(c, VGX_MESH_SLOT);
+    VgxLaunchScope scope(c, VGX_SLOT_MESH);
     mesh_count_kernel<<<g128, 128, 0, st>>>(d_jobs, nj, n_vox, min_weight, d_cnt, d_flag);
   }
   {
-    VgxLaunchScope scope(c, VGX_MESH_SLOT, 0);
+    VgxLaunchScope scope(c, VGX_SLOT_MESH, 0);
     rc = vgx_exclusive_scan_u32(c, d_cnt, d_toff, n_vox, d_tmp);
-    c->prof[VGX_MESH_SLOT].launches += 3;
+    c->prof[VGX_SLOT_MESH].launches += 3;
   }
   if (rc != VGX_OK) return rc;
   {
-    VgxLaunchScope scope(c, VGX_MESH_SLOT);
+    VgxLaunchScope scope(c, VGX_SLOT_MESH);
     mesh_popc_kernel<<<g256, 256, 0, st>>>(d_flag, n_vox, d_cnt);
   }
   {
-    VgxLaunchScope scope(c, VGX_MESH_SLOT, 0);
+    VgxLaunchScope scope(c, VGX_SLOT_MESH, 0);
     rc = vgx_exclusive_scan_u32(c, d_cnt, d_voff, n_vox, d_tmp);
-    c->prof[VGX_MESH_SLOT].launches += 3;
+    c->prof[VGX_SLOT_MESH].launches += 3;
   }
   if (rc != VGX_OK) return rc;
   {
-    VgxLaunchScope scope(c, VGX_MESH_SLOT);
+    VgxLaunchScope scope(c, VGX_SLOT_MESH);
     mesh_offsets_kernel<<<(nj + 1 + 127) / 128, 128, 0, st>>>(d_jobs, nj, n_vox, d_toff, d_voff, d_offs);
   }
   VGX_CUDA(c, cudaGetLastError());
@@ -483,11 +481,11 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
                  3 * sizeof(uint32_t) * tbase);
   if (rc != VGX_OK) return rc;
   {
-    VgxLaunchScope scope(c, VGX_MESH_SLOT);
+    VgxLaunchScope scope(c, VGX_SLOT_MESH);
     mesh_vertex_kernel<<<g128, 128, 0, st>>>(d_jobs, nj, n_vox, d_flag, d_voff, vbase, c->d_mesh_xyz);
   }
   {
-    VgxLaunchScope scope(c, VGX_MESH_SLOT);
+    VgxLaunchScope scope(c, VGX_SLOT_MESH);
     mesh_triangle_kernel<<<g128, 128, 0, st>>>(d_jobs, nj, n_vox, min_weight, d_toff, d_flag, d_voff, vbase,
                                                tbase, c->d_mesh_tri);
   }
@@ -619,7 +617,7 @@ extern "C" int vgx_mesh_ply(vgx_ctx* c, const uint8_t* rgba, uint8_t* out, uint6
   VGX_CUDA(c, cudaMemcpyAsync(d_col, col.data(), col.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
   const int64_t recs = c->mesh_nv + c->mesh_nt;
   {
-    VgxLaunchScope scope(c, VGX_MESH_SLOT);
+    VgxLaunchScope scope(c, VGX_SLOT_MESH);
     mesh_ply_kernel<<<(unsigned)((recs + 255) / 256), 256, 0, c->stream>>>(c->d_mesh_xyz, c->d_mesh_tri, c->mesh_nv,
                                                                           c->mesh_nt, d_voff, ns, d_col, d_body);
   }

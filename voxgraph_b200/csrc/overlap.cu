@@ -15,13 +15,6 @@
 
 namespace {
 
-inline void ov_inverse(const float T[7], float o[7]) {
-  const float qi[4] = {T[0], -T[1], -T[2], -T[3]};
-  float r[3];
-  ov_rotate(qi, T + 4, r);
-  o[0] = qi[0]; o[1] = qi[1]; o[2] = qi[2]; o[3] = qi[3];
-  o[4] = -r[0]; o[5] = -r[1]; o[6] = -r[2];
-}
 inline void ov_compose(const float A[7], const float B[7], float o[7]) {
   const float aw = A[0], ax = A[1], ay = A[2], az = A[3];
   const float bw = B[0], bx = B[1], by = B[2], bz = B[3];

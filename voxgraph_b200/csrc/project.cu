@@ -45,8 +45,6 @@
 
 #include "layer_access.cuh"
 
-#define VGX_PROJECT_SLOT 13   // vgx_profile_get: projection kernels
-#define VGX_EVAL_SLOT 14      // vgx_profile_get: map evaluation kernels (vgx_submap_transform's fold)
 // 63 bits set: a packed key never reaches it (each 21-bit field is at most 2^21 - 2), so it sorts last
 #define PROJ_NO_KEY 0x7FFFFFFFFFFFFFFFull
 #define PROJ_KEY_BITS 63
@@ -288,17 +286,6 @@ transform_fold_kernel(const ProjSrc* __restrict__ src, const uint64_t* __restric
 }
 
 // ------------------------------------------------------------------ host
-static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
-// minkindr QuatTransformation::inverse, float (oracle vgo_T_inverse)
-static void proj_T_inverse(const float T[7], float o[7]) {
-  const float qi[4] = {T[0], -T[1], -T[2], -T[3]};
-  float r[3];
-  ov_rotate(qi, T + 4, r);
-  o[0] = qi[0]; o[1] = qi[1]; o[2] = qi[2]; o[3] = qi[3];
-  o[4] = -r[0]; o[5] = -r[1]; o[6] = -r[2];
-}
-
 static int launch_fold(vgx_ctx* c, int vps, unsigned n_keys, const ProjSrc* d_src, const uint64_t* ukey,
                        const uint32_t* urank, const uint32_t* useg, const unsigned* slot, VgxSubmap* s) {
   cudaStream_t st = c->stream;
@@ -331,7 +318,7 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
     memset(&h[r], 0, sizeof(ProjSrc));
     h[r].L = layer_of(subs[r]);
     memcpy(h[r].T, poses[r], 7 * sizeof(float));
-    proj_T_inverse(h[r].T, h[r].T_inv);
+    ov_inverse(h[r].T, h[r].T_inv);
     h[r].first_block = (int)n_in;
     n_in += (size_t)subs[r]->n_blocks;
   }
@@ -372,32 +359,32 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
     VGX_CUDA(c, cudaMemcpyAsync(d_src, h.data(), sizeof(ProjSrc) * (size_t)ns, cudaMemcpyHostToDevice, st));
     VGX_CUDA(c, cudaMemsetAsync(d_ctl, 0, sizeof(int), st));
     {
-      VgxLaunchScope scope(c, VGX_PROJECT_SLOT);
+      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
       project_candidate_kernel<<<(unsigned)((n_in + 127) / 128), 128, 0, st>>>(d_src, ns, (int)n_in, transform,
                                                                             keys_a, ranks_a, d_ctl);
     }
     VGX_CUDA(c, cudaGetLastError());
     {
-      VgxLaunchScope scope(c, VGX_PROJECT_SLOT);
+      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
       VGX_CUDA(c, cub::DeviceRadixSort::SortPairs(d_sort_tmp, sort_tmp, (unsigned long long*)keys_a,
                                                   (unsigned long long*)keys_b, ranks_a, ranks_b, (int)P, 0,
                                                   PROJ_KEY_BITS, st));
     }
     const unsigned gp = (unsigned)((P + 255) / 256);
     {
-      VgxLaunchScope scope(c, VGX_PROJECT_SLOT);
+      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
       project_flag_kernel<<<gp, 256, 0, st>>>(keys_b, ranks_b, P, pair_head, key_head);
     }
     VGX_CUDA(c, cudaGetLastError());
     {
-      VgxLaunchScope scope(c, VGX_PROJECT_SLOT, 0);
+      VgxLaunchScope scope(c, VGX_SLOT_PROJECT, 0);
       rc = vgx_exclusive_scan_u32(c, pair_head, pair_pos, P, scan_tmp);
       if (rc == VGX_OK) rc = vgx_exclusive_scan_u32(c, key_head, key_pos, P, scan_tmp);
-      c->prof[VGX_PROJECT_SLOT].launches += 6;
+      c->prof[VGX_SLOT_PROJECT].launches += 6;
     }
     if (rc != VGX_OK) return rc;
     {
-      VgxLaunchScope scope(c, VGX_PROJECT_SLOT);
+      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
       project_scatter_kernel<<<gp, 256, 0, st>>>(keys_b, ranks_b, P, pair_head, key_head, pair_pos, key_pos, keys_a,
                                                  ranks_a, useg);
     }
@@ -416,15 +403,15 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
   unsigned* slot = pair_pos;
   if (n_keys > 0) {
     {
-      VgxLaunchScope scope(c, VGX_PROJECT_SLOT);
+      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
       project_occupancy_kernel<<<n_keys, std::min(PROJ_THREADS, g0.vox_per_block), 0, st>>>(d_src, keys_a, ranks_a,
                                                                                             useg, transform, keep);
     }
     VGX_CUDA(c, cudaGetLastError());
     {
-      VgxLaunchScope scope(c, VGX_PROJECT_SLOT, 0);
+      VgxLaunchScope scope(c, VGX_SLOT_PROJECT, 0);
       rc = vgx_exclusive_scan_u32(c, keep, slot, n_keys, scan_tmp);
-      c->prof[VGX_PROJECT_SLOT].launches += 3;
+      c->prof[VGX_SLOT_PROJECT].launches += 3;
     }
     if (rc != VGX_OK) return rc;
     VGX_CUDA(c, cudaMemcpyAsync(&n_out, slot + n_keys, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
@@ -437,14 +424,14 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
   s->finished = true;
   if (n_out > 0 && transform) {
     {
-      VgxLaunchScope scope(c, VGX_EVAL_SLOT);
+      VgxLaunchScope scope(c, VGX_SLOT_EVAL);
       transform_fold_kernel<<<n_keys, std::min(PROJ_THREADS, g0.vox_per_block), 0, st>>>(d_src, keys_a, slot, s->d_dw,
                                                                                         s->d_block_idx);
     }
     VGX_CUDA(c, cudaGetLastError());
   } else if (n_out > 0) {
     {
-      VgxLaunchScope scope(c, VGX_PROJECT_SLOT);
+      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
       rc = launch_fold(c, g0.vps, n_keys, d_src, keys_a, ranks_a, useg, slot, s);
     }
     if (rc != VGX_OK) return rc;
@@ -485,11 +472,7 @@ extern "C" int vgx_project_map(vgx_ctx* c, int n, const uint32_t* ids, const flo
   int nb = 0;
   const int rc = project(c, subs, poses, out_id, &nb);
   if (rc != VGX_OK) {
-    if (c->find(out_id)) {   // a failure after the allocation: drop the half-built submap, keep the message
-      const std::string msg = c->error;
-      vgx_submap_free(c, out_id);
-      c->set_error(msg);
-    }
+    vgx_submap_drop(c, out_id);   // a failure after the allocation leaves a half-built submap
     return rc;
   }
   if (n_blocks) *n_blocks = nb;
@@ -508,11 +491,7 @@ extern "C" int vgx_submap_transform(vgx_ctx* c, uint32_t id, const float* T_new_
   int nb = 0;
   const int rc = project(c, {s}, {T_new_old}, tmp, &nb, true);
   if (rc != VGX_OK) {
-    if (c->find(tmp)) {
-      const std::string msg = c->error;
-      vgx_submap_free(c, tmp);
-      c->set_error(msg);
-    }
+    vgx_submap_drop(c, tmp);
     return rc;
   }
   return vgx_submap_move(c, tmp, id);

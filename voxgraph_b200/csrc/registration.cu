@@ -578,8 +578,7 @@ int vgx_fill_constraint(vgx_ctx* c, uint32_t ref_id, uint32_t read_id, const vgx
   C.grid16 = rd->d_grid16;
   C.gmin0 = rd->grid_min[0]; C.gmin1 = rd->grid_min[1]; C.gmin2 = rd->grid_min[2];
   C.gd0 = rd->grid_dim[0]; C.gd1 = rd->grid_dim[1]; C.gd2 = rd->grid_dim[2];
-  C.vps_shift = 0;
-  while ((1 << C.vps_shift) < rd->vps) C.vps_shift++;
+  C.vps_shift = rd->sh;
   // cpp:274 factor = num_residuals / summed_reference_weight; sampled points all weigh 1
   if (is_sampled) C.factor = (C.n > 0 && p.n > 0) ? 1.0 : 0.0;
   else C.factor = (p.sum_w != 0.0) ? (double)p.n / p.sum_w : 0.0;
@@ -646,7 +645,7 @@ extern "C" int vgx_reg_eval_emit(vgx_ctx* c, uint32_t ref_id, uint32_t read_id,
   double* d_jr = jac_ref ? d_r + Kp : nullptr;
   double* d_je = jac_read ? d_r + 5 * Kp : nullptr;
   {
-    VgxLaunchScope scope(c, 1);
+    VgxLaunchScope scope(c, VGX_SLOT_REG_EMIT);
     reg_emit_kernel<<<(unsigned)((K + 255) / 256), 256, 0, c->stream>>>(C, P, d_r, d_jr, d_je);
   }
   VGX_CUDA(c, cudaGetLastError());

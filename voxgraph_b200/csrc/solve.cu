@@ -792,7 +792,7 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
   VGX_CUDA(c, cudaMemsetAsync(g->d_A, 0, sizeof(double) * M * M, st));
   VGX_CUDA(c, cudaMemcpyAsync(g->d_state, init, sizeof(*init), cudaMemcpyHostToDevice, st));
   {
-    VgxLaunchScope s(c, 4, 3);
+    VgxLaunchScope s(c, VGX_SLOT_SOLVE, 3);
     enqueue_lm_build(st, g, n, lo);
     VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->d_A, n, g->d_state, g->d_diag, VGX_COV_RANK_TOL));
   }
@@ -803,7 +803,7 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
     VGX_CUDA(c, cudaFuncSetAttribute(cov_column_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)(sizeof(double) * (size_t)n)));
   {
-    VgxLaunchScope s(c, 4);
+    VgxLaunchScope s(c, VGX_SLOT_SOLVE);
     cov_column_kernel<<<(unsigned)ncols, 256, sizeof(double) * (size_t)n, st>>>(g->d_A, n, d_cols, d_X);
   }
   VGX_CUDA(c, cudaGetLastError());
@@ -898,7 +898,7 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
   rc = eval_enqueue(c, g, g->d_x, g->d_packed[0], true, excl);
   if (rc != VGX_OK) return rc;
   {
-    VgxLaunchScope s(c, 4);
+    VgxLaunchScope s(c, VGX_SLOT_SOLVE);
     lm_init_kernel<<<1, 256, 0, st>>>(g->d_packed[0], g->d_red_offset, N, g->d_state,
                                       o->initial_trust_region_radius, lo);
   }
@@ -915,7 +915,7 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
   const int* skip = &g->d_state->done;
   auto enqueue_iteration = [&](int k) -> int {
     {
-      VgxLaunchScope s(c, 4, 4);
+      VgxLaunchScope s(c, VGX_SLOT_SOLVE, 4);
       if (!use_smem_chol)   // the shared-memory solver reads the written blocks only
         VGX_CUDA(c, cudaMemsetAsync(g->d_A, 0, sizeof(double) * (size_t)(n + 1) * (n + 1), st));
       enqueue_lm_build(st, g, n, lo);
@@ -935,7 +935,7 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
     int rc2 = eval_enqueue(c, g, g->d_xc, g->d_packed[1], true, excl, skip);
     if (rc2 != VGX_OK) return rc2;
     {
-      VgxLaunchScope s(c, 4, 2);
+      VgxLaunchScope s(c, VGX_SLOT_SOLVE, 2);
       lm_decide_kernel<<<1, 256, 0, st>>>(g->d_packed[0], g->d_packed[1], g->d_red_offset, N, g->d_x,
                                           g->d_xc, g->d_state, lo, 1, g->d_snap + (k & 1));
       lm_accept_kernel<<<std::max(1, std::min(64, (int)(g->packed_len / 2048))), 256, 0, st>>>(

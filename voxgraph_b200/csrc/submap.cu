@@ -186,8 +186,7 @@ static int check_uploaded_blocks(vgx_ctx* c, VgxSubmap* s, const char* what) {
   VGX_CUDA(c, cudaMemcpyAsync(&bad, s->d_counters + 2, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   if (!bad) return VGX_OK;
-  c->submaps.erase(s->id);
-  free_submap(s);
+  vgx_submap_drop(c, s->id);
   c->set_error(std::string(what) + ((bad & 2) ? ": block index outside the accepted range"
                                               : ": repeated block index"));
   return VGX_ERR_INVALID;
@@ -293,10 +292,8 @@ int vgx_submap_build_grid(vgx_ctx* c, VgxSubmap* s) {
 int vgx_submap_build_view(vgx_ctx* c, VgxSubmap* s, const float2* bricks, float* view) {
   const size_t used = (size_t)s->n_blocks * s->vox_per_block;
   if (used == 0) return VGX_OK;
-  int sh = 0;
-  while ((1 << sh) < s->vps) sh++;
   build_view_kernel<<<(unsigned)((used + 255) / 256), 256, 0, c->stream>>>(bricks, s->d_block_idx, s->hash, view,
-                                                                          s->n_blocks, s->vps, sh);
+                                                                          s->n_blocks, s->vps, s->sh);
   c->launches++;
   VGX_CUDA(c, cudaGetLastError());
   return VGX_OK;
@@ -341,6 +338,8 @@ int vgx_submap_alloc(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int cap
   s->block_size = voxel_size * (float)vps;
   s->block_size_inv = (float)(1.0 / (double)s->block_size);
   s->vps = vps;
+  s->sh = 0;
+  while ((1 << s->sh) < vps) s->sh++;
   s->vox_per_block = vps * vps * vps;
   s->cap_blocks = cap > 0 ? cap : 1;
   const uint32_t tsize = table_size_for(s->cap_blocks);
@@ -386,22 +385,10 @@ extern "C" int vgx_submap_upload(vgx_ctx* c, uint32_t id, float voxel_size, int 
   VGX_CUDA(c, cudaMemcpyAsync(tmp_w, weight, nvox * sizeof(float), cudaMemcpyHostToDevice, c->stream));
   VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx, block_idx, sizeof(int32_t) * 3 * n_blocks,
                               cudaMemcpyHostToDevice, c->stream));
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_counters, &s->n_blocks, sizeof(int), cudaMemcpyHostToDevice,
-                              c->stream));
-  hash_insert_kernel<<<(n_blocks + 127) / 128, 128, 0, c->stream>>>(s->hash, s->d_block_idx, n_blocks,
-                                                                    s->d_counters + 2);
   interleave_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(tmp_d, tmp_w, s->d_dw, nvox);
-  {
-    int sh = 0;
-    while ((1 << sh) < vps) sh++;
-    build_view_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(
-        s->d_dw, s->d_block_idx, s->hash, s->d_view, n_blocks, vps, sh);
-  }
-  c->launches += 3;
-  VGX_CUDA(c, cudaGetLastError());
-  rc = check_uploaded_blocks(c, s, "vgx_submap_upload");  // synchronises: host buffers are the caller's
-  if (rc != VGX_OK) return rc;
-  return vgx_submap_build_grid(c, s);
+  c->launches++;
+  // synchronises: the host buffers are the caller's
+  return vgx_submap_upload_finish(c, s, "vgx_submap_upload");
 }
 
 extern "C" int vgx_submap_peek_device(vgx_ctx* c, uint32_t id, const int32_t** d_block_idx,
@@ -470,14 +457,8 @@ extern "C" int vgx_submap_finish(vgx_ctx* c, uint32_t id) {
   // integration capacity (128 KiB per brick)
   const size_t used = (size_t)s->n_blocks * s->vox_per_block;
   if (!s->d_view) VGX_CUDA(c, cudaMalloc(&s->d_view, sizeof(float) * 8 * (used > 0 ? used : 1)));
-  if (used > 0) {
-    int sh = 0;
-    while ((1 << sh) < s->vps) sh++;
-    build_view_kernel<<<(unsigned)((used + 255) / 256), 256, 0, c->stream>>>(
-        s->d_dw, s->d_block_idx, s->hash, s->d_view, s->n_blocks, s->vps, sh);
-    c->launches++;
-    VGX_CUDA(c, cudaGetLastError());
-  }
+  const int rc = vgx_submap_build_view(c, s, s->d_dw, s->d_view);
+  if (rc != VGX_OK) return rc;
   s->finished = true;
   vgx_graph_invalidate_registration(c);
   return vgx_submap_build_grid(c, s);
@@ -493,6 +474,13 @@ extern "C" int vgx_submap_free(vgx_ctx* c, uint32_t id) {
   c->submaps.erase(id);
   vgx_graph_invalidate_registration(c);
   return VGX_OK;
+}
+
+void vgx_submap_drop(vgx_ctx* c, uint32_t id) {
+  if (!c->find(id)) return;
+  const std::string msg = c->error;
+  vgx_submap_free(c, id);
+  c->set_error(msg);
 }
 
 int vgx_submap_move(vgx_ctx* c, uint32_t from_id, uint32_t id) {

@@ -580,8 +580,7 @@ extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7],
   P.voxel_size = s->voxel_size;
   P.voxel_size_inv = s->voxel_size_inv;
   P.vps = s->vps;
-  P.vps_shift = 0;
-  while ((1 << P.vps_shift) < s->vps) P.vps_shift++;
+  P.vps_shift = s->sh;
   P.n = n;
   vgx_tsdf_stats st;
   memset(&st, 0, sizeof(st));
@@ -609,7 +608,7 @@ extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7],
   if (P.cfg.mode == 0) {
     // ---- ray-ordered path: allocate -> count -> scan -> emit -> stable sort by voxel -> apply
     {
-      VgxLaunchScope scope(c, 3);
+      VgxLaunchScope scope(c, VGX_SLOT_TSDF_ALLOCATE);
       tsdf_allocate_kernel<<<grid, 128, 0, stream>>>(P, d_pts, s->hash, s->d_block_idx, s->d_counters,
                                                     s->cap_blocks);
     }
@@ -622,7 +621,7 @@ extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7],
     unsigned* d_scan_tmp = (unsigned*)((char*)c->d_sort + 2 * cnt_bytes);
     unsigned total = 0;
     {
-      VgxLaunchScope scope(c, 2, 1);
+      VgxLaunchScope scope(c, VGX_SLOT_TSDF_INTEGRATE, 1);
       tsdf_count_kernel<<<grid, 128, 0, stream>>>(P, d_pts, d_counts);
       rc = vgx_exclusive_scan_u32(c, d_counts, d_offsets, (size_t)n, d_scan_tmp);   // hand-written, 3 launches
       if (rc != VGX_OK) return rc;
@@ -655,7 +654,7 @@ extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7],
       unsigned* d_heads = d_nlong + 64;
       void* d_sort_tmp = b2 + 2 * key_bytes + 2 * val_bytes + 256 + heads_bytes;
       {
-        VgxLaunchScope scope(c, 2, 4);
+        VgxLaunchScope scope(c, VGX_SLOT_TSDF_INTEGRATE, 4);
         VGX_CUDA(c, cudaMemsetAsync(d_nlong, 0, 256, stream));
         tsdf_emit_kernel<<<grid, 128, 0, stream>>>(P, d_pts, s->hash, d_offsets, sentinel, k_in, v_in, d_stats);
         cub::DeviceRadixSort::SortPairs(d_sort_tmp, sort_tmp, k_in, k_out, (unsigned long long*)v_in,
@@ -672,7 +671,7 @@ extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7],
     }
   } else {
     // ---- Fast scheduling: one kernel, blocks allocated on demand
-    VgxLaunchScope scope(c, 2);
+    VgxLaunchScope scope(c, VGX_SLOT_TSDF_INTEGRATE);
     tsdf_integrate_kernel<<<grid, 128, 0, stream>>>(P, d_pts, s->hash, s->d_block_idx, s->d_counters,
                                                    s->cap_blocks, s->d_dw, d_stats, d_start, d_obs);
   }

@@ -108,6 +108,7 @@ struct VgxSubmap {
   uint32_t id = 0;
   float voxel_size = 0, voxel_size_inv = 0, block_size = 0, block_size_inv = 0;
   int vps = 16, vox_per_block = 4096;
+  int sh = 4;                  // log2(vps)
   int cap_blocks = 0;
   int n_blocks = 0;            // host mirror (valid after upload / integrate sync)
   bool finished = false;
@@ -146,7 +147,25 @@ struct VgxRelEdge {
 
 struct VgxGraph;  // defined in graph.h
 
-#define VGX_PROFILE_SLOTS 15   // vgx_profile_get's `which`
+// vgx_profile_get's `which` (documented in voxgraph_b200.h); the values are part of the C-ABI
+enum VgxProfileSlotId {
+  VGX_SLOT_REG_REDUCE = 0,       // registration reduce kernel
+  VGX_SLOT_REG_EMIT = 1,         // registration emit kernel
+  VGX_SLOT_TSDF_INTEGRATE = 2,
+  VGX_SLOT_TSDF_ALLOCATE = 3,
+  VGX_SLOT_SOLVE = 4,            // Cholesky / LM kernels
+  VGX_SLOT_OTHER = 5,            // everything else
+  VGX_SLOT_REG_POSE_SETUP = 6,
+  VGX_SLOT_REG_SUMS = 7,         // per-constraint sums
+  VGX_SLOT_ASSEMBLY = 8,         // normal equations (+ the fused peer exchange)
+  VGX_SLOT_COLL_CODEC = 9,       // submap collection decode / encode kernels
+  VGX_SLOT_COLL_COPY = 10,       // submap collection stream copies (host <-> device)
+  VGX_SLOT_COLL_UPLOAD = 11,     // submap collection upload (block hash, registration view, grid)
+  VGX_SLOT_MESH = 12,
+  VGX_SLOT_PROJECT = 13,
+  VGX_SLOT_EVAL = 14,            // map evaluation kernels
+  VGX_PROFILE_SLOTS = 15
+};
 struct VgxProfileSlot {
   double total_ms = 0;
   int64_t launches = 0;
@@ -232,6 +251,8 @@ int vgx_submap_alloc(vgx_ctx* ctx, uint32_t submap_id, float voxel_size, int vps
 // hash, registration view, the upload rules (a bad block list drops the submap: VGX_ERR_INVALID) and
 // the dense grid.  Synchronises.
 int vgx_submap_upload_finish(vgx_ctx* ctx, VgxSubmap* s, const char* what);
+// frees submap_id if it exists and keeps the error message of the failure that leads to the drop
+void vgx_submap_drop(vgx_ctx* ctx, uint32_t submap_id);
 // moves the submap from_id to id (whose previous content is freed); from_id no longer exists.  Synchronises.
 int vgx_submap_move(vgx_ctx* ctx, uint32_t from_id, uint32_t id);
 // an id for a scratch submap: the first unused one counting down from 2^32 - 2 (2^32 - 1 is a valid cblox id)
@@ -241,6 +262,8 @@ int vgx_submap_build_view(vgx_ctx* ctx, VgxSubmap* s, const float2* bricks, floa
 // clears the block hash and re-inserts the first s->n_blocks blocks (after a capacity overflow
 // left keys without a brick behind)
 int vgx_submap_rebuild_hash(vgx_ctx* ctx, VgxSubmap* s);
+// sub-buffer size in a scratch layout (keeps every sub-buffer 256-byte aligned)
+static inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 // hand-written exclusive scan (extract.cu): out[0..n], out[n] = total; d_tmp: vgx_scan_tmp_count(n) words
 int vgx_exclusive_scan_u32(vgx_ctx* c, const unsigned* d_in, unsigned* d_out, size_t n, unsigned* d_tmp);
 size_t vgx_scan_tmp_count(size_t n);
