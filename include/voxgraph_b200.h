@@ -46,16 +46,27 @@ void* vgx_ctx_stream(vgx_ctx* ctx);
 int vgx_ctx_synchronize(vgx_ctx* ctx);
 
 /* Kernel accounting: when enabled the library brackets each of its kernels with
- * CUDA events on the context stream. which: 0 = registration reduce kernel,
- * 1 = registration emit kernel, 2 = TSDF integrate kernel, 3 = TSDF allocate kernel,
- * 4 = Cholesky/LM kernels, 5 = everything else, 6 = registration pose set-up, 7 = per-constraint sums,
- * 8 = assembly of the normal equations (+ the peer exchange when it is fused into it),
- * 9 = submap collection codec kernels (decode / encode), 10 = submap collection stream copies
- * (host <-> device), 11 = submap collection upload (block hash, registration view, grid),
- * 12 = mesh kernels (vgx_mesh_build's passes and scans, the PLY pack of vgx_mesh_ply),
- * 13 = projection kernels (vgx_project_map's passes, sort and scans; the upload of the result is not
- * included), 14 = map evaluation kernels (vgx_submap_transform's resampling kernel, the two
- * vgx_evaluate_layers_rmse kernels). */
+ * CUDA events on the context stream and adds them to one slot, vgx_profile_get's `which`. */
+enum VgxProfileSlotId {
+  VGX_SLOT_REG_REDUCE = 0,       /* registration reduce kernel */
+  VGX_SLOT_REG_EMIT = 1,         /* registration emit kernel */
+  VGX_SLOT_TSDF_INTEGRATE = 2,   /* TSDF integrate kernel */
+  VGX_SLOT_TSDF_ALLOCATE = 3,    /* TSDF allocate kernel */
+  VGX_SLOT_SOLVE = 4,            /* Cholesky / LM kernels */
+  VGX_SLOT_OTHER = 5,            /* everything else */
+  VGX_SLOT_REG_POSE_SETUP = 6,   /* registration pose set-up */
+  VGX_SLOT_REG_SUMS = 7,         /* per-constraint sums */
+  VGX_SLOT_ASSEMBLY = 8,         /* assembly of the normal equations (+ the peer exchange when it is fused into it) */
+  VGX_SLOT_COLL_CODEC = 9,       /* submap collection codec kernels (decode / encode) */
+  VGX_SLOT_COLL_COPY = 10,       /* submap collection stream copies (host <-> device) */
+  VGX_SLOT_COLL_UPLOAD = 11,     /* submap collection upload (block hash, registration view, grid) */
+  VGX_SLOT_MESH = 12,            /* mesh kernels (vgx_mesh_build's passes and scans, the PLY pack of vgx_mesh_ply) */
+  VGX_SLOT_PROJECT = 13,         /* projection kernels (vgx_project_map's passes, sort and scans; the upload of
+                                    the result is not included) */
+  VGX_SLOT_EVAL = 14,            /* map evaluation kernels (vgx_submap_transform's resampling kernel, the two
+                                    vgx_evaluate_layers_rmse kernels) */
+  VGX_PROFILE_SLOTS = 15
+};
 int vgx_profile_enable(vgx_ctx* ctx, int on);
 int vgx_profile_reset(vgx_ctx* ctx);
 int vgx_profile_get(vgx_ctx* ctx, int which, double* total_ms, int64_t* launches);

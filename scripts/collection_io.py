@@ -11,56 +11,23 @@ registration view, grid).  Host framing is timed on its own through vgx_collecti
 same parser as a load.  The card's name and power limit are read in the same run.  Needs a GPU.
 """
 import argparse
-import json
-import os
-import subprocess
-import sys
 import time
 
-import numpy as np
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-WORKLOADS = {"config2": dict(submaps=50, voxel_size=0.2, seed=2), "config4": dict(submaps=200, voxel_size=0.1, seed=4)}
-SLOT_KERNELS, SLOT_COPIES, SLOT_UPLOAD = 9, 10, 11
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             stdout=subprocess.PIPE, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clock = [s.strip() for s in out.split(",")]
-        return dict(name=name, power_limit=power, max_sm_clock=clock)
-    except Exception as e:   # the figures are still reported, without the card's description
-        return dict(error=str(e))
-
-
-def split(ctx):
-    return {name: ctx.profile_get(slot)[0] for name, slot in
-            (("codec_kernels_ms", SLOT_KERNELS), ("stream_copies_ms", SLOT_COPIES), ("upload_ms", SLOT_UPLOAD))}
+import _measure as M
 
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", default="config2", choices=sorted(WORKLOADS))
+    ap.add_argument("--workload", default="config2", choices=sorted(M.WORKLOADS))
     ap.add_argument("--submaps", type=int, default=None)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    from voxgraph_b200 import api, synth
-    w = dict(WORKLOADS[a.workload])
-    if a.submaps:
-        w["submaps"] = a.submaps
+    from voxgraph_b200 import _lib, api
+    w = M.WORKLOADS[a.workload]
     t0 = time.time()
-    sc = synth.make_scene(seed=w["seed"], n_submaps=w["submaps"], n_points=100, voxel_size=w["voxel_size"],
-                          trunc=0.6 if abs(w["voxel_size"] - 0.2) < 1e-9 else None, workers=os.cpu_count() or 1)
+    ctx, sc, ids, T = M.upload_scene(w, a.submaps)
     t_scene = time.time() - t0
-    ctx = api.Context(0)
-    for s in sc.submaps:
-        ctx.submap_upload(s.submap_id, s.voxel_size, s.vps, s.block_idx, s.distance, s.weight)
-    ids = [s.submap_id for s in sc.submaps]
-    T = np.array([synth.pose_to_T(p) for p in sc.poses_init], np.float32)
     n_blocks = sum(s.num_blocks for s in sc.submaps)
     n_vox = n_blocks * sc.submaps[0].vps ** 3
     observed = int(sum((s.weight > 1e-6).sum() for s in sc.submaps))
@@ -68,40 +35,35 @@ def main():
     data = ctx.collection_save(ids, T)   # warm-up: staging buffers, module load
     ctx2 = api.Context(0)
 
-    def load_once(profiled=False):
+    def save():
+        host, _, out = M.timed(ctx, lambda: ctx.collection_save(ids, T))
+        assert out == data
+        return host
+
+    def free_loaded():
         for i in ids:
             try:
                 ctx2.submap_free(i)
             except api.VgxError:
                 pass
-        ctx2.synchronize()
-        ctx2.profile_enable(profiled)
-        ctx2.profile_reset()
-        t = time.perf_counter()
-        ctx2.collection_load(data)
-        ctx2.synchronize()
-        dt = time.perf_counter() - t
-        ctx2.profile_enable(False)
-        return dt
 
-    def save_once(profiled=False):
-        ctx.synchronize()
-        ctx.profile_enable(profiled)
-        ctx.profile_reset()
-        t = time.perf_counter()
-        out = ctx.collection_save(ids, T)
-        dt = time.perf_counter() - t
-        ctx.profile_enable(False)
-        assert out == data
-        return dt
+    def load():
+        free_loaded()
+        return M.timed(ctx2, lambda: ctx2.collection_load(data))[0]
 
-    load_once()
-    save_t = [save_once() for _ in range(a.repeats)]
-    load_t = [load_once() for _ in range(a.repeats)]
-    save_once(True)
-    save_split = split(ctx)
-    load_once(True)
-    load_split = split(ctx2)
+    def split(c, fn):
+        """fn's codec kernel, stream copy and upload time from one profiled call."""
+        codec_ms, _, _ = M.profiled(c, _lib.VGX_SLOT_COLL_CODEC, fn)
+        return dict(codec_kernels_ms=round(codec_ms, 3),
+                    stream_copies_ms=round(c.profile_get(_lib.VGX_SLOT_COLL_COPY)[0], 3),
+                    upload_ms=round(c.profile_get(_lib.VGX_SLOT_COLL_UPLOAD)[0], 3))
+
+    load()
+    save_t = [save() for _ in range(a.repeats)]
+    load_t = [load() for _ in range(a.repeats)]
+    save_split = split(ctx, lambda: ctx.collection_save(ids, T))
+    free_loaded()
+    load_split = split(ctx2, lambda: ctx2.collection_load(data))
     scan_t = []
     for _ in range(a.repeats):
         t = time.perf_counter()
@@ -113,22 +75,15 @@ def main():
 
     def rates(ts):
         best = min(ts)
-        return dict(wall_ms=[round(1e3 * x, 3) for x in ts], best_ms=round(1e3 * best, 3),
-                    file_GBps=round(len(data) / best / 1e9, 3), voxels_per_s=float("%.4g" % (n_vox / best)))
+        return dict(wall_ms=[round(x, 3) for x in ts], best_ms=round(best, 3),
+                    file_GBps=round(len(data) / best / 1e6, 3), voxels_per_s=float("%.4g" % (n_vox / best * 1e3)))
 
-    res = dict(
+    M.emit(dict(
         workload=a.workload, submaps=len(ids), blocks=n_blocks, voxels=n_vox, observed_voxels=observed,
         voxel_size=w["voxel_size"], file_bytes=len(data), file_bytes_per_voxel=round(len(data) / n_vox, 3),
-        hbm_bytes_per_voxel=8, scene_build_s=round(t_scene, 1), gpu=gpu_info(),
-        save=dict(rates(save_t), profiled_split_ms={k: round(v, 3) for k, v in save_split.items()}),
-        load=dict(rates(load_t), host_framing_ms=round(1e3 * min(scan_t), 3),
-                  profiled_split_ms={k: round(v, 3) for k, v in load_split.items()}))
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "a") as f:
-            f.write(line + "\n")
+        hbm_bytes_per_voxel=8, scene_build_s=round(t_scene, 1), gpu=M.gpu_info(),
+        save=dict(rates(save_t), profiled_split_ms=save_split),
+        load=dict(rates(load_t), host_framing_ms=round(1e3 * min(scan_t), 3), profiled_split_ms=load_split)), a.out)
     ctx.close()
     ctx2.close()
 

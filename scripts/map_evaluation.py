@@ -12,33 +12,17 @@ alignment has a known answer.  The map is the submaps at their true poses.  Repo
   - the whole vgx_map_evaluate call by a host clock ending in a synchronise (best of --repeats, each from a
     fresh copy of the ground truth);
   - the aligned pose against the known offset, the RMSE before and after;
-  - the card's name and power limit, read in the same run.  Needs a GPU.
+  - the card's name, power limit and max SM clock, read in the same run.  Needs a GPU.
 """
 import argparse
-import json
-import os
-import subprocess
-import sys
-import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import _measure as M
 
 GT_ID = 0xFFFFFF00
 PROJ_ID = 0xFFFFFF01
 OFFSET = (0.1, -0.05, 0.03, 0.01)   # where the ground truth is moved to: the alignment should undo it
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                             stdout=subprocess.PIPE, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power = [s.strip() for s in out.split(",")]
-        return dict(name=name, power_limit=power)
-    except Exception as e:
-        return dict(error=str(e))
 
 
 def main():
@@ -48,14 +32,8 @@ def main():
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    import torch
     from voxgraph_b200 import api, synth
-    sc = synth.make_scene(seed=2, n_submaps=a.submaps, n_points=100, voxel_size=a.voxel_size,
-                          trunc=0.6 if abs(a.voxel_size - 0.2) < 1e-9 else None, workers=os.cpu_count() or 1)
-    ctx = api.Context(0)
-    for s in sc.submaps:
-        ctx.submap_upload(s.submap_id, s.voxel_size, s.vps, s.block_idx, s.distance, s.weight)
-    ids = [s.submap_id for s in sc.submaps]
+    ctx, sc, ids, _ = M.upload_scene(dict(submaps=a.submaps, voxel_size=a.voxel_size, seed=2))
     vps = sc.submaps[0].vps
     T = np.array([synth.pose_to_T(p) for p in sc.poses_gt], np.float32)
     # the ground truth: the whole area at the true poses, moved by the inverse of OFFSET (so that the alignment
@@ -68,17 +46,6 @@ def main():
     gt_layer = ctx.submap_download(GT_ID)
     gt_vs = ctx.submap_info(GT_ID)[0]
 
-    stream = torch.cuda.ExternalStream(ctx.stream_ptr)
-
-    def timed(fn):
-        ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
-        ctx.synchronize()
-        ev[0].record(stream)
-        out = fn()
-        ev[1].record(stream)
-        ctx.synchronize()
-        return ev[0].elapsed_time(ev[1]), out
-
     def fresh_gt():
         ctx.submap_upload(GT_ID, gt_vs, vps, *gt_layer)
 
@@ -86,7 +53,7 @@ def main():
     fresh_gt()
     filt = ctx.registration_filter(min_voxel_weight=1.0, max_voxel_distance=0.3, use_esdf_distance=1)
     stages = {}
-    stages["projection_ms"], _ = timed(lambda: ctx.project_map(ids, T, PROJ_ID))
+    _, stages["projection_ms"], _ = M.timed(ctx, lambda: ctx.project_map(ids, T, PROJ_ID))
 
     def finish_projected():
         ctx.submap_finish(PROJ_ID)
@@ -97,15 +64,15 @@ def main():
         ctx.submap_finish(GT_ID)
         ctx.submap_generate_esdf(GT_ID)
 
-    stages["finish_projected_ms"], _ = timed(finish_projected)
-    stages["finish_ground_truth_ms"], _ = timed(finish_gt)
+    _, stages["finish_projected_ms"], _ = M.timed(ctx, finish_projected)
+    _, stages["finish_ground_truth_ms"], _ = M.timed(ctx, finish_gt)
     before = ctx.evaluate_layers_rmse(GT_ID, PROJ_ID)
     ctx.graph_set_nodes([PROJ_ID, GT_ID], np.zeros((2, 4)), np.array([1, 0], np.uint8))
     ctx.graph_set_registration_constraints([PROJ_ID], [GT_ID], ctx.reg_config(
         registration_point_type=api.K_VOXELS, no_correspondence_cost=0.0, sampling_ratio=-1.0,
         use_esdf_distance=1))
     opts = ctx.solver_options(max_num_iterations=200, parameter_tolerance=1e-12, max_solver_time_s=1e9)
-    stages["lm_ms"], (x, summ) = timed(lambda: ctx.graph_solve(2, opts))
+    _, stages["lm_ms"], (x, summ) = M.timed(ctx, lambda: ctx.graph_solve(2, opts))
     pose = x[1]
     Tal = synth.pose_to_T(pose)
 
@@ -113,20 +80,17 @@ def main():
         ctx.submap_transform(GT_ID, Tal)
         finish_gt()
 
-    stages["transform_ms"], _ = timed(transform)
-    stages["rmse_ms"], after = timed(lambda: ctx.evaluate_layers_rmse(GT_ID, PROJ_ID))
+    _, stages["transform_ms"], _ = M.timed(ctx, transform)
+    _, stages["rmse_ms"], after = M.timed(ctx, lambda: ctx.evaluate_layers_rmse(GT_ID, PROJ_ID))
     ctx.graph_set_nodes([], np.zeros((0, 4)), np.zeros(0, np.uint8))
     ctx.submap_free(PROJ_ID)
     # the whole call
     host = []
     for _ in range(a.repeats):
         fresh_gt()
-        ctx.synchronize()
-        t0 = time.perf_counter()
-        r = ctx.map_evaluate(GT_ID, ids, T)
-        ctx.synchronize()
-        host.append(1e3 * (time.perf_counter() - t0))
-    res = dict(gpu=gpu_info(), submaps=len(ids), voxel_size=a.voxel_size,
+        h, _, r = M.timed(ctx, lambda: ctx.map_evaluate(GT_ID, ids, T))
+        host.append(h)
+    res = dict(gpu=M.gpu_info(), submaps=len(ids), voxel_size=a.voxel_size,
                ground_truth_blocks=int(len(gt_layer[0])),
                stages_event_ms={k: round(v, 3) for k, v in stages.items()},
                map_evaluate_host_ms=[round(h, 3) for h in host], map_evaluate_best_ms=round(min(host), 3),
@@ -136,12 +100,7 @@ def main():
                rmse_before=float(before.rmse), rmse_after=float(r.details.rmse),
                evaluated_voxels=int(r.details.num_evaluated_voxels))
     ctx.close()
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "a") as f:
-            f.write(line + "\n")
+    M.emit(res, a.out)
 
 
 if __name__ == "__main__":

@@ -14,64 +14,33 @@ the restated reference.  min_weight defaults to voxgraph's mesh_min_weight 2.0 (
 1 to 10).  The card's name and power limit are read in the same run.  Needs a GPU.
 """
 import argparse
-import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "tests"))
+import _measure as M
 
-WORKLOADS = {"config2": dict(submaps=50, voxel_size=0.2, seed=2), "config4": dict(submaps=200, voxel_size=0.1, seed=4)}
-SLOT_MESH = 12
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             stdout=subprocess.PIPE, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clock = [s.strip() for s in out.split(",")]
-        return dict(name=name, power_limit=power, max_sm_clock=clock)
-    except Exception as e:   # the figures are still reported, without the card's description
-        return dict(error=str(e))
+sys.path.insert(0, os.path.join(M.ROOT, "tests"))
 
 
 def measure(ctx, ids, T, min_weight, repeats, restate_layers):
-    import torch
-    from voxgraph_b200 import api
+    from voxgraph_b200 import _lib, api
     cfg = ctx.mesh_config(min_weight=min_weight)
     n_vox = 0
     for i in ids:
         _, vps, nb, _ = ctx.submap_info(i)
         n_vox += nb * vps ** 3
     ctx.mesh_build(ids, T, cfg)   # warm-up: table upload, scratch and output buffers
-    stream = torch.cuda.ExternalStream(ctx.stream_ptr)
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
     host, dev = [], []
     for _ in range(repeats):
-        ctx.synchronize()
-        t = time.perf_counter()
-        ev[0].record(stream)
-        vo, to = ctx.mesh_build(ids, T, cfg)
-        ev[1].record(stream)
-        ctx.synchronize()
-        host.append(1e3 * (time.perf_counter() - t))
-        dev.append(ev[0].elapsed_time(ev[1]))
-    ctx.profile_enable(True)
-    ctx.profile_reset()
-    ctx.mesh_build(ids, T, cfg)
-    kern_ms, launches = ctx.profile_get(SLOT_MESH)
-    ctx.profile_enable(False)
-    t = time.perf_counter()
-    xyz, tri = ctx.mesh_download()
-    t_dl = 1e3 * (time.perf_counter() - t)
-    t = time.perf_counter()
-    ply = ctx.mesh_ply()
-    t_ply = 1e3 * (time.perf_counter() - t)
+        h, d, _ = M.timed(ctx, lambda: ctx.mesh_build(ids, T, cfg))
+        host.append(h)
+        dev.append(d)
+    kern_ms, launches, _ = M.profiled(ctx, _lib.VGX_SLOT_MESH, lambda: ctx.mesh_build(ids, T, cfg))
+    t_dl, _, (xyz, tri) = M.timed(ctx, ctx.mesh_download)
+    t_ply, _, ply = M.timed(ctx, ctx.mesh_ply)
     res = dict(submaps=len(ids), voxels=n_vox, min_weight=min_weight, vertices=len(xyz), triangles=len(tri),
                build_host_ms=[round(x, 3) for x in host], build_event_ms=[round(x, 3) for x in dev],
                build_best_ms=round(min(host), 3), voxels_per_s=float("%.4g" % (n_vox / (min(host) / 1e3))),
@@ -116,35 +85,20 @@ def stream_active(min_weight, repeats):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", default="config2", choices=sorted(WORKLOADS))
+    ap.add_argument("--workload", default="config2", choices=sorted(M.WORKLOADS))
     ap.add_argument("--submaps", type=int, default=None)
     ap.add_argument("--repeats", type=int, default=5)
     ap.add_argument("--restate-submaps", type=int, default=3)
     ap.add_argument("--min-weight", type=float, default=2.0)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    from voxgraph_b200 import api, synth
-    w = dict(WORKLOADS[a.workload])
-    if a.submaps:
-        w["submaps"] = a.submaps
-    sc = synth.make_scene(seed=w["seed"], n_submaps=w["submaps"], n_points=100, voxel_size=w["voxel_size"],
-                          trunc=0.6 if abs(w["voxel_size"] - 0.2) < 1e-9 else None, workers=os.cpu_count() or 1)
-    ctx = api.Context(0)
-    for s in sc.submaps:
-        ctx.submap_upload(s.submap_id, s.voxel_size, s.vps, s.block_idx, s.distance, s.weight)
-    ids = [s.submap_id for s in sc.submaps]
-    T = np.array([synth.pose_to_T(p) for p in sc.poses_init], np.float32)
+    w = M.WORKLOADS[a.workload]
+    ctx, sc, ids, T = M.upload_scene(w, a.submaps)
     layers = [(s.voxel_size, s.vps, s.block_idx, s.distance, s.weight) for s in sc.submaps[:a.restate_submaps]]
     scene = measure(ctx, ids, T, a.min_weight, a.repeats, layers)
     ctx.close()
-    res = dict(gpu=gpu_info(), workload=a.workload, voxel_size=w["voxel_size"], scene=scene,
-               active_submap=stream_active(a.min_weight, a.repeats))
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "a") as f:
-            f.write(line + "\n")
+    M.emit(dict(gpu=M.gpu_info(), workload=a.workload, voxel_size=w["voxel_size"], scene=scene,
+                active_submap=stream_active(a.min_weight, a.repeats)), a.out)
 
 
 if __name__ == "__main__":

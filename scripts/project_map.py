@@ -14,35 +14,15 @@ sort scratch, from cudaMemGetInfo).  Two projections are checked bit-equal.  The
 limit are read in the same run.  Needs a GPU.
 """
 import argparse
-import json
-import os
-import subprocess
-import sys
-import time
 
-import numpy as np
+import _measure as M
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-
-WORKLOADS = {"config2": dict(submaps=50, voxel_size=0.2, seed=2), "config4": dict(submaps=200, voxel_size=0.1, seed=4)}
-SLOT_PROJECT = 13
-SLOT_MESH = 12
 OUT_ID = 0xFFFFFFF0
-
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                             stdout=subprocess.PIPE, text=True, timeout=30).stdout.strip().splitlines()[0]
-        name, power, clock = [s.strip() for s in out.split(",")]
-        return dict(name=name, power_limit=power, max_sm_clock=clock)
-    except Exception as e:   # the figures are still reported, without the card's description
-        return dict(error=str(e))
 
 
 def measure(ctx, ids, T, min_weight, repeats):
     import torch
+    from voxgraph_b200 import _lib
     n_in = 0
     for i in ids:
         _, vps, nb, _ = ctx.submap_info(i)
@@ -54,41 +34,20 @@ def measure(ctx, ids, T, min_weight, repeats):
     free1, _ = torch.cuda.mem_get_info()
     first = ctx.submap_download(OUT_ID)
     ctx.submap_free(OUT_ID)
-    stream = torch.cuda.ExternalStream(ctx.stream_ptr)
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
     host, dev = [], []
     for _ in range(repeats):
-        ctx.synchronize()
-        t = time.perf_counter()
-        ev[0].record(stream)
-        ctx.project_map(ids, T, OUT_ID)
-        ev[1].record(stream)
-        ctx.synchronize()
-        host.append(1e3 * (time.perf_counter() - t))
-        dev.append(ev[0].elapsed_time(ev[1]))
+        h, d, _ = M.timed(ctx, lambda: ctx.project_map(ids, T, OUT_ID))
+        host.append(h)
+        dev.append(d)
         ctx.submap_free(OUT_ID)
-    ctx.profile_enable(True)
-    ctx.profile_reset()
-    ctx.project_map(ids, T, OUT_ID)
-    kern_ms, launches = ctx.profile_get(SLOT_PROJECT)
-    ctx.profile_enable(False)
+    kern_ms, launches, _ = M.profiled(ctx, _lib.VGX_SLOT_PROJECT, lambda: ctx.project_map(ids, T, OUT_ID))
     again = ctx.submap_download(OUT_ID)
     deterministic = all(a.tobytes() == b.tobytes() for a, b in zip(first, again))
     _, vps, _, _ = ctx.submap_info(OUT_ID)
     cfg = ctx.mesh_config(min_weight=min_weight)
     ctx.mesh_build([OUT_ID], None, cfg)                      # warm-up
-    mesh_ms = []
-    for _ in range(repeats):
-        ctx.synchronize()
-        t = time.perf_counter()
-        ctx.mesh_build([OUT_ID], None, cfg)
-        ctx.synchronize()
-        mesh_ms.append(1e3 * (time.perf_counter() - t))
-    ctx.profile_enable(True)
-    ctx.profile_reset()
-    ctx.mesh_build([OUT_ID], None, cfg)
-    mesh_kern_ms, _ = ctx.profile_get(SLOT_MESH)
-    ctx.profile_enable(False)
+    mesh_ms = [M.timed(ctx, lambda: ctx.mesh_build([OUT_ID], None, cfg))[0] for _ in range(repeats)]
+    mesh_kern_ms, _, _ = M.profiled(ctx, _lib.VGX_SLOT_MESH, lambda: ctx.mesh_build([OUT_ID], None, cfg))
     xyz, tri = ctx.mesh_download()
     ctx.submap_free(OUT_ID)
     return dict(submaps=len(ids), input_voxels=n_in, output_blocks=n_out_blocks,
@@ -111,30 +70,16 @@ def main():
     ap.add_argument("--min-weight", type=float, default=2.0)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    from voxgraph_b200 import api, synth
-    res = dict(gpu=gpu_info(), results={})
+    res = dict(gpu=M.gpu_info(), results={})
     for name in a.workloads.split(","):
-        w = dict(WORKLOADS[name])
-        if a.submaps:
-            w["submaps"] = a.submaps
-        sc = synth.make_scene(seed=w["seed"], n_submaps=w["submaps"], n_points=100, voxel_size=w["voxel_size"],
-                              trunc=0.6 if abs(w["voxel_size"] - 0.2) < 1e-9 else None, workers=os.cpu_count() or 1)
-        ctx = api.Context(0)
-        for s in sc.submaps:
-            ctx.submap_upload(s.submap_id, s.voxel_size, s.vps, s.block_idx, s.distance, s.weight)
-        ids = [s.submap_id for s in sc.submaps]
-        T = np.array([synth.pose_to_T(p) for p in sc.poses_init], np.float32)
+        w = M.WORKLOADS[name]
+        ctx, sc, ids, T = M.upload_scene(w, a.submaps)
         r = measure(ctx, ids, T, a.min_weight, a.repeats)
         r["voxel_size"] = w["voxel_size"]
         res["results"][name] = r
         ctx.close()
         del sc
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "a") as f:
-            f.write(line + "\n")
+    M.emit(res, a.out)
 
 
 if __name__ == "__main__":

@@ -15,7 +15,7 @@ import bench  # noqa: E402
 sys.stdout = bench._REAL_STDOUT
 w = dict(bench.WORKLOADS["config4"]); w["name"] = "config4"
 sc = bench.build_scene(w)
-from voxgraph_b200 import api  # noqa: E402
+from voxgraph_b200 import _lib, api  # noqa: E402
 
 ctx = api.Context(0)
 P = bench.Problem(ctx, api, sc)
@@ -34,7 +34,7 @@ def kernel_us(sel):
     for _ in range(6):
         ctx.graph_eval_async()
     ctx.synchronize()
-    ms, n = ctx.profile_get(0)
+    ms, n = ctx.profile_get(_lib.VGX_SLOT_REG_REDUCE)
     ctx.profile_enable(False)
     return ms / max(n, 1) * 1e3
 

@@ -1,5 +1,7 @@
 """Exact models of finishSubmap on the device (ESDF, relevant voxels, surface OBB, isosurface vertices)
 for tests/test_oracle_finish.py and tests/test_gpu_finish_exact.py.  Test support, not product code.
+MATRIX (the layer matrix), FILTERS and ESDF_CASES are the cases that the finishSubmap, mesh, projection,
+registration-lookup and map evaluation tests run over.
 
 Every model works on `Grid`, a dense embedding of a block layer over its block AABB with "absent"
 cells, so neighbour logic owes nothing to block tables, hashes or slot order.  Block coordinates are
@@ -491,3 +493,51 @@ def noise_layer(vs, vps, nblocks_xyz, seed=0, origin=(0, 0, 0)):
                     for i in range(nx)], np.int32)
     d = np.random.RandomState(seed).uniform(-0.05, 0.05, (len(idx), vps ** 3)).astype(F32)
     return vs, vps, idx, d, np.full(d.shape, 2.0, F32)
+
+
+# filters: min_voxel_weight 0 / 0.1 with weights 0.1f / 0.5 / 1, weights at 1e-6, zero-weight slabs,
+# max_voxel_distance 0, 0.3 and exactly a voxel's value
+def filter_cases():
+    out = []
+    for res in [(0.25, 8), (0.2, 16)]:
+        vs, vps, idx, d, w = layer(res, "box", "tilted")
+        w01 = np.full_like(w, np.float32(0.1))
+        wz = w.copy().reshape(len(idx), vps, vps, vps)
+        wz[:, :, 3, :] = 0.0                      # a zero-weight slab (y = 3) in every block
+        wz[:, 5, :, :] = np.float32(1e-6)         # ... and a slab at the observation threshold
+        wz = wz.reshape(len(idx), -1)
+        v = float(d.reshape(-1)[len(d.reshape(-1)) // 2])
+        for mw, ww, md in [(0.0, w, 0.3), (0.1, w01, 0.3), (0.5, w, 0.3), (1.0, w, 0.3), (0.0, wz, 0.3),
+                           (1.0, w, 0.0), (1.0, w, abs(v)), (0.0, wz, 0.6)]:
+            out.append(("%g/%d-minw%g-maxd%g-%s" % (res[0], res[1], mw, md, "slabs" if ww is wz else
+                                                     "w0.1f" if ww is w01 else "w2"),
+                        (vs, vps, idx, d, ww, mw, md)))
+    return out
+
+
+def esdf_cases():
+    sph = layer((0.2, 16), "box", "sphere")
+    pl = layer((0.25, 8), "edge", "plane")
+    cr = layer((0.125, 16), "straddle", "crafted")
+    long = layer((0.05, 32), "one", "plane")
+    idx5 = np.array([(i, 0, 0) for i in range(4)], np.int32)
+    d5 = np.full((4, 32 ** 3), 0.6, np.float32)
+    d5.reshape(4, 32, 32, 32)[0, :, :, 0] = 0.01          # one seed plane at x = 0: 127 voxels to go
+    far = (0.05, 32, idx5, d5, np.full_like(d5, 2.0))
+    de = np.full((1, 8 ** 3), 0.5, np.float32)
+    de.reshape(8, 8, 8)[:, :, 0] = 0.25                   # seeds at x = 0: 0.25 + 3 * 0.25 is exactly 1.0
+    exact_max = (0.25, 8, np.zeros((1, 3), np.int32), de, np.full_like(de, 2.0))
+    return [("defaults-sphere", sph, {}), ("max<vs", sph, dict(max_distance_m=0.15)),
+            ("max-not-multiple", sph, dict(max_distance_m=0.93)),
+            ("default<max", sph, dict(default_distance_m=0.5, max_distance_m=2.0)),
+            ("min0", sph, dict(min_distance_m=0.0)), ("min>=trunc", sph, dict(min_distance_m=0.7)),
+            ("edge-join", pl, {}), ("crafted-zeros", cr, dict(min_distance_m=0.3)),
+            ("crafted-min0", cr, dict(min_distance_m=0.0)),
+            ("weights-1e-6", (long[0], long[1], long[2], long[3], np.full_like(long[4], np.float32(1e-6))), {}),
+            ("5m-at-0.05", far, dict(max_distance_m=5.0, default_distance_m=5.0)),
+            ("max-reached-exactly", exact_max, dict(min_distance_m=0.3, max_distance_m=1.0))]
+
+
+MATRIX = matrix()
+FILTERS = filter_cases()
+ESDF_CASES = esdf_cases()

@@ -1,6 +1,6 @@
 """Test support for the fused registration reduction (not product code).
 
-Three pieces:
+Four pieces:
 
 * Poses whose pose blocks are the same on the host and on the device.  The oracle (and emit mode)
   evaluates cos_e, sin_e, cos(the - tho), sin(the - tho) with libm cosf/sinf; the device pose set-up
@@ -13,6 +13,8 @@ Three pieces:
 * A float32 restatement of the reduce kernel's transform, block index, unit bounds and unit cull test
   (vgx_reg_transform, vgx_block_index, reg_unit_bounds_kernel, reg_unit_may_hit), operation by
   operation and without FMA, used to build units on the cull decision and to check its margin.
+* `Problem`, a registration problem on the device with its exact reference, and `check_eval`, which
+  checks the fused evaluation of a problem against that reference.
 """
 import ctypes
 import ctypes.util
@@ -525,3 +527,108 @@ def cull_problem_scenes(bsi, seed=5):
         P = pose_block(x[ref], x[read])
         out.append((ref, read, P, cull_scene(P, off, rng, bsi)))
     return x, out
+
+
+# --------------------------------------------------------------------------- device problems
+GRID_MAX_CELLS = 4096   # larger block AABBs get no block grid (submap.cu, VGX_GRID_MAX_CELLS)
+
+
+class Problem:
+    """Submaps (uploaded to the device and mirrored as oracle layers), nodes and registration
+    constraints; builds the PoseGraph at exact-trig poses and the exact reference."""
+
+    def __init__(self, ctx, oracle):
+        self.ctx, self.oracle = ctx, oracle
+        self.sub = {}
+        self.nodes = {}      # sid -> (base pose, constant)
+        self.cons = []
+
+    def submap(self, sid, vs, vps, idx, d, w, iso=None, vox=None, esdf=False):
+        from voxgraph_b200 import api
+        o = self.oracle
+        self.ctx.submap_upload(sid, vs, vps, idx, d, w)
+        e = dict(layer=o.Layer.from_blocks(vs, vps, idx, d, w), pts={})
+        for ptype, pts in ((api.K_ISOSURFACE_POINTS, iso), (api.K_VOXELS, vox)):
+            if pts is not None:
+                pts = tuple(np.ascontiguousarray(a, np.float32) for a in pts)
+                self.ctx.submap_upload_points(sid, ptype, *pts)
+                e["pts"][ptype] = pts
+        if esdf:
+            self.ctx.submap_generate_esdf(sid)
+            eo, obo, _ = o.generate_esdf(e["layer"])
+            e["esdf"] = o.Layer.from_blocks(vs, vps, idx, eo, obo)
+        self.sub[sid] = e
+
+    def synth_submap(self, s, sid=None, **kw):
+        sid = s.submap_id if sid is None else sid
+        self.submap(sid, s.voxel_size, s.vps, s.block_idx, s.distance, s.weight,
+                    iso=(s.points_xyz, s.points_distance, s.points_weight), **kw)
+
+    def node(self, sid, pose, constant=False):
+        self.nodes[sid] = (np.asarray(pose, np.float64), constant)
+
+    def constrain(self, a, b, **kw):
+        from voxgraph_b200 import api
+        self.cons.append(api.RegistrationConstraintConfig(a, b, **kw))
+
+    def build(self, seed, fixed=None, sigma=(0.03, 0.03, 0.02, 0.01)):
+        """Draw exact-trig poses, build the PoseGraph (node order = sorted submap ids)."""
+        from voxgraph_b200 import api
+        ids = sorted(self.nodes)
+        col = {s: k for k, s in enumerate(ids)}
+        pairs = []
+        for c in self.cons:
+            a, b = col[c.first_submap_id], col[c.second_submap_id]
+            pairs += [(a, b), (b, a)]
+        fx = {col[s]: p for s, p in (fixed or {}).items()}
+        self.x = exact_trig_poses(np.array([self.nodes[s][0] for s in ids]), pairs,
+                                     np.random.default_rng(seed), sigma=sigma, fixed=fx)
+        self.col = col
+        pg = api.PoseGraph(self.ctx)
+        for s in ids:
+            pg.addSubmapNode(api.SubmapNodeConfig(s, self.x[col[s]], set_constant=self.nodes[s][1]))
+        for c in self.cons:
+            pg.addRegistrationConstraint(c)
+        pg._sync()
+        self.pg = pg
+        return pg
+
+    def exact(self, emit=True):
+        """Exact sums of the oracle's terms over pg.registration_blocks; each non-sampled block is
+        also checked bit for bit against emit mode at the same poses."""
+        o, ctx, pg = self.oracle, self.ctx, self.pg
+        ex = Exact(len(self.col))
+        self.n_terms = 0
+        for k, ((a, b), cfg) in enumerate(zip(pg.registration_blocks, pg._reg_cfgs)):
+            ia, ib = self.col[a], self.col[b]
+            ref, read = self.x[ia], self.x[ib]
+            check_pose_block(o, ref, read)
+            xyz, d, w = self.sub[a]["pts"][cfg.registration_point_type]
+            layer = self.sub[b]["esdf" if cfg.use_esdf_distance else "layer"]
+            nc = cfg.no_correspondence_cost
+            if cfg.sampling_ratio != -1.0:
+                K = o.sampled_num_residuals(cfg.sampling_ratio, len(w))
+                idx = ctx.graph_get_sample_indices(k, K)
+                assert len(idx) == K
+                ok, r, jr, je = o.reg_evaluate_sampled(layer, xyz, d, idx, ref, read, no_correspondence_cost=nc)
+            else:
+                ok, r, jr, je = o.reg_evaluate(layer, xyz, d, w, ref, read, no_correspondence_cost=nc)
+                if emit:
+                    ok_g, r_g, jr_g, je_g = ctx.reg_eval_emit(a, b, ref, read, cfg)
+                    assert ok_g and np.array_equal(r_g, r) and np.array_equal(jr_g, jr) and \
+                        np.array_equal(je_g, je), "emit mode differs from the oracle on block %d" % k
+            assert ok
+            ex.add_block(ia, ib, r, jr, je)
+            self.n_terms += len(r)
+        ex.finish()
+        return ex
+
+
+def check_eval(pb, ex, label, costs=True):
+    ok, cost, g, H = pb.pg.evaluate()
+    assert ok
+    worst = check_bound(ex, cost, g, H, label=label)
+    if costs:
+        worst = max(worst, check_costs_bound(ex, pb.pg.getVisualizationEdgeResiduals(), label=label + " costs"))
+    print("%s: max |fused - exact| / bound = %.3g over %d residuals" % (label, worst, pb.n_terms))
+    return worst

@@ -6,6 +6,8 @@ import re
 
 import pytest
 
+import support
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -27,41 +29,47 @@ def test_header_symbols_exported(lib):
         assert hasattr(lib, name), name
 
 
+# the header typedef of every ctypes.Structure in voxgraph_b200/_lib.py
+HEADER_STRUCTS = {"TsdfConfig": "vgx_tsdf_config", "TsdfStats": "vgx_tsdf_stats",
+                  "RegistrationFilter": "vgx_registration_filter", "RegConfig": "vgx_reg_config",
+                  "EsdfConfig": "vgx_esdf_config", "SolverOptions": "vgx_solver_options",
+                  "SolverSummary": "vgx_solver_summary", "CollectionEntry": "vgx_collection_entry",
+                  "MeshConfig": "vgx_mesh_config", "VoxelEvaluationDetails": "vgx_voxel_evaluation_details",
+                  "MapEvaluationResult": "vgx_map_evaluation"}
+
+
 def test_struct_layouts_match_header(tmp_path):
-    """ctypes mirrors vs the C compiler's view of include/voxgraph_b200.h (size and every field offset)."""
-    import subprocess
+    """Every ctypes mirror in _lib.py against the C compiler's view of include/voxgraph_b200.h (size and
+    every field offset), and every VGX_ constant of _lib.py (status codes, layer selectors, profiling
+    slots) against its value in the header."""
     from voxgraph_b200 import _lib
-    structs = {"vgx_tsdf_config": _lib.TsdfConfig, "vgx_tsdf_stats": _lib.TsdfStats,
-               "vgx_reg_config": _lib.RegConfig, "vgx_solver_options": _lib.SolverOptions,
-               "vgx_solver_summary": _lib.SolverSummary, "vgx_registration_filter": _lib.RegistrationFilter,
-               "vgx_esdf_config": _lib.EsdfConfig}
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "voxgraph_b200.h"', 'int main(void) {']
+    mirrors = {n: v for n, v in vars(_lib).items()
+               if isinstance(v, type) and issubclass(v, C.Structure) and v.__module__ == _lib.__name__}
+    assert set(mirrors) == set(HEADER_STRUCTS), "a ctypes struct without its header typedef, or a stale entry"
+    structs = {HEADER_STRUCTS[n]: ct for n, ct in mirrors.items()}
+    constants = {n: v for n, v in vars(_lib).items() if n.startswith("VGX_") and isinstance(v, int)}
+    assert "VGX_SLOT_EVAL" in constants and "VGX_PROFILE_SLOTS" in constants
+    out = support.c_layout(tmp_path, {c: [f for f, _ in ct._fields_] for c, ct in structs.items()}, constants)
     for cname, ct in structs.items():
-        lines.append('printf("%s %%zu\\n", sizeof(%s));' % (cname, cname))
+        assert out[cname] == C.sizeof(ct), cname
         for fname, _ in ct._fields_:
-            lines.append('printf("%s.%s %%zu\\n", offsetof(%s, %s));' % (cname, fname, cname, fname))
-    lines += ['return 0;', '}']
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-I" + os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
-    out = dict(l.split() for l in subprocess.run([str(exe)], check=True, stdout=subprocess.PIPE,
-                                                 text=True).stdout.strip().splitlines())
-    for cname, ct in structs.items():
-        assert int(out[cname]) == C.sizeof(ct), cname
-        for fname, _ in ct._fields_:
-            assert int(out["%s.%s" % (cname, fname)]) == getattr(ct, fname).offset, (cname, fname)
+            assert out["%s.%s" % (cname, fname)] == getattr(ct, fname).offset, (cname, fname)
+    for name, value in constants.items():
+        assert out[name] == value, name
     assert C.sizeof(_lib.TsdfConfig) == 14 * 4 and C.sizeof(_lib.TsdfStats) == 5 * 8
+    assert C.sizeof(_lib.CollectionEntry) == 44
+    assert C.sizeof(_lib.VoxelEvaluationDetails) == 48
+    assert C.sizeof(_lib.MeshConfig) == 4 and _lib.MeshConfig.min_weight.offset == 0
 
 
 def test_no_cpu_fallback(lib):
     import torch
     if torch.cuda.is_available():
         pytest.skip("GPU present")
+    from voxgraph_b200 import _lib, api
     h = C.c_void_p()
     assert lib.vgx_device_count() == 0
-    assert lib.vgx_ctx_create(0, C.byref(h)) == -2   # VGX_ERR_CUDA
-    from voxgraph_b200 import api
+    assert lib.vgx_ctx_create(0, C.byref(h)) == _lib.VGX_ERR_CUDA
     with pytest.raises(api.VgxError):
         api.Context(0)
 

@@ -10,9 +10,10 @@ import numpy as np
 import pytest
 
 import collection_stream as cs
+from voxgraph_b200 import _lib
 
 pytestmark = pytest.mark.gpu
-INVALID = -1
+INVALID = _lib.VGX_ERR_INVALID
 
 
 @pytest.fixture(scope="module")
@@ -91,7 +92,8 @@ def test_save_is_byte_identical_to_protobuf(exp, tmp_path):
     ids32 = np.ascontiguousarray(exp["ids"], np.uint32); T = np.ascontiguousarray(exp["poses"], np.float32)
     args = (ctx._h, 3, ids32.ctypes.data_as(C.POINTER(C.c_uint32)), T.ctypes.data_as(C.POINTER(C.c_float)))
     small = C.create_string_buffer(len(data) - 1)
-    assert L.vgx_collection_save(*args, small, len(data) - 1, C.byref(size)) == -6 and size.value == len(data)
+    assert L.vgx_collection_save(*args, small, len(data) - 1, C.byref(size)) == _lib.VGX_ERR_CAPACITY
+    assert size.value == len(data)
     try:
         sys.path.insert(0, cs.GOLDEN)
         import make_collection_golden as g
@@ -203,11 +205,11 @@ def _finished_state(ctx, ids, poses_T, xyzyaw):
     return out, pairs, (ok, cost, g, H)
 
 
-def _same_bits(a, b):
+def _identical(a, b):
     if isinstance(a, (tuple, list)):
         assert len(a) == len(b)
         for x, y in zip(a, b):
-            _same_bits(x, y)
+            _identical(x, y)
     elif isinstance(a, np.ndarray):
         assert a.shape == b.shape and a.dtype == b.dtype and a.tobytes() == b.tobytes()
     else:
@@ -242,8 +244,8 @@ def test_mapper_round_trip(tmp_path):
     b = _finished_state(ctx2, ids_l, poses, xyzyaw)
     assert a[1] and a[1] == b[1]   # overlapping pairs
     for sid in ids_l:
-        _same_bits(a[0][sid], b[0][sid])
-    _same_bits(a[2], b[2])
+        _identical(a[0][sid], b[0][sid])
+    _identical(a[2], b[2])
     assert a[2][0] and a[2][1] > 0
     ctx.close()
     ctx2.close()

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 import solve_exact as SX
+from support import ctx  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -15,12 +16,9 @@ ANCHORS = ["first", "interleaved", "frame"]
 WORST = {}                     # largest ratio to the bound per path, printed at the end of the module
 
 
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
+@pytest.fixture(scope="module", autouse=True)
+def _report_worst():
+    yield
     for k in sorted(WORST):
         print("dense solve: largest ratio to the bound, %-36s %.3g" % (k, WORST[k]))
 

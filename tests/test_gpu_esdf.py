@@ -3,18 +3,11 @@ point, and the use_esdf_distance registration branch (registration_cost_function
 import numpy as np
 import pytest
 
+from support import ctx  # noqa: F401
 from voxgraph_b200 import synth
 
 pytestmark = pytest.mark.gpu
 VS, VPS = 0.2, 16
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
 
 
 def _esdf_check(ctx, oracle, sid, vs, vps, idx, d, w, **cfg):

@@ -3,19 +3,12 @@ oracle's findRelevantVoxelIndices / findIsosurfaceVertices / surface OBB - bit-e
 import numpy as np
 import pytest
 
+from support import ctx  # noqa: F401
 from voxgraph_b200 import synth
 
 pytestmark = pytest.mark.gpu
 
 VS, VPS = 0.2, 16
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
 
 
 def _check(ctx, oracle, sid, voxel_size, vps, idx, d, w, min_w=1.0, max_d=0.3):

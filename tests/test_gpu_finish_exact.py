@@ -9,19 +9,12 @@ import numpy as np
 import pytest
 
 import finish_exact as fx
-from test_oracle_finish import ESDF_CASES, FILTERS, MATRIX
-from voxgraph_b200 import synth
+from finish_exact import ESDF_CASES, FILTERS, MATRIX
+from support import ctx  # noqa: F401
+from voxgraph_b200 import _lib, synth
 
 pytestmark = pytest.mark.gpu
 _ids = itertools.count(5000)
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
 
 
 def _esdf_kw(cfg):
@@ -220,7 +213,7 @@ def _run_overlap(ctx, oracle, subs, T, max_pairs=None):
         p = lambda a, t: a.ctypes.data_as(C.POINTER(t))
         rc = ctx._L.vgx_find_overlapping_pairs(ctx._h, len(ids), p(idv, C.c_uint32), p(Tv, C.c_float),
                                                len(want) - 1, p(out, C.c_uint32), C.byref(n))
-        assert rc == -6 and n.value == len(want)
+        assert rc == _lib.VGX_ERR_CAPACITY and n.value == len(want)
         rc = ctx._L.vgx_find_overlapping_pairs(ctx._h, len(ids), p(idv, C.c_uint32), p(Tv, C.c_float),
                                                len(want), p(out, C.c_uint32), C.byref(n))
         assert rc == 0 and [tuple(int(v) for v in r) for r in out] == [(ids[i], ids[j]) for i, j in want]
@@ -333,7 +326,7 @@ def test_upload_rejects_repeated_and_out_of_range_indices(ctx, oracle, path):
         sid = next(_ids)
         with pytest.raises(api.VgxError) as e:
             up(sid, vs, vps, idx, d, w)
-        assert e.value.code == -1
+        assert e.value.code == _lib.VGX_ERR_INVALID
         with pytest.raises(api.VgxError):
             ctx.submap_info(sid)
     for v in (lo, hi):

@@ -11,17 +11,10 @@ unit test, so parity is established through size-independent properties:
 import numpy as np
 import pytest
 
+from support import ctx  # noqa: F401
 from voxgraph_b200 import synth
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
 
 
 @pytest.fixture(scope="module")

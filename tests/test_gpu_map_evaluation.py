@@ -18,55 +18,19 @@ import finish_exact as fx
 import rmse_exact as rx
 import transform_oracle as to
 from collection_stream import field, varint
-from test_oracle_finish import MATRIX
-from voxgraph_b200 import synth
+from finish_exact import MATRIX
+from support import IDENTITY, ctx, exists, poses_for, same_bits, yaw_T  # noqa: F401
+from voxgraph_b200 import _lib, synth
 
 pytestmark = pytest.mark.gpu
 _ids = itertools.count(30000)
 F32 = np.float32
-IDENTITY = np.array([1, 0, 0, 0, 0, 0, 0], F32)
-SLOT = 14
 SCRATCH = 0xFFFFFFFE   # the first id the library's scratch submaps take (then counting down)
 
 
 def _no_scratch(ctx):
     """No scratch submap left: none of the 16 ids the library's scratch submaps take first."""
-    return not any(_exists(ctx, SCRATCH - k) for k in range(16))
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
-
-
-def _same(exp, got, what):
-    """Bit-equal arrays, NaN equal to NaN whatever its payload."""
-    exp = np.asarray(exp); got = np.asarray(got)
-    assert exp.shape == got.shape, (what, exp.shape, got.shape)
-    if exp.dtype == np.float32:
-        ne, ng = np.isnan(exp), np.isnan(got)
-        assert np.array_equal(ne, ng), (what, "NaN positions")
-        exp = np.where(ne, 0, exp).astype(F32); got = np.where(ng, 0, got).astype(F32)
-        fx.assert_bits(exp, got, what)
-    else:
-        assert np.array_equal(exp, got), (what, exp[:3], got[:3])
-
-
-def _exists(ctx, sid):
-    from voxgraph_b200 import api
-    try:
-        ctx.submap_info(sid)
-        return True
-    except api.VgxError as e:
-        assert e.code == -3
-        return False
-
-
-def _yaw_T(yaw, t=(0.0, 0.0, 0.0)):
-    return np.array([np.cos(yaw / 2), 0, 0, np.sin(yaw / 2), *t], F32)
+    return not any(exists(ctx, SCRATCH - k) for k in range(16))
 
 
 # ---------------------------------------------------------------- layer files
@@ -107,9 +71,9 @@ def test_layer_load_bit_exact(ctx, res):
     gvs, gvps, nb, fin = ctx.submap_info(sid)
     assert fin and nb == n and gvps == vps and gvs == F32(vs)
     got = ctx.submap_download(sid)
-    _same(idx.astype(np.int32), got[0], "block indices")
-    _same(d, got[1], "distance")
-    _same(w, got[2], "weight")
+    same_bits(idx.astype(np.int32), got[0], "block indices")
+    same_bits(d, got[1], "distance")
+    same_bits(w, got[2], "weight")
     ctx.submap_free(sid)
     # an empty layer is a submap without blocks
     ctx.layer_load(sid, layer_stream(vs, vps, idx[:0], d[:0], w[:0]))
@@ -155,27 +119,17 @@ def test_layer_load_refusals_leave_nothing(ctx):
         sid = next(_ids)
         with pytest.raises(api.VgxError) as e:
             ctx.layer_load(sid, data)
-        assert e.value.code == -1, name
-        assert not _exists(ctx, sid), name
+        assert e.value.code == _lib.VGX_ERR_INVALID, name
+        assert not exists(ctx, sid), name
     # an existing id is refused and kept
     with pytest.raises(api.VgxError) as e:
         ctx.layer_load(keep, layer_stream(vs, vps, idx, d, w))
-    assert e.value.code == -1
-    _same(d, ctx.submap_download(keep)[1], "kept submap")
+    assert e.value.code == _lib.VGX_ERR_INVALID
+    same_bits(d, ctx.submap_download(keep)[1], "kept submap")
     ctx.submap_free(keep)
 
 
 # ---------------------------------------------------------------- transform
-def _poses_for(vs, vps):
-    bs = float(F32(vs) * vps)
-    rs = np.random.RandomState(int(vs * 1000) + vps)
-    q = rs.normal(size=4); q /= np.linalg.norm(q)
-    return {"identity": IDENTITY,
-            "translation": np.array([1, 0, 0, 0, 2 * bs, -bs, 0.37 * bs], F32),
-            "yaw": _yaw_T(0.7, (0.3 * bs, 0.1 * bs, 0.0)),
-            "random": np.array([*q, *rs.uniform(-bs, bs, 3)], F32)}
-
-
 def _check_transform(ctx, oracle, lay, T):
     from voxgraph_b200 import api
     sid = next(_ids)
@@ -187,10 +141,10 @@ def _check_transform(ctx, oracle, lay, T):
     if exp is None:
         with pytest.raises(api.VgxError) as e:
             ctx.submap_transform(sid, T)
-        assert e.value.code == -1 and _no_scratch(ctx)
+        assert e.value.code == _lib.VGX_ERR_INVALID and _no_scratch(ctx)
         got = ctx.submap_download(sid)   # unchanged
-        _same(np.asarray(lay[2], np.int32), got[0], "refused: block indices")
-        _same(lay[3], got[1], "refused: distance")
+        same_bits(np.asarray(lay[2], np.int32), got[0], "refused: block indices")
+        same_bits(lay[3], got[1], "refused: distance")
         ctx.submap_free(sid)
         return None
     ctx.submap_transform(sid, T)
@@ -198,16 +152,16 @@ def _check_transform(ctx, oracle, lay, T):
     assert fin and nb == len(exp[0]) and vps == lay[1]
     got = ctx.submap_download(sid)
     ctx.submap_free(sid)
-    _same(exp[0], got[0], "block indices")
-    _same(exp[1], got[1], "distance")
-    _same(exp[2], got[2], "weight")
+    same_bits(exp[0], got[0], "block indices")
+    same_bits(exp[1], got[1], "distance")
+    same_bits(exp[2], got[2], "weight")
     return got
 
 
 @pytest.mark.parametrize("case", range(len(MATRIX)), ids=[m[0] for m in MATRIX])
 def test_transform_matrix(ctx, oracle, case):
     lay = MATRIX[case][1]
-    for name, T in _poses_for(lay[0], lay[1]).items():
+    for name, T in poses_for(lay[0], lay[1]).items():
         _check_transform(ctx, oracle, lay, T)
 
 
@@ -217,12 +171,12 @@ def test_transform_identity_and_nan(ctx, oracle, res):
     lay = _layer(3, *res, nan=False)
     assert np.all(np.isfinite(lay[3])) and not np.any((lay[3] == 0) & np.signbit(lay[3]))
     got = _check_transform(ctx, oracle, lay, IDENTITY)
-    _same(lay[3], got[1], "identity distance")
-    _same(lay[4], got[2], "identity weight")
+    same_bits(lay[3], got[1], "identity distance")
+    same_bits(lay[4], got[2], "identity weight")
     # with NaN distances the identity spreads them to the neighbours that interpolate over them
     lay = _layer(3, *res)
     _check_transform(ctx, oracle, lay, IDENTITY)
-    _check_transform(ctx, oracle, lay, _yaw_T(0.3, (0.07, -0.02, 0.01)))
+    _check_transform(ctx, oracle, lay, yaw_T(0.3, (0.07, -0.02, 0.01)))
 
 
 def test_transform_refuses_out_of_range(ctx, oracle):
@@ -235,7 +189,7 @@ def test_transform_refuses_out_of_range(ctx, oracle):
     assert _check_transform(ctx, oracle, (vs, vps, idx, d, w), np.array([1, 0, 0, 0, 2 * bs, 0, 0], F32)) is None
     with pytest.raises(api.VgxError) as e:
         ctx.submap_transform(next(_ids), IDENTITY)
-    assert e.value.code == -3
+    assert e.value.code == _lib.VGX_ERR_NOT_FOUND
 
 
 # ---------------------------------------------------------------- RMSE
@@ -293,15 +247,15 @@ def test_rmse_crafted_tsdf(ctx):
     from voxgraph_b200 import api
     with pytest.raises(api.VgxError) as e:
         ctx.evaluate_layers_rmse(g, t, _lib.VGX_LAYER_ESDF, _lib.VGX_LAYER_TSDF)
-    assert e.value.code == -1
+    assert e.value.code == _lib.VGX_ERR_INVALID
     o = next(_ids)
     ctx.submap_upload(o, 0.2, vps, gidx, gd, gw)
     with pytest.raises(api.VgxError) as e:
         ctx.evaluate_layers_rmse(g, o, _lib.VGX_LAYER_TSDF, _lib.VGX_LAYER_TSDF)
-    assert e.value.code == -1
+    assert e.value.code == _lib.VGX_ERR_INVALID
     with pytest.raises(api.VgxError) as e:
         ctx.evaluate_layers_rmse(g, next(_ids), _lib.VGX_LAYER_TSDF, _lib.VGX_LAYER_TSDF)
-    assert e.value.code == -3
+    assert e.value.code == _lib.VGX_ERR_NOT_FOUND
     for s in (g, t, o):
         ctx.submap_free(s)
 
@@ -383,7 +337,7 @@ def test_map_evaluate_recovers_offset(ctx, oracle, scene):
     gt_layer = _download_all(ctx, gt)
     ctx.profile_reset()
     r = ctx.map_evaluate(gt, [map_id], T)
-    assert ctx.profile_get(SLOT)[1] == 3   # the transform's fold and the two RMSE kernels
+    assert ctx.profile_get(_lib.VGX_SLOT_EVAL)[1] == 3   # the transform's fold and the two RMSE kernels
     assert _no_scratch(ctx)
     pose = np.array(r.aligned_pose[:])
     err_t = np.abs(pose[:3] - np.array(OFFSET[:3]))
@@ -406,7 +360,7 @@ def test_map_evaluate_recovers_offset(ctx, oracle, scene):
     exp = to.transform_layer(oracle.Layer.from_blocks(VS, 16, *gt_layer), Texp).export()
     got = ctx.submap_download(gt)
     for x, y, what in zip(exp, got, ("block indices", "distance", "weight")):
-        _same(x, y, what)
+        same_bits(x, y, what)
     # the reported RMSE equals the restatement on the two ESDFs
     p = next(_ids)
     ctx.project_map([map_id], T, p)
@@ -487,11 +441,12 @@ def test_map_evaluate_errors_leave_everything(ctx, scene):
     other = next(_ids)
     ctx.submap_upload(other, 0.2, 16, lay[2], lay[3], lay[4])
     T = _offset_T()[None]
-    cases = [(next(_ids), [map_id], T, -3),               # unknown ground truth
-             (gt, [next(_ids)], T, -3),                    # unknown submap
-             (gt, [gt], T, -1),                            # the ground truth among the submaps
-             (gt, [other], T, -1),                         # voxel size differs
-             (gt, [map_id, map_id], np.repeat(T, 2, 0), -1)]   # a projection refusal: repeated id
+    INVALID, NOT_FOUND = _lib.VGX_ERR_INVALID, _lib.VGX_ERR_NOT_FOUND
+    cases = [(next(_ids), [map_id], T, NOT_FOUND),                  # unknown ground truth
+             (gt, [next(_ids)], T, NOT_FOUND),                      # unknown submap
+             (gt, [gt], T, INVALID),                                # the ground truth among the submaps
+             (gt, [other], T, INVALID),                             # voxel size differs
+             (gt, [map_id, map_id], np.repeat(T, 2, 0), INVALID)]   # a projection refusal: repeated id
     for g, ids, poses, code in cases:
         with pytest.raises(api.VgxError) as e:
             ctx.map_evaluate(g, ids, poses)

@@ -11,33 +11,12 @@ import pytest
 
 import finish_exact as fx
 import mesh_exact as me
-from test_oracle_finish import MATRIX
-from voxgraph_b200 import synth
+from finish_exact import MATRIX
+from support import ctx, same_bits  # noqa: F401
+from voxgraph_b200 import _lib, synth
 
 pytestmark = pytest.mark.gpu
 _ids = itertools.count(9000)
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
-
-
-def _same(exp, got, what):
-    """Bit-equal arrays, NaN equal to NaN whatever its payload."""
-    exp = np.asarray(exp); got = np.asarray(got)
-    assert exp.shape == got.shape, (what, exp.shape, got.shape)
-    if exp.dtype == np.float32:
-        ne, ng = np.isnan(exp), np.isnan(got)
-        assert np.array_equal(ne, ng), (what, "NaN positions")
-        exp = np.where(ne, 0, exp).astype(np.float32); got = np.where(ng, 0, got).astype(np.float32)
-        fx.assert_bits(exp, got, what)
-    else:
-        bad = np.nonzero(exp != got)
-        assert bad[0].size == 0, (what, "first difference at", bad[0][:1], exp[bad][:3], got[bad][:3])
 
 
 def _check(ctx, layers, poses=None, min_weight=1.0, upload=True, ids=None):
@@ -50,8 +29,8 @@ def _check(ctx, layers, poses=None, min_weight=1.0, upload=True, ids=None):
     xyz, tri, vo, to = api.separated_mesh(ctx, ids, poses, min_weight)
     ex, et, evo, eto = me.separated([fx.Grid(*lay) for lay in layers], poses, min_weight)
     assert vo.tolist() == evo.tolist() and to.tolist() == eto.tolist()
-    _same(ex, xyz, "vertices")
-    _same(et, tri, "triangles")
+    same_bits(ex, xyz, "vertices")
+    same_bits(et, tri, "triangles")
     return ids, xyz, tri
 
 
@@ -68,7 +47,7 @@ def test_matrix_in_one_build(ctx):
     T = np.stack([synth.pose_to_T([*rs.uniform(-5, 5, 3), rs.uniform(-3, 3)]) for _ in layers]).astype(np.float32)
     ctx.profile_reset()
     ids, xyz, tri = _check(ctx, layers, T)
-    ms, launches = ctx.profile_get(12)
+    ms, launches = ctx.profile_get(_lib.VGX_SLOT_MESH)
     assert launches == 11      # count, scan (3), popcount, scan (3), offsets, vertices, triangles
     assert len(tri) > 10000
     for sid in ids:
@@ -166,7 +145,7 @@ def test_separated_mesh_poses_and_mixed_resolutions(ctx):
     from voxgraph_b200 import api
     xyz0, tri0, _, _ = api.separated_mesh(ctx, ids, None, 1.0)
     ex, et, _, _ = me.separated([fx.Grid(*lay) for lay in layers], None, 1.0)
-    _same(ex, xyz0, "submap frame"); _same(et, tri0, "submap frame triangles")
+    same_bits(ex, xyz0, "submap frame"); same_bits(et, tri0, "submap frame triangles")
     for sid in ids:
         ctx.submap_free(sid)
 
@@ -185,7 +164,7 @@ def test_errors_release_and_ply_paths(ctx):
     data = ctx.mesh_ply()
     assert bytes(data) == bytes(ctx.mesh_ply(np.stack([api.submap_colour(a), api.submap_colour(b)])))
     px, prgba, ptri = me.read_ply(data)
-    _same(xyz, px, "ply vertices")
+    same_bits(xyz, px, "ply vertices")
     assert np.array_equal(ptri, tri.astype(np.int64))
     for k, sid in enumerate((a, b)):
         assert (prgba[vo[k]:vo[k + 1]] == api.submap_colour(sid)).all()
@@ -194,18 +173,19 @@ def test_errors_release_and_ply_paths(ctx):
     size = C.c_uint64(0)
     assert L.vgx_mesh_ply(h, None, None, 0, C.byref(size)) == 0 and size.value == len(data)
     buf = (C.c_char * len(data))()
-    assert L.vgx_mesh_ply(h, None, buf, len(data) - 1, C.byref(size)) == -6 and size.value == len(data)
+    assert L.vgx_mesh_ply(h, None, buf, len(data) - 1, C.byref(size)) == _lib.VGX_ERR_CAPACITY
+    assert size.value == len(data)
     assert L.vgx_mesh_ply(h, None, buf, len(data), C.byref(size)) == 0 and bytes(buf) == bytes(data)
     # download capacity and NULL outputs
     nv, nt = C.c_int64(0), C.c_int64(0)
     small = np.zeros((len(xyz) - 1, 3), np.float32)
     assert L.vgx_mesh_download(h, len(xyz) - 1, small.ctypes.data_as(C.POINTER(C.c_float)), 0, None,
-                               C.byref(nv), C.byref(nt)) == -6
+                               C.byref(nv), C.byref(nt)) == _lib.VGX_ERR_CAPACITY
     assert nv.value == len(xyz) and nt.value == len(tri)
     # unknown id: VGX_ERR_NOT_FOUND and an empty mesh
     with pytest.raises(api.VgxError) as e:
         ctx.mesh_build([a, 4242424242], None, cfg)
-    assert e.value.code == -3
+    assert e.value.code == _lib.VGX_ERR_NOT_FOUND
     x2, t2 = ctx.mesh_download()
     assert len(x2) == 0 and len(t2) == 0
     # n = 0 releases the buffer; the PLY of nothing is a header
@@ -277,5 +257,5 @@ def test_mapper_save_separated_mesh(tmp_path):
     ax, at = m.activeSubmapMesh()
     idx, d, w = c.submap_download(m.active_id)
     ex, et = me.mesh(fx.Grid(0.2, 16, idx, d, w), 2.0)
-    _same(ex, ax, "active submap"); _same(et.astype(np.uint32), at, "active submap triangles")
+    same_bits(ex, ax, "active submap"); same_bits(et.astype(np.uint32), at, "active submap triangles")
     c.close()

@@ -13,46 +13,14 @@ import pytest
 import finish_exact as fx
 import mesh_exact as me
 import project_oracle as po
-from test_oracle_finish import MATRIX
-from voxgraph_b200 import synth
+from finish_exact import MATRIX
+from support import IDENTITY, ctx, exists, poses_for, same_bits, yaw_T  # noqa: F401
+from voxgraph_b200 import _lib, synth
 
 pytestmark = pytest.mark.gpu
 _ids = itertools.count(20000)
 F32 = np.float32
-IDENTITY = np.array([1, 0, 0, 0, 0, 0, 0], F32)
-SLOT = 13
 LAUNCHES = 15    # candidates, sort, flags, 2 scans (3 each), scatter, occupancy, scan (3), fold
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
-
-
-def _same(exp, got, what):
-    """Bit-equal arrays, NaN equal to NaN whatever its payload."""
-    exp = np.asarray(exp); got = np.asarray(got)
-    assert exp.shape == got.shape, (what, exp.shape, got.shape)
-    if exp.dtype == np.float32:
-        ne, ng = np.isnan(exp), np.isnan(got)
-        assert np.array_equal(ne, ng), (what, "NaN positions")
-        exp = np.where(ne, 0, exp).astype(F32); got = np.where(ng, 0, got).astype(F32)
-        fx.assert_bits(exp, got, what)
-    else:
-        assert np.array_equal(exp, got), (what, exp[:3], got[:3])
-
-
-def _exists(ctx, sid):
-    from voxgraph_b200 import api
-    try:
-        ctx.submap_info(sid)
-        return True
-    except api.VgxError as e:
-        assert e.code == -3
-        return False
 
 
 def _oracle(oracle, layers, poses, ids):
@@ -76,38 +44,24 @@ def _check(ctx, oracle, layers, poses, ids=None, upload=True):
     if exp is None:
         with pytest.raises(api.VgxError) as e:
             ctx.project_map(ids, poses, out)
-        assert e.value.code == -1 and not _exists(ctx, out)
+        assert e.value.code == _lib.VGX_ERR_INVALID and not exists(ctx, out)
         return ids, None
     n = ctx.project_map(ids, poses, out)
     vs, vps, nb, fin = ctx.submap_info(out)
     assert fin and nb == n == len(exp[0]) and vps == layers[0][1] and vs == F32(layers[0][0])
     got = ctx.submap_download(out)
     ctx.submap_free(out)
-    _same(exp[0], got[0], "block indices")
-    _same(exp[1], got[1], "distance")
-    _same(exp[2], got[2], "weight")
+    same_bits(exp[0], got[0], "block indices")
+    same_bits(exp[1], got[1], "distance")
+    same_bits(exp[2], got[2], "weight")
     return ids, got
-
-
-def _yaw_T(yaw, t=(0.0, 0.0, 0.0)):
-    return np.array([np.cos(yaw / 2), 0, 0, np.sin(yaw / 2), *t], F32)
-
-
-def _poses_for(vs, vps):
-    bs = float(F32(vs) * vps)
-    rs = np.random.RandomState(int(vs * 1000) + vps)
-    q = rs.normal(size=4); q /= np.linalg.norm(q)
-    return {"identity": IDENTITY,
-            "translation": np.array([1, 0, 0, 0, 2 * bs, -bs, 0.37 * bs], F32),
-            "yaw": _yaw_T(0.7, (0.3 * bs, 0.1 * bs, 0.0)),
-            "random": np.array([*q, *rs.uniform(-bs, bs, 3)], F32)}
 
 
 @pytest.mark.parametrize("case", range(len(MATRIX)), ids=[m[0] for m in MATRIX])
 def test_matrix(ctx, oracle, case):
     lay = MATRIX[case][1]
     ids = None
-    for name, T in _poses_for(lay[0], lay[1]).items():
+    for name, T in poses_for(lay[0], lay[1]).items():
         ids, _ = _check(ctx, oracle, [lay], T[None], ids=ids, upload=ids is None)
     ctx.submap_free(ids[0])
 
@@ -125,7 +79,7 @@ def _overlapping(vs, vps, n, seed):
         w[rs.uniform(size=w.shape) < 0.05] = 0
         d[rs.uniform(size=d.shape) < 0.002] = np.nan
         layers.append((vs, vps, lay[2], d, w))
-        poses.append(_yaw_T(rs.uniform(-0.5, 0.5), rs.uniform(-0.5 * bs, 0.5 * bs, 3)))
+        poses.append(yaw_T(rs.uniform(-0.5, 0.5), rs.uniform(-0.5 * bs, 0.5 * bs, 3)))
     return layers, np.stack(poses)
 
 
@@ -160,7 +114,7 @@ def test_device_integrated_active_and_finished(ctx, oracle, mode):
     ctx.submap_finish_ex(a, ctx.registration_filter(min_voxel_weight=1e-6))   # b stays active
     assert ctx.submap_info(a)[3] and not ctx.submap_info(b)[3]
     layers = [(0.2, 16, *ctx.submap_download(s)) for s in (a, b)]
-    T = np.stack([_yaw_T(0.0), _yaw_T(0.3, (0.4, -0.2, 0.0))])
+    T = np.stack([yaw_T(0.0), yaw_T(0.3, (0.4, -0.2, 0.0))])
     _, got = _check(ctx, oracle, layers, T, ids=[a, b], upload=False)
     assert len(got[0]) > 20 and (got[2] > 0).sum() > 1000
     ctx.submap_free(a); ctx.submap_free(b)
@@ -180,21 +134,21 @@ def test_errors_leave_nothing(ctx):
 
     before = state()
     shift = IDENTITY.copy(); shift[4] = 2 * 1.6     # two blocks of 1.6 along x
-    cases = [([a, 4242424242], -3, out),                # unknown id
-             ([a], -1, a),                              # out_id is an input
-             ([a], -1, b),                              # out_id exists
-             ([a, b], -1, out),                         # voxel size differs
-             ([a, c8], -1, out),                        # voxels per side differ
-             ([a, a], -1, out),                         # repeated id
-             ([], -1, out),                             # n < 1
-             ([far], -1, out)]                          # candidates beyond VGX_BLOCK_INDEX_MAX
+    cases = [([a, 4242424242], _lib.VGX_ERR_NOT_FOUND, out),  # unknown id
+             ([a], _lib.VGX_ERR_INVALID, a),                  # out_id is an input
+             ([a], _lib.VGX_ERR_INVALID, b),                  # out_id exists
+             ([a, b], _lib.VGX_ERR_INVALID, out),             # voxel size differs
+             ([a, c8], _lib.VGX_ERR_INVALID, out),            # voxels per side differ
+             ([a, a], _lib.VGX_ERR_INVALID, out),             # repeated id
+             ([], _lib.VGX_ERR_INVALID, out),                 # n < 1
+             ([far], _lib.VGX_ERR_INVALID, out)]              # candidates beyond VGX_BLOCK_INDEX_MAX
     for ids, code, oid in cases:
         T = np.tile(shift if ids == [far] else IDENTITY, (len(ids), 1))
         with pytest.raises(api.VgxError) as e:
             ctx.project_map(ids, T, oid)
         assert e.value.code == code, (ids, oid, e.value)
         if oid == out:
-            assert not _exists(ctx, out)
+            assert not exists(ctx, out)
     assert state() == before
     # an empty submap projects to an empty map
     e = next(_ids)
@@ -213,7 +167,7 @@ def test_launch_count_and_determinism(ctx, oracle):
     ctx.profile_enable(True)
     out = next(_ids)
     ctx.project_map(ids, poses, out)
-    ms, launches = ctx.profile_get(SLOT)
+    ms, launches = ctx.profile_get(_lib.VGX_SLOT_PROJECT)
     ctx.profile_enable(False)
     assert launches == LAUNCHES and ms > 0
     again = ctx.submap_download(out)
@@ -228,7 +182,7 @@ def test_combined_mesh_equals_restatement(ctx, oracle):
     from voxgraph_b200 import api
     layers = [fx.layer((0.1, 16), "box", "sphere"), fx.layer((0.1, 16), "box", "tilted"),
               fx.layer((0.1, 16), "checker", "plane")]
-    T = np.stack([_yaw_T(0.0), _yaw_T(0.4, (0.3, -0.2, 0.05)), _yaw_T(-0.2, (-0.5, 0.4, 0.0))])
+    T = np.stack([yaw_T(0.0), yaw_T(0.4, (0.3, -0.2, 0.05)), yaw_T(-0.2, (-0.5, 0.4, 0.0))])
     ids = [next(_ids) for _ in layers]
     for sid, lay in zip(ids, layers):
         ctx.submap_upload(sid, *lay)
@@ -236,15 +190,15 @@ def test_combined_mesh_equals_restatement(ctx, oracle):
     for min_weight in (1.0, 2.0):
         xyz, tri = api.combined_mesh(ctx, ids, T, min_weight)
         ex, et = me.mesh(fx.Grid(0.1, 16, idx, d, w), min_weight)
-        _same(ex, xyz, "combined vertices")
-        _same(et.astype(np.uint32), tri, "combined triangles")
+        same_bits(ex, xyz, "combined vertices")
+        same_bits(et.astype(np.uint32), tri, "combined triangles")
         assert len(tri) > 0
-        assert not _exists(ctx, api.PROJECTION_SCRATCH_ID)
+        assert not exists(ctx, api.PROJECTION_SCRATCH_ID)
     # projected_map returns the same layer and frees its scratch submap
     got = api.projected_map(ctx, ids, T)
     for x, y in zip((idx, d, w), got):
         assert np.asarray(x).tobytes() == y.tobytes()
-    assert not _exists(ctx, api.PROJECTION_SCRATCH_ID)
+    assert not exists(ctx, api.PROJECTION_SCRATCH_ID)
     for sid in ids:
         ctx.submap_free(sid)
 
@@ -295,5 +249,5 @@ def test_mapper_save_combined_mesh(tmp_path):
     xyz, rgba, tri = me.read_ply(data)
     assert len(tri) > 0 and (rgba == 255).all()
     ax, at = m.combinedMesh()
-    _same(xyz, ax, "mapper combined mesh")
+    same_bits(xyz, ax, "mapper combined mesh")
     c.close()

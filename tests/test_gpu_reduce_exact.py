@@ -11,122 +11,14 @@ import numpy as np
 import pytest
 
 import reduce_exact as RX
+from reduce_exact import GRID_MAX_CELLS, Problem, check_eval
+from support import ctx, oracle_layer  # noqa: F401
 from voxgraph_b200 import synth
 
 pytestmark = pytest.mark.gpu
 
-GRID_MAX_CELLS = 4096   # larger block AABBs get no block grid (submap.cu, VGX_GRID_MAX_CELLS)
 RAGGED = (1, 31, 32, 33, 95, 2047, 2048, 2049, 3000, 5000)
 PI_F = float(np.float32(np.pi))
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
-
-
-class Problem:
-    """Submaps (uploaded to the device and mirrored as oracle layers), nodes and registration
-    constraints; builds the PoseGraph at exact-trig poses and the exact reference."""
-
-    def __init__(self, ctx, oracle):
-        self.ctx, self.oracle = ctx, oracle
-        self.sub = {}
-        self.nodes = {}      # sid -> (base pose, constant)
-        self.cons = []
-
-    def submap(self, sid, vs, vps, idx, d, w, iso=None, vox=None, esdf=False):
-        from voxgraph_b200 import api
-        o = self.oracle
-        self.ctx.submap_upload(sid, vs, vps, idx, d, w)
-        e = dict(layer=o.Layer.from_blocks(vs, vps, idx, d, w), pts={})
-        for ptype, pts in ((api.K_ISOSURFACE_POINTS, iso), (api.K_VOXELS, vox)):
-            if pts is not None:
-                pts = tuple(np.ascontiguousarray(a, np.float32) for a in pts)
-                self.ctx.submap_upload_points(sid, ptype, *pts)
-                e["pts"][ptype] = pts
-        if esdf:
-            self.ctx.submap_generate_esdf(sid)
-            eo, obo, _ = o.generate_esdf(e["layer"])
-            e["esdf"] = o.Layer.from_blocks(vs, vps, idx, eo, obo)
-        self.sub[sid] = e
-
-    def synth_submap(self, s, sid=None, **kw):
-        sid = s.submap_id if sid is None else sid
-        self.submap(sid, s.voxel_size, s.vps, s.block_idx, s.distance, s.weight,
-                    iso=(s.points_xyz, s.points_distance, s.points_weight), **kw)
-
-    def node(self, sid, pose, constant=False):
-        self.nodes[sid] = (np.asarray(pose, np.float64), constant)
-
-    def constrain(self, a, b, **kw):
-        from voxgraph_b200 import api
-        self.cons.append(api.RegistrationConstraintConfig(a, b, **kw))
-
-    def build(self, seed, fixed=None, sigma=(0.03, 0.03, 0.02, 0.01)):
-        """Draw exact-trig poses, build the PoseGraph (node order = sorted submap ids)."""
-        from voxgraph_b200 import api
-        ids = sorted(self.nodes)
-        col = {s: k for k, s in enumerate(ids)}
-        pairs = []
-        for c in self.cons:
-            a, b = col[c.first_submap_id], col[c.second_submap_id]
-            pairs += [(a, b), (b, a)]
-        fx = {col[s]: p for s, p in (fixed or {}).items()}
-        self.x = RX.exact_trig_poses(np.array([self.nodes[s][0] for s in ids]), pairs,
-                                     np.random.default_rng(seed), sigma=sigma, fixed=fx)
-        self.col = col
-        pg = api.PoseGraph(self.ctx)
-        for s in ids:
-            pg.addSubmapNode(api.SubmapNodeConfig(s, self.x[col[s]], set_constant=self.nodes[s][1]))
-        for c in self.cons:
-            pg.addRegistrationConstraint(c)
-        pg._sync()
-        self.pg = pg
-        return pg
-
-    def exact(self, emit=True):
-        """Exact sums of the oracle's terms over pg.registration_blocks; each non-sampled block is
-        also checked bit for bit against emit mode at the same poses."""
-        o, ctx, pg = self.oracle, self.ctx, self.pg
-        ex = RX.Exact(len(self.col))
-        self.n_terms = 0
-        for k, ((a, b), cfg) in enumerate(zip(pg.registration_blocks, pg._reg_cfgs)):
-            ia, ib = self.col[a], self.col[b]
-            ref, read = self.x[ia], self.x[ib]
-            RX.check_pose_block(o, ref, read)
-            xyz, d, w = self.sub[a]["pts"][cfg.registration_point_type]
-            layer = self.sub[b]["esdf" if cfg.use_esdf_distance else "layer"]
-            nc = cfg.no_correspondence_cost
-            if cfg.sampling_ratio != -1.0:
-                K = o.sampled_num_residuals(cfg.sampling_ratio, len(w))
-                idx = ctx.graph_get_sample_indices(k, K)
-                assert len(idx) == K
-                ok, r, jr, je = o.reg_evaluate_sampled(layer, xyz, d, idx, ref, read, no_correspondence_cost=nc)
-            else:
-                ok, r, jr, je = o.reg_evaluate(layer, xyz, d, w, ref, read, no_correspondence_cost=nc)
-                if emit:
-                    ok_g, r_g, jr_g, je_g = ctx.reg_eval_emit(a, b, ref, read, cfg)
-                    assert ok_g and np.array_equal(r_g, r) and np.array_equal(jr_g, jr) and \
-                        np.array_equal(je_g, je), "emit mode differs from the oracle on block %d" % k
-            assert ok
-            ex.add_block(ia, ib, r, jr, je)
-            self.n_terms += len(r)
-        ex.finish()
-        return ex
-
-
-def _check_eval(pb, ex, label, costs=True):
-    ok, cost, g, H = pb.pg.evaluate()
-    assert ok
-    worst = RX.check_bound(ex, cost, g, H, label=label)
-    if costs:
-        worst = max(worst, RX.check_costs_bound(ex, pb.pg.getVisualizationEdgeResiduals(), label=label + " costs"))
-    print("%s: max |fused - exact| / bound = %.3g over %d residuals" % (label, worst, pb.n_terms))
-    return worst
 
 
 # --------------------------------------------------------------------------- scenes
@@ -201,7 +93,7 @@ def test_baseline_small_scene(ctx, oracle, small_scene):
     pb.build(seed=1, fixed=fixed)
     assert pb.x[0, 3] == 0.0 and abs(pb.x[5, 3]) < RX.SERIES_THETA
     ex = pb.exact()
-    _check_eval(pb, ex, "baseline")
+    check_eval(pb, ex, "baseline")
 
 
 # --------------------------------------------------------------------------- 2. tile shapes
@@ -232,7 +124,7 @@ def test_tile_shapes(ctx, tile_problem, monkeypatch, tile_units):
     assert pg.registration_blocks == pg0.registration_blocks
     pb.pg = pg
     try:
-        _check_eval(pb, ex, "tile_units=%s" % tile_units, costs=(tile_units in ("1", "2", "129")))
+        check_eval(pb, ex, "tile_units=%s" % tile_units, costs=(tile_units in ("1", "2", "129")))
     finally:
         pb.pg = pg0
 
@@ -297,7 +189,7 @@ def cull_problem(ctx, oracle):
 def test_culling_edges(ctx, oracle):
     pb, _ = cull_problem(ctx, oracle)
     ex = pb.exact()
-    _check_eval(pb, ex, "culling edges")
+    check_eval(pb, ex, "culling edges")
 
 
 # --------------------------------------------------------------------------- 4. options
@@ -316,7 +208,7 @@ def test_constraint_options(ctx, oracle, small_scene):
     pb = Problem(ctx, oracle)
     for i in range(4):
         s = sc.submaps[i]
-        vx, vd, vw = oracle.find_relevant_voxels(pb_layer(oracle, s), 1.0, 0.3)
+        vx, vd, vw = oracle.find_relevant_voxels(oracle_layer(oracle, s), 1.0, 0.3)
         pb.submap(100 + i, s.voxel_size, s.vps, s.block_idx, s.distance, s.weight,
                   iso=(s.points_xyz, s.points_distance, s.points_weight), vox=(vx, vd, vw), esdf=True)
         pb.node(100 + i, sc.poses_init[i], constant=(i == 0))
@@ -345,8 +237,4 @@ def test_constraint_options(ctx, oracle, small_scene):
         pb.constrain(200 + 2 * k, 201 + 2 * k)
     pb.build(seed=4, fixed={100: sc.poses_init[0]})
     ex = pb.exact()
-    _check_eval(pb, ex, "constraint options")
-
-
-def pb_layer(oracle, s):
-    return oracle.Layer.from_blocks(s.voxel_size, s.vps, s.block_idx, s.distance, s.weight)
+    check_eval(pb, ex, "constraint options")

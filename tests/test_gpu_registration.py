@@ -2,23 +2,12 @@
 import numpy as np
 import pytest
 
+from support import ctx, oracle_layer  # noqa: F401
 from voxgraph_b200 import synth
 
 pytestmark = pytest.mark.gpu
 
 VS, VPS = 0.2, 16
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
-
-
-def _olayer(oracle, s):
-    return oracle.Layer.from_blocks(s.voxel_size, s.vps, s.block_idx, s.distance, s.weight)
 
 
 def _bit_equal(a, b):
@@ -31,7 +20,7 @@ def test_emit_bit_exact_pair_scene(ctx, oracle, pair_scene):
         ctx.upload_synth_submap(s)
     s0, s1 = pair_scene.submaps
     for (a, b) in ((s0, s1), (s1, s0)):
-        layer = _olayer(oracle, b)
+        layer = oracle_layer(oracle, b)
         ia, ib = a.submap_id, b.submap_id
         ref, read = pair_scene.poses_init[ia], pair_scene.poses_init[ib]
         ok_o, r_o, jr_o, je_o = oracle.reg_evaluate(layer, a.points_xyz, a.points_distance,
@@ -52,7 +41,7 @@ def test_emit_bit_exact_many_poses(ctx, oracle, small_scene):
     sc = small_scene
     for s in sc.submaps:
         ctx.upload_synth_submap(s)
-    layers = [_olayer(oracle, s) for s in sc.submaps]
+    layers = [oracle_layer(oracle, s) for s in sc.submaps]
     rs = np.random.RandomState(0)
     n_checked = 0
     for (i, j) in sc.pairs:
@@ -179,7 +168,7 @@ def _build_graphs(ctx, oracle, sc, api):
         ctx.upload_synth_submap(s)
     pg = api.PoseGraph(ctx)
     og = oracle.Graph()
-    layers = [_olayer(oracle, s) for s in sc.submaps]
+    layers = [oracle_layer(oracle, s) for s in sc.submaps]
     for i, s in enumerate(sc.submaps):
         pg.addSubmapNode(api.SubmapNodeConfig(i, sc.poses_init[i], set_constant=(i == 0)))
         og.add_node(i, sc.poses_init[i], constant=(i == 0))
@@ -271,7 +260,7 @@ def test_emit_sampling_mode_bit_exact(ctx, oracle, pair_scene):
     for s in pair_scene.submaps:
         ctx.upload_synth_submap(s)      # fresh upload = fresh default-seeded generator
     s0, s1 = pair_scene.submaps
-    layer = _olayer(oracle, s1)
+    layer = oracle_layer(oracle, s1)
     sampler = oracle.WeightedSampler(s0.points_weight)
     ref, read = pair_scene.poses_init[0], pair_scene.poses_init[1]
     for ratio in (0.2, 0.05, 0.2):
@@ -295,7 +284,7 @@ def test_graph_sampling_mode_matches_oracle(ctx, oracle, small_scene):
         ctx.upload_synth_submap(s)
     pg = api.PoseGraph(ctx)
     og = oracle.Graph()
-    layers = [_olayer(oracle, s) for s in sc.submaps]
+    layers = [oracle_layer(oracle, s) for s in sc.submaps]
     for i, s in enumerate(sc.submaps):
         pg.addSubmapNode(api.SubmapNodeConfig(i, sc.poses_init[i], set_constant=(i == 0)))
         og.add_node(i, sc.poses_init[i], constant=(i == 0))

@@ -24,21 +24,14 @@ import finish_exact as fx
 import reduce_exact as RX
 import registration_layers as RL
 import tsdf_exact as tx
-from test_gpu_reduce_exact import GRID_MAX_CELLS, Problem, _check_eval
+from finish_exact import MATRIX
+from reduce_exact import GRID_MAX_CELLS, Problem, check_eval
+from support import ctx  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
-MATRIX = fx.matrix()
 _ids = itertools.count(3000)
 PI_F = float(np.float32(np.pi))
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
 
 
 def _reference_points(xyz, ref, read):
@@ -183,7 +176,7 @@ def test_fused_layouts_both_loops(ctx, oracle, res):
         for label, fixed in (("identity", poses), ("random", {400: np.zeros(4)})):
             pb.build(seed=7, fixed=fixed)
             ex = pb.exact()
-            _check_eval(pb, ex, "%g/%d %s type=%d nc=%g" % (res[0], res[1], label, point_type, nc))
+            check_eval(pb, ex, "%g/%d %s type=%d nc=%g" % (res[0], res[1], label, point_type, nc))
 
 
 @pytest.mark.parametrize("nc", [0.0, 0.3])
@@ -205,7 +198,7 @@ def test_fused_far_translation_aliases_nothing(ctx, oracle, nc):
         ok, r, _, _ = oracle.reg_evaluate(pb.sub[b]["layer"], xyz, d, w, pb.x[pb.col[a]], pb.x[pb.col[b]],
                                           no_correspondence_cost=float("nan"), jacobians=False)
         assert ok and np.isnan(r).all(), "block %d: a correspondence 2^21 blocks away" % k
-    _check_eval(pb, ex, "far translation nc=%g" % nc)
+    check_eval(pb, ex, "far translation nc=%g" % nc)
     if nc == 0.0:
         ok, cost, g, H = pb.pg.evaluate()
         assert ok and cost == 0.0 and not np.any(g) and not np.any(H)

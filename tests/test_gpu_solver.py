@@ -2,21 +2,10 @@
 import numpy as np
 import pytest
 
+from support import ctx, oracle_layer  # noqa: F401
 from voxgraph_b200 import synth
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
-
-
-def _olayer(oracle, s):
-    return oracle.Layer.from_blocks(s.voxel_size, s.vps, s.block_idx, s.distance, s.weight)
 
 
 def _wrap(a):
@@ -84,7 +73,7 @@ def test_self_registration_ka5(ctx, oracle, pair_scene, pert):
     og = oracle.Graph()
     og.add_node(0, s.pose_gt, constant=True)
     og.add_node(1, s.pose_gt + np.array(pert))
-    og.add_registration(0, 1, _olayer(oracle, s), s.points_xyz, s.points_distance, s.points_weight)
+    og.add_registration(0, 1, oracle_layer(oracle, s), s.points_xyz, s.points_distance, s.points_weight)
     rc, so = og.solve(oracle.solver_options(parameter_tolerance=3e-9, max_num_iterations=40))
     xg = pg.getSubmapPoses()[11]; xo = og.poses()[1]
     err = xg - s.pose_gt
@@ -98,7 +87,7 @@ def _graphs(ctx, oracle, sc, api):
     for s in sc.submaps:
         ctx.upload_synth_submap(s)
     pg = api.PoseGraph(ctx); og = oracle.Graph()
-    layers = [_olayer(oracle, s) for s in sc.submaps]
+    layers = [oracle_layer(oracle, s) for s in sc.submaps]
     for i in range(len(sc.submaps)):
         pg.addSubmapNode(api.SubmapNodeConfig(i, sc.poses_init[i], set_constant=(i == 0)))
         og.add_node(i, sc.poses_init[i], constant=(i == 0))

@@ -2,20 +2,13 @@
 import numpy as np
 import pytest
 
-from voxgraph_b200 import synth
+from support import ctx  # noqa: F401
+from voxgraph_b200 import _lib, synth
 
 pytestmark = pytest.mark.gpu
 
 VS = 0.2
 IDENT = np.array([1, 0, 0, 0, 0, 0, 0], np.float32)
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
 
 
 def _as_dict(idx, d, w):
@@ -196,14 +189,14 @@ def test_capacity_overflow_reports_error(ctx):
     pts = np.array([[10.0, 3.0, 1.0], [-8.0, 2.0, 0.5]], np.float32)
     with pytest.raises(api.VgxError) as e:
         ctx.tsdf_integrate(305, IDENT, pts, ctx.tsdf_config())
-    assert e.value.code == -6
+    assert e.value.code == _lib.VGX_ERR_CAPACITY
     # the overflow leaves a consistent submap behind (hash rebuilt from the blocks that exist):
     # further calls keep failing cleanly instead of hanging on a full table, in both modes
     assert ctx.submap_block_count(305) == 2
     for mode in (1, 0, 1):
         with pytest.raises(api.VgxError) as e:
             ctx.tsdf_integrate(305, IDENT, pts, ctx.tsdf_config(mode=mode))
-        assert e.value.code == -6
+        assert e.value.code == _lib.VGX_ERR_CAPACITY
     far = np.array([[60.0, 3.0, 1.0], [-70.0, 2.0, 0.5], [5.0, 80.0, 9.0]], np.float32)
     with pytest.raises(api.VgxError):
         ctx.tsdf_integrate(305, IDENT, far, ctx.tsdf_config(mode=1, max_ray_length_m=100.0))

@@ -12,20 +12,13 @@ import numpy as np
 import pytest
 
 import tsdf_exact as tx
-from voxgraph_b200 import synth
+from support import ctx  # noqa: F401
+from voxgraph_b200 import _lib, synth
 
 pytestmark = pytest.mark.gpu
 
 _ids = itertools.count(2000)
 FAST_ALL = dict(mode=1, start_voxel_subsampling_factor=1e3, max_consecutive_ray_collisions=1 << 30)
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from voxgraph_b200 import api
-    c = api.Context(0)
-    yield c
-    c.close()
 
 
 @pytest.fixture(scope="module")
@@ -257,7 +250,7 @@ def test_capacity_at_the_edge(ctx, oracle, world, mode):
             else:
                 with pytest.raises(api.VgxError) as e:
                     ctx.tsdf_integrate(sid, T, pts, ctx.tsdf_config(**kw))
-                assert e.value.code == -6
+                assert e.value.code == _lib.VGX_ERR_CAPACITY
             assert ctx.submap_block_count(sid) == cap
             gi = ctx.submap_download(sid)[0]
             assert len(gi) == cap and set(map(tuple, gi.tolist())) <= oset

@@ -6,28 +6,15 @@ import subprocess
 import numpy as np
 import pytest
 
+from support import compile_cpp_mirror
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FIXTURE = os.path.join(ROOT, "tests", "golden", "layer_tsdf.bin")
 
 
-def _compile(tmp_path):
-    from voxgraph_b200 import build
-    build.build()
-    exe = str(tmp_path / "map_evaluation_test")
-    lib_dir = os.path.join(ROOT, "voxgraph_b200")
-    cmd = ["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"),
-           "-I" + os.path.join(ROOT, "voxgraph_b200", "host"),
-           os.path.join(ROOT, "tests", "cpp", "map_evaluation_test.cpp"), "-o", exe,
-           "-L" + lib_dir, "-lvoxgraph_b200", "-Wl,-rpath," + lib_dir]
-    env = dict(os.environ); env.pop("CXX", None)
-    p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env)
-    assert p.returncode == 0, p.stdout
-    return exe
-
-
 def test_cpp_map_evaluation_compiles_and_refuses_cpu(tmp_path):
     import torch
-    exe = _compile(tmp_path)
+    exe = compile_cpp_mirror(tmp_path, "map_evaluation_test.cpp")
     if torch.cuda.is_available():
         pytest.skip("GPU present: covered by the gpu test")
     p = subprocess.run([exe, FIXTURE], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
@@ -40,7 +27,7 @@ def test_cpp_and_python_report_the_same_evaluation():
     from voxgraph_b200 import api
     with tempfile.TemporaryDirectory() as tmp:
         import pathlib
-        exe = _compile(pathlib.Path(tmp))
+        exe = compile_cpp_mirror(pathlib.Path(tmp), "map_evaluation_test.cpp")
         p = subprocess.run([exe, FIXTURE], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,
                            timeout=300)
     assert p.returncode == 0 and "MAPEVAL_OK" in p.stdout, p.stdout

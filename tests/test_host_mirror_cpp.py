@@ -1,32 +1,16 @@
 """The C++ host mirror (voxgraph_b200/host/voxgraph_b200.hpp) compiles against the C-ABI with plain
 g++ (the reference is C++: this is the layer a maintainer links); on a GPU it must reproduce the
 closed-form plane residuals, solve, and integrate a scan."""
-import os
 import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _compile(tmp_path):
-    from voxgraph_b200 import build
-    build.build()
-    exe = str(tmp_path / "host_mirror_test")
-    lib_dir = os.path.join(ROOT, "voxgraph_b200")
-    cmd = ["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"),
-           "-I" + os.path.join(ROOT, "voxgraph_b200", "host"),
-           os.path.join(ROOT, "tests", "cpp", "host_mirror_test.cpp"), "-o", exe,
-           "-L" + lib_dir, "-lvoxgraph_b200", "-Wl,-rpath," + lib_dir]
-    env = dict(os.environ); env.pop("CXX", None)
-    p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env)
-    assert p.returncode == 0, p.stdout
-    return exe
+from support import compile_cpp_mirror
 
 
 def test_cpp_mirror_compiles_and_refuses_cpu(tmp_path):
     import torch
-    exe = _compile(tmp_path)
+    exe = compile_cpp_mirror(tmp_path, "host_mirror_test.cpp")
     if torch.cuda.is_available():
         pytest.skip("GPU present: covered by the gpu test")
     p = subprocess.run([exe], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
@@ -35,6 +19,6 @@ def test_cpp_mirror_compiles_and_refuses_cpu(tmp_path):
 
 @pytest.mark.gpu
 def test_cpp_mirror_on_gpu(tmp_path):
-    exe = _compile(tmp_path)
+    exe = compile_cpp_mirror(tmp_path, "host_mirror_test.cpp")
     p = subprocess.run([exe], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=300)
     assert p.returncode == 0 and "HOST_MIRROR_OK" in p.stdout, p.stdout

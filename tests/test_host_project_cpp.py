@@ -6,28 +6,15 @@ import subprocess
 
 import pytest
 
+from support import compile_cpp_mirror
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FIXTURE = os.path.join(ROOT, "tests", "golden", "collection_unpacked.bin")
 
 
-def _compile(tmp_path):
-    from voxgraph_b200 import build
-    build.build()
-    exe = str(tmp_path / "combined_mesh_test")
-    lib_dir = os.path.join(ROOT, "voxgraph_b200")
-    cmd = ["g++", "-std=c++17", "-O2", "-I" + os.path.join(ROOT, "include"),
-           "-I" + os.path.join(ROOT, "voxgraph_b200", "host"),
-           os.path.join(ROOT, "tests", "cpp", "combined_mesh_test.cpp"), "-o", exe,
-           "-L" + lib_dir, "-lvoxgraph_b200", "-Wl,-rpath," + lib_dir]
-    env = dict(os.environ); env.pop("CXX", None)
-    p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env)
-    assert p.returncode == 0, p.stdout
-    return exe
-
-
 def test_cpp_combined_mesh_compiles_and_refuses_cpu(tmp_path):
     import torch
-    exe = _compile(tmp_path)
+    exe = compile_cpp_mirror(tmp_path, "combined_mesh_test.cpp")
     if torch.cuda.is_available():
         pytest.skip("GPU present: covered by the gpu test")
     p = subprocess.run([exe, FIXTURE, str(tmp_path / "out.ply")], stdout=subprocess.PIPE,
@@ -38,7 +25,7 @@ def test_cpp_combined_mesh_compiles_and_refuses_cpu(tmp_path):
 @pytest.mark.gpu
 def test_cpp_and_python_write_the_same_combined_ply(tmp_path):
     from voxgraph_b200 import api
-    exe = _compile(tmp_path)
+    exe = compile_cpp_mirror(tmp_path, "combined_mesh_test.cpp")
     out = tmp_path / "cpp.ply"
     p = subprocess.run([exe, FIXTURE, str(out)], stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True,
                        timeout=300)

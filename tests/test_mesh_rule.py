@@ -1,20 +1,14 @@
 """The submap mesh rule (tests/mesh_exact.py, restated by vgx_mesh_build) on the CPU: the face-walk
 triangulation over all 256 cube configurations, closed and consistently oriented surfaces on analytic
 fields, vertex accuracy, open boundaries only where the valid region ends, the shared-edge property
-over the finishSubmap layer matrix, the palette, and the layout of vgx_mesh_config."""
-import ctypes as C
-import os
-import subprocess
-
+over the finishSubmap layer matrix, and the palette."""
 import numpy as np
 import pytest
 
 import finish_exact as fx
 import mesh_exact as me
-from test_oracle_finish import MATRIX
+from finish_exact import MATRIX
 from voxgraph_b200 import synth
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 # --------------------------------------------------------------------------- the rule over 256 configurations
@@ -206,16 +200,3 @@ def test_palette():
         assert api.submap_colour(i).tolist() == me.rainbow((i % 20) / 20.0)
     assert api.submap_colour(2 ** 32 - 1).tolist() == me.rainbow(((2 ** 32 - 1) % 20) / 20.0)
     assert len({tuple(api.submap_colour(i)) for i in range(20)}) == 20
-
-
-def test_mesh_config_layout(tmp_path):
-    """The ctypes mirror of vgx_mesh_config against the C compiler's view of the header."""
-    from voxgraph_b200 import _lib
-    src = tmp_path / "layout.c"
-    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "voxgraph_b200.h"\nint main(void) {\n'
-                   'printf("%zu %zu\\n", sizeof(vgx_mesh_config), offsetof(vgx_mesh_config, min_weight));\n'
-                   'return 0;\n}\n')
-    exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-I" + os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
-    size, off = map(int, subprocess.run([str(exe)], check=True, stdout=subprocess.PIPE, text=True).stdout.split())
-    assert size == C.sizeof(_lib.MeshConfig) == 4 and off == _lib.MeshConfig.min_weight.offset == 0

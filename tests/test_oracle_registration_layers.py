@@ -16,8 +16,8 @@ import pytest
 
 import finish_exact as fx
 import registration_layers as RL
+from finish_exact import MATRIX
 
-MATRIX = fx.matrix()
 IDENTITY = np.zeros(4)
 
 

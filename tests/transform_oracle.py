@@ -1,19 +1,13 @@
 """ctypes front-end of tests/transform_oracle.c, the CPU restatement of voxblox transformLayer into a submap's
 own layer (VoxgraphSubmap::transformSubmap) that vgx_submap_transform is checked against.  Compiled on first use
 into a temporary directory (never into the tree) and linked against oracle/libvg_oracle.so."""
-import atexit
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
 from oracle import oracle as o
+from support import build_oracle_harness
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_ROOT = os.path.dirname(_HERE)
 _lib = None
 
 
@@ -21,20 +15,7 @@ def lib():
     global _lib
     if _lib is not None:
         return _lib
-    o.lib()   # builds and loads oracle/libvg_oracle.so first
-    odir = os.path.join(_ROOT, "oracle")
-    tmp = tempfile.mkdtemp(prefix="vgx_transform_oracle_")
-    atexit.register(shutil.rmtree, tmp, True)
-    so = os.path.join(tmp, "libvg_transform_oracle.so")
-    env = dict(os.environ)
-    env.pop("CC", None)
-    cmd = ["gcc", "-O2", "-ffp-contract=off", "-fno-fast-math", "-fPIC", "-shared", "-std=c11", "-Wall", "-Wextra",
-           "-I" + odir, os.path.join(_HERE, "transform_oracle.c"), "-o", so, "-L" + odir, "-lvg_oracle",
-           "-Wl,-rpath," + odir, "-lm"]
-    p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env)
-    if p.returncode != 0:
-        raise RuntimeError("building tests/transform_oracle.c failed:\n" + p.stdout)
-    L = C.CDLL(so)
+    L = build_oracle_harness("transform_oracle.c", "libvg_transform_oracle.so")
     L.vgt_transform_layer.restype = C.c_void_p
     L.vgt_transform_layer.argtypes = [C.c_void_p, C.c_float, C.c_int, C.POINTER(C.c_float)]
     _lib = L

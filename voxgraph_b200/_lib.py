@@ -18,6 +18,24 @@ VGX_ERR_NOMEM = -4
 VGX_ERR_NCCL = -5
 VGX_ERR_CAPACITY = -6
 
+# vgx_profile_get's `which` (enum VgxProfileSlotId)
+VGX_SLOT_REG_REDUCE = 0
+VGX_SLOT_REG_EMIT = 1
+VGX_SLOT_TSDF_INTEGRATE = 2
+VGX_SLOT_TSDF_ALLOCATE = 3
+VGX_SLOT_SOLVE = 4
+VGX_SLOT_OTHER = 5
+VGX_SLOT_REG_POSE_SETUP = 6
+VGX_SLOT_REG_SUMS = 7
+VGX_SLOT_ASSEMBLY = 8
+VGX_SLOT_COLL_CODEC = 9
+VGX_SLOT_COLL_COPY = 10
+VGX_SLOT_COLL_UPLOAD = 11
+VGX_SLOT_MESH = 12
+VGX_SLOT_PROJECT = 13
+VGX_SLOT_EVAL = 14
+VGX_PROFILE_SLOTS = 15
+
 
 class TsdfConfig(C.Structure):
     _fields_ = [("default_truncation_distance", C.c_float),

@@ -147,26 +147,7 @@ struct VgxRelEdge {
 
 struct VgxGraph;  // defined in graph.h
 
-// vgx_profile_get's `which` (documented in voxgraph_b200.h); the values are part of the C-ABI
-enum VgxProfileSlotId {
-  VGX_SLOT_REG_REDUCE = 0,       // registration reduce kernel
-  VGX_SLOT_REG_EMIT = 1,         // registration emit kernel
-  VGX_SLOT_TSDF_INTEGRATE = 2,
-  VGX_SLOT_TSDF_ALLOCATE = 3,
-  VGX_SLOT_SOLVE = 4,            // Cholesky / LM kernels
-  VGX_SLOT_OTHER = 5,            // everything else
-  VGX_SLOT_REG_POSE_SETUP = 6,
-  VGX_SLOT_REG_SUMS = 7,         // per-constraint sums
-  VGX_SLOT_ASSEMBLY = 8,         // normal equations (+ the fused peer exchange)
-  VGX_SLOT_COLL_CODEC = 9,       // submap collection decode / encode kernels
-  VGX_SLOT_COLL_COPY = 10,       // submap collection stream copies (host <-> device)
-  VGX_SLOT_COLL_UPLOAD = 11,     // submap collection upload (block hash, registration view, grid)
-  VGX_SLOT_MESH = 12,
-  VGX_SLOT_PROJECT = 13,
-  VGX_SLOT_EVAL = 14,            // map evaluation kernels
-  VGX_PROFILE_SLOTS = 15
-};
-struct VgxProfileSlot {
+struct VgxProfileSlot {   // one per VgxProfileSlotId (voxgraph_b200.h)
   double total_ms = 0;
   int64_t launches = 0;
 };
