@@ -712,11 +712,11 @@ struct EventPair {
 
 int copy_h2d_chunked(vgx_ctx* c, uint8_t* d, const uint8_t* h, uint64_t n) {
   if (n == 0) return VGX_OK;
-  int rc = c->ensure_pinned(2 * kChunk);
+  uint8_t* stage;
+  int rc = vgx_carve(c, c->h_pinned, vgx_part(stage, 2 * kChunk));
   if (rc != VGX_OK) return rc;
   EventPair ev;
   if ((rc = ev.init(c)) != VGX_OK) return rc;
-  uint8_t* stage = (uint8_t*)c->h_pinned;
   uint64_t off = 0;
   for (int k = 0; off < n; ++k) {
     const size_t len = (size_t)std::min<uint64_t>(kChunk, n - off);
@@ -733,11 +733,11 @@ int copy_h2d_chunked(vgx_ctx* c, uint8_t* d, const uint8_t* h, uint64_t n) {
 
 int copy_d2h_chunked(vgx_ctx* c, uint8_t* h, const uint8_t* d, uint64_t n) {
   if (n == 0) return VGX_OK;
-  int rc = c->ensure_pinned(2 * kChunk);
+  uint8_t* stage;
+  int rc = vgx_carve(c, c->h_pinned, vgx_part(stage, 2 * kChunk));
   if (rc != VGX_OK) return rc;
   EventPair ev;
   if ((rc = ev.init(c)) != VGX_OK) return rc;
-  uint8_t* stage = (uint8_t*)c->h_pinned;
   const uint64_t chunks = (n + kChunk - 1) / kChunk;
   for (uint64_t k = 0; k <= chunks; ++k) {
     if (k < chunks) {   // enqueue chunk k, then drain chunk k - 1 while it runs
@@ -784,20 +784,19 @@ extern "C" int vgx_collection_scan(const uint8_t* bytes, uint64_t n, int max_sub
 static int decode_layout(vgx_ctx* c, const char* what, const CollLayout& L, const uint8_t* bytes, uint64_t n) {
   VGX_CUDA(c, cudaSetDevice(c->device));
   const int vpb = (int)(L.vps * L.vps * L.vps);
-  const size_t table_bytes = (L.blocks.size() * sizeof(CollBlockRef) + 15) & ~(size_t)15;
-  const size_t bytes_off = table_bytes + 16;   // [regions | error word | stream bytes]
-  int rc = c->ensure_scratch(bytes_off + (size_t)n);
+  CollBlockRef* d_regions;
+  int* d_err;
+  uint8_t* d_bytes;
+  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_regions, L.blocks.size()), vgx_part(d_err, 1),
+                     vgx_part(d_bytes, (size_t)n));
   if (rc != VGX_OK) return rc;
-  uint8_t* d = (uint8_t*)c->d_scratch;
-  CollBlockRef* d_regions = (CollBlockRef*)d;
-  int* d_err = (int*)(d + table_bytes);
   {
     VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
     if (!L.blocks.empty())
       VGX_CUDA(c, cudaMemcpyAsync(d_regions, L.blocks.data(), L.blocks.size() * sizeof(CollBlockRef),
                                   cudaMemcpyHostToDevice, c->stream));
     VGX_CUDA(c, cudaMemsetAsync(d_err, 0, sizeof(int), c->stream));
-    rc = copy_h2d_chunked(c, d + bytes_off, bytes, n);
+    rc = copy_h2d_chunked(c, d_bytes, bytes, n);
     if (rc != VGX_OK) return rc;
   }
   for (const CollSubmapRef& s : L.submaps) {
@@ -809,7 +808,7 @@ static int decode_layout(vgx_ctx* c, const char* what, const CollLayout& L, cons
     if (s.n_blocks == 0) continue;
     {
       VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
-      const cudaError_t e = cudaMemcpyAsync(sm->d_block_idx, L.block_idx.data() + 3 * s.first_block,
+      const cudaError_t e = cudaMemcpyAsync(sm->d_block_idx.get(), L.block_idx.data() + 3 * s.first_block,
                                             sizeof(int32_t) * 3 * s.n_blocks, cudaMemcpyHostToDevice, c->stream);
       if (e != cudaSuccess) {
         c->set_error(std::string(what) + ": " + cudaGetErrorString(e));
@@ -818,7 +817,7 @@ static int decode_layout(vgx_ctx* c, const char* what, const CollLayout& L, cons
     }
     VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
     collection_decode_kernel<<<s.n_blocks, COLL_THREADS, 0, c->stream>>>(
-        d + bytes_off, d_regions + s.first_block, vpb, reinterpret_cast<float*>(sm->d_dw), d_err);
+        d_bytes, d_regions + s.first_block, vpb, reinterpret_cast<float*>(sm->d_dw.get()), d_err);
   }
   int h_err = 0;
   cudaError_t e = cudaGetLastError();
@@ -893,19 +892,19 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
   size_t total_blocks = 0;
   for (VgxSubmap* s : subs) total_blocks += (size_t)s->n_blocks;
   // scratch: [payload sizes | block offsets | block messages]
-  const size_t sizes_bytes = (total_blocks * sizeof(uint32_t) + 15) & ~(size_t)15;
-  const size_t offs_bytes = total_blocks * sizeof(uint64_t);
-  int rc = c->ensure_scratch(sizes_bytes + offs_bytes);
+  uint32_t* d_sizes;
+  uint64_t* d_offs;
+  uint8_t* d_msgs;
+  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_sizes, total_blocks), vgx_part(d_offs, total_blocks));
   if (rc != VGX_OK) return rc;
-  uint32_t* d_sizes = (uint32_t*)c->d_scratch;
   CollEncodeArgs a{};
   a.vps = vps;
   a.header_bytes = hdr;
   size_t first = 0;
   for (VgxSubmap* s : subs) {
     if (s->n_blocks > 0) {
-      a.dw = s->d_dw;
-      a.block_idx = s->d_block_idx;
+      a.dw = s->d_dw.get();
+      a.block_idx = s->d_block_idx.get();
       a.vox_per_block = s->vox_per_block;
       a.out_sizes = d_sizes + first;
       VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
@@ -942,11 +941,10 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
   *size = total;
   if (!out) return VGX_OK;
   if (capacity < total) VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_collection_save: capacity too small");
-  rc = c->ensure_scratch(sizes_bytes + offs_bytes + (size_t)dev_bytes);
+  // the second carve of d_scratch may move it: the sizes are re-sent
+  rc = vgx_carve(c, c->d_scratch, vgx_part(d_sizes, total_blocks), vgx_part(d_offs, total_blocks),
+                 vgx_part(d_msgs, (size_t)dev_bytes));
   if (rc != VGX_OK) return rc;
-  d_sizes = (uint32_t*)c->d_scratch;   // ensure_scratch may have moved the buffer: the sizes are re-sent
-  uint64_t* d_offs = (uint64_t*)((uint8_t*)c->d_scratch + sizes_bytes);
-  uint8_t* d_msgs = (uint8_t*)c->d_scratch + sizes_bytes + offs_bytes;
   if (total_blocks) {
     VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
     VGX_CUDA(c, cudaMemcpyAsync(d_sizes, sizes.data(), total_blocks * sizeof(uint32_t), cudaMemcpyHostToDevice,
@@ -958,8 +956,8 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
   first = 0;
   for (VgxSubmap* s : subs) {
     if (s->n_blocks > 0) {
-      a.dw = s->d_dw;
-      a.block_idx = s->d_block_idx;
+      a.dw = s->d_dw.get();
+      a.block_idx = s->d_block_idx.get();
       a.vox_per_block = s->vox_per_block;
       a.voxel_size = s->voxel_size;
       a.block_size = s->block_size;

@@ -120,14 +120,11 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
   if (!(dc.max_distance_m > 0) || !(dc.min_distance_m >= 0))
     VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_generate_esdf: invalid distances");
   vgx_graph_invalidate_registration(c);
-  cudaFree(s->d_esdf); s->d_esdf = nullptr;
-  cudaFree(s->d_view_esdf); s->d_view_esdf = nullptr;
+  s->d_esdf.reset();
+  s->d_view_esdf.reset();
   const size_t nvox = (size_t)s->n_blocks * s->vox_per_block;
   if (sweeps_out) *sweeps_out = 0;
-  if (nvox == 0) {
-    VGX_CUDA(c, cudaMalloc((void**)&s->d_view_esdf, 32));
-    return VGX_OK;
-  }
+  if (nvox == 0) return s->d_view_esdf.alloc(c, 32, "ESDF registration view");
   EsdfParams P;
   P.voxel_size = s->voxel_size;
   P.max_distance = dc.max_distance_m; P.default_distance = dc.default_distance_m;
@@ -136,18 +133,17 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
   P.sh = s->sh;
   P.n_blocks = s->n_blocks;
   cudaStream_t st = c->stream;
-  VGX_CUDA(c, cudaMalloc((void**)&s->d_esdf, sizeof(float2) * nvox));
-  // scratch: fixed mask | neighbour table | changed flag
-  const size_t fixed_b = (nvox + 255) & ~(size_t)255;
-  const size_t nb_b = ((size_t)27 * s->n_blocks * sizeof(int) + 255) & ~(size_t)255;
-  int rc = c->ensure_sort(fixed_b + nb_b + 256);
+  int rc = s->d_esdf.alloc(c, sizeof(float2) * nvox, "ESDF bricks");
   if (rc != VGX_OK) return rc;
-  unsigned char* d_fixed = (unsigned char*)c->d_sort;
-  int* d_nb = (int*)((char*)c->d_sort + fixed_b);
-  int* d_changed = (int*)((char*)c->d_sort + fixed_b + nb_b);
+  unsigned char* d_fixed;
+  int *d_nb, *d_changed;
+  rc = vgx_carve(c, c->d_work, vgx_part(d_fixed, nvox), vgx_part(d_nb, (size_t)27 * s->n_blocks),
+                 vgx_part(d_changed, 1));
+  if (rc != VGX_OK) return rc;
   const unsigned grid = (unsigned)((nvox + 255) / 256);
-  esdf_init_kernel<<<grid, 256, 0, st>>>(P, s->d_dw, s->d_esdf, d_fixed);
-  esdf_neighbours_kernel<<<(27 * s->n_blocks + 127) / 128, 128, 0, st>>>(s->hash, s->d_block_idx, s->n_blocks, d_nb);
+  esdf_init_kernel<<<grid, 256, 0, st>>>(P, s->d_dw.get(), s->d_esdf.get(), d_fixed);
+  esdf_neighbours_kernel<<<(27 * s->n_blocks + 127) / 128, 128, 0, st>>>(s->hash(), s->d_block_idx.get(), s->n_blocks,
+                                                                          d_nb);
   c->launches += 2;
   // relax to convergence: the flag is read back every other sweep
   int sweeps = 0;
@@ -155,7 +151,7 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
   for (;;) {
     VGX_CUDA(c, cudaMemsetAsync(d_changed, 0, sizeof(int), st));
     for (int k = 0; k < 2; ++k) {
-      esdf_sweep_kernel<<<grid, 256, 0, st>>>(P, s->d_esdf, d_fixed, d_nb, d_changed);
+      esdf_sweep_kernel<<<grid, 256, 0, st>>>(P, s->d_esdf.get(), d_fixed, d_nb, d_changed);
       c->launches++;
       ++sweeps;
     }
@@ -168,8 +164,9 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
   VGX_CUDA(c, cudaGetLastError());
   if (sweeps_out) *sweeps_out = sweeps;
   // registration view of the ESDF layer (observed <=> weight 1), same octet layout as the TSDF view
-  VGX_CUDA(c, cudaMalloc((void**)&s->d_view_esdf, sizeof(float) * 8 * nvox));
-  rc = vgx_submap_build_view(c, s, s->d_esdf, s->d_view_esdf);
+  rc = s->d_view_esdf.alloc(c, sizeof(float) * 8 * nvox, "ESDF registration view");
+  if (rc != VGX_OK) return rc;
+  rc = vgx_submap_build_view(c, s, s->d_esdf.get(), s->d_view_esdf.get());
   if (rc != VGX_OK) return rc;
   VGX_CUDA(c, cudaStreamSynchronize(st));
   return VGX_OK;
@@ -180,7 +177,7 @@ extern "C" int vgx_submap_download_esdf(vgx_ctx* c, uint32_t id, int max_blocks,
   if (!c) return VGX_ERR_INVALID;
   VgxSubmap* s = c->find(id);
   if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_download_esdf: unknown submap");
-  if (!s->d_esdf && s->n_blocks > 0) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_download_esdf: no ESDF generated");
+  if (!s->d_esdf.get() && s->n_blocks > 0) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_download_esdf: no ESDF generated");
   VGX_CUDA(c, cudaSetDevice(c->device));
   const int n = s->n_blocks;
   if (n_out) *n_out = n;
@@ -188,7 +185,7 @@ extern "C" int vgx_submap_download_esdf(vgx_ctx* c, uint32_t id, int max_blocks,
   if (n == 0) return VGX_OK;
   const size_t nvox = (size_t)n * s->vox_per_block;
   std::vector<float2> h(nvox);
-  VGX_CUDA(c, cudaMemcpyAsync(h.data(), s->d_esdf, sizeof(float2) * nvox, cudaMemcpyDeviceToHost, c->stream));
+  VGX_CUDA(c, cudaMemcpyAsync(h.data(), s->d_esdf.get(), sizeof(float2) * nvox, cudaMemcpyDeviceToHost, c->stream));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   for (size_t i = 0; i < nvox; ++i) {
     if (distance) distance[i] = h[i].x;

@@ -134,11 +134,11 @@ static int rmse_layer(vgx_ctx* c, VgxSubmap* s, int which, const char* name, Rms
   if (which != VGX_LAYER_TSDF && which != VGX_LAYER_ESDF)
     VGX_FAIL(c, VGX_ERR_INVALID, std::string("vgx_evaluate_layers_rmse: unknown layer selector for the ") + name);
   if (!s->finished) VGX_FAIL(c, VGX_ERR_INVALID, std::string("vgx_evaluate_layers_rmse: the ") + name + " is not finished");
-  if (which == VGX_LAYER_ESDF && !s->d_view_esdf)
+  if (which == VGX_LAYER_ESDF && !s->d_view_esdf.get())
     VGX_FAIL(c, VGX_ERR_INVALID, std::string("vgx_evaluate_layers_rmse: the ") + name + " has no ESDF");
-  L->hash = s->hash;
-  L->dw = which == VGX_LAYER_ESDF ? s->d_esdf : s->d_dw;
-  L->block_idx = s->d_block_idx;
+  L->hash = s->hash();
+  L->dw = which == VGX_LAYER_ESDF ? s->d_esdf.get() : s->d_dw.get();
+  L->block_idx = s->d_block_idx.get();
   L->n_blocks = s->n_blocks;
   L->esdf = which == VGX_LAYER_ESDF;
   return VGX_OK;
@@ -164,9 +164,9 @@ extern "C" int vgx_evaluate_layers_rmse(vgx_ctx* c, uint32_t gt_id, int gt_layer
   RmsePartial total;
   memset(&total, 0, sizeof(total));
   if (n_part > 0) {
-    rc = c->ensure_sort(sizeof(RmsePartial) * (n_part + 1));
+    RmsePartial* d_part;
+    rc = vgx_carve(c, c->d_work, vgx_part(d_part, n_part + 1));
     if (rc != VGX_OK) return rc;
-    RmsePartial* d_part = (RmsePartial*)c->d_sort;
     cudaStream_t st = c->stream;
     const int threads = std::min(RMSE_THREADS, g->vox_per_block);
     {

@@ -323,25 +323,24 @@ __global__ void unpack_points_kernel(const float* __restrict__ pts, int n, float
 }
 
 // ------------------------------------------------------------------ host orchestration
-// takes ownership of d_pts (n points, unit-major, zero padded); weights come back to the host once
-// for the sampler's cumulative sums and summed_reference_weight (cpp:124), in point order
-static int install_points(vgx_ctx* c, VgxSubmap* s, int type, float* d_pts, int n) {
+// takes d_pts (n points, unit-major, zero padded) over; weights come back to the host once for the
+// sampler's cumulative sums and summed_reference_weight (cpp:124), in point order
+static int install_points(vgx_ctx* c, VgxSubmap* s, int type, VgxBuffer<float>&& d_pts, int n) {
   VgxPoints& p = s->points[type];
-  if (p.data) cudaFree(p.data);
   p = VgxPoints();
   if (n == 0) {
-    cudaFree(d_pts);
+    d_pts.reset();
     return VGX_OK;
   }
   std::vector<float> w((size_t)n);
-  int rc = c->ensure_scratch(sizeof(float) * (size_t)n);
-  if (rc != VGX_OK) { cudaFree(d_pts); return rc; }
-  gather_weights_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(d_pts, n, (float*)c->d_scratch);
+  float* d_w;
+  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_w, (size_t)n));
+  if (rc != VGX_OK) return rc;
+  gather_weights_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(d_pts.get(), n, d_w);
   c->launches++;
-  cudaError_t e = cudaMemcpyAsync(w.data(), c->d_scratch, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, c->stream);
+  cudaError_t e = cudaMemcpyAsync(w.data(), d_w, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, c->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
   if (e != cudaSuccess) {
-    cudaFree(d_pts);
     c->set_error(std::string("registration point extraction: ") + cudaGetErrorString(e));
     return VGX_ERR_CUDA;
   }
@@ -349,16 +348,16 @@ static int install_points(vgx_ctx* c, VgxSubmap* s, int type, float* d_pts, int 
   double sum = 0;
   for (int i = 0; i < n; ++i) { sum += (double)w[i]; p.cumulative_w[i] = sum; }
   p.n = n;
-  p.data = d_pts;
+  p.data = std::move(d_pts);
   p.sum_w = sum;
   return VGX_OK;
 }
 
-static int alloc_points(vgx_ctx* c, int n, float** out) {
-  *out = nullptr;
+static int alloc_points(vgx_ctx* c, int n, VgxBuffer<float>& out) {
   const size_t units = ((size_t)std::max(n, 1) + VGX_PT_UNIT - 1) / VGX_PT_UNIT;
-  VGX_CUDA(c, cudaMalloc((void**)out, units * VGX_PT_UNIT_FLOATS * sizeof(float)));
-  VGX_CUDA(c, cudaMemsetAsync(*out, 0, units * VGX_PT_UNIT_FLOATS * sizeof(float), c->stream));
+  const int rc = out.alloc(c, units * VGX_PT_UNIT_FLOATS * sizeof(float), "registration points");
+  if (rc != VGX_OK) return rc;
+  VGX_CUDA(c, cudaMemsetAsync(out.get(), 0, units * VGX_PT_UNIT_FLOATS * sizeof(float), c->stream));
   return VGX_OK;
 }
 
@@ -377,7 +376,7 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
   vgx_registration_filter f;
   vgx_registration_filter_default(&f);
   if (filter) f = *filter;
-  if (f.use_esdf_distance && !s->d_esdf && s->n_blocks > 0)
+  if (f.use_esdf_distance && !s->d_esdf.get() && s->n_blocks > 0)
     VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_extract_points: use_esdf_distance needs the submap's ESDF "
                                  "(vgx_submap_generate_esdf first, as finishSubmap does)");
   VGX_CUDA(c, cudaSetDevice(c->device));
@@ -386,29 +385,22 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
   const size_t nvox = (size_t)s->n_blocks * s->vox_per_block;
   s->surface_obb_valid = false;
   s->iso_blocks.clear();
-  cudaFree(s->d_iso_idx);
-  s->d_iso_idx = nullptr;
+  s->d_iso_idx.reset();
   s->n_iso = 0;
   s->points_extracted = true;
   if (nvox == 0) {
-    int rc = install_points(c, s, VGX_POINTS_VOXELS, nullptr, 0);
-    if (rc == VGX_OK) rc = install_points(c, s, VGX_POINTS_ISOSURFACE, nullptr, 0);
+    int rc = install_points(c, s, VGX_POINTS_VOXELS, VgxBuffer<float>(), 0);
+    if (rc == VGX_OK) rc = install_points(c, s, VGX_POINTS_ISOSURFACE, VgxBuffer<float>(), 0);
     return rc;
   }
   if (nvox >= 0xFFFFFFFFull / 12) VGX_FAIL(c, VGX_ERR_CAPACITY, "submap too large for 32-bit candidate indices");
   cudaStream_t st = c->stream;
-  // scratch: counts | offsets (+1) | scan tmp | obb[6] | block flags
-  const size_t cnt_b = ((nvox + 1) * sizeof(unsigned) + 255) & ~(size_t)255;
-  const size_t tmp_b = (vgx_scan_tmp_count(nvox * 12) * sizeof(unsigned) + 255) & ~(size_t)255;
-  const size_t flag_b = ((size_t)s->n_blocks * sizeof(unsigned) + 255) & ~(size_t)255;
-  int rc = c->ensure_sort(2 * cnt_b + tmp_b + 256 + flag_b);
+  unsigned *d_counts, *d_offsets, *d_tmp, *d_flags;
+  float* d_obb;
+  int rc = vgx_carve(c, c->d_work, vgx_part(d_counts, nvox + 1), vgx_part(d_offsets, nvox + 1),
+                     vgx_part(d_tmp, vgx_scan_tmp_count(nvox * 12)), vgx_part(d_obb, 6),
+                     vgx_part(d_flags, (size_t)s->n_blocks));
   if (rc != VGX_OK) return rc;
-  char* base = (char*)c->d_sort;
-  unsigned* d_counts = (unsigned*)base;
-  unsigned* d_offsets = (unsigned*)(base + cnt_b);
-  unsigned* d_tmp = (unsigned*)(base + 2 * cnt_b);
-  float* d_obb = (float*)(base + 2 * cnt_b + tmp_b);
-  unsigned* d_flags = (unsigned*)(base + 2 * cnt_b + tmp_b + 256);
   const unsigned grid256 = (unsigned)((nvox + 255) / 256), grid128 = (unsigned)((nvox + 127) / 128);
 
   // ---- relevant voxels + surface OBB
@@ -423,11 +415,11 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
     unsigned total = 0;
     VGX_CUDA(c, cudaMemcpyAsync(&total, d_offsets + nvox, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     VGX_CUDA(c, cudaStreamSynchronize(st));
-    float* d_pts = nullptr;
-    rc = alloc_points(c, (int)total, &d_pts);
+    VgxBuffer<float> d_pts;
+    rc = alloc_points(c, (int)total, d_pts);
     if (rc != VGX_OK) return rc;
-    relevant_emit_kernel<<<grid256, 256, 0, st>>>(L, d_counts, d_offsets, f.use_esdf_distance ? s->d_esdf : nullptr,
-                                                 d_pts, d_obb);
+    relevant_emit_kernel<<<grid256, 256, 0, st>>>(L, d_counts, d_offsets, f.use_esdf_distance ? s->d_esdf.get() : nullptr,
+                                                 d_pts.get(), d_obb);
     c->launches++;
     VGX_CUDA(c, cudaGetLastError());
     float obb[6];
@@ -435,7 +427,7 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
     VGX_CUDA(c, cudaStreamSynchronize(st));
     for (int a = 0; a < 3; ++a) { s->surface_obb_min[a] = obb[a]; s->surface_obb_max[a] = obb[3 + a]; }
     s->surface_obb_valid = total > 0;
-    rc = install_points(c, s, VGX_POINTS_VOXELS, d_pts, (int)total);
+    rc = install_points(c, s, VGX_POINTS_VOXELS, std::move(d_pts), (int)total);
     if (rc != VGX_OK) return rc;
   }
   // ---- isosurface vertices
@@ -451,25 +443,19 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
     VGX_CUDA(c, cudaMemcpyAsync(&M, d_offsets + nvox, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     VGX_CUDA(c, cudaStreamSynchronize(st));
     unsigned kept = 0;
-    float* d_pts = nullptr;
+    VgxBuffer<float> d_pts;
     if (M > 0) {
       size_t tsize = 1024;
       while (tsize < 2 * (size_t)M) tsize <<= 1;
-      const size_t cand_b = ((size_t)M * 3 * sizeof(float) + 255) & ~(size_t)255;
-      const size_t key_b = ((size_t)M * sizeof(unsigned long long) + 255) & ~(size_t)255;
-      const size_t keep_b = (((size_t)M + 1) * sizeof(unsigned) + 255) & ~(size_t)255;
-      const size_t dw_b = ((size_t)M * sizeof(float2) + 255) & ~(size_t)255;
-      const size_t tmp2_b = (vgx_scan_tmp_count(M) * sizeof(unsigned) + 255) & ~(size_t)255;
-      rc = c->ensure_sort2(cand_b + key_b + 2 * keep_b + dw_b + tmp2_b + tsize * sizeof(IsoBucket));
+      IsoBucket* d_table;
+      float* d_cand;
+      unsigned long long* d_key;
+      unsigned *d_keep, *d_koff, *d_tmp2;
+      float2* d_cdw;
+      rc = vgx_carve(c, c->d_work2, vgx_part(d_table, tsize), vgx_part(d_cand, (size_t)M * 3), vgx_part(d_key, M),
+                     vgx_part(d_keep, (size_t)M + 1), vgx_part(d_koff, (size_t)M + 1), vgx_part(d_cdw, M),
+                     vgx_part(d_tmp2, vgx_scan_tmp_count(M)));
       if (rc != VGX_OK) return rc;
-      char* b2 = (char*)c->d_sort2;
-      IsoBucket* d_table = (IsoBucket*)b2;
-      float* d_cand = (float*)(b2 + tsize * sizeof(IsoBucket));
-      unsigned long long* d_key = (unsigned long long*)((char*)d_cand + cand_b);
-      unsigned* d_keep = (unsigned*)((char*)d_key + key_b);
-      unsigned* d_koff = (unsigned*)((char*)d_keep + keep_b);
-      float2* d_cdw = (float2*)((char*)d_koff + keep_b);
-      unsigned* d_tmp2 = (unsigned*)((char*)d_cdw + dw_b);
       iso_table_clear_kernel<<<(unsigned)((tsize + 255) / 256), 256, 0, st>>>(d_table, tsize);
       iso_emit_kernel<<<grid128, 128, 0, st>>>(L, min_weight, threshold_inv, d_counts, d_offsets, d_cand, d_key,
                                               d_table, tsize - 1);
@@ -479,10 +465,10 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
       if (rc != VGX_OK) return rc;
       VGX_CUDA(c, cudaMemcpyAsync(&kept, d_koff + M, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
       VGX_CUDA(c, cudaStreamSynchronize(st));
-      rc = alloc_points(c, (int)kept, &d_pts);
+      rc = alloc_points(c, (int)kept, d_pts);
       if (rc != VGX_OK) return rc;
-      VGX_CUDA(c, cudaMemsetAsync(d_flags, 0, flag_b, st));
-      iso_compact_kernel<<<(M + 127) / 128, 128, 0, st>>>(L, d_cand, d_cdw, d_keep, d_koff, M, d_pts, d_flags);
+      VGX_CUDA(c, cudaMemsetAsync(d_flags, 0, sizeof(unsigned) * (size_t)s->n_blocks, st));
+      iso_compact_kernel<<<(M + 127) / 128, 128, 0, st>>>(L, d_cand, d_cdw, d_keep, d_koff, M, d_pts.get(), d_flags);
       c->launches++;
       VGX_CUDA(c, cudaGetLastError());
       // isosurface block list (slots, ascending) for overlapsWith
@@ -494,22 +480,23 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
         if (flags[b]) s->iso_blocks.push_back(b);
       if (!s->iso_blocks.empty()) {
         std::vector<int32_t> bidx(3 * (size_t)s->n_blocks), iso(3 * s->iso_blocks.size());
-        VGX_CUDA(c, cudaMemcpyAsync(bidx.data(), s->d_block_idx, sizeof(int32_t) * bidx.size(),
+        VGX_CUDA(c, cudaMemcpyAsync(bidx.data(), s->d_block_idx.get(), sizeof(int32_t) * bidx.size(),
                                     cudaMemcpyDeviceToHost, st));
         VGX_CUDA(c, cudaStreamSynchronize(st));
         for (size_t k = 0; k < s->iso_blocks.size(); ++k)
           for (int a = 0; a < 3; ++a) iso[3 * k + a] = bidx[3 * (size_t)s->iso_blocks[k] + a];
-        VGX_CUDA(c, cudaMalloc((void**)&s->d_iso_idx, sizeof(int32_t) * iso.size()));
-        VGX_CUDA(c, cudaMemcpyAsync(s->d_iso_idx, iso.data(), sizeof(int32_t) * iso.size(),
+        rc = s->d_iso_idx.alloc(c, sizeof(int32_t) * iso.size(), "isosurface block list");
+        if (rc != VGX_OK) return rc;
+        VGX_CUDA(c, cudaMemcpyAsync(s->d_iso_idx.get(), iso.data(), sizeof(int32_t) * iso.size(),
                                     cudaMemcpyHostToDevice, st));
         VGX_CUDA(c, cudaStreamSynchronize(st));
         s->n_iso = (int)s->iso_blocks.size();
       }
     } else {
-      rc = alloc_points(c, 0, &d_pts);
+      rc = alloc_points(c, 0, d_pts);
       if (rc != VGX_OK) return rc;
     }
-    rc = install_points(c, s, VGX_POINTS_ISOSURFACE, d_pts, (int)kept);
+    rc = install_points(c, s, VGX_POINTS_ISOSURFACE, std::move(d_pts), (int)kept);
     if (rc != VGX_OK) return rc;
   }
   return VGX_OK;
@@ -540,12 +527,10 @@ extern "C" int vgx_submap_download_points(vgx_ctx* c, uint32_t id, int type, int
   if (p.n == 0) return VGX_OK;
   VGX_CUDA(c, cudaSetDevice(c->device));
   const size_t n = (size_t)p.n;
-  int rc = c->ensure_scratch(5 * n * sizeof(float));
+  float *d_xyz, *d_d, *d_w;
+  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_xyz, 3 * n), vgx_part(d_d, n), vgx_part(d_w, n));
   if (rc != VGX_OK) return rc;
-  float* d_xyz = (float*)c->d_scratch;
-  float* d_d = d_xyz + 3 * n;
-  float* d_w = d_d + n;
-  unpack_points_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(p.data, p.n, d_xyz, d_d, d_w);
+  unpack_points_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(p.data.get(), p.n, d_xyz, d_d, d_w);
   c->launches++;
   if (xyz) VGX_CUDA(c, cudaMemcpyAsync(xyz, d_xyz, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
   if (distance) VGX_CUDA(c, cudaMemcpyAsync(distance, d_d, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));

@@ -19,37 +19,9 @@
 #include "registration.cuh"
 #include "registration_kernels.h"
 
-static void free_tables(VgxGraph* g) {
-  cudaFree(g->d_cons); cudaFree(g->d_poses); cudaFree(g->d_tiles); cudaFree(g->d_tile_begin);
-  cudaFree(g->d_unit_bounds); g->d_unit_bounds = nullptr;
-  cudaFree(g->d_partials); cudaFree(g->d_csum); cudaFree(g->d_rel);
-  cudaFree(g->d_tile_order); cudaFree(g->d_tile_cost); cudaFree(g->d_block_mask);
-  g->d_tile_order = nullptr; g->d_tile_cost = nullptr; g->d_block_mask = nullptr;
-  cudaFree(g->d_csr_begin); cudaFree(g->d_csr_items); cudaFree(g->d_block_nodes);
-  cudaFree(g->d_red_offset); cudaFree(g->d_x); cudaFree(g->d_xc);
-  cudaFree(g->d_packed[0]); cudaFree(g->d_packed[1]);
-  cudaFree(g->d_A); cudaFree(g->d_scale); cudaFree(g->d_diag); cudaFree(g->d_gs); cudaFree(g->d_step);
-  cudaFree(g->d_state);
-  cudaFree(g->d_sample_pts); cudaFree(g->d_sample_idx);
-  g->d_sample_pts = nullptr; g->d_sample_idx = nullptr;
-  cudaFree(g->d_snap); g->d_snap = nullptr;
-  // the pinned host buffers (h_state, h_snap, h_x) outlive the tables: cudaMallocHost costs ~0.2 ms each
-  g->d_cons = nullptr; g->d_poses = nullptr; g->d_tiles = nullptr; g->d_tile_begin = nullptr;
-  g->d_partials = nullptr; g->d_csum = nullptr; g->d_rel = nullptr;
-  g->d_csr_begin = nullptr; g->d_csr_items = nullptr; g->d_block_nodes = nullptr;
-  g->d_red_offset = nullptr; g->d_x = nullptr; g->d_xc = nullptr;
-  g->d_packed[0] = g->d_packed[1] = nullptr;
-  g->d_A = nullptr; g->d_scale = nullptr; g->d_diag = nullptr; g->d_gs = nullptr; g->d_step = nullptr;
-  g->d_state = nullptr;
-}
-
 void vgx_graph_free(vgx_ctx* c) {
   if (!c->graph) return;
   cudaStreamSynchronize(c->stream);
-  free_tables(c->graph);
-  if (c->graph->h_state) cudaFreeHost(c->graph->h_state);
-  if (c->graph->h_snap) cudaFreeHost(c->graph->h_snap);
-  if (c->graph->h_x) cudaFreeHost(c->graph->h_x);
   if (c->graph->copy_stream) {
     cudaStreamDestroy(c->graph->copy_stream);
     for (int k = 0; k < 2; ++k) { cudaEventDestroy(c->graph->ev_iter[k]); cudaEventDestroy(c->graph->ev_copy[k]); }
@@ -349,20 +321,11 @@ extern "C" int vgx_shard_constraints(int nranks, int n, const int32_t* num_resid
 }
 
 // ------------------------------------------------------------------ table construction
-template <class T>
-static cudaError_t upload_vec(T** dptr, const std::vector<T>& v, cudaStream_t st) {
-  *dptr = nullptr;
-  const size_t bytes = sizeof(T) * std::max<size_t>(v.size(), 1);
-  cudaError_t e = cudaMalloc((void**)dptr, bytes);
-  if (e != cudaSuccess) return e;
-  if (!v.empty()) e = cudaMemcpyAsync(*dptr, v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice, st);
-  return e;
-}
 
 static int build_tables(vgx_ctx* c, VgxGraph* g) {
   VGX_CUDA(c, cudaSetDevice(c->device));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  free_tables(g);
+  g->dev = VgxGraphTables();
   const int N = g->N;
   const int P = (int)g->reg_ref.size();
   // ---- shard registration constraints over ranks: greedy by descending point count
@@ -420,17 +383,18 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
     for (int k = 0; k < g->n_local; ++k)
       if (is_sampled[g->local[k]]) { units += ((size_t)cons[k].n + 31) / 32; nidx += (size_t)cons[k].n; }
     if (units > 0) {
-      VGX_CUDA(c, cudaMalloc((void**)&g->d_sample_pts, units * VGX_PT_UNIT_FLOATS * sizeof(float)));
-      VGX_CUDA(c, cudaMalloc((void**)&g->d_sample_idx, nidx * sizeof(int32_t)));
+      int rc = g->dev.d_sample_pts.alloc(c, units * VGX_PT_UNIT_FLOATS * sizeof(float), "registration sample points");
+      if (rc == VGX_OK) rc = g->dev.d_sample_idx.alloc(c, nidx * sizeof(int32_t), "registration sample points");
+      if (rc != VGX_OK) return rc;
       size_t uo = 0, io = 0;
       for (int k = 0; k < g->n_local; ++k) {
         const int i = g->local[k];
         if (!is_sampled[i]) continue;
         const VgxPoints& p = c->find(g->reg_ref[i])->points[g->reg_cfgs[i].registration_point_type];
-        VGX_CUDA(c, cudaMemcpyAsync(g->d_sample_idx + io, g->samples[i].data(), sizeof(int32_t) * cons[k].n,
+        VGX_CUDA(c, cudaMemcpyAsync(g->dev.d_sample_idx.get() + io, g->samples[i].data(), sizeof(int32_t) * cons[k].n,
                                     cudaMemcpyHostToDevice, c->stream));
-        float* dst = g->d_sample_pts + uo * VGX_PT_UNIT_FLOATS;
-        vgx_launch_reg_gather_samples(c->stream, p.data, g->d_sample_idx + io, cons[k].n, dst);
+        float* dst = g->dev.d_sample_pts.get() + uo * VGX_PT_UNIT_FLOATS;
+        vgx_launch_reg_gather_samples(c->stream, p.data.get(), g->dev.d_sample_idx.get() + io, cons[k].n, dst);
         c->launches++;
         cons[k].pts = dst;
         uo += ((size_t)cons[k].n + 31) / 32;
@@ -547,67 +511,74 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
   g->n_free = n;
   g->packed_len = PACK_HDR + 20 * (size_t)N + 16 * (size_t)g->E;
 
-  cudaError_t e = cudaSuccess;
+  // every failure here reads "graph table build: <CUDA error>"; out of memory is VGX_ERR_NOMEM
+  const char* what = "graph table build";
+  VgxGraphTables& t = g->dev;
   cudaStream_t st = c->stream;
-  if (e == cudaSuccess) e = upload_vec(&g->d_cons, cons, st);
-  if (e == cudaSuccess) e = upload_vec(&g->d_tiles, tiles, st);
-  if (e == cudaSuccess) e = upload_vec(&g->d_tile_begin, tile_begin, st);
+  int rc = VGX_OK;
+  auto check = [&](cudaError_t e) {
+    if (rc != VGX_OK || e == cudaSuccess) return;
+    c->set_error(std::string(what) + ": " + cudaGetErrorString(e));
+    rc = e == cudaErrorMemoryAllocation ? VGX_ERR_NOMEM : VGX_ERR_CUDA;
+  };
+  auto dmalloc = [&](auto& d, size_t bytes) {
+    if (rc == VGX_OK) rc = d.alloc(c, std::max<size_t>(bytes, 8), what, VGX_ERR_NOMEM);
+  };
+  auto upload = [&](auto& d, const auto& v) {
+    dmalloc(d, sizeof(v[0]) * std::max<size_t>(v.size(), 1));
+    if (rc == VGX_OK && !v.empty())
+      check(cudaMemcpyAsync(d.get(), v.data(), sizeof(v[0]) * v.size(), cudaMemcpyHostToDevice, st));
+  };
+  upload(t.d_cons, cons);
+  upload(t.d_tiles, tiles);
+  upload(t.d_tile_begin, tile_begin);
   {
     std::vector<int> ident(tiles.size()), zero(tiles.size(), 0);
     std::iota(ident.begin(), ident.end(), 0);
-    if (e == cudaSuccess) e = upload_vec(&g->d_tile_order, ident, st);
-    if (e == cudaSuccess) e = upload_vec(&g->d_tile_cost, zero, st);
+    upload(t.d_tile_order, ident);
+    upload(t.d_tile_cost, zero);
   }
-  if (e == cudaSuccess) e = upload_vec(&g->d_rel, g->rel, st);
-  if (e == cudaSuccess) e = upload_vec(&g->d_csr_begin, csr_begin, st);
-  if (e == cudaSuccess) e = upload_vec(&g->d_csr_items, items, st);
-  if (e == cudaSuccess) e = upload_vec(&g->d_block_mask, block_mask, st);
-  if (e == cudaSuccess) e = upload_vec(&g->d_block_nodes, block_nodes, st);
-  if (e == cudaSuccess) e = upload_vec(&g->d_red_offset, red, st);
-  if (e == cudaSuccess) e = upload_vec(&g->d_x, g->x, st);
-  auto dmalloc = [&](void** p, size_t bytes) {
-    if (e == cudaSuccess) e = cudaMalloc(p, std::max<size_t>(bytes, 8));
-  };
-  dmalloc((void**)&g->d_unit_bounds, sizeof(float4) * (size_t)n_units);
-  if (e == cudaSuccess && g->n_tiles > 0) {
-    vgx_launch_reg_unit_bounds(st, g->d_tiles, g->n_tiles, g->d_unit_bounds);
+  upload(t.d_rel, g->rel);
+  upload(t.d_csr_begin, csr_begin);
+  upload(t.d_csr_items, items);
+  upload(t.d_block_mask, block_mask);
+  upload(t.d_block_nodes, block_nodes);
+  upload(t.d_red_offset, red);
+  upload(t.d_x, g->x);
+  dmalloc(t.d_unit_bounds, sizeof(float4) * (size_t)n_units);
+  if (rc == VGX_OK && g->n_tiles > 0) {
+    vgx_launch_reg_unit_bounds(st, t.d_tiles.get(), g->n_tiles, t.d_unit_bounds.get());
     c->launches++;
-    e = cudaGetLastError();
+    check(cudaGetLastError());
   }
-  dmalloc((void**)&g->d_poses, sizeof(RegPoseConst) * g->n_local);
-  dmalloc((void**)&g->d_partials, sizeof(double) * VGX_REG_NSTRIDE * (size_t)g->n_tiles);
-  dmalloc((void**)&g->d_csum, sizeof(double) * VGX_REG_NSTRIDE * (size_t)g->n_local);
-  dmalloc((void**)&g->d_xc, sizeof(double) * 4 * N);
-  dmalloc((void**)&g->d_packed[0], sizeof(double) * g->packed_len);
-  dmalloc((void**)&g->d_packed[1], sizeof(double) * g->packed_len);
-  dmalloc((void**)&g->d_A, sizeof(double) * (size_t)(n + 1) * (n + 1));
-  dmalloc((void**)&g->d_scale, sizeof(double) * n);
-  dmalloc((void**)&g->d_diag, sizeof(double) * n);
-  dmalloc((void**)&g->d_gs, sizeof(double) * n);
-  dmalloc((void**)&g->d_step, sizeof(double) * n);
-  dmalloc((void**)&g->d_state, sizeof(LmState));
-  if (e == cudaSuccess && !g->h_state) e = cudaMallocHost((void**)&g->h_state, sizeof(LmState));
-  dmalloc((void**)&g->d_snap, 2 * sizeof(LmState));
-  if (e == cudaSuccess && !g->h_snap) e = cudaMallocHost((void**)&g->h_snap, 2 * sizeof(LmState));
-  if (e == cudaSuccess && g->h_x_cap < N) {
-    if (g->h_x) cudaFreeHost(g->h_x);
-    g->h_x = nullptr;
-    g->h_x_cap = std::max(2 * N, 64);
-    e = cudaMallocHost((void**)&g->h_x, sizeof(double) * 4 * (size_t)g->h_x_cap);
-    if (e != cudaSuccess) g->h_x_cap = 0;
-  }
-  if (e == cudaSuccess && !g->copy_stream) {
-    e = cudaStreamCreateWithFlags(&g->copy_stream, cudaStreamNonBlocking);
-    for (int k = 0; k < 2 && e == cudaSuccess; ++k) {
-      e = cudaEventCreateWithFlags(&g->ev_iter[k], cudaEventDisableTiming);
-      if (e == cudaSuccess) e = cudaEventCreateWithFlags(&g->ev_copy[k], cudaEventDisableTiming);
+  dmalloc(t.d_poses, sizeof(RegPoseConst) * g->n_local);
+  dmalloc(t.d_partials, sizeof(double) * VGX_REG_NSTRIDE * (size_t)g->n_tiles);
+  dmalloc(t.d_csum, sizeof(double) * VGX_REG_NSTRIDE * (size_t)g->n_local);
+  dmalloc(t.d_xc, sizeof(double) * 4 * N);
+  dmalloc(t.d_packed[0], sizeof(double) * g->packed_len);
+  dmalloc(t.d_packed[1], sizeof(double) * g->packed_len);
+  dmalloc(t.d_A, sizeof(double) * (size_t)(n + 1) * (n + 1));
+  dmalloc(t.d_scale, sizeof(double) * n);
+  dmalloc(t.d_diag, sizeof(double) * n);
+  dmalloc(t.d_gs, sizeof(double) * n);
+  dmalloc(t.d_step, sizeof(double) * n);
+  dmalloc(t.d_state, sizeof(LmState));
+  if (rc == VGX_OK && !g->h_state.get()) rc = g->h_state.alloc(c, sizeof(LmState), what, VGX_ERR_NOMEM);
+  dmalloc(t.d_snap, 2 * sizeof(LmState));
+  if (rc == VGX_OK && !g->h_snap.get()) rc = g->h_snap.alloc(c, 2 * sizeof(LmState), what, VGX_ERR_NOMEM);
+  if (rc == VGX_OK && g->h_x.bytes() < sizeof(double) * 4 * (size_t)N)
+    rc = g->h_x.alloc(c, sizeof(double) * 4 * (size_t)std::max(2 * N, 64), what, VGX_ERR_NOMEM);
+  if (rc == VGX_OK && !g->copy_stream) {
+    check(cudaStreamCreateWithFlags(&g->copy_stream, cudaStreamNonBlocking));
+    for (int k = 0; k < 2 && rc == VGX_OK; ++k) {
+      check(cudaEventCreateWithFlags(&g->ev_iter[k], cudaEventDisableTiming));
+      check(cudaEventCreateWithFlags(&g->ev_copy[k], cudaEventDisableTiming));
     }
   }
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) {
-    free_tables(g);
-    c->set_error(std::string("graph table build: ") + cudaGetErrorString(e));
-    return e == cudaErrorMemoryAllocation ? VGX_ERR_NOMEM : VGX_ERR_CUDA;
+  if (rc == VGX_OK) check(cudaStreamSynchronize(st));
+  if (rc != VGX_OK) {
+    g->dev = VgxGraphTables();
+    return rc;
   }
   g->dirty = false;
   return VGX_OK;
@@ -623,18 +594,19 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
     // the second evaluation on new tables, then every 32nd (the poses move little inside a solve)
     if (g->n_tiles > 1 && (g->evals_since_order == -2 || g->evals_since_order >= 32)) {
       VgxLaunchScope s(c, VGX_SLOT_OTHER);
-      vgx_launch_reg_order(st, g->d_tile_cost, g->n_tiles, g->d_tile_order);
+      vgx_launch_reg_order(st, g->dev.d_tile_cost.get(), g->n_tiles, g->dev.d_tile_order.get());
       g->evals_since_order = 0;
     }
     if (g->evals_since_order >= 0) ++g->evals_since_order;
     {
       VgxLaunchScope s(c, VGX_SLOT_REG_POSE_SETUP);
-      vgx_launch_reg_pose_setup(st, g->d_cons, d_x, g->d_poses, g->n_local, skip);
+      vgx_launch_reg_pose_setup(st, g->dev.d_cons.get(), d_x, g->dev.d_poses.get(), g->n_local, skip);
     }
     {
       VgxLaunchScope s(c, VGX_SLOT_REG_REDUCE);
-      vgx_launch_reg_reduce(st, g->d_cons, g->d_poses, g->d_tiles, g->n_tiles, g->d_tile_order,
-                            g->d_tile_cost, g->d_partials, g->grid_capacity, g->d_unit_bounds, jacobian, skip);
+      vgx_launch_reg_reduce(st, g->dev.d_cons.get(), g->dev.d_poses.get(), g->dev.d_tiles.get(), g->n_tiles,
+                            g->dev.d_tile_order.get(), g->dev.d_tile_cost.get(), g->dev.d_partials.get(),
+                            g->grid_capacity, g->dev.d_unit_bounds.get(), jacobian, skip);
     }
     if (g->evals_since_order < 0) g->evals_since_order = -2;   // a cost has been measured now
   }
@@ -652,10 +624,11 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
   const int excl = do_reg ? 0 : 1;
   if (do_reg) {
     RegSums sums;
-    sums.partials = g->d_partials; sums.tile_begin = g->d_tile_begin; sums.cons = g->d_cons;
+    sums.partials = g->dev.d_partials.get(); sums.tile_begin = g->dev.d_tile_begin.get();
+    sums.cons = g->dev.d_cons.get();
     VgxLaunchScope s(c, VGX_SLOT_REG_SUMS);
     L.cfg.gridDim = dim3((unsigned)((g->n_local + 3) / 4));
-    cudaLaunchKernelEx(&L.cfg, reg_csum_kernel, sums, g->n_local, g->d_csum, skip);
+    cudaLaunchKernelEx(&L.cfg, reg_csum_kernel, sums, g->n_local, g->dev.d_csum.get(), skip);
   }
   if (p2p) {
     int rc = vgx_p2p_begin(c, g->packed_len, &push, &gat);
@@ -675,10 +648,11 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
     {
       VgxLaunchScope s(c, VGX_SLOT_ASSEMBLY);
       L.cfg.gridDim = dim3((unsigned)grid);
-      cudaLaunchKernelEx(&L.cfg, assemble_exchange_kernel, (const double*)g->d_csum, (const VgxRelEdge*)g->d_rel, d_x,
-                         (const int*)g->d_csr_begin, (const int4*)g->d_csr_items, push, g->N, g->E, g->n_local,
+      cudaLaunchKernelEx(&L.cfg, assemble_exchange_kernel, (const double*)g->dev.d_csum.get(),
+                         (const VgxRelEdge*)g->dev.d_rel.get(), d_x, (const int*)g->dev.d_csr_begin.get(),
+                         (const int4*)g->dev.d_csr_items.get(), push, g->N, g->E, g->n_local,
                          g->n_rel_local, excl, gat, d_packed, (int)g->packed_len, skip,
-                         (const unsigned char*)g->d_block_mask);
+                         (const unsigned char*)g->dev.d_block_mask.get());
     }
     VGX_CUDA(c, cudaGetLastError());
     return VGX_OK;
@@ -686,11 +660,12 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
   {
     VgxLaunchScope s(c, VGX_SLOT_ASSEMBLY);
     L.cfg.gridDim = dim3((unsigned)(g->N + g->E + 1));
-    cudaLaunchKernelEx(&L.cfg, assemble_kernel, (const double*)g->d_csum, (const VgxRelEdge*)g->d_rel, d_x, (const int*)g->d_csr_begin,
-                       (const int4*)g->d_csr_items, push, g->N, g->E, g->n_local, g->n_rel_local, excl, skip);
+    cudaLaunchKernelEx(&L.cfg, assemble_kernel, (const double*)g->dev.d_csum.get(),
+                       (const VgxRelEdge*)g->dev.d_rel.get(), d_x, (const int*)g->dev.d_csr_begin.get(),
+                       (const int4*)g->dev.d_csr_items.get(), push, g->N, g->E, g->n_local, g->n_rel_local, excl, skip);
   }
   VGX_CUDA(c, cudaGetLastError());
-  if (p2p) return vgx_p2p_gather(c, gat, d_packed, g->packed_len, g->d_block_mask, g->N);
+  if (p2p) return vgx_p2p_gather(c, gat, d_packed, g->packed_len, g->dev.d_block_mask.get(), g->N);
   return vgx_nccl_allreduce_sum_f64(c, d_packed, g->packed_len);
 }
 
@@ -743,12 +718,12 @@ extern "C" int vgx_graph_set_poses(vgx_ctx* c, const double* xyzyaw) {
   if (!g->dirty) {
     VGX_CUDA(c, cudaSetDevice(c->device));
     // stage through pinned memory so the copy is a true async H2D
-    int rc = c->ensure_pinned(sizeof(double) * 4 * g->N);
+    double* h;
+    int rc = vgx_carve(c, c->h_pinned, vgx_part(h, 4 * (size_t)g->N));
     if (rc != VGX_OK) return rc;
     VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    memcpy(c->h_pinned, xyzyaw, sizeof(double) * 4 * g->N);
-    VGX_CUDA(c, cudaMemcpyAsync(g->d_x, c->h_pinned, sizeof(double) * 4 * g->N, cudaMemcpyHostToDevice,
-                                c->stream));
+    memcpy(h, xyzyaw, sizeof(double) * 4 * g->N);
+    VGX_CUDA(c, cudaMemcpyAsync(g->dev.d_x.get(), h, sizeof(double) * 4 * g->N, cudaMemcpyHostToDevice, c->stream));
   }
   return VGX_OK;
 }
@@ -859,7 +834,7 @@ extern "C" int vgx_graph_eval_async(vgx_ctx* c, int exclude_registration) {
   VgxGraph* g = nullptr;
   int rc = prepare(c, &g);
   if (rc != VGX_OK) return rc;
-  return eval_enqueue(c, g, g->d_x, g->d_packed[0], true, exclude_registration != 0);
+  return eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, exclude_registration != 0);
 }
 
 extern "C" int vgx_graph_eval(vgx_ctx* c, int exclude_registration, double* cost, double* gradient,
@@ -867,12 +842,12 @@ extern "C" int vgx_graph_eval(vgx_ctx* c, int exclude_registration, double* cost
   VgxGraph* g = nullptr;
   int rc = prepare(c, &g);
   if (rc != VGX_OK) return rc;
-  rc = eval_enqueue(c, g, g->d_x, g->d_packed[0], true, exclude_registration != 0);
+  rc = eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, exclude_registration != 0);
   if (rc != VGX_OK) return rc;
-  rc = c->ensure_pinned(sizeof(double) * g->packed_len);
+  double* h;
+  rc = vgx_carve(c, c->h_pinned, vgx_part(h, g->packed_len));
   if (rc != VGX_OK) return rc;
-  double* h = (double*)c->h_pinned;
-  VGX_CUDA(c, cudaMemcpyAsync(h, g->d_packed[0], sizeof(double) * g->packed_len, cudaMemcpyDeviceToHost,
+  VGX_CUDA(c, cudaMemcpyAsync(h, g->dev.d_packed[0].get(), sizeof(double) * g->packed_len, cudaMemcpyDeviceToHost,
                               c->stream));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   const int N = g->N, dim = 4 * N;
@@ -909,12 +884,12 @@ extern "C" int vgx_graph_registration_costs(vgx_ctx* c, double* per_constraint) 
   int rc = prepare(c, &g);
   if (rc != VGX_OK) return rc;
   if (!per_constraint) return VGX_ERR_INVALID;
-  rc = eval_enqueue(c, g, g->d_x, g->d_packed[1], false, false);
+  rc = eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[1].get(), false, false);
   if (rc != VGX_OK) return rc;
   const int P = (int)g->reg_ref.size();
   std::vector<double> cs((size_t)g->n_local * VGX_REG_NSTRIDE + 1);
   if (g->n_local > 0)
-    VGX_CUDA(c, cudaMemcpyAsync(cs.data(), g->d_csum, sizeof(double) * VGX_REG_NSTRIDE * g->n_local,
+    VGX_CUDA(c, cudaMemcpyAsync(cs.data(), g->dev.d_csum.get(), sizeof(double) * VGX_REG_NSTRIDE * g->n_local,
                                 cudaMemcpyDeviceToHost, c->stream));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   for (int i = 0; i < P; ++i) per_constraint[i] = 0.0;

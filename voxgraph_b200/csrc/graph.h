@@ -18,6 +18,37 @@ struct LmState {
   int termination, done, accepted, step_valid, scale_ready;
 };
 
+// The device buffers of one table build: all of them are released when the tables are rebuilt.
+struct VgxGraphTables {
+  VgxBuffer<RegConstraintDev> d_cons;
+  VgxBuffer<RegPoseConst> d_poses;
+  VgxBuffer<RegTile> d_tiles;
+  VgxBuffer<float4> d_unit_bounds;   // bounding sphere per 32-point unit of the tiles (RegTile::unit0)
+  VgxBuffer<int> d_tile_begin;
+  VgxBuffer<double> d_partials;
+  VgxBuffer<double> d_csum;
+  VgxBuffer<VgxRelEdge> d_rel;
+  VgxBuffer<unsigned char> d_block_mask;   // per output block: bit r = rank r contributes (peer exchange)
+  VgxBuffer<int> d_tile_order;  // CTA b of the reduce kernel runs tile d_tile_order[b] (longest first)
+  VgxBuffer<int> d_tile_cost;   // SM cycles each tile took in the latest evaluation
+  VgxBuffer<int> d_csr_begin;   // N + E + 1
+  VgxBuffer<int4> d_csr_items;  // (source, role, first tile, end tile)
+  VgxBuffer<int> d_block_nodes; // E x 2
+  VgxBuffer<int> d_red_offset;  // N: reduced offset or -1
+  VgxBuffer<double> d_x;
+  VgxBuffer<double> d_xc;
+  VgxBuffer<double> d_packed[2];
+  VgxBuffer<double> d_A;
+  VgxBuffer<double> d_scale;
+  VgxBuffer<double> d_diag;
+  VgxBuffer<double> d_gs;
+  VgxBuffer<double> d_step;
+  VgxBuffer<LmState> d_state;
+  VgxBuffer<LmState> d_snap;    // [2] outcome of iteration k (written by lm_decide), parity k & 1
+  VgxBuffer<float> d_sample_pts;   // gathered unit-major points of the local sampled blocks
+  VgxBuffer<int32_t> d_sample_idx;
+};
+
 struct VgxGraph {
   int N = 0;
   std::vector<uint32_t> ids;
@@ -41,42 +72,16 @@ struct VgxGraph {
   int64_t residuals_local = 0, residuals_global = 0;
   bool zero_weight = false;
   size_t packed_len = 0;
+  int evals_since_order = -1;   // -1: no cost measured yet since the tables were built
 
   // device
-  RegConstraintDev* d_cons = nullptr;
-  RegPoseConst* d_poses = nullptr;
-  RegTile* d_tiles = nullptr;
-  float4* d_unit_bounds = nullptr;   // bounding sphere per 32-point unit of the tiles (RegTile::unit0)
-  int* d_tile_begin = nullptr;
-  double* d_partials = nullptr;
-  double* d_csum = nullptr;
-  VgxRelEdge* d_rel = nullptr;
-  unsigned char* d_block_mask = nullptr;   // per output block: bit r = rank r contributes (peer exchange)
-  int* d_tile_order = nullptr;  // CTA b of the reduce kernel runs tile d_tile_order[b] (longest first)
-  int* d_tile_cost = nullptr;   // SM cycles each tile took in the latest evaluation
-  int evals_since_order = -1;   // -1: no cost measured yet since the tables were built
-  int* d_csr_begin = nullptr;   // N + E + 1
-  int4* d_csr_items = nullptr;  // (source, role, first tile, end tile)
-  int* d_block_nodes = nullptr; // E x 2
-  int* d_red_offset = nullptr;  // N: reduced offset or -1
-  double* d_x = nullptr;
-  double* d_xc = nullptr;
-  double* d_packed[2] = {nullptr, nullptr};
-  double* d_A = nullptr;
-  double* d_scale = nullptr;
-  double* d_diag = nullptr;
-  double* d_gs = nullptr;
-  double* d_step = nullptr;
-  LmState* d_state = nullptr;
-  LmState* h_state = nullptr;
-  LmState* d_snap = nullptr;    // [2] outcome of iteration k (written by lm_decide), parity k & 1
-  LmState* h_snap = nullptr;    // [2] pinned
-  double* h_x = nullptr;        // pinned, 4 * h_x_cap
-  int h_x_cap = 0;
+  VgxGraphTables dev;
+  // pinned; they outlive the tables: a page-locked allocation costs ~0.2 ms
+  VgxBuffer<LmState> h_state{VgxMem::pinned};
+  VgxBuffer<LmState> h_snap{VgxMem::pinned};    // [2]
+  VgxBuffer<double> h_x{VgxMem::pinned};        // 4 x (at least N)
   cudaStream_t copy_stream = nullptr;
   cudaEvent_t ev_iter[2] = {nullptr, nullptr}, ev_copy[2] = {nullptr, nullptr};
-  float* d_sample_pts = nullptr;   // gathered unit-major points of the local sampled blocks
-  int32_t* d_sample_idx = nullptr;
 };
 
 __device__ __forceinline__ double normalize_angle(double a) {

@@ -16,9 +16,9 @@ struct LayerDev {
 
 static inline LayerDev layer_of(const VgxSubmap* s) {
   LayerDev L;
-  L.hash = s->hash;
-  L.dw = s->d_dw;
-  L.block_idx = s->d_block_idx;
+  L.hash = s->hash();
+  L.dw = s->d_dw.get();
+  L.block_idx = s->d_block_idx.get();
   L.voxel_size = s->voxel_size; L.voxel_size_inv = s->voxel_size_inv;
   L.block_size = s->block_size; L.block_size_inv = s->block_size_inv;
   L.vps = s->vps;

@@ -383,31 +383,11 @@ mesh_ply_kernel(const float* __restrict__ xyz, const uint32_t* __restrict__ tri,
 
 // ------------------------------------------------------------------ host
 void vgx_mesh_free(vgx_ctx* c) {
-  cudaFree(c->d_mesh_xyz);
-  cudaFree(c->d_mesh_tri);
-  c->d_mesh_xyz = nullptr;
-  c->d_mesh_tri = nullptr;
-  c->mesh_vcap = c->mesh_tcap = 0;
+  c->d_mesh_xyz.reset();
+  c->d_mesh_tri.reset();
   c->mesh_nv = c->mesh_nt = 0;
   c->mesh_ids.clear();
   c->mesh_voff.assign(1, 0);
-}
-
-// grows a device buffer to `need` bytes keeping its first `used` bytes
-static int grow_keep(vgx_ctx* c, void** p, size_t* cap, size_t need, size_t used) {
-  if (need <= *cap) return VGX_OK;
-  const size_t want = need + need / 4;
-  void* q = nullptr;
-  VGX_CUDA(c, cudaMalloc(&q, want));
-  if (used) {
-    const cudaError_t e = cudaMemcpyAsync(q, *p, used, cudaMemcpyDeviceToDevice, c->stream);
-    if (e != cudaSuccess) { cudaFree(q); VGX_CUDA(c, e); }
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  }
-  cudaFree(*p);
-  *p = q;
-  *cap = want;
-  return VGX_OK;
 }
 
 
@@ -421,20 +401,13 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
                       std::vector<int64_t>& voff, std::vector<int64_t>& toff) {
   const int nj = (int)jobs.size();
   cudaStream_t st = c->stream;
-  const size_t cnt_b = align256((n_vox + 1) * sizeof(unsigned));
-  const size_t tmp_b = align256(vgx_scan_tmp_count(n_vox) * sizeof(unsigned));
-  const size_t job_b = align256((size_t)nj * sizeof(MeshJob));
-  const size_t off_b = align256(2 * ((size_t)nj + 1) * sizeof(unsigned));
-  int rc = c->ensure_sort(4 * cnt_b + tmp_b + job_b + off_b);
+  unsigned *d_cnt, *d_toff, *d_flag, *d_voff, *d_tmp, *d_offs;
+  MeshJob* d_jobs;
+  int rc = vgx_carve(c, c->d_work, vgx_part(d_cnt, n_vox + 1), vgx_part(d_toff, n_vox + 1),
+                     vgx_part(d_flag, n_vox + 1), vgx_part(d_voff, n_vox + 1),
+                     vgx_part(d_tmp, vgx_scan_tmp_count(n_vox)), vgx_part(d_jobs, (size_t)nj),
+                     vgx_part(d_offs, 2 * ((size_t)nj + 1)));
   if (rc != VGX_OK) return rc;
-  char* base = (char*)c->d_sort;
-  unsigned* d_cnt = (unsigned*)base;
-  unsigned* d_toff = (unsigned*)(base + cnt_b);
-  unsigned* d_flag = (unsigned*)(base + 2 * cnt_b);
-  unsigned* d_voff = (unsigned*)(base + 3 * cnt_b);
-  unsigned* d_tmp = (unsigned*)(base + 4 * cnt_b);
-  MeshJob* d_jobs = (MeshJob*)(base + 4 * cnt_b + tmp_b);
-  unsigned* d_offs = (unsigned*)(base + 4 * cnt_b + tmp_b + job_b);
   VGX_CUDA(c, cudaMemcpyAsync(d_jobs, jobs.data(), (size_t)nj * sizeof(MeshJob), cudaMemcpyHostToDevice, st));
   VGX_CUDA(c, cudaMemsetAsync(d_flag, 0, n_vox * sizeof(unsigned), st));
   const unsigned g128 = (unsigned)((n_vox + 127) / 128), g256 = (unsigned)((n_vox + 255) / 256);
@@ -474,20 +447,20 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
     toff.push_back((int64_t)(tbase + offs[2 * (size_t)k]));
     voff.push_back((int64_t)(vbase + offs[2 * (size_t)k + 1]));
   }
-  rc = grow_keep(c, (void**)&c->d_mesh_xyz, &c->mesh_vcap, 3 * sizeof(float) * std::max(nv, (size_t)1),
-                 3 * sizeof(float) * vbase);
+  rc = c->d_mesh_xyz.grow_keep(c, 3 * sizeof(float) * std::max(nv, (size_t)1), 3 * sizeof(float) * vbase,
+                                "mesh vertices");
   if (rc != VGX_OK) return rc;
-  rc = grow_keep(c, (void**)&c->d_mesh_tri, &c->mesh_tcap, 3 * sizeof(uint32_t) * std::max(nt, (size_t)1),
-                 3 * sizeof(uint32_t) * tbase);
+  rc = c->d_mesh_tri.grow_keep(c, 3 * sizeof(uint32_t) * std::max(nt, (size_t)1), 3 * sizeof(uint32_t) * tbase,
+                               "mesh triangles");
   if (rc != VGX_OK) return rc;
   {
     VgxLaunchScope scope(c, VGX_SLOT_MESH);
-    mesh_vertex_kernel<<<g128, 128, 0, st>>>(d_jobs, nj, n_vox, d_flag, d_voff, vbase, c->d_mesh_xyz);
+    mesh_vertex_kernel<<<g128, 128, 0, st>>>(d_jobs, nj, n_vox, d_flag, d_voff, vbase, c->d_mesh_xyz.get());
   }
   {
     VgxLaunchScope scope(c, VGX_SLOT_MESH);
     mesh_triangle_kernel<<<g128, 128, 0, st>>>(d_jobs, nj, n_vox, min_weight, d_toff, d_flag, d_voff, vbase,
-                                               tbase, c->d_mesh_tri);
+                                               tbase, c->d_mesh_tri.get());
   }
   VGX_CUDA(c, cudaGetLastError());
   VGX_CUDA(c, cudaStreamSynchronize(st));   // the scratch is reused by the next batch
@@ -573,10 +546,10 @@ extern "C" int vgx_mesh_download(vgx_ctx* c, int64_t max_vertices, float* xyz, i
     VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_mesh_download: output too small");
   VGX_CUDA(c, cudaSetDevice(c->device));
   if (xyz && c->mesh_nv)
-    VGX_CUDA(c, cudaMemcpyAsync(xyz, c->d_mesh_xyz, 3 * sizeof(float) * (size_t)c->mesh_nv, cudaMemcpyDeviceToHost,
+    VGX_CUDA(c, cudaMemcpyAsync(xyz, c->d_mesh_xyz.get(), 3 * sizeof(float) * (size_t)c->mesh_nv, cudaMemcpyDeviceToHost,
                                 c->stream));
   if (triangles && c->mesh_nt)
-    VGX_CUDA(c, cudaMemcpyAsync(triangles, c->d_mesh_tri, 3 * sizeof(uint32_t) * (size_t)c->mesh_nt,
+    VGX_CUDA(c, cudaMemcpyAsync(triangles, c->d_mesh_tri.get(), 3 * sizeof(uint32_t) * (size_t)c->mesh_nt,
                                 cudaMemcpyDeviceToHost, c->stream));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   return VGX_OK;
@@ -606,19 +579,19 @@ extern "C" int vgx_mesh_ply(vgx_ctx* c, const uint8_t* rgba, uint8_t* out, uint6
     if (rgba) memcpy(q, rgba + 4 * (size_t)k, 4); else rainbow(c->mesh_ids[k], q);
     col[k] = (uint32_t)q[0] | ((uint32_t)q[1] << 8) | ((uint32_t)q[2] << 16) | ((uint32_t)q[3] << 24);
   }
-  const size_t body_b = align256((size_t)body), voff_b = align256(c->mesh_voff.size() * sizeof(int64_t));
-  int rc = c->ensure_scratch(body_b + voff_b + col.size() * sizeof(uint32_t));
+  uint8_t* d_body;
+  int64_t* d_voff;
+  uint32_t* d_col;
+  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_body, (size_t)body), vgx_part(d_voff, c->mesh_voff.size()),
+                     vgx_part(d_col, col.size()));
   if (rc != VGX_OK) return rc;
-  uint8_t* d_body = (uint8_t*)c->d_scratch;
-  int64_t* d_voff = (int64_t*)(d_body + body_b);
-  uint32_t* d_col = (uint32_t*)((char*)d_voff + voff_b);
   VGX_CUDA(c, cudaMemcpyAsync(d_voff, c->mesh_voff.data(), c->mesh_voff.size() * sizeof(int64_t),
                               cudaMemcpyHostToDevice, c->stream));
   VGX_CUDA(c, cudaMemcpyAsync(d_col, col.data(), col.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
   const int64_t recs = c->mesh_nv + c->mesh_nt;
   {
     VgxLaunchScope scope(c, VGX_SLOT_MESH);
-    mesh_ply_kernel<<<(unsigned)((recs + 255) / 256), 256, 0, c->stream>>>(c->d_mesh_xyz, c->d_mesh_tri, c->mesh_nv,
+    mesh_ply_kernel<<<(unsigned)((recs + 255) / 256), 256, 0, c->stream>>>(c->d_mesh_xyz.get(), c->d_mesh_tri.get(), c->mesh_nv,
                                                                           c->mesh_nt, d_voff, ns, d_col, d_body);
   }
   VGX_CUDA(c, cudaGetLastError());

@@ -110,8 +110,8 @@ extern "C" int vgx_find_overlapping_pairs(vgx_ctx* c, int n, const uint32_t* ids
         if (amax[3 * (size_t)i + a] < amin[3 * (size_t)j + a] || amin[3 * (size_t)i + a] > amax[3 * (size_t)j + a]) sep = true;
       if (sep || sm[i]->n_iso == 0) continue;
       OverlapJob J;
-      J.other_hash = sm[j]->hash;
-      J.iso_idx = sm[i]->d_iso_idx;
+      J.other_hash = sm[j]->hash();
+      J.iso_idx = sm[i]->d_iso_idx.get();
       J.n_iso = sm[i]->n_iso;
       J.block_size = sm[i]->block_size;
       J.other_block_size_inv = sm[j]->block_size_inv;
@@ -123,11 +123,10 @@ extern "C" int vgx_find_overlapping_pairs(vgx_ctx* c, int n, const uint32_t* ids
     }
   }
   if (jobs.empty()) return VGX_OK;
-  const size_t jb = ((jobs.size() * sizeof(OverlapJob)) + 255) & ~(size_t)255;
-  int rc = c->ensure_scratch(jb + jobs.size() * sizeof(int));
+  OverlapJob* d_jobs;
+  int* d_flags;
+  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_jobs, jobs.size()), vgx_part(d_flags, jobs.size()));
   if (rc != VGX_OK) return rc;
-  OverlapJob* d_jobs = (OverlapJob*)c->d_scratch;
-  int* d_flags = (int*)((char*)c->d_scratch + jb);
   VGX_CUDA(c, cudaMemcpyAsync(d_jobs, jobs.data(), jobs.size() * sizeof(OverlapJob), cudaMemcpyHostToDevice, c->stream));
   overlap_pairs_kernel<<<(unsigned)jobs.size(), 128, 0, c->stream>>>(d_jobs, d_flags);
   c->launches++;

@@ -291,8 +291,8 @@ static int launch_fold(vgx_ctx* c, int vps, unsigned n_keys, const ProjSrc* d_sr
   cudaStream_t st = c->stream;
   switch (vps) {
 #define PROJ_FOLD(VPT, REGS, THREADS)                                                                   \
-  project_fold_kernel<VPT, REGS><<<n_keys, THREADS, 0, st>>>(d_src, ukey, urank, useg, slot, s->d_dw, \
-                                                             s->d_block_idx);                          \
+  project_fold_kernel<VPT, REGS><<<n_keys, THREADS, 0, st>>>(d_src, ukey, urank, useg, slot, s->d_dw.get(), \
+                                                             s->d_block_idx.get());                          \
   break;
     case 2: PROJ_FOLD(1, true, 8)
     case 4: PROJ_FOLD(1, true, 64)
@@ -329,32 +329,28 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
   const size_t P = per_block * n_in;
   cudaStream_t st = c->stream;
   unsigned n_keys = 0, n_out = 0;
-  // scratch in c->d_sort: pairs (double-buffered for the sort), flags, scans, segments, source table
+  // scratch in d_work: pairs (double-buffered for the sort), flags, scans, segments, source table
   size_t sort_tmp = 0;
   if (P > 0)
     VGX_CUDA(c, cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (unsigned long long*)nullptr,
                                                 (unsigned long long*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr,
                                                 (int)P, 0, PROJ_KEY_BITS, st));
-  const size_t k8 = align256(8 * P + 8), u4 = align256(4 * (P + 1)), tmp4 = align256(4 * vgx_scan_tmp_count(P + 1));
-  const size_t src_b = align256(sizeof(ProjSrc) * (size_t)ns), ctl_b = 256;
-  const size_t total = 2 * k8 + 7 * u4 + tmp4 + src_b + ctl_b + align256(sort_tmp);
-  int rc = c->ensure_sort(total);
+  uint64_t* keys_a;     // candidates, then the distinct keys
+  uint64_t* keys_b;     // sorted keys
+  uint32_t* ranks_a;    // candidates, then the distinct ranks per key
+  uint32_t* ranks_b;    // sorted ranks
+  unsigned* pair_head;  // then keep flags
+  unsigned *key_head, *pair_pos /* then output slots */, *key_pos, *scan_tmp;
+  uint32_t* useg;
+  ProjSrc* d_src;
+  int* d_ctl;
+  char* d_sort_tmp;
+  int rc = vgx_carve(c, c->d_work, vgx_part(keys_a, P + 1), vgx_part(keys_b, P + 1), vgx_part(ranks_a, P + 1),
+                     vgx_part(ranks_b, P + 1), vgx_part(pair_head, P + 1), vgx_part(key_head, P + 1),
+                     vgx_part(pair_pos, P + 1), vgx_part(key_pos, P + 1), vgx_part(useg, P + 1),
+                     vgx_part(scan_tmp, vgx_scan_tmp_count(P + 1)), vgx_part(d_src, (size_t)ns), vgx_part(d_ctl, 1),
+                     vgx_part(d_sort_tmp, sort_tmp));
   if (rc != VGX_OK) return rc;
-  char* at = (char*)c->d_sort;
-  auto take = [&](size_t b) { char* p = at; at += b; return (void*)p; };
-  uint64_t* keys_a = (uint64_t*)take(k8);       // candidates, then the distinct keys
-  uint64_t* keys_b = (uint64_t*)take(k8);       // sorted keys
-  uint32_t* ranks_a = (uint32_t*)take(u4);      // candidates, then the distinct ranks per key
-  uint32_t* ranks_b = (uint32_t*)take(u4);      // sorted ranks
-  unsigned* pair_head = (unsigned*)take(u4);    // then keep flags
-  unsigned* key_head = (unsigned*)take(u4);
-  unsigned* pair_pos = (unsigned*)take(u4);     // then output slots
-  unsigned* key_pos = (unsigned*)take(u4);
-  uint32_t* useg = (uint32_t*)take(u4);
-  unsigned* scan_tmp = (unsigned*)take(tmp4);
-  ProjSrc* d_src = (ProjSrc*)take(src_b);
-  int* d_ctl = (int*)take(ctl_b);
-  void* d_sort_tmp = take(align256(sort_tmp));
   if (P > 0) {
     VGX_CUDA(c, cudaMemcpyAsync(d_src, h.data(), sizeof(ProjSrc) * (size_t)ns, cudaMemcpyHostToDevice, st));
     VGX_CUDA(c, cudaMemsetAsync(d_ctl, 0, sizeof(int), st));
@@ -425,8 +421,8 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
   if (n_out > 0 && transform) {
     {
       VgxLaunchScope scope(c, VGX_SLOT_EVAL);
-      transform_fold_kernel<<<n_keys, std::min(PROJ_THREADS, g0.vox_per_block), 0, st>>>(d_src, keys_a, slot, s->d_dw,
-                                                                                        s->d_block_idx);
+      transform_fold_kernel<<<n_keys, std::min(PROJ_THREADS, g0.vox_per_block), 0, st>>>(d_src, keys_a, slot, s->d_dw.get(),
+                                                                                        s->d_block_idx.get());
     }
     VGX_CUDA(c, cudaGetLastError());
   } else if (n_out > 0) {

@@ -558,24 +558,24 @@ int vgx_fill_constraint(vgx_ctx* c, uint32_t ref_id, uint32_t read_id, const vgx
   VgxSubmap* ref = c->find(ref_id);
   VgxSubmap* rd = c->find(read_id);
   if (!ref || !rd) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "registration constraint: unknown submap");
-  if (!rd->finished || !rd->d_view)
+  if (!rd->finished || !rd->d_view.get())
     VGX_FAIL(c, VGX_ERR_INVALID, "registration constraint: reading submap is not finished");
-  if (cfg->use_esdf_distance && !rd->d_view_esdf)
+  if (cfg->use_esdf_distance && !rd->d_view_esdf.get())
     VGX_FAIL(c, VGX_ERR_INVALID, "registration constraint: use_esdf_distance needs the reading submap's ESDF "
                                  "(vgx_submap_generate_esdf)");
   const VgxPoints& p = ref->points[cfg->registration_point_type];
   const bool is_sampled = cfg->sampling_ratio != -1.0f;
   RegConstraintDev C;
-  C.pts = is_sampled ? nullptr : p.data;
+  C.pts = is_sampled ? nullptr : p.data.get();
   C.n = reg_num_residuals(p, cfg);
   C.ref_node = -1; C.read_node = -1;
-  C.hash = rd->hash;
-  C.view = cfg->use_esdf_distance ? rd->d_view_esdf : rd->d_view;   // cpp:133-153
+  C.hash = rd->hash();
+  C.view = cfg->use_esdf_distance ? rd->d_view_esdf.get() : rd->d_view.get();   // cpp:133-153
   C.voxel_size = rd->voxel_size; C.voxel_size_inv = rd->voxel_size_inv;
   C.block_size = rd->block_size; C.block_size_inv = rd->block_size_inv;
   C.vps = rd->vps;
-  C.grid = rd->d_grid;
-  C.grid16 = rd->d_grid16;
+  C.grid = rd->d_grid.get();
+  C.grid16 = rd->d_grid16.get();
   C.gmin0 = rd->grid_min[0]; C.gmin1 = rd->grid_min[1]; C.gmin2 = rd->grid_min[2];
   C.gd0 = rd->grid_dim[0]; C.gd1 = rd->grid_dim[1]; C.gd2 = rd->grid_dim[2];
   C.vps_shift = rd->sh;
@@ -622,26 +622,28 @@ extern "C" int vgx_reg_eval_emit(vgx_ctx* c, uint32_t ref_id, uint32_t read_id,
   const size_t K = (size_t)C.n;
   const size_t Kp = (K + 3) & ~(size_t)3;  // keep the Jacobian blocks 32-byte aligned
   const size_t units = (K + 31) / 32;
-  const size_t sample_bytes = sampled ? ((units * VGX_PT_UNIT_FLOATS * sizeof(float) + Kp * sizeof(int32_t) + 255) & ~(size_t)255) : 0;
-  rc = c->ensure_scratch(9 * Kp * sizeof(double) + sample_bytes);
+  // scratch: residuals and both Jacobians (9 x Kp) | (sampling mode) the drawn points and their indices
+  double* d_r;
+  float* d_pts;
+  int32_t* d_idx;
+  rc = vgx_carve(c, c->d_scratch, vgx_part(d_r, 9 * Kp), vgx_part(d_pts, sampled ? units * VGX_PT_UNIT_FLOATS : 0),
+                 vgx_part(d_idx, sampled ? Kp : 0));
   if (rc != VGX_OK) return rc;
   if (sampled) {
     // cpp:118-122: every Evaluate draws its points anew from the reference submap's sampler
     VgxPoints& p = c->find(ref_id)->points[cfg->registration_point_type];
-    rc = c->ensure_pinned(Kp * sizeof(int32_t));
+    int32_t* h_idx;
+    rc = vgx_carve(c, c->h_pinned, vgx_part(h_idx, Kp));
     if (rc != VGX_OK) return rc;
     VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    vgx_points_draw(p, (int)K, (int32_t*)c->h_pinned);
-    float* d_pts = (float*)((char*)c->d_scratch + 9 * Kp * sizeof(double));
-    int32_t* d_idx = (int32_t*)(d_pts + units * VGX_PT_UNIT_FLOATS);
-    VGX_CUDA(c, cudaMemcpyAsync(d_idx, c->h_pinned, K * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    vgx_launch_reg_gather_samples(c->stream, p.data, d_idx, (int)K, d_pts);
+    vgx_points_draw(p, (int)K, h_idx);
+    VGX_CUDA(c, cudaMemcpyAsync(d_idx, h_idx, K * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    vgx_launch_reg_gather_samples(c->stream, p.data.get(), d_idx, (int)K, d_pts);
     c->launches++;
     C.pts = d_pts;
   }
   RegPoseConst P;
   vgx_reg_pose_setup<TrigHostLibm>(ref_pose, read_pose, P);
-  double* d_r = (double*)c->d_scratch;
   double* d_jr = jac_ref ? d_r + Kp : nullptr;
   double* d_je = jac_read ? d_r + 5 * Kp : nullptr;
   {

@@ -672,10 +672,10 @@ static void enqueue_lm_build(cudaStream_t st, VgxGraph* g, int n, const LmOpts& 
   const int N = g->N;
   const int nthreads = std::max(16 * (N + g->E), 4 * N);
   lm_build_kernel<<<std::min(296, (nthreads + 255) / 256), 256, 0, st>>>(
-      g->d_packed[0], g->d_red_offset, g->d_block_nodes, N, g->E, n, g->d_A, g->d_scale, g->d_diag,
-      g->d_gs, g->d_state, lo);
-  lm_persist_kernel<<<1, 256, 0, st>>>(g->d_packed[0], g->d_red_offset, N, g->d_scale, g->d_diag,
-                                       g->d_state, lo);
+      g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), g->dev.d_block_nodes.get(), N, g->E, n, g->dev.d_A.get(),
+      g->dev.d_scale.get(), g->dev.d_diag.get(), g->dev.d_gs.get(), g->dev.d_state.get(), lo);
+  lm_persist_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), N, g->dev.d_scale.get(),
+                                       g->dev.d_diag.get(), g->dev.d_state.get(), lo);
 }
 
 // ------------------------------------------------------------------ edge covariances
@@ -763,16 +763,15 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
   for (int k = 0; k < 16 * m; ++k) cov[k] = 0.0;   // constant blocks: zero covariance
   if (n == 0 || cols.empty()) return VGX_OK;
   cudaStream_t st = c->stream;
-  rc = eval_enqueue(c, g, g->d_x, g->d_packed[0], true, false);
+  rc = eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, false);
   if (rc != VGX_OK) return rc;
   const size_t M = (size_t)n + 1;
   // scratch: requested column indices | X (ncols x n)
   const size_t ncols = cols.size();
-  const size_t x_off = (sizeof(int) * ncols + 255) & ~(size_t)255;
-  rc = c->ensure_scratch(x_off + sizeof(double) * ncols * (size_t)n);
+  int* d_cols;
+  double* d_X;
+  rc = vgx_carve(c, c->d_scratch, vgx_part(d_cols, ncols), vgx_part(d_X, ncols * (size_t)n));
   if (rc != VGX_OK) return rc;
-  int* d_cols = (int*)c->d_scratch;
-  double* d_X = (double*)((char*)c->d_scratch + x_off);
   size_t no_smem = 0;
   int coop_grid = 0;
   rc = chol_dispatch(c, n, false, &no_smem, &coop_grid);
@@ -785,16 +784,17 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
   lo.min_lm_diagonal = 0.0;
   lo.max_lm_diagonal = INFINITY;
   lo.jacobi_scaling = 0;
-  LmState* init = g->h_state;   // pinned: the copy stays asynchronous (the stream is synchronised below)
+  LmState* init = g->h_state.get();   // pinned: the copy stays asynchronous (the stream is synchronised below)
   memset(init, 0, sizeof(*init));
   init->radius = INFINITY;
   init->step_valid = 1;
-  VGX_CUDA(c, cudaMemsetAsync(g->d_A, 0, sizeof(double) * M * M, st));
-  VGX_CUDA(c, cudaMemcpyAsync(g->d_state, init, sizeof(*init), cudaMemcpyHostToDevice, st));
+  VGX_CUDA(c, cudaMemsetAsync(g->dev.d_A.get(), 0, sizeof(double) * M * M, st));
+  VGX_CUDA(c, cudaMemcpyAsync(g->dev.d_state.get(), init, sizeof(*init), cudaMemcpyHostToDevice, st));
   {
     VgxLaunchScope s(c, VGX_SLOT_SOLVE, 3);
     enqueue_lm_build(st, g, n, lo);
-    VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->d_A, n, g->d_state, g->d_diag, VGX_COV_RANK_TOL));
+    VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->dev.d_A.get(), n, g->dev.d_state.get(), g->dev.d_diag.get(),
+                                 VGX_COV_RANK_TOL));
   }
   VGX_CUDA(c, cudaGetLastError());
   // inverse columns
@@ -804,13 +804,13 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
                                      (int)(sizeof(double) * (size_t)n)));
   {
     VgxLaunchScope s(c, VGX_SLOT_SOLVE);
-    cov_column_kernel<<<(unsigned)ncols, 256, sizeof(double) * (size_t)n, st>>>(g->d_A, n, d_cols, d_X);
+    cov_column_kernel<<<(unsigned)ncols, 256, sizeof(double) * (size_t)n, st>>>(g->dev.d_A.get(), n, d_cols, d_X);
   }
   VGX_CUDA(c, cudaGetLastError());
   std::vector<double> X(ncols * (size_t)n);
   LmState hs;
   VGX_CUDA(c, cudaMemcpyAsync(X.data(), d_X, sizeof(double) * X.size(), cudaMemcpyDeviceToHost, st));
-  VGX_CUDA(c, cudaMemcpyAsync(&hs, g->d_state, sizeof(hs), cudaMemcpyDeviceToHost, st));
+  VGX_CUDA(c, cudaMemcpyAsync(&hs, g->dev.d_state.get(), sizeof(hs), cudaMemcpyDeviceToHost, st));
   VGX_CUDA(c, cudaStreamSynchronize(st));
   if (!hs.step_valid)   // a pivot failed the rank rule above (ceres::Covariance::Compute returns false)
     VGX_FAIL(c, VGX_ERR_INVALID, "vgx_graph_edge_covariances: J^T J is not positive definite (rank deficient)");
@@ -895,62 +895,68 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
   // a snapshot the decide kernel writes); every kernel of an iteration returns at once when the
   // solve has ended, so the speculative iteration after the last one is a row of empty launches
   // that drain while the host already returns.  Multi-rank: no run-ahead (the ranks stay in step).
-  rc = eval_enqueue(c, g, g->d_x, g->d_packed[0], true, excl);
+  rc = eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, excl);
   if (rc != VGX_OK) return rc;
   {
     VgxLaunchScope s(c, VGX_SLOT_SOLVE);
-    lm_init_kernel<<<1, 256, 0, st>>>(g->d_packed[0], g->d_red_offset, N, g->d_state,
+    lm_init_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), N, g->dev.d_state.get(),
                                       o->initial_trust_region_radius, lo);
   }
-  VGX_CUDA(c, cudaMemcpyAsync(g->h_state, g->d_state, sizeof(LmState), cudaMemcpyDeviceToHost, st));
+  VGX_CUDA(c, cudaMemcpyAsync(g->h_state.get(), g->dev.d_state.get(), sizeof(LmState), cudaMemcpyDeviceToHost, st));
   VGX_CUDA(c, cudaStreamSynchronize(st));
-  S.initial_cost = g->h_state->cost;
+  S.initial_cost = g->h_state.get()->cost;
   bool timed_out = false;
   static const char* no_spec = getenv("VGX_LM_NO_RUNAHEAD");
   const int ahead = (c->nranks == 1 && !(no_spec && no_spec[0] == '1')) ? 1 : 0;
   // VGX_CHOL_DEBUG=1: phase cycle counts of the last shared-memory Cholesky, printed after the solve
   static const char* chol_dbg_env = getenv("VGX_CHOL_DEBUG");
-  long long* d_chol_dbg = nullptr;
-  if (chol_dbg_env && chol_dbg_env[0] == '1' && use_smem_chol) cudaMalloc((void**)&d_chol_dbg, 8 * sizeof(long long));
-  const int* skip = &g->d_state->done;
+  VgxBuffer<long long> chol_dbg;
+  if (chol_dbg_env && chol_dbg_env[0] == '1' && use_smem_chol)
+    chol_dbg.alloc(c, 8 * sizeof(long long), "VGX_CHOL_DEBUG");
+  long long* d_chol_dbg = chol_dbg.get();
+  const int* skip = &g->dev.d_state.get()->done;
   auto enqueue_iteration = [&](int k) -> int {
     {
       VgxLaunchScope s(c, VGX_SLOT_SOLVE, 4);
       if (!use_smem_chol)   // the shared-memory solver reads the written blocks only
-        VGX_CUDA(c, cudaMemsetAsync(g->d_A, 0, sizeof(double) * (size_t)(n + 1) * (n + 1), st));
+        VGX_CUDA(c, cudaMemsetAsync(g->dev.d_A.get(), 0, sizeof(double) * (size_t)(n + 1) * (n + 1), st));
       enqueue_lm_build(st, g, n, lo);
       if (use_smem_chol) {
-        chol_solve_smem_kernel<<<1, 512, smem_chol_bytes, st>>>(g->d_A, n, g->d_step, g->d_state, g->d_red_offset,
-                                                                g->d_block_nodes, N, g->E, d_chol_dbg);
+        chol_solve_smem_kernel<<<1, 512, smem_chol_bytes, st>>>(g->dev.d_A.get(), n, g->dev.d_step.get(),
+                                                                g->dev.d_state.get(), g->dev.d_red_offset.get(),
+                                                                g->dev.d_block_nodes.get(), N, g->E, d_chol_dbg);
       } else {
         // LM: sign test only (as Eigen's LLT in the reference)
-        VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->d_A, n, g->d_state, nullptr, 0.0));
+        VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->dev.d_A.get(), n, g->dev.d_state.get(), nullptr, 0.0));
       }
-      lm_step_kernel<<<1, 1024, sizeof(double) * n, st>>>(g->d_A, n, N, g->d_red_offset, g->d_scale,
-                                                         g->d_diag, g->d_gs, g->d_x, g->d_xc, g->d_step,
-                                                         g->d_state, use_smem_chol ? g->d_step : nullptr);
+      lm_step_kernel<<<1, 1024, sizeof(double) * n, st>>>(g->dev.d_A.get(), n, N, g->dev.d_red_offset.get(),
+                                                         g->dev.d_scale.get(), g->dev.d_diag.get(), g->dev.d_gs.get(),
+                                                         g->dev.d_x.get(), g->dev.d_xc.get(), g->dev.d_step.get(),
+                                                         g->dev.d_state.get(),
+                                                         use_smem_chol ? g->dev.d_step.get() : nullptr);
     }
     VGX_CUDA(c, cudaGetLastError());
     // candidate evaluated with Jacobians so an accepted step needs no second pass
-    int rc2 = eval_enqueue(c, g, g->d_xc, g->d_packed[1], true, excl, skip);
+    int rc2 = eval_enqueue(c, g, g->dev.d_xc.get(), g->dev.d_packed[1].get(), true, excl, skip);
     if (rc2 != VGX_OK) return rc2;
     {
       VgxLaunchScope s(c, VGX_SLOT_SOLVE, 2);
-      lm_decide_kernel<<<1, 256, 0, st>>>(g->d_packed[0], g->d_packed[1], g->d_red_offset, N, g->d_x,
-                                          g->d_xc, g->d_state, lo, 1, g->d_snap + (k & 1));
+      lm_decide_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_packed[1].get(), g->dev.d_red_offset.get(),
+                                          N, g->dev.d_x.get(), g->dev.d_xc.get(), g->dev.d_state.get(), lo, 1,
+                                          g->dev.d_snap.get() + (k & 1));
       lm_accept_kernel<<<std::max(1, std::min(64, (int)(g->packed_len / 2048))), 256, 0, st>>>(
-          g->d_packed[1], g->d_packed[0], g->packed_len, g->d_state);
+          g->dev.d_packed[1].get(), g->dev.d_packed[0].get(), g->packed_len, g->dev.d_state.get());
     }
     VGX_CUDA(c, cudaGetLastError());
     // outcome of iteration k -> host, on the copy stream (the main stream keeps running ahead)
     VGX_CUDA(c, cudaEventRecord(g->ev_iter[k & 1], st));
     VGX_CUDA(c, cudaStreamWaitEvent(g->copy_stream, g->ev_iter[k & 1], 0));
-    VGX_CUDA(c, cudaMemcpyAsync(g->h_snap + (k & 1), g->d_snap + (k & 1), sizeof(LmState),
+    VGX_CUDA(c, cudaMemcpyAsync(g->h_snap.get() + (k & 1), g->dev.d_snap.get() + (k & 1), sizeof(LmState),
                                 cudaMemcpyDeviceToHost, g->copy_stream));
     VGX_CUDA(c, cudaEventRecord(g->ev_copy[k & 1], g->copy_stream));
     return VGX_OK;
   };
-  bool run = !g->h_state->done && n > 0;
+  bool run = !g->h_state.get()->done && n > 0;
   if (run) {
     int enq = 0, k = 0;   // iterations enqueued / the one whose outcome is awaited
     for (;;) {
@@ -962,40 +968,39 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
         ++enq;
       }
       VGX_CUDA(c, cudaEventSynchronize(g->ev_copy[k & 1]));
-      *g->h_state = g->h_snap[k & 1];
-      if (g->h_state->done) break;
+      *g->h_state.get() = g->h_snap.get()[k & 1];
+      if (g->h_state.get()->done) break;
       if (c->nranks == 1 && wall_s() - t0 >= o->max_solver_time_s) { timed_out = true; break; }
       ++k;
     }
     if (timed_out) VGX_CUDA(c, cudaStreamSynchronize(st));   // iterations in flight still move x
     // final poses: the main stream may still be draining the empty launches of the speculative
     // iteration; the copy stream is ordered after the deciding iteration only
-    VGX_CUDA(c, cudaMemcpyAsync(g->h_x, g->d_x, sizeof(double) * 4 * N, cudaMemcpyDeviceToHost,
+    VGX_CUDA(c, cudaMemcpyAsync(g->h_x.get(), g->dev.d_x.get(), sizeof(double) * 4 * N, cudaMemcpyDeviceToHost,
                                 timed_out ? st : g->copy_stream));
     VGX_CUDA(c, cudaStreamSynchronize(timed_out ? st : g->copy_stream));
     if (timed_out) {
-      VGX_CUDA(c, cudaMemcpyAsync(g->h_state, g->d_state, sizeof(LmState), cudaMemcpyDeviceToHost, st));
+      VGX_CUDA(c, cudaMemcpyAsync(g->h_state.get(), g->dev.d_state.get(), sizeof(LmState), cudaMemcpyDeviceToHost, st));
       VGX_CUDA(c, cudaStreamSynchronize(st));
     }
-    memcpy(g->x.data(), g->h_x, sizeof(double) * 4 * N);
+    memcpy(g->x.data(), g->h_x.get(), sizeof(double) * 4 * N);
   } else {
-    VGX_CUDA(c, cudaMemcpyAsync(g->x.data(), g->d_x, sizeof(double) * 4 * N, cudaMemcpyDeviceToHost, st));
+    VGX_CUDA(c, cudaMemcpyAsync(g->x.data(), g->dev.d_x.get(), sizeof(double) * 4 * N, cudaMemcpyDeviceToHost, st));
     VGX_CUDA(c, cudaStreamSynchronize(st));
   }
-  if (n == 0) { g->h_state->termination = 2; }
+  if (n == 0) { g->h_state.get()->termination = 2; }
   if (d_chol_dbg) {
     long long h[5] = {0, 0, 0, 0, 0};
     cudaStreamSynchronize(st);
     cudaMemcpy(h, d_chol_dbg, sizeof(h), cudaMemcpyDeviceToHost);
     fprintf(stderr, "[vgx] chol n=%d cycles: load %lld update %lld factor+solve %lld back %lld total %lld\n", n, h[0],
             h[1], h[2], h[3], h[4]);
-    cudaFree(d_chol_dbg);
   }
-  S.iterations = g->h_state->iterations;
-  S.num_successful_steps = g->h_state->successful;
-  S.num_residual_evals = g->h_state->evals;
-  S.termination = timed_out ? 4 : g->h_state->termination;
-  S.final_cost = g->h_state->cost;
+  S.iterations = g->h_state.get()->iterations;
+  S.num_successful_steps = g->h_state.get()->successful;
+  S.num_residual_evals = g->h_state.get()->evals;
+  S.termination = timed_out ? 4 : g->h_state.get()->termination;
+  S.final_cost = g->h_state.get()->cost;
   S.total_time_s = wall_s() - t0;
   if (xyzyaw_out) memcpy(xyzyaw_out, g->x.data(), sizeof(double) * 4 * N);
   if (summary) *summary = S;

@@ -13,41 +13,6 @@
 #include "vgx_internal.h"
 
 // ------------------------------------------------------------------ context
-int vgx_ctx::ensure_scratch(size_t bytes) {
-  if (bytes <= scratch_bytes) return VGX_OK;
-  if (d_scratch) cudaFree(d_scratch);
-  d_scratch = nullptr;
-  scratch_bytes = 0;
-  size_t want = bytes + bytes / 4;
-  VGX_CUDA(this, cudaMalloc(&d_scratch, want));
-  scratch_bytes = want;
-  return VGX_OK;
-}
-
-int vgx_ctx::ensure_pinned(size_t bytes) {
-  if (bytes <= pinned_bytes) return VGX_OK;
-  if (h_pinned) cudaFreeHost(h_pinned);
-  h_pinned = nullptr;
-  pinned_bytes = 0;
-  size_t want = bytes + bytes / 4;
-  VGX_CUDA(this, cudaMallocHost(&h_pinned, want));
-  pinned_bytes = want;
-  return VGX_OK;
-}
-
-static int grow(vgx_ctx* c, void** p, size_t* cap, size_t bytes) {
-  if (bytes <= *cap) return VGX_OK;
-  if (*p) cudaFree(*p);
-  *p = nullptr;
-  *cap = 0;
-  const size_t want = bytes + bytes / 4;
-  VGX_CUDA(c, cudaMalloc(p, want));
-  *cap = want;
-  return VGX_OK;
-}
-int vgx_ctx::ensure_sort(size_t bytes) { return grow(this, &d_sort, &sort_bytes, bytes); }
-int vgx_ctx::ensure_sort2(size_t bytes) { return grow(this, &d_sort2, &sort2_bytes, bytes); }
-
 extern "C" int vgx_device_count(void) {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;
@@ -73,28 +38,6 @@ extern "C" int vgx_ctx_create(int device, vgx_ctx** out) {
   return VGX_OK;
 }
 
-static void free_points(VgxPoints& p) {
-  if (p.data) cudaFree(p.data);
-  p = VgxPoints();
-}
-
-static void free_submap(VgxSubmap* s) {
-  if (!s) return;
-  cudaFree(s->hash.entries);
-  cudaFree(s->d_block_idx);
-  cudaFree(s->d_dw);
-  cudaFree(s->d_view);
-  cudaFree(s->d_esdf);
-  cudaFree(s->d_view_esdf);
-  cudaFree(s->d_counters);
-  cudaFree(s->d_grid);
-  cudaFree(s->d_grid16);
-  cudaFree(s->d_iso_idx);
-  free_points(s->points[0]);
-  free_points(s->points[1]);
-  delete s;
-}
-
 extern "C" void vgx_ctx_destroy(vgx_ctx* c) {
   if (!c) return;
   cudaSetDevice(c->device);
@@ -102,12 +45,7 @@ extern "C" void vgx_ctx_destroy(vgx_ctx* c) {
   vgx_comm_destroy(c);
   vgx_p2p_free(c);
   vgx_graph_free(c);
-  vgx_mesh_free(c);
-  for (auto& kv : c->submaps) free_submap(kv.second);
-  if (c->d_scratch) cudaFree(c->d_scratch);
-  if (c->d_sort) cudaFree(c->d_sort);
-  if (c->d_sort2) cudaFree(c->d_sort2);
-  if (c->h_pinned) cudaFreeHost(c->h_pinned);
+  for (auto& kv : c->submaps) delete kv.second;
   cudaEventDestroy(c->ev0);
   cudaEventDestroy(c->ev1);
   cudaStreamDestroy(c->stream);
@@ -183,7 +121,7 @@ __global__ void hash_insert_kernel(VgxHash h, const int32_t* block_idx, int n, i
 // new submap is dropped and the upload fails.
 static int check_uploaded_blocks(vgx_ctx* c, VgxSubmap* s, const char* what) {
   int bad = 0;
-  VGX_CUDA(c, cudaMemcpyAsync(&bad, s->d_counters + 2, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  VGX_CUDA(c, cudaMemcpyAsync(&bad, s->d_counters.get() + 2, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   if (!bad) return VGX_OK;
   vgx_submap_drop(c, s->id);
@@ -252,15 +190,13 @@ __global__ void deinterleave_kernel(const float2* __restrict__ dw, float* __rest
 // Dense block index over the blocks' AABB (host-built: off the hot path, once per finished submap).
 #define VGX_GRID_MAX_CELLS 4096
 int vgx_submap_build_grid(vgx_ctx* c, VgxSubmap* s) {
-  cudaFree(s->d_grid);
-  cudaFree(s->d_grid16);
-  s->d_grid = nullptr;
-  s->d_grid16 = nullptr;
+  s->d_grid.reset();
+  s->d_grid16.reset();
   s->grid_dim[0] = s->grid_dim[1] = s->grid_dim[2] = 0;
   const int n = s->n_blocks;
   if (n <= 0) return VGX_OK;
   std::vector<int32_t> idx(3 * (size_t)n);
-  VGX_CUDA(c, cudaMemcpyAsync(idx.data(), s->d_block_idx, sizeof(int32_t) * 3 * n, cudaMemcpyDeviceToHost,
+  VGX_CUDA(c, cudaMemcpyAsync(idx.data(), s->d_block_idx.get(), sizeof(int32_t) * 3 * n, cudaMemcpyDeviceToHost,
                               c->stream));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
@@ -277,13 +213,15 @@ int vgx_submap_build_grid(vgx_ctx* c, VgxSubmap* s) {
   for (int i = 0; i < n; ++i)
     grid[(size_t)(idx[3 * i + 2] - lo[2]) * dy * dx + (size_t)(idx[3 * i + 1] - lo[1]) * dx +
          (idx[3 * i] - lo[0])] = i;
-  VGX_CUDA(c, cudaMalloc(&s->d_grid, sizeof(int32_t) * cells));
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_grid, grid.data(), sizeof(int32_t) * cells, cudaMemcpyHostToDevice, c->stream));
+  int rc = s->d_grid.alloc(c, sizeof(int32_t) * cells, "dense block grid");
+  if (rc != VGX_OK) return rc;
+  VGX_CUDA(c, cudaMemcpyAsync(s->d_grid.get(), grid.data(), sizeof(int32_t) * cells, cudaMemcpyHostToDevice, c->stream));
   // 16-bit copy for the registration kernel's shared-memory grid (one bulk copy per tile)
   std::vector<uint16_t> g16(((size_t)cells + 7) & ~(size_t)7, 0xFFFF);
   for (long long k = 0; k < cells; ++k) g16[(size_t)k] = grid[(size_t)k] < 0 ? 0xFFFF : (uint16_t)grid[(size_t)k];
-  VGX_CUDA(c, cudaMalloc(&s->d_grid16, sizeof(uint16_t) * g16.size()));
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_grid16, g16.data(), sizeof(uint16_t) * g16.size(), cudaMemcpyHostToDevice, c->stream));
+  rc = s->d_grid16.alloc(c, sizeof(uint16_t) * g16.size(), "dense block grid");
+  if (rc != VGX_OK) return rc;
+  VGX_CUDA(c, cudaMemcpyAsync(s->d_grid16.get(), g16.data(), sizeof(uint16_t) * g16.size(), cudaMemcpyHostToDevice, c->stream));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   for (int a = 0; a < 3; ++a) { s->grid_min[a] = lo[a]; s->grid_dim[a] = hi[a] - lo[a] + 1; }
   return VGX_OK;
@@ -292,7 +230,7 @@ int vgx_submap_build_grid(vgx_ctx* c, VgxSubmap* s) {
 int vgx_submap_build_view(vgx_ctx* c, VgxSubmap* s, const float2* bricks, float* view) {
   const size_t used = (size_t)s->n_blocks * s->vox_per_block;
   if (used == 0) return VGX_OK;
-  build_view_kernel<<<(unsigned)((used + 255) / 256), 256, 0, c->stream>>>(bricks, s->d_block_idx, s->hash, view,
+  build_view_kernel<<<(unsigned)((used + 255) / 256), 256, 0, c->stream>>>(bricks, s->d_block_idx.get(), s->hash(), view,
                                                                           s->n_blocks, s->vps, s->sh);
   c->launches++;
   VGX_CUDA(c, cudaGetLastError());
@@ -300,10 +238,10 @@ int vgx_submap_build_view(vgx_ctx* c, VgxSubmap* s, const float2* bricks, float*
 }
 
 int vgx_submap_rebuild_hash(vgx_ctx* c, VgxSubmap* s) {
-  const uint32_t tsize = s->hash.mask + 1;
-  hash_clear_kernel<<<(tsize + 255) / 256, 256, 0, c->stream>>>(s->hash.entries, tsize);
+  const uint32_t tsize = s->hash_mask + 1;
+  hash_clear_kernel<<<(tsize + 255) / 256, 256, 0, c->stream>>>(s->d_hash.get(), tsize);
   if (s->n_blocks > 0)
-    hash_insert_kernel<<<(s->n_blocks + 127) / 128, 128, 0, c->stream>>>(s->hash, s->d_block_idx, s->n_blocks,
+    hash_insert_kernel<<<(s->n_blocks + 127) / 128, 128, 0, c->stream>>>(s->hash(), s->d_block_idx.get(), s->n_blocks,
                                                                          nullptr);
   c->launches += 2;
   VGX_CUDA(c, cudaGetLastError());
@@ -325,7 +263,7 @@ int vgx_submap_alloc(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int cap
   VgxSubmap* old = c->find(id);
   if (old) {
     VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    free_submap(old);
+    delete old;
     c->submaps.erase(id);
     vgx_graph_invalidate_registration(c);
   }
@@ -343,22 +281,21 @@ int vgx_submap_alloc(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int cap
   s->vox_per_block = vps * vps * vps;
   s->cap_blocks = cap > 0 ? cap : 1;
   const uint32_t tsize = table_size_for(s->cap_blocks);
-  s->hash.mask = tsize - 1;
+  s->hash_mask = tsize - 1;
   const size_t nvox = (size_t)s->cap_blocks * s->vox_per_block;
-  cudaError_t e = cudaSuccess;
-  if (e == cudaSuccess) e = cudaMalloc(&s->hash.entries, sizeof(VgxHashEntry) * tsize);
-  if (e == cudaSuccess) e = cudaMalloc(&s->d_block_idx, sizeof(int32_t) * 3 * s->cap_blocks);
-  if (e == cudaSuccess) e = cudaMalloc(&s->d_dw, sizeof(float2) * nvox);
-  if (e == cudaSuccess && with_view) e = cudaMalloc(&s->d_view, sizeof(float) * 8 * nvox);
-  if (e == cudaSuccess) e = cudaMalloc(&s->d_counters, sizeof(int) * 4);
-  if (e != cudaSuccess) {
-    free_submap(s);
-    c->set_error(std::string("submap allocation: ") + cudaGetErrorString(e));
-    return e == cudaErrorMemoryAllocation ? VGX_ERR_NOMEM : VGX_ERR_CUDA;
+  const char* what = "submap allocation";
+  int rc = s->d_hash.alloc(c, sizeof(VgxHashEntry) * tsize, what, VGX_ERR_NOMEM);
+  if (rc == VGX_OK) rc = s->d_block_idx.alloc(c, sizeof(int32_t) * 3 * s->cap_blocks, what, VGX_ERR_NOMEM);
+  if (rc == VGX_OK) rc = s->d_dw.alloc(c, sizeof(float2) * nvox, what, VGX_ERR_NOMEM);
+  if (rc == VGX_OK && with_view) rc = s->d_view.alloc(c, sizeof(float) * 8 * nvox, what, VGX_ERR_NOMEM);
+  if (rc == VGX_OK) rc = s->d_counters.alloc(c, sizeof(int) * 4, what, VGX_ERR_NOMEM);
+  if (rc != VGX_OK) {
+    delete s;
+    return rc;
   }
-  hash_clear_kernel<<<(tsize + 255) / 256, 256, 0, c->stream>>>(s->hash.entries, tsize);
+  hash_clear_kernel<<<(tsize + 255) / 256, 256, 0, c->stream>>>(s->d_hash.get(), tsize);
   c->launches++;
-  VGX_CUDA(c, cudaMemsetAsync(s->d_counters, 0, sizeof(int) * 4, c->stream));
+  VGX_CUDA(c, cudaMemsetAsync(s->d_counters.get(), 0, sizeof(int) * 4, c->stream));
   c->submaps[id] = s;
   *out = s;
   return VGX_OK;
@@ -377,15 +314,14 @@ extern "C" int vgx_submap_upload(vgx_ctx* c, uint32_t id, float voxel_size, int 
   s->finished = true;
   if (n_blocks == 0) return VGX_OK;
   const size_t nvox = (size_t)n_blocks * s->vox_per_block;
-  rc = c->ensure_scratch(2 * nvox * sizeof(float));
+  float *tmp_d, *tmp_w;
+  rc = vgx_carve(c, c->d_scratch, vgx_part(tmp_d, nvox), vgx_part(tmp_w, nvox));
   if (rc != VGX_OK) return rc;
-  float* tmp_d = (float*)c->d_scratch;
-  float* tmp_w = tmp_d + nvox;
   VGX_CUDA(c, cudaMemcpyAsync(tmp_d, distance, nvox * sizeof(float), cudaMemcpyHostToDevice, c->stream));
   VGX_CUDA(c, cudaMemcpyAsync(tmp_w, weight, nvox * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx, block_idx, sizeof(int32_t) * 3 * n_blocks,
+  VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx.get(), block_idx, sizeof(int32_t) * 3 * n_blocks,
                               cudaMemcpyHostToDevice, c->stream));
-  interleave_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(tmp_d, tmp_w, s->d_dw, nvox);
+  interleave_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(tmp_d, tmp_w, s->d_dw.get(), nvox);
   c->launches++;
   // synchronises: the host buffers are the caller's
   return vgx_submap_upload_finish(c, s, "vgx_submap_upload");
@@ -398,8 +334,8 @@ extern "C" int vgx_submap_peek_device(vgx_ctx* c, uint32_t id, const int32_t** d
   if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_peek_device: unknown submap");
   VGX_CUDA(c, cudaSetDevice(c->device));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // the caller reads the bricks on its own stream
-  if (d_block_idx) *d_block_idx = s->d_block_idx;
-  if (d_dw) *d_dw = reinterpret_cast<const float*>(s->d_dw);
+  if (d_block_idx) *d_block_idx = s->d_block_idx.get();
+  if (d_dw) *d_dw = reinterpret_cast<const float*>(s->d_dw.get());
   if (n_blocks) *n_blocks = s->n_blocks;
   return VGX_OK;
 }
@@ -416,19 +352,20 @@ extern "C" int vgx_submap_upload_device(vgx_ctx* c, uint32_t id, float voxel_siz
   s->finished = true;
   if (n_blocks == 0) return VGX_OK;
   const size_t nvox = (size_t)n_blocks * s->vox_per_block;
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx, d_block_idx, sizeof(int32_t) * 3 * n_blocks, cudaMemcpyDeviceToDevice, c->stream));
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_dw, d_dw, sizeof(float2) * nvox, cudaMemcpyDeviceToDevice, c->stream));
+  VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx.get(), d_block_idx, sizeof(int32_t) * 3 * n_blocks,
+                              cudaMemcpyDeviceToDevice, c->stream));
+  VGX_CUDA(c, cudaMemcpyAsync(s->d_dw.get(), d_dw, sizeof(float2) * nvox, cudaMemcpyDeviceToDevice, c->stream));
   // synchronises: the source buffers are the caller's
   return vgx_submap_upload_finish(c, s, "vgx_submap_upload_device");
 }
 
 int vgx_submap_upload_finish(vgx_ctx* c, VgxSubmap* s, const char* what) {
   if (s->n_blocks == 0) return VGX_OK;
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_counters, &s->n_blocks, sizeof(int), cudaMemcpyHostToDevice, c->stream));
-  hash_insert_kernel<<<(s->n_blocks + 127) / 128, 128, 0, c->stream>>>(s->hash, s->d_block_idx, s->n_blocks,
-                                                                       s->d_counters + 2);
+  VGX_CUDA(c, cudaMemcpyAsync(s->d_counters.get(), &s->n_blocks, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  hash_insert_kernel<<<(s->n_blocks + 127) / 128, 128, 0, c->stream>>>(s->hash(), s->d_block_idx.get(), s->n_blocks,
+                                                                       s->d_counters.get() + 2);
   c->launches++;
-  int rc = vgx_submap_build_view(c, s, s->d_dw, s->d_view);
+  int rc = vgx_submap_build_view(c, s, s->d_dw.get(), s->d_view.get());
   if (rc != VGX_OK) return rc;
   rc = check_uploaded_blocks(c, s, what);
   if (rc != VGX_OK) return rc;
@@ -442,7 +379,7 @@ extern "C" int vgx_submap_create(vgx_ctx* c, uint32_t id, float voxel_size, int 
   int rc = vgx_submap_alloc(c, id, voxel_size, vps, capacity, false, &s);
   if (rc != VGX_OK) return rc;
   // new voxblox blocks are zero-initialised (distance 0, weight 0)
-  VGX_CUDA(c, cudaMemsetAsync(s->d_dw, 0, sizeof(float2) * (size_t)capacity * s->vox_per_block,
+  VGX_CUDA(c, cudaMemsetAsync(s->d_dw.get(), 0, sizeof(float2) * (size_t)capacity * s->vox_per_block,
                               c->stream));
   s->finished = false;
   return VGX_OK;
@@ -456,8 +393,11 @@ extern "C" int vgx_submap_finish(vgx_ctx* c, uint32_t id) {
   // the layer is frozen from here on: the view only needs the blocks that exist, not the
   // integration capacity (128 KiB per brick)
   const size_t used = (size_t)s->n_blocks * s->vox_per_block;
-  if (!s->d_view) VGX_CUDA(c, cudaMalloc(&s->d_view, sizeof(float) * 8 * (used > 0 ? used : 1)));
-  const int rc = vgx_submap_build_view(c, s, s->d_dw, s->d_view);
+  if (!s->d_view.get()) {
+    const int rc = s->d_view.alloc(c, sizeof(float) * 8 * (used > 0 ? used : 1), "registration view");
+    if (rc != VGX_OK) return rc;
+  }
+  const int rc = vgx_submap_build_view(c, s, s->d_dw.get(), s->d_view.get());
   if (rc != VGX_OK) return rc;
   s->finished = true;
   vgx_graph_invalidate_registration(c);
@@ -470,7 +410,7 @@ extern "C" int vgx_submap_free(vgx_ctx* c, uint32_t id) {
   if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_free: unknown submap");
   VGX_CUDA(c, cudaSetDevice(c->device));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  free_submap(s);
+  delete s;
   c->submaps.erase(id);
   vgx_graph_invalidate_registration(c);
   return VGX_OK;
@@ -488,7 +428,7 @@ int vgx_submap_move(vgx_ctx* c, uint32_t from_id, uint32_t id) {
   if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_move: unknown submap");
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   VgxSubmap* old = c->find(id);
-  if (old) free_submap(old);
+  delete old;
   c->submaps.erase(from_id);
   s->id = id;
   c->submaps[id] = s;
@@ -534,14 +474,13 @@ extern "C" int vgx_submap_download(vgx_ctx* c, uint32_t id, int max_blocks, int3
   if (n == 0) return VGX_OK;
   const size_t nvox = (size_t)n * s->vox_per_block;
   if (block_idx)
-    VGX_CUDA(c, cudaMemcpyAsync(block_idx, s->d_block_idx, sizeof(int32_t) * 3 * n,
+    VGX_CUDA(c, cudaMemcpyAsync(block_idx, s->d_block_idx.get(), sizeof(int32_t) * 3 * n,
                                 cudaMemcpyDeviceToHost, c->stream));
   if (distance || weight) {
-    int rc = c->ensure_scratch(2 * nvox * sizeof(float));
+    float *tmp_d, *tmp_w;
+    int rc = vgx_carve(c, c->d_scratch, vgx_part(tmp_d, nvox), vgx_part(tmp_w, nvox));
     if (rc != VGX_OK) return rc;
-    float* tmp_d = (float*)c->d_scratch;
-    float* tmp_w = tmp_d + nvox;
-    deinterleave_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(s->d_dw, tmp_d, tmp_w, nvox);
+    deinterleave_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(s->d_dw.get(), tmp_d, tmp_w, nvox);
     c->launches++;
     VGX_CUDA(c, cudaGetLastError());
     if (distance)
@@ -563,15 +502,15 @@ extern "C" int vgx_submap_upload_points(vgx_ctx* c, uint32_t id, int type, int n
   VGX_CUDA(c, cudaSetDevice(c->device));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   VgxPoints& p = s->points[type];
-  free_points(p);
+  p = VgxPoints();
   vgx_graph_invalidate_registration(c);
   if (n == 0) return VGX_OK;
   // unit-major AoSoA staging on the host (pinned): unit u = {x[32], y[32], z[32], d[32], w[32]}
   const size_t units = ((size_t)n + VGX_PT_UNIT - 1) / VGX_PT_UNIT;
   const size_t floats = units * VGX_PT_UNIT_FLOATS;
-  int rc = c->ensure_pinned(floats * sizeof(float));
+  float* h;
+  int rc = vgx_carve(c, c->h_pinned, vgx_part(h, floats));
   if (rc != VGX_OK) return rc;
-  float* h = (float*)c->h_pinned;
   memset(h, 0, floats * sizeof(float));
   double sum_w = 0;
   std::vector<double> cumulative((size_t)n);
@@ -585,17 +524,17 @@ extern "C" int vgx_submap_upload_points(vgx_ctx* c, uint32_t id, int type, int n
     sum_w += (double)weight[i];  // cpp:124, in point order
     cumulative[i] = sum_w;       // WeightedSampler::addItem (weighted_sampler_inl.h:6-17)
   }
-  float* d = nullptr;
-  VGX_CUDA(c, cudaMalloc(&d, floats * sizeof(float)));
-  cudaError_t e = cudaMemcpyAsync(d, h, floats * sizeof(float), cudaMemcpyHostToDevice, c->stream);
+  VgxBuffer<float> d;
+  rc = d.alloc(c, floats * sizeof(float), "points upload");
+  if (rc != VGX_OK) return rc;
+  cudaError_t e = cudaMemcpyAsync(d.get(), h, floats * sizeof(float), cudaMemcpyHostToDevice, c->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
   if (e != cudaSuccess) {
-    cudaFree(d);
     c->set_error(std::string("points upload: ") + cudaGetErrorString(e));
     return VGX_ERR_CUDA;
   }
   p.n = n;
-  p.data = d;
+  p.data = std::move(d);
   p.sum_w = sum_w;
   p.cumulative_w.swap(cumulative);
   return VGX_OK;

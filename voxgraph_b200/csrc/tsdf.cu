@@ -588,16 +588,13 @@ extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7],
     if (stats) *stats = st;
     return VGX_OK;
   }
-  // scratch: points | stats[4] | (fast) two 2^20-entry approximate sets
-  const size_t pts_bytes = ((sizeof(float) * 3 * (size_t)n) + 255) & ~(size_t)255;
+  // scratch: points | stats[4] (cleared as 256 bytes) | (fast) two 2^20-entry approximate sets
   const size_t set_bytes = sizeof(unsigned long long) << 20;
-  const size_t need = pts_bytes + 256 + (P.cfg.mode == 1 ? 2 * set_bytes : 0);
-  int rc = c->ensure_scratch(need);
+  float* d_pts;
+  unsigned long long *d_stats, *d_start;
+  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_pts, 3 * (size_t)n), vgx_part(d_stats, 32),
+                     vgx_part(d_start, P.cfg.mode == 1 ? 2u << 20 : 0));
   if (rc != VGX_OK) return rc;
-  char* base = (char*)c->d_scratch;
-  float* d_pts = (float*)base;
-  unsigned long long* d_stats = (unsigned long long*)(base + pts_bytes);
-  unsigned long long* d_start = (unsigned long long*)(base + pts_bytes + 256);
   unsigned long long* d_obs = d_start + (1u << 20);
   cudaStream_t stream = c->stream;
   VGX_CUDA(c, cudaMemcpyAsync(d_pts, points_C, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice, stream));
@@ -609,16 +606,13 @@ extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7],
     // ---- ray-ordered path: allocate -> count -> scan -> emit -> stable sort by voxel -> apply
     {
       VgxLaunchScope scope(c, VGX_SLOT_TSDF_ALLOCATE);
-      tsdf_allocate_kernel<<<grid, 128, 0, stream>>>(P, d_pts, s->hash, s->d_block_idx, s->d_counters,
+      tsdf_allocate_kernel<<<grid, 128, 0, stream>>>(P, d_pts, s->hash(), s->d_block_idx.get(), s->d_counters.get(),
                                                     s->cap_blocks);
     }
-    const size_t cnt_bytes = ((sizeof(unsigned) * ((size_t)n + 2)) + 255) & ~(size_t)255;
-    const size_t scan_tmp = ((vgx_scan_tmp_count((size_t)n) * sizeof(unsigned)) + 255) & ~(size_t)255;
-    rc = c->ensure_sort(2 * cnt_bytes + scan_tmp + 256);
+    unsigned *d_counts, *d_offsets, *d_scan_tmp;
+    rc = vgx_carve(c, c->d_work, vgx_part(d_counts, (size_t)n + 2), vgx_part(d_offsets, (size_t)n + 2),
+                   vgx_part(d_scan_tmp, vgx_scan_tmp_count((size_t)n)));
     if (rc != VGX_OK) return rc;
-    unsigned* d_counts = (unsigned*)c->d_sort;
-    unsigned* d_offsets = (unsigned*)((char*)c->d_sort + cnt_bytes);
-    unsigned* d_scan_tmp = (unsigned*)((char*)c->d_sort + 2 * cnt_bytes);
     unsigned total = 0;
     {
       VgxLaunchScope scope(c, VGX_SLOT_TSDF_INTEGRATE, 1);
@@ -629,9 +623,7 @@ extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7],
     VGX_CUDA(c, cudaMemcpyAsync(&total, d_offsets + n, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
     VGX_CUDA(c, cudaStreamSynchronize(stream));
     if (total > 0) {
-      // offsets live in d_sort; the tuple buffers go to d_scratch behind the points
-      const size_t key_bytes = ((sizeof(unsigned) * (size_t)total) + 255) & ~(size_t)255;
-      const size_t val_bytes = ((sizeof(float2) * (size_t)total) + 255) & ~(size_t)255;
+      // offsets live in d_work; the tuple buffers and the sort temp go to d_work2
       // keys = slot * 4096 + voxel; the sentinel (unmapped block) is one past the largest key
       const unsigned long long sent64 = (unsigned long long)s->cap_blocks << (3 * P.vps_shift);
       if (sent64 >= 0xFFFFFFFFull) VGX_FAIL(c, VGX_ERR_CAPACITY, "submap too large for 32-bit voxel keys");
@@ -642,44 +634,40 @@ extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7],
       cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (unsigned*)nullptr, (unsigned*)nullptr,
                                       (unsigned long long*)nullptr, (unsigned long long*)nullptr,
                                       (int)total, 0, end_bit, stream);
-      const size_t heads_bytes = ((sizeof(unsigned) * ((size_t)total / VGX_TSDF_LONG_SEGMENT + 2)) + 255) & ~(size_t)255;
-      rc = c->ensure_sort2(2 * key_bytes + 2 * val_bytes + sort_tmp + heads_bytes + 1024);
+      unsigned *k_in, *k_out, *d_nlong, *d_heads;
+      float2 *v_in, *v_out;
+      char* d_sort_tmp;
+      rc = vgx_carve(c, c->d_work2, vgx_part(k_in, total), vgx_part(k_out, total), vgx_part(v_in, total),
+                     vgx_part(v_out, total), vgx_part(d_nlong, 64),
+                     vgx_part(d_heads, (size_t)total / VGX_TSDF_LONG_SEGMENT + 2), vgx_part(d_sort_tmp, sort_tmp));
       if (rc != VGX_OK) return rc;
-      char* b2 = (char*)c->d_sort2;
-      unsigned* k_in = (unsigned*)b2;
-      unsigned* k_out = (unsigned*)(b2 + key_bytes);
-      float2* v_in = (float2*)(b2 + 2 * key_bytes);
-      float2* v_out = (float2*)(b2 + 2 * key_bytes + val_bytes);
-      unsigned* d_nlong = (unsigned*)(b2 + 2 * key_bytes + 2 * val_bytes);
-      unsigned* d_heads = d_nlong + 64;
-      void* d_sort_tmp = b2 + 2 * key_bytes + 2 * val_bytes + 256 + heads_bytes;
       {
         VgxLaunchScope scope(c, VGX_SLOT_TSDF_INTEGRATE, 4);
         VGX_CUDA(c, cudaMemsetAsync(d_nlong, 0, 256, stream));
-        tsdf_emit_kernel<<<grid, 128, 0, stream>>>(P, d_pts, s->hash, d_offsets, sentinel, k_in, v_in, d_stats);
+        tsdf_emit_kernel<<<grid, 128, 0, stream>>>(P, d_pts, s->hash(), d_offsets, sentinel, k_in, v_in, d_stats);
         cub::DeviceRadixSort::SortPairs(d_sort_tmp, sort_tmp, k_in, k_out, (unsigned long long*)v_in,
                                         (unsigned long long*)v_out, (int)total, 0, end_bit, stream);
         tsdf_apply_kernel<<<(total + 255) / 256, 256, 0, stream>>>(
-            k_out, v_out, total, sentinel, s->d_dw, P.cfg.default_truncation_distance, P.cfg.max_weight,
+            k_out, v_out, total, sentinel, s->d_dw.get(), P.cfg.default_truncation_distance, P.cfg.max_weight,
             d_heads, d_nlong);
         // at most total / 64 long segments; launch enough warps, the surplus exits
         const unsigned max_long = total / VGX_TSDF_LONG_SEGMENT + 1;
         tsdf_apply_long_kernel<<<(max_long + 3) / 4, 128, 0, stream>>>(
-            k_out, v_out, total, s->d_dw, P.cfg.default_truncation_distance, P.cfg.max_weight, d_heads,
+            k_out, v_out, total, s->d_dw.get(), P.cfg.default_truncation_distance, P.cfg.max_weight, d_heads,
             d_nlong, d_stats + 3);
       }
     }
   } else {
     // ---- Fast scheduling: one kernel, blocks allocated on demand
     VgxLaunchScope scope(c, VGX_SLOT_TSDF_INTEGRATE);
-    tsdf_integrate_kernel<<<grid, 128, 0, stream>>>(P, d_pts, s->hash, s->d_block_idx, s->d_counters,
-                                                   s->cap_blocks, s->d_dw, d_stats, d_start, d_obs);
+    tsdf_integrate_kernel<<<grid, 128, 0, stream>>>(P, d_pts, s->hash(), s->d_block_idx.get(), s->d_counters.get(),
+                                                   s->cap_blocks, s->d_dw.get(), d_stats, d_start, d_obs);
   }
   VGX_CUDA(c, cudaGetLastError());
   unsigned long long h_stats[4];
   int h_counters[2];
   VGX_CUDA(c, cudaMemcpyAsync(h_stats, d_stats, sizeof(h_stats), cudaMemcpyDeviceToHost, stream));
-  VGX_CUDA(c, cudaMemcpyAsync(h_counters, s->d_counters, sizeof(h_counters), cudaMemcpyDeviceToHost, stream));
+  VGX_CUDA(c, cudaMemcpyAsync(h_counters, s->d_counters.get(), sizeof(h_counters), cudaMemcpyDeviceToHost, stream));
   VGX_CUDA(c, cudaStreamSynchronize(stream));
   const bool overflow = h_counters[1] != 0 || h_counters[0] > s->cap_blocks;
   s->n_blocks = h_counters[0] < s->cap_blocks ? h_counters[0] : s->cap_blocks;
@@ -692,7 +680,7 @@ extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7],
   if (overflow) {
     // keys without a brick must not stay in the table: rebuild it from the blocks that exist
     int fixed[2] = {s->n_blocks, 0};
-    cudaMemcpyAsync(s->d_counters, fixed, sizeof(fixed), cudaMemcpyHostToDevice, stream);
+    cudaMemcpyAsync(s->d_counters.get(), fixed, sizeof(fixed), cudaMemcpyHostToDevice, stream);
     vgx_submap_rebuild_hash(c, s);
     cudaStreamSynchronize(stream);
     VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_tsdf_integrate: submap block capacity exhausted");

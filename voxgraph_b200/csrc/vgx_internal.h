@@ -7,6 +7,7 @@
 #include <map>
 #include <random>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "voxgraph_b200.h"
@@ -26,6 +27,58 @@
     (ctx)->set_error(msg);       \
     return (code);               \
   } while (0)
+
+// ------------------------------------------------------------------ memory owner
+// The one owner of device (cudaMalloc) and page-locked host (cudaMallocHost) allocations: a buffer
+// of T that is freed by reset(), by its destructor or by a new allocation.  Move-only.  Freeing a
+// buffer the stream may still read is the owner's caller's concern: it synchronises first.
+// Kernel-facing structs hold the raw pointer, taken with get().
+enum class VgxMem { device, pinned };
+struct vgx_ctx;
+
+template <class T = char>
+class VgxBuffer {
+ public:
+  VgxBuffer() = default;
+  explicit VgxBuffer(VgxMem kind) : kind_(kind) {}
+  VgxBuffer(VgxBuffer&& o) noexcept { *this = std::move(o); }
+  VgxBuffer& operator=(VgxBuffer&& o) noexcept {
+    if (this != &o) {
+      reset();
+      std::swap(p_, o.p_);
+      std::swap(bytes_, o.bytes_);
+      std::swap(kind_, o.kind_);
+    }
+    return *this;
+  }
+  VgxBuffer(const VgxBuffer&) = delete;
+  VgxBuffer& operator=(const VgxBuffer&) = delete;
+  ~VgxBuffer() { reset(); }
+
+  T* get() const { return p_; }
+  size_t bytes() const { return bytes_; }
+  void reset() {
+    if (p_) kind_ == VgxMem::pinned ? cudaFreeHost(p_) : cudaFree(p_);
+    p_ = nullptr;
+    bytes_ = 0;
+  }
+  // frees what it holds and allocates `bytes`.  On failure the owner is empty, the context's error
+  // reads "<what>: <CUDA error>" and the status is VGX_ERR_CUDA (`nomem` when out of memory).
+  int alloc(vgx_ctx* c, size_t bytes, const char* what, int nomem = VGX_ERR_CUDA);
+  // discard-and-grow: when it holds fewer than `need` bytes, a new allocation of need + need / 4
+  // bytes replaces the old one and its contents
+  int grow(vgx_ctx* c, size_t need, const char* what) {
+    return need <= bytes_ ? VGX_OK : alloc(c, need + need / 4, what);
+  }
+  // grow-and-keep: as grow, but the first `used` bytes are copied over on the context's stream, which
+  // is synchronised before the old allocation is freed; a failed allocation leaves the old one in place
+  int grow_keep(vgx_ctx* c, size_t need, size_t used, const char* what);
+
+ private:
+  T* p_ = nullptr;
+  size_t bytes_ = 0;
+  VgxMem kind_ = VgxMem::device;
+};
 
 // ------------------------------------------------------------------ block hash
 // voxblox AnyIndexHash (block_hash.h): x + 17191*y + 17191^2*z, then masked into an
@@ -95,7 +148,7 @@ __device__ __forceinline__ int vgx_hash_find(const VgxHash& h, int bx, int by, i
 #define VGX_PT_UNIT_FLOATS 160
 struct VgxPoints {
   int n = 0;
-  float* data = nullptr;        // ceil(n / 32) units
+  VgxBuffer<float> data;        // ceil(n / 32) units
   double sum_w = 0;             // summed_reference_weight (cpp:124), sequential double sum
   std::vector<double> cumulative_w;  // WeightedSampler::cumulative_item_weights_ (host, sampling mode)
   std::mt19937 rng;                  // WeightedSampler::random_number_generator_ (default seed)
@@ -112,21 +165,22 @@ struct VgxSubmap {
   int cap_blocks = 0;
   int n_blocks = 0;            // host mirror (valid after upload / integrate sync)
   bool finished = false;
-  VgxHash hash{nullptr, 0};
-  int32_t* d_block_idx = nullptr;  // cap x 3
-  float2* d_dw = nullptr;          // cap x vps^3 (distance, weight)
+  VgxBuffer<VgxHashEntry> d_hash;   // hash_mask + 1 entries
+  uint32_t hash_mask = 0;
+  VgxBuffer<int32_t> d_block_idx;  // cap x 3
+  VgxBuffer<float2> d_dw;          // cap x vps^3 (distance, weight)
   // Registration view ("octets"): for every voxel the distances of its 2x2x2 forward
   // neighbourhood (corner i: x = bit2, y = bit1, z = bit0; apron across bricks baked in),
   // NaN where the voxel is unobserved or its block missing. One 32-byte sector per point.
-  float* d_view = nullptr;         // cap x vps^3 x 8
-  float2* d_esdf = nullptr;        // ESDF bricks (distance, observed 1/0), n_blocks x vps^3 (vgx_submap_generate_esdf)
-  float* d_view_esdf = nullptr;    // registration view of the ESDF bricks
-  int* d_counters = nullptr;       // [0] = n_blocks (device), [1] = overflow flag, [2] = bad upload input
+  VgxBuffer<float> d_view;         // cap x vps^3 x 8
+  VgxBuffer<float2> d_esdf;        // ESDF bricks (distance, observed 1/0), n_blocks x vps^3 (vgx_submap_generate_esdf)
+  VgxBuffer<float> d_view_esdf;    // registration view of the ESDF bricks
+  VgxBuffer<int> d_counters;       // [0] = n_blocks (device), [1] = overflow flag, [2] = bad upload input
   // Dense block index over the AABB of the allocated blocks (finished submaps): slot or -1.
   // Small enough to be staged in shared memory by the registration kernel; the hash stays
   // the general structure (integration, view construction, sparse/huge submaps).
-  int32_t* d_grid = nullptr;
-  uint16_t* d_grid16 = nullptr;   // 16-bit copy (0xFFFF = no block), padded to a multiple of 16 bytes
+  VgxBuffer<int32_t> d_grid;
+  VgxBuffer<uint16_t> d_grid16;   // 16-bit copy (0xFFFF = no block), padded to a multiple of 16 bytes
   int grid_min[3] = {0, 0, 0};
   int grid_dim[3] = {0, 0, 0};
   VgxPoints points[2];
@@ -135,8 +189,10 @@ struct VgxSubmap {
   float surface_obb_min[3] = {0, 0, 0}, surface_obb_max[3] = {0, 0, 0};
   std::vector<int> iso_blocks;
   bool points_extracted = false;
-  int32_t* d_iso_idx = nullptr;   // block indices of the isosurface blocks (n_iso x 3)
+  VgxBuffer<int32_t> d_iso_idx;   // block indices of the isosurface blocks (n_iso x 3)
   int n_iso = 0;
+
+  VgxHash hash() const { return {d_hash.get(), hash_mask}; }
 };
 
 // ------------------------------------------------------------------ pose graph
@@ -163,15 +219,15 @@ struct vgx_ctx {
   VgxProfileSlot prof[VGX_PROFILE_SLOTS];
   int64_t launches = 0;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  // scratch
-  void* d_scratch = nullptr;
-  size_t scratch_bytes = 0;
-  void* h_pinned = nullptr;
-  size_t pinned_bytes = 0;
-  void* d_sort = nullptr;    // TSDF deterministic path: counts / offsets / scan temp
-  size_t sort_bytes = 0;
-  void* d_sort2 = nullptr;   // ... tuple buffers + radix-sort temp
-  size_t sort2_bytes = 0;
+  // Scratch arenas.  They grow (discard-and-grow) and never shrink; a call lays its parts out in one
+  // with vgx_carve, and the parts are valid until the next vgx_carve of the same arena.  A function
+  // may hold parts of several arenas at once, but a callee must not carve an arena its caller holds
+  // parts of: the arena may move.  A function that carves the same arena twice re-sends what the
+  // first parts held.
+  VgxBuffer<> d_scratch;   // a call's inputs and outputs on their way to or from the host
+  VgxBuffer<> d_work;      // a pass's working buffers: counts, offsets, flags, scan and sort temp
+  VgxBuffer<> d_work2;     // the second set of a pass that holds d_work parts (sort tuples, candidates)
+  VgxBuffer<> h_pinned{VgxMem::pinned};   // page-locked host staging of copies to and from the device
   // NCCL
   void* nccl_comm = nullptr;
   int nranks = 1, rank = 0;
@@ -185,9 +241,8 @@ struct vgx_ctx {
   bool p2p_fused = true;           // one-launch assemble + exchange (VGX_P2P_FUSED=0: two launches)
   long long p2p_timeout_cycles = 0;
   // separated submap mesh of the last vgx_mesh_build (mesh.cu)
-  float* d_mesh_xyz = nullptr;        // n_vertices x 3
-  uint32_t* d_mesh_tri = nullptr;     // n_triangles x 3
-  size_t mesh_vcap = 0, mesh_tcap = 0;
+  VgxBuffer<float> d_mesh_xyz;        // n_vertices x 3
+  VgxBuffer<uint32_t> d_mesh_tri;     // n_triangles x 3
   int64_t mesh_nv = 0, mesh_nt = 0;
   std::vector<uint32_t> mesh_ids;     // the submaps of the build, in build order
   std::vector<int64_t> mesh_voff;     // their first vertices (+ the total)
@@ -198,11 +253,57 @@ struct vgx_ctx {
     auto it = submaps.find(id);
     return it == submaps.end() ? nullptr : it->second;
   }
-  int ensure_scratch(size_t bytes);
-  int ensure_pinned(size_t bytes);
-  int ensure_sort(size_t bytes);
-  int ensure_sort2(size_t bytes);
 };
+
+template <class T>
+int VgxBuffer<T>::alloc(vgx_ctx* c, size_t bytes, const char* what, int nomem) {
+  reset();
+  void* p = nullptr;
+  const cudaError_t e = kind_ == VgxMem::pinned ? cudaMallocHost(&p, bytes) : cudaMalloc(&p, bytes);
+  if (e != cudaSuccess) {
+    c->set_error(std::string(what) + ": " + cudaGetErrorString(e));
+    return e == cudaErrorMemoryAllocation ? nomem : VGX_ERR_CUDA;
+  }
+  p_ = static_cast<T*>(p);
+  bytes_ = bytes;
+  return VGX_OK;
+}
+
+template <class T>
+int VgxBuffer<T>::grow_keep(vgx_ctx* c, size_t need, size_t used, const char* what) {
+  if (need <= bytes_) return VGX_OK;
+  VgxBuffer q(kind_);
+  const int rc = q.alloc(c, need + need / 4, what);
+  if (rc != VGX_OK) return rc;
+  if (used) {
+    VGX_CUDA(c, cudaMemcpyAsync(q.p_, p_, used, cudaMemcpyDefault, c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+  }
+  *this = std::move(q);
+  return VGX_OK;
+}
+
+// ------------------------------------------------------------------ scratch layout
+// one part of a vgx_carve layout: n elements of T at *at
+template <class T>
+struct VgxPart {
+  T*& at;
+  size_t bytes;
+};
+template <class T>
+VgxPart<T> vgx_part(T*& at, size_t n) { return {at, sizeof(T) * n}; }
+static inline size_t vgx_part_span(size_t bytes) { return (bytes + 255) & ~(size_t)255; }
+
+// Lays the parts out in `arena` in order, each rounded up to 256 bytes (so every part starts
+// 256-byte aligned), growing the arena to the total first; no CUDA call when it is large enough.
+template <class... T>
+int vgx_carve(vgx_ctx* c, VgxBuffer<>& arena, VgxPart<T>... parts) {
+  const int rc = arena.grow(c, (vgx_part_span(parts.bytes) + ...), "scratch arena");
+  if (rc != VGX_OK) return rc;
+  char* at = arena.get();
+  ((parts.at = reinterpret_cast<T*>(at), at += vgx_part_span(parts.bytes)), ...);
+  return VGX_OK;
+}
 
 // RAII-less helper to bracket kernel launches for accounting.
 struct VgxLaunchScope {
@@ -243,8 +344,6 @@ int vgx_submap_build_view(vgx_ctx* ctx, VgxSubmap* s, const float2* bricks, floa
 // clears the block hash and re-inserts the first s->n_blocks blocks (after a capacity overflow
 // left keys without a brick behind)
 int vgx_submap_rebuild_hash(vgx_ctx* ctx, VgxSubmap* s);
-// sub-buffer size in a scratch layout (keeps every sub-buffer 256-byte aligned)
-static inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 // hand-written exclusive scan (extract.cu): out[0..n], out[n] = total; d_tmp: vgx_scan_tmp_count(n) words
 int vgx_exclusive_scan_u32(vgx_ctx* c, const unsigned* d_in, unsigned* d_out, size_t n, unsigned* d_tmp);
 size_t vgx_scan_tmp_count(size_t n);
