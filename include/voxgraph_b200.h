@@ -420,7 +420,9 @@ typedef struct vgx_solver_options {       /* ceres::Solver::Options subset, pose
 typedef struct vgx_solver_summary {       /* what voxgraph reads off ceres::Solver::Summary */
   int iterations;
   int num_successful_steps;
-  int num_residual_evals;
+  int num_residual_evals;  /* 1 (the start) + one per candidate evaluated; Ceres also counts the
+                             re-evaluation after an accepted step, which the device fuses into the
+                             candidate's */
   int termination;  /* 0 parameter tol, 1 function tol, 2 gradient tol, 3 max iterations,
                        4 max time, 5 min radius, 6 failure */
   double initial_cost, final_cost;

@@ -221,8 +221,9 @@ def _max_ratio(r, bound):
     return float(np.max(r[~zero] / bound[~zero]))
 
 
-def backward_ratio(A, b, y, delta=None):
-    """max_i |b - A y|_i / (c u (|L||L^T||y|)_i + (|A| delta)_i), residual in long double."""
+def backward_ratio(A, b, y, delta=None, extra=None):
+    """max_i |b - A y|_i / (c u (|L||L^T||y|)_i + (|A| delta)_i + extra_i), residual in long double.
+    extra: a known perturbation of A times |y| (e.g. an uncertain damping term)."""
     ld = np.longdouble
     n = len(b)
     aL = np.abs(np.linalg.cholesky(A))
@@ -230,6 +231,8 @@ def backward_ratio(A, b, y, delta=None):
     bound = gamma_c(n) * U * (aL @ (aL.T @ ay))
     if delta is not None:
         bound = bound + np.abs(A) @ delta
+    if extra is not None:
+        bound = bound + extra
     r = np.asarray(b, ld) - np.dot(np.asarray(A, ld), np.asarray(y, ld))
     return _max_ratio(r, bound)
 

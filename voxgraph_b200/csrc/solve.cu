@@ -628,6 +628,7 @@ __global__ void lm_init_kernel(const double* __restrict__ packed, const int* __r
     S.termination = 3;
     if (o.max_num_iterations <= 0) { S.termination = 3; S.done = 1; }
     else if (gm <= o.gradient_tolerance) { S.termination = 2; S.done = 1; }
+    else if (radius <= o.min_radius) { S.termination = 5; S.done = 1; }
     *st = S;
   }
 }
@@ -905,7 +906,9 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
   VGX_CUDA(c, cudaMemcpyAsync(g->h_state.get(), g->dev.d_state.get(), sizeof(LmState), cudaMemcpyDeviceToHost, st));
   VGX_CUDA(c, cudaStreamSynchronize(st));
   S.initial_cost = g->h_state.get()->cost;
-  bool timed_out = false;
+  // Ceres checks the time budget before every iteration, the first included, and before the other
+  // tests (iterations, gradient, radius): a budget spent by now ends the solve with x untouched.
+  bool timed_out = c->nranks == 1 && wall_s() - t0 >= o->max_solver_time_s;
   static const char* no_spec = getenv("VGX_LM_NO_RUNAHEAD");
   const int ahead = (c->nranks == 1 && !(no_spec && no_spec[0] == '1')) ? 1 : 0;
   // VGX_CHOL_DEBUG=1: phase cycle counts of the last shared-memory Cholesky, printed after the solve
@@ -956,7 +959,7 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
     VGX_CUDA(c, cudaEventRecord(g->ev_copy[k & 1], g->copy_stream));
     return VGX_OK;
   };
-  bool run = !g->h_state.get()->done && n > 0;
+  bool run = !timed_out && !g->h_state.get()->done && n > 0;
   if (run) {
     int enq = 0, k = 0;   // iterations enqueued / the one whose outcome is awaited
     for (;;) {
