@@ -290,7 +290,11 @@ typedef struct vgx_tsdf_config {          /* voxblox::TsdfIntegratorBase::Config
   int use_sparsity_compensation_factor;   /* yaml:27  1 */
   float sparsity_compensation_factor;     /* yaml:28  20 */
   float start_voxel_subsampling_factor;   /* FastTsdfIntegrator, 2 */
-  int max_consecutive_ray_collisions;     /* FastTsdfIntegrator, 2 */
+  int max_consecutive_ray_collisions;     /* FastTsdfIntegrator, 2.  Both approximate sets start each
+                                             call filled with ~0, which index (-1, 0, 0) also hashes to:
+                                             its first visit counts as a collision, and a point whose
+                                             start cell is (-1, 0, 0) is never cast.  A point with a NaN
+                                             or infinite coordinate touches neither set. */
   int mode;                               /* 0 simple (every ray, every voxel; the updates of each
                                              voxel are applied in ray order = bit-identical to the
                                              single-threaded reference), 1 fast (FastTsdfIntegrator

@@ -1627,7 +1627,9 @@ static void tsdf_integrate(vgo_layer* l, const vgo_tsdf_config* c, const float T
   if (c->mode == 1) {
     start_set = (uint64_t*)malloc(sizeof(uint64_t) * (mask + 1));
     obs_set = (uint64_t*)malloc(sizeof(uint64_t) * (mask + 1));
-    /* "empty" marker: a hash value that real indices practically never produce */
+    /* "empty" marker ~0, as on the device.  It is a real hash: index (-1, 0, 0) (and (17190, -1, 0))
+     * hashes to ~0, so the first visit of that voxel counts as a collision and a point whose start
+     * cell is (-1, 0, 0) is never cast (tests/fast_schedule.py) */
     for (uint64_t i = 0; i <= mask; ++i) { start_set[i] = ~(uint64_t)0; obs_set[i] = ~(uint64_t)0; }
   }
   for (int i = 0; i < n; ++i) {
