@@ -26,17 +26,6 @@ def world():
     return synth.make_world(3, size_xy=(30.0, 30.0), n_clutter=40, n_walls=4)
 
 
-def _scans(world, n_beams=16, n_azimuth=256, origin=(0.0, 0.0, 0.0)):
-    """Three scans from different poses (two with clearing rays), sensor poses offset by `origin`."""
-    out = []
-    for k, (px, py, yaw) in enumerate([(15.0, 15.0, 0.4), (16.5, 14.0, 1.9), (13.0, 16.0, -2.6)]):
-        pts = synth.lidar_scan(world, np.array([px, py, 1.2, yaw]), n_beams=n_beams, n_azimuth=n_azimuth,
-                               seed=k, miss_range=40.0 if k != 1 else None)
-        T = synth.pose_to_T([px - 15.0 + origin[0], py - 15.0 + origin[1], 0.1 * k + origin[2], yaw])
-        out.append((T, pts))
-    return out
-
-
 def _run_mode0(ctx, oracle, vs, vps, scans, capacity=None, **kw):
     """Integrate `scans` = [(T, points[, cfg overrides])] on both sides; returns per-scan stats and the
     model's closed-form batch counts.  Capacity defaults to the oracle's final block count."""
@@ -64,55 +53,22 @@ def _run_mode0(ctx, oracle, vs, vps, scans, capacity=None, **kw):
     return exp
 
 
-MW24 = 2.0 ** 24
-CONFIGS = [
-    dict(),
-    dict(use_const_weight=0),
-    dict(use_weight_dropoff=0),
-    dict(use_sparsity_compensation_factor=0),
-    dict(sparsity_compensation_factor=1.0),
-    dict(sparsity_compensation_factor=2.5),
-    dict(allow_clear=0),
-    dict(voxel_carving_enabled=0),
-    dict(use_const_weight=0, use_weight_dropoff=0),
-    dict(use_const_weight=0, sparsity_compensation_factor=2.5, allow_clear=0),
-    dict(voxel_carving_enabled=0, use_weight_dropoff=0, use_sparsity_compensation_factor=0),
-    dict(min_ray_length_m=1.5, max_ray_length_m=9.0),
-    dict(default_truncation_distance=0.1),
-    dict(default_truncation_distance=0.2),    # = voxel size: the drop-off denominator is 0
-    dict(default_truncation_distance=2.0),
-    dict(max_weight=3.0),
-    dict(max_weight=40.0),
-    dict(max_weight=100.5),
-    dict(max_weight=MW24 - 8),
-    dict(max_weight=MW24),
-]
-
-
-@pytest.mark.parametrize("kw", CONFIGS, ids=lambda kw: ",".join("%s=%r" % i for i in kw.items()) or "default")
+@pytest.mark.parametrize("kw", tx.CONFIGS, ids=tx.config_id)
 def test_simple_bit_exact_config_matrix(ctx, oracle, world, kw):
-    exp = _run_mode0(ctx, oracle, 0.2, 16, _scans(world), **kw)
+    exp = _run_mode0(ctx, oracle, 0.2, 16, tx.scans(world), **kw)
     sat = sum(e[4] for e in exp)
     if kw.get("use_const_weight", 1) and kw.get("max_weight", 1e4) <= 2.0 ** 20 and kw.get("voxel_carving_enabled", 1):
         assert sat > 0     # integer weights >= 2^-20 max_weight: the closed form runs
-    if kw.get("max_weight", 0) >= MW24 - 8:
+    if kw.get("max_weight", 0) >= tx.MW24 - 8:
         assert sat == 0
 
 
-def _ring(n, z, ranges, az0=0.1):
-    """n points around the sensor at height z (sensor frame) and the given horizontal ranges."""
-    a = az0 + 2 * np.pi * np.arange(n) / n
-    r = np.resize(np.asarray(ranges, np.float64), n)
-    zz = np.resize(np.asarray(z, np.float64), n)
-    return np.stack([r * np.cos(a), r * np.sin(a), zz], -1).astype(np.float32)
-
-
-@pytest.mark.parametrize("mw", [3.0, 40.0, 100.5, 1e4, MW24 - 8, MW24])
+@pytest.mark.parametrize("mw", [3.0, 40.0, 100.5, 1e4, tx.MW24 - 8, tx.MW24])
 def test_saturated_batches_cross_the_cap(ctx, oracle, mw):
     """Integer update weights of 2^14 (|z| = 2^-7, use_const_weight=0) reach 2^24 within 1024 rays:
     the cap is crossed inside a closed-form batch at small, fractional and near-2^24 caps.  At 2^24
     the integer closed form is refused and only the batches after a voxel sits at the cap collapse."""
-    pts = _ring(1100, [2.0 ** -7, -2.0 ** -7], [3.0, 4.5, 6.0])
+    pts = tx.ring(1100, [2.0 ** -7, -2.0 ** -7], [3.0, 4.5, 6.0])
     T = synth.pose_to_T([0.1, 0.1, 0.1, 0.3])
     exp = _run_mode0(ctx, oracle, 0.2, 16, [(T, pts)], use_const_weight=0, max_weight=mw)
     assert exp[0][4] > 0
@@ -122,7 +78,7 @@ def test_saturated_batches_cross_the_cap(ctx, oracle, mw):
 def test_simple_bit_exact_resolutions(ctx, oracle, world, vs, vps):
     """Other voxel sizes and block sizes (key = slot << 3 log2(vps), sort end bit, sentinel), a sensor
     at negative coordinates, one 2 km from the origin, and a float quaternion that is not exactly unit."""
-    scans = _scans(world, n_beams=8, n_azimuth=128)
+    scans = tx.scans(world, n_beams=8, n_azimuth=128)
     T_neg = scans[0][0].copy(); T_neg[4:] = [-7.3, -11.9, -2.05]
     T_far = scans[1][0].copy(); T_far[4:] += np.array([2000.0, -1312.5, 3.0], np.float32)
     q = np.array([0.71, 0.12, -0.2, 0.67], np.float32)        # |q|^2 = 0.9894
@@ -132,36 +88,14 @@ def test_simple_bit_exact_resolutions(ctx, oracle, world, vs, vps):
     _run_mode0(ctx, oracle, vs, vps, [(T_far, scans[1][1]), (T_far, scans[0][1])], **cfg)
 
 
-def _edge_points():
-    f = np.float32
-    up = lambda v: np.nextafter(f(v), f(np.inf)); dn = lambda v: np.nextafter(f(v), f(-np.inf))
-    p = []
-    for r in (0.5, 8.0):                       # min / max ray length exactly, and one ulp either side
-        for v in (dn(r), f(r), up(r)):
-            p += [[v, 0, 0], [0, -v, 0], [0, 0, v]]     # axis-aligned: t = 2 on the degenerate axes
-    p += [[0, 0, 0]]                           # sdf = 0/0 at the sensor voxel when min_ray_length_m = 0
-    p += [[np.nan, 0, 0], [1, np.nan, 2], [np.inf, 0, 0], [-np.inf, 0, 0], [0, np.inf, 1]]
-    p += [[3e19, 0, 0], [-2e19, 2e19, 0], [1.1e19, 1.1e19, 1.1e19], [1e19, -1e19, 1e19]]
-    p += [[2.0, 0.5, 0.25], [4.0, -2.0, 1.0], [-2.0, 2.0, -0.75], [6.0, 4.0, 0.0], [0.0, -4.0, 2.0]]
-    p += [[3.1 + 0.02 * k, 1.3 + 0.01 * k, -0.6 + 0.015 * k] for k in range(5)]   # one voxel
-    p += [[12.0, 3.0, -1.0], [-9.0, 10.0, 0.5], [0.3, -15.0, 2.0]]             # clearing rays
-    return np.array(p, np.float32)
-
-
-EDGE_CFGS = [dict(min_ray_length_m=0.5, max_ray_length_m=8.0),
-             dict(min_ray_length_m=0.0, max_ray_length_m=8.0, voxel_carving_enabled=0),
-             dict(min_ray_length_m=0.0, max_ray_length_m=8.0, allow_clear=0),
-             dict(min_ray_length_m=0.0, max_ray_length_m=8.0, use_weight_dropoff=0)]
-
-
 def test_ray_edges_simple_bit_exact(ctx, oracle):
     """Crafted points at 0.25 m voxels (faces exactly representable) from a sensor on a block corner
     and from one inside a voxel, under four configurations, accumulated in one submap."""
-    pts = _edge_points()
+    pts = tx.edge_points()
     scans = []
     for t in ([0.0, 0.0, 0.0], [0.3, -0.45, 0.1]):
         T = np.array([1, 0, 0, 0, *t], np.float32)
-        scans += [(T, pts, c) for c in EDGE_CFGS]
+        scans += [(T, pts, c) for c in tx.EDGE_CFGS]
     exp = _run_mode0(ctx, oracle, 0.25, 8, scans)
     assert all(e[0] == e[1] for e in exp)
     # 15 axis points within or beyond the lengths, 4 huge finite, 5 on faces, 5 in one voxel, 3 clearing
@@ -201,9 +135,9 @@ def test_fast_serialisation_ray_edges(ctx, oracle):
     """The crafted points in the Fast schedule.  The one-ulp neighbours of the length limits are left
     out: after the sensor translation they can land on the same float point, and the Fast schedule
     then rightly casts only one of them."""
-    pts = _edge_points()
+    pts = tx.edge_points()
     keep = np.ones(len(pts), bool); keep[[0, 1, 2, 6, 7, 8, 9, 10, 11, 15, 16, 17]] = False
-    for c in EDGE_CFGS:
+    for c in tx.EDGE_CFGS:
         _run_fast(ctx, oracle, 0.25, 8, np.array([1, 0, 0, 0, 0.3, -0.45, 0.1], np.float32), pts[keep],
                   **{**c, "use_weight_dropoff": 0})
 
@@ -215,8 +149,8 @@ def test_segment_lengths(ctx, oracle, n):
     weights 2^6 far behind the sensor; mixed stream: some sdf below 2 trunc at the sensor voxel and
     fractional weights."""
     T = synth.pose_to_T([0.1, 0.1, 0.1, 0.0])
-    sat_pts = _ring(n, 0.125, [3.0, 4.2, 5.5])
-    mixed = _ring(n, [0.125, 0.3, 0.125, -0.2, 0.125, 0.125, 0.125], [3.0, 1.0, 4.2, 5.5, 1.1])
+    sat_pts = tx.ring(n, 0.125, [3.0, 4.2, 5.5])
+    mixed = tx.ring(n, [0.125, 0.3, 0.125, -0.2, 0.125, 0.125, 0.125], [3.0, 1.0, 4.2, 5.5, 1.1])
     for pts in (sat_pts, mixed):
         layer = oracle.Layer(0.2, 16)
         st, g, s, u = oracle.tsdf_integrate_trace(layer, oracle.tsdf_config(use_const_weight=0), T, pts)

@@ -65,7 +65,9 @@ def test_colour_rule_band_and_early_out():
 
 def test_replay_matches_oracle_distance_and_weight(oracle):
     """The coloured sequential replay built on the per-ray trace reproduces the oracle's (distance, weight) bit
-    for bit, and colours exactly the voxels that received a band update; clearing rays colour nothing."""
+    for bit, and colours exactly the voxels that received a band update.  The clearing rays here (points at
+    40 m, cut at max_ray_length_m = 16 m) end far in front of anything and colour nothing; a clearing point
+    within a truncation distance of the limit does reach the band (test_clearing_rays_reach_the_band)."""
     world = synth.make_world(3, size_xy=(30.0, 30.0), n_clutter=40, n_walls=4)
     pts = synth.lidar_scan(world, np.array([15.0, 15.0, 1.2, 0.4]), n_beams=8, n_azimuth=64, seed=1, miss_range=40.0)
     T = synth.pose_to_T([0.3, -0.2, 0.1, 0.4])
@@ -91,6 +93,31 @@ def test_replay_matches_oracle_distance_and_weight(oracle):
     assert len(band) > 100 and np.array_equal(st.keys[st.c != 0], band)
     clearing = np.linalg.norm(pts, axis=1) > cfg.max_ray_length_m
     assert clearing.any() and not np.isin(keys[clearing[r]], band).any()
+
+
+def test_clearing_rays_reach_the_band(oracle):
+    """A clearing ray (norm > max_ray_length_m) ends at norm - trunc, so its last voxel's centre can lie
+    further along the ray, less than trunc in front of the point: an update inside the band, which the colour
+    rule blends.  400 points at 8 m + U(0.001, trunc + one voxel) with max_ray_length_m = 8: every one is a
+    clearing ray, and a hundred or more of them reach the band, with sdf > 0 (in front of the point)."""
+    T = synth.pose_to_T([0.1, 0.1, 0.1, 0.3])
+    cfg = oracle.tsdf_config(max_ray_length_m=8.0)
+    trunc = F32(cfg.default_truncation_distance)
+    for vs in (0.2, 0.1, 0.05):
+        rs = np.random.RandomState(0)
+        d = rs.normal(size=(400, 3))
+        d /= np.linalg.norm(d, axis=1)[:, None]
+        pts = (d * (8.0 + rs.uniform(0.001, float(trunc) + vs, 400))[:, None]).astype(F32)
+        assert (np.linalg.norm(pts.astype(np.float64), axis=1) > 8.0).all()
+        g, s, u, r = cx.trace_rays(oracle, oracle.Layer(vs, 8), cfg, T, pts)
+        band = np.abs(s) < trunc
+        assert len(np.unique(r[band])) > 100, vs
+        assert (s[band] > 0).all() and (u[band] > 0).all()
+        # and the replay colours those voxels with the clearing rays' colours
+        st = cx.State()
+        words = cx.pack(np.full((400, 4), [10, 20, 30, 40], np.uint8))
+        cx.replay(tx.voxel_keys(g), s, u, words[r], trunc, cfg.max_weight, st)
+        assert np.array_equal(st.keys[st.c != 0], np.unique(tx.voxel_keys(g[band])))
 
 
 def test_merge_known_answers():

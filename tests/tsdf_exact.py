@@ -149,6 +149,82 @@ def replay(keys, sdf, uw, trunc, max_weight, state=None, order=None):
     return uniq, d_out, w_out, sat
 
 
+# ---------------------------------------------------------------------- the parity matrix
+# Scans, configurations and crafted points that tests/test_gpu_tsdf_exact.py runs colourless and
+# tests/test_gpu_colour_exact.py runs with ray colours.
+MW24 = 2.0 ** 24
+CONFIGS = [
+    dict(),
+    dict(use_const_weight=0),
+    dict(use_weight_dropoff=0),
+    dict(use_sparsity_compensation_factor=0),
+    dict(sparsity_compensation_factor=1.0),
+    dict(sparsity_compensation_factor=2.5),
+    dict(allow_clear=0),
+    dict(voxel_carving_enabled=0),
+    dict(use_const_weight=0, use_weight_dropoff=0),
+    dict(use_const_weight=0, sparsity_compensation_factor=2.5, allow_clear=0),
+    dict(voxel_carving_enabled=0, use_weight_dropoff=0, use_sparsity_compensation_factor=0),
+    dict(min_ray_length_m=1.5, max_ray_length_m=9.0),
+    dict(default_truncation_distance=0.1),
+    dict(default_truncation_distance=0.2),    # = voxel size: the drop-off denominator is 0
+    dict(default_truncation_distance=2.0),
+    dict(max_weight=3.0),
+    dict(max_weight=40.0),
+    dict(max_weight=100.5),
+    dict(max_weight=MW24 - 8),
+    dict(max_weight=MW24),
+]
+
+
+def config_id(kw):
+    return ",".join("%s=%r" % i for i in kw.items()) or "default"
+
+
+def scans(world, n_beams=16, n_azimuth=256, origin=(0.0, 0.0, 0.0)):
+    """Three scans from different poses (two with clearing rays), sensor poses offset by `origin`."""
+    from voxgraph_b200 import synth
+    out = []
+    for k, (px, py, yaw) in enumerate([(15.0, 15.0, 0.4), (16.5, 14.0, 1.9), (13.0, 16.0, -2.6)]):
+        pts = synth.lidar_scan(world, np.array([px, py, 1.2, yaw]), n_beams=n_beams, n_azimuth=n_azimuth,
+                               seed=k, miss_range=40.0 if k != 1 else None)
+        T = synth.pose_to_T([px - 15.0 + origin[0], py - 15.0 + origin[1], 0.1 * k + origin[2], yaw])
+        out.append((T, pts))
+    return out
+
+
+def ring(n, z, ranges, az0=0.1):
+    """n points around the sensor at height z (sensor frame) and the given horizontal ranges."""
+    a = az0 + 2 * np.pi * np.arange(n) / n
+    r = np.resize(np.asarray(ranges, np.float64), n)
+    zz = np.resize(np.asarray(z, np.float64), n)
+    return np.stack([r * np.cos(a), r * np.sin(a), zz], -1).astype(np.float32)
+
+
+def edge_points():
+    """Crafted points for 0.25 m voxels: the ray-length limits and one ulp either side, the sensor
+    point, NaN, inf and huge finite points, points on voxel faces, in one voxel, and clearing rays."""
+    f = np.float32
+    up = lambda v: np.nextafter(f(v), f(np.inf)); dn = lambda v: np.nextafter(f(v), f(-np.inf))
+    p = []
+    for r in (0.5, 8.0):                       # min / max ray length exactly, and one ulp either side
+        for v in (dn(r), f(r), up(r)):
+            p += [[v, 0, 0], [0, -v, 0], [0, 0, v]]     # axis-aligned: t = 2 on the degenerate axes
+    p += [[0, 0, 0]]                           # sdf = 0/0 at the sensor voxel when min_ray_length_m = 0
+    p += [[np.nan, 0, 0], [1, np.nan, 2], [np.inf, 0, 0], [-np.inf, 0, 0], [0, np.inf, 1]]
+    p += [[3e19, 0, 0], [-2e19, 2e19, 0], [1.1e19, 1.1e19, 1.1e19], [1e19, -1e19, 1e19]]
+    p += [[2.0, 0.5, 0.25], [4.0, -2.0, 1.0], [-2.0, 2.0, -0.75], [6.0, 4.0, 0.0], [0.0, -4.0, 2.0]]
+    p += [[3.1 + 0.02 * k, 1.3 + 0.01 * k, -0.6 + 0.015 * k] for k in range(5)]   # one voxel
+    p += [[12.0, 3.0, -1.0], [-9.0, 10.0, 0.5], [0.3, -15.0, 2.0]]             # clearing rays
+    return np.array(p, np.float32)
+
+
+EDGE_CFGS = [dict(min_ray_length_m=0.5, max_ray_length_m=8.0),
+             dict(min_ray_length_m=0.0, max_ray_length_m=8.0, voxel_carving_enabled=0),
+             dict(min_ray_length_m=0.0, max_ray_length_m=8.0, allow_clear=0),
+             dict(min_ray_length_m=0.0, max_ray_length_m=8.0, use_weight_dropoff=0)]
+
+
 def check_fast(cand, keys, sdf, uw, trunc, max_weight, exact=None):
     """Serialisation check of one Fast integration into an empty layer.
 

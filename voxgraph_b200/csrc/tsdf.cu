@@ -20,8 +20,10 @@
 // published voxblox sources and not checked against a compiled voxblox: with w the voxel's weight BEFORE
 // the update and uw the update weight, after the new_weight < 1e-6 early-out,
 //   if (|sdf| < truncation) colour = blendTwoColors(colour, w, ray colour, uw).
-// Clearing rays and every update outside the band leave the colour alone (a clearing ray ends
-// truncation in front of its point, so it never reaches the band).  The colourless call (rgba == NULL)
+// Every update outside the band leaves the colour alone.  The rule looks at |sdf| only, so clearing rays
+// follow it too: a clearing ray ends at norm - truncation, and the centre of its last voxel can lie
+// further along, within truncation of the point (a point just beyond max_ray_length_m); that update is in
+// the band and blends the ray's colour.  The colourless call (rgba == NULL)
 // runs the kernels it always ran (the <false> instantiations below) and leaves an existing channel
 // untouched - the one place this differs from voxblox, which would blend in its default Color().
 //   mode 0: the emitted tuple carries the ray's colour (16 bytes instead of 8 through the sort) and the
