@@ -377,17 +377,27 @@ def ray_world_range(world, origin, dirs, max_range):
     return best
 
 
+def quat_to_matrix(q):
+    """Unit quaternion [qw qx qy qz] -> 3x3 rotation matrix (float64)."""
+    w, x, y, z = [float(v) for v in q]
+    return np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
+                     [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
+                     [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]])
+
+
 def lidar_scan(world, sensor_pose, n_beams=64, n_azimuth=1024, vfov_deg=16.6, max_range=16.0,
-               range_noise=0.02, seed=0, miss_range=None):
+               range_noise=0.02, seed=0, miss_range=None, R_world_sensor=None):
     """64x1024 spinning LiDAR (config 3). Returns points in the sensor frame (n,3) f32.
     Rays that hit nothing within max_range are dropped unless miss_range is given
-    (then they are reported at miss_range, producing voxblox clearing rays)."""
+    (then they are reported at miss_range, producing voxblox clearing rays).
+    R_world_sensor: the sensor's full 3x3 orientation (a tilted sensor); sensor_pose[3] (yaw) is then
+    not used, and only sensor_pose[:3] places the sensor."""
     rng = np.random.default_rng(seed)
     el = np.deg2rad(np.linspace(-vfov_deg, vfov_deg, n_beams))
     az = np.linspace(-np.pi, np.pi, n_azimuth, endpoint=False)
     E, A = np.meshgrid(el, az, indexing="ij")
     dirs_c = np.stack([np.cos(E) * np.cos(A), np.cos(E) * np.sin(A), np.sin(E)], -1).reshape(-1, 3)
-    Rw = rot_z(sensor_pose[3])
+    Rw = rot_z(sensor_pose[3]) if R_world_sensor is None else np.asarray(R_world_sensor, np.float64)
     dirs_w = dirs_c @ Rw.T
     rng_m = ray_world_range(world, np.asarray(sensor_pose[:3], np.float64), dirs_w, max_range * 2)
     rng_m = rng_m + rng.normal(0, range_noise, rng_m.shape)
