@@ -13,9 +13,11 @@
  *
  * Conventions: plain pointers and sizes, caller owns every host buffer, the context
  * owns all device memory, every function returns an int status (no exceptions or
- * aborts cross the boundary; vgx_last_error() gives the message).  One context per
- * GPU; a context is not thread-safe.  There is NO CPU fallback: every entry point
- * needs a CUDA device and fails with VGX_ERR_CUDA without one.
+ * aborts cross the boundary: a host allocation failure is VGX_ERR_NOMEM).  Every
+ * call on a context selects the context's device first.  vgx_last_error() gives the
+ * message of the last call on the context, prefixed with the name of the function the
+ * caller called.  One context per GPU; a context is not thread-safe.  There is NO CPU
+ * fallback: every entry point needs a CUDA device and fails with VGX_ERR_CUDA without one.
  */
 #ifndef VOXGRAPH_B200_H_
 #define VOXGRAPH_B200_H_
@@ -41,6 +43,8 @@ typedef struct vgx_ctx vgx_ctx;
 int vgx_device_count(void);
 int vgx_ctx_create(int device, vgx_ctx** out);
 void vgx_ctx_destroy(vgx_ctx* ctx);
+/* The message of the last call on ctx: "<function>: <reason>" after a failure, the
+ * function being the one the caller called; empty after a call that returned VGX_OK. */
 const char* vgx_last_error(const vgx_ctx* ctx);
 /* cudaStream_t all work of this context is enqueued on (for event timing). */
 void* vgx_ctx_stream(vgx_ctx* ctx);

@@ -109,7 +109,6 @@ cloud_compact_kernel(int n, const float* __restrict__ pts, const uint32_t* __res
 // the validation rules of the header -> the record count
 static int cloud_check(vgx_ctx* c, const vgx_cloud_layout* L, const uint8_t* data, uint64_t n_bytes, float colour_max,
                        int* n) {
-  if (!c) return VGX_ERR_INVALID;
   if (!L) VGX_FAIL(c, VGX_ERR_INVALID, "point cloud: no layout");
   if (L->point_step == 0) VGX_FAIL(c, VGX_ERR_INVALID, "point cloud: point_step is 0");
   const auto inside = [&](int32_t off) { return off >= 0 && (uint64_t)off + 4 <= L->point_step; };
@@ -151,77 +150,71 @@ static int cloud_decode_launch(vgx_ctx* c, const vgx_cloud_layout& L, const uint
 
 extern "C" int vgx_cloud_decode(vgx_ctx* c, const vgx_cloud_layout* L, const uint8_t* data, uint64_t n_bytes,
                                 float colour_max, int max_points, float* points_C, uint8_t* rgba, int* n_points) {
-  int n = 0;
-  int rc = cloud_check(c, L, data, n_bytes, colour_max, &n);
-  if (rc != VGX_OK) return rc;
-  if (max_points < 0) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_cloud_decode: negative max_points");
-  if (n_points) *n_points = 0;
-  if (n == 0) return VGX_OK;
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  uint8_t* d_raw;
-  float *d_pts, *d_out_pts;
-  uint32_t *d_rgba, *d_out_rgba;
-  unsigned long long* d_kept;
-  unsigned *d_flags, *d_offsets, *d_scan_tmp;
-  rc = vgx_carve(c, c->d_scratch, vgx_part(d_raw, (size_t)L->height * L->row_step), vgx_part(d_pts, 3 * (size_t)n),
-                 vgx_part(d_rgba, (size_t)n), vgx_part(d_out_pts, 3 * (size_t)n), vgx_part(d_out_rgba, (size_t)n),
-                 vgx_part(d_kept, 1));
-  if (rc != VGX_OK) return rc;
-  rc = vgx_carve(c, c->d_work, vgx_part(d_flags, (size_t)n + 2), vgx_part(d_offsets, (size_t)n + 2),
-                 vgx_part(d_scan_tmp, vgx_scan_tmp_count((size_t)n)));
-  if (rc != VGX_OK) return rc;
-  cudaStream_t stream = c->stream;
-  VGX_CUDA(c, cudaMemsetAsync(d_kept, 0, sizeof(*d_kept), stream));
-  rc = cloud_decode_launch(c, *L, data, colour_max, d_raw, d_pts, d_rgba, d_flags, d_kept);
-  if (rc != VGX_OK) return rc;
-  {
-    VgxLaunchScope scope(c, VGX_SLOT_CLOUD_DECODE);
-    rc = vgx_exclusive_scan_u32(c, d_flags, d_offsets, (size_t)n, d_scan_tmp);
-    if (rc != VGX_OK) return rc;
-    cloud_compact_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(n, d_pts, d_rgba, d_flags, d_offsets, d_out_pts,
-                                                                          d_out_rgba);
-  }
-  VGX_CUDA(c, cudaGetLastError());
-  unsigned kept = 0;
-  VGX_CUDA(c, cudaMemcpyAsync(&kept, d_offsets + n, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
-  VGX_CUDA(c, cudaStreamSynchronize(stream));
-  if (n_points) *n_points = (int)kept;
-  if ((points_C || rgba) && kept > (unsigned)max_points)
-    VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_cloud_decode: more kept points than max_points");
-  if (points_C) VGX_CUDA(c, cudaMemcpyAsync(points_C, d_out_pts, sizeof(float) * 3 * (size_t)kept, cudaMemcpyDeviceToHost, stream));
-  if (rgba) VGX_CUDA(c, cudaMemcpyAsync(rgba, d_out_rgba, 4 * (size_t)kept, cudaMemcpyDeviceToHost, stream));
-  VGX_CUDA(c, cudaStreamSynchronize(stream));
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    int n = 0;
+    VGX_TRY(cloud_check(c, L, data, n_bytes, colour_max, &n));
+    if (max_points < 0) VGX_FAIL(c, VGX_ERR_INVALID, "negative max_points");
+    if (n_points) *n_points = 0;
+    if (n == 0) return VGX_OK;
+    uint8_t* d_raw;
+    float *d_pts, *d_out_pts;
+    uint32_t *d_rgba, *d_out_rgba;
+    unsigned long long* d_kept;
+    unsigned *d_flags, *d_offsets, *d_scan_tmp;
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_raw, (size_t)L->height * L->row_step), vgx_part(d_pts, 3 * (size_t)n),
+                      vgx_part(d_rgba, (size_t)n), vgx_part(d_out_pts, 3 * (size_t)n), vgx_part(d_out_rgba, (size_t)n),
+                      vgx_part(d_kept, 1)));
+    VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_flags, (size_t)n + 2), vgx_part(d_offsets, (size_t)n + 2),
+                      vgx_part(d_scan_tmp, vgx_scan_tmp_count((size_t)n))));
+    cudaStream_t stream = c->stream;
+    VGX_CUDA(c, cudaMemsetAsync(d_kept, 0, sizeof(*d_kept), stream));
+    VGX_TRY(cloud_decode_launch(c, *L, data, colour_max, d_raw, d_pts, d_rgba, d_flags, d_kept));
+    {
+      VgxLaunchScope scope(c, VGX_SLOT_CLOUD_DECODE);
+      VGX_TRY(vgx_exclusive_scan_u32(c, d_flags, d_offsets, (size_t)n, d_scan_tmp));
+      cloud_compact_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(n, d_pts, d_rgba, d_flags, d_offsets, d_out_pts,
+                                                                            d_out_rgba);
+    }
+    VGX_CUDA(c, cudaGetLastError());
+    unsigned kept = 0;
+    VGX_CUDA(c, cudaMemcpyAsync(&kept, d_offsets + n, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
+    VGX_CUDA(c, cudaStreamSynchronize(stream));
+    if (n_points) *n_points = (int)kept;
+    if ((points_C || rgba) && kept > (unsigned)max_points)
+      VGX_FAIL(c, VGX_ERR_CAPACITY, "more kept points than max_points");
+    if (points_C) VGX_CUDA(c, cudaMemcpyAsync(points_C, d_out_pts, sizeof(float) * 3 * (size_t)kept, cudaMemcpyDeviceToHost, stream));
+    if (rgba) VGX_CUDA(c, cudaMemcpyAsync(rgba, d_out_rgba, 4 * (size_t)kept, cudaMemcpyDeviceToHost, stream));
+    VGX_CUDA(c, cudaStreamSynchronize(stream));
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_tsdf_integrate_cloud(vgx_ctx* c, uint32_t id, const float T_G_C[7], const vgx_cloud_layout* L,
                                         const uint8_t* data, uint64_t n_bytes, int colours, float colour_max,
                                         const vgx_tsdf_config* cfg, vgx_tsdf_stats* stats, int* n_points) {
-  int n = 0;
-  int rc = cloud_check(c, L, data, n_bytes, colour_max, &n);
-  if (rc != VGX_OK) return rc;
-  VgxSubmap* s;
-  vgx_tsdf_config rcfg;
-  rc = vgx_tsdf_check(c, id, T_G_C, cfg, &s, &rcfg);
-  if (rc != VGX_OK) return rc;
-  if (n == 0) {
-    if (stats) memset(stats, 0, sizeof(*stats));
-    if (n_points) *n_points = 0;
-    return VGX_OK;
-  }
-  // scratch: message bytes | point slots | stats | (fast) the two approximate sets | colour slots
-  uint8_t* d_raw;
-  float* d_pts;
-  unsigned long long *d_stats, *d_sets;
-  uint32_t* d_rgba;
-  rc = vgx_carve(c, c->d_scratch, vgx_part(d_raw, (size_t)L->height * L->row_step), vgx_part(d_pts, 3 * (size_t)n),
-                 vgx_part(d_stats, VGX_TSDF_STAT_WORDS), vgx_part(d_sets, vgx_tsdf_set_words(rcfg)),
-                 vgx_part(d_rgba, colours ? (size_t)n : 0));
-  if (rc != VGX_OK) return rc;
-  VGX_CUDA(c, cudaMemsetAsync(d_stats, 0, sizeof(unsigned long long) * VGX_TSDF_STAT_WORDS, c->stream));
-  rc = cloud_decode_launch(c, *L, data, colour_max, d_raw, d_pts, colours ? d_rgba : nullptr, nullptr,
-                           d_stats + VGX_TSDF_STAT_CALLER);
-  if (rc != VGX_OK) return rc;
-  return vgx_tsdf_integrate_resident(c, s, T_G_C, rcfg, n, d_pts, colours ? d_rgba : nullptr, d_stats, d_sets, stats,
-                                     n_points);
+  return vgx_entry(c, __func__, [&] {
+    int n = 0;
+    VGX_TRY(cloud_check(c, L, data, n_bytes, colour_max, &n));
+    VgxSubmap* s;
+    vgx_tsdf_config rcfg;
+    VGX_TRY(vgx_tsdf_check(c, id, T_G_C, cfg, &s, &rcfg));
+    if (n == 0) {
+      if (stats) memset(stats, 0, sizeof(*stats));
+      if (n_points) *n_points = 0;
+      return VGX_OK;
+    }
+    // scratch: message bytes | point slots | stats | (fast) the two approximate sets | colour slots
+    uint8_t* d_raw;
+    float* d_pts;
+    unsigned long long *d_stats, *d_sets;
+    uint32_t* d_rgba;
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_raw, (size_t)L->height * L->row_step), vgx_part(d_pts, 3 * (size_t)n),
+                      vgx_part(d_stats, VGX_TSDF_STAT_WORDS), vgx_part(d_sets, vgx_tsdf_set_words(rcfg)),
+                      vgx_part(d_rgba, colours ? (size_t)n : 0)));
+    VGX_CUDA(c, cudaMemsetAsync(d_stats, 0, sizeof(unsigned long long) * VGX_TSDF_STAT_WORDS, c->stream));
+    VGX_TRY(cloud_decode_launch(c, *L, data, colour_max, d_raw, d_pts, colours ? d_rgba : nullptr, nullptr,
+                                d_stats + VGX_TSDF_STAT_CALLER));
+    return vgx_tsdf_integrate_resident(c, s, T_G_C, rcfg, n, d_pts, colours ? d_rgba : nullptr, d_stats, d_sets, stats,
+                                       n_points);
+  });
 }

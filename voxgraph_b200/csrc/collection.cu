@@ -725,10 +725,9 @@ struct EventPair {
 int copy_h2d_chunked(vgx_ctx* c, uint8_t* d, const uint8_t* h, uint64_t n) {
   if (n == 0) return VGX_OK;
   uint8_t* stage;
-  int rc = vgx_carve(c, c->h_pinned, vgx_part(stage, 2 * kChunk));
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(vgx_carve(c, c->h_pinned, vgx_part(stage, 2 * kChunk)));
   EventPair ev;
-  if ((rc = ev.init(c)) != VGX_OK) return rc;
+  VGX_TRY(ev.init(c));
   uint64_t off = 0;
   for (int k = 0; off < n; ++k) {
     const size_t len = (size_t)std::min<uint64_t>(kChunk, n - off);
@@ -746,10 +745,9 @@ int copy_h2d_chunked(vgx_ctx* c, uint8_t* d, const uint8_t* h, uint64_t n) {
 int copy_d2h_chunked(vgx_ctx* c, uint8_t* h, const uint8_t* d, uint64_t n) {
   if (n == 0) return VGX_OK;
   uint8_t* stage;
-  int rc = vgx_carve(c, c->h_pinned, vgx_part(stage, 2 * kChunk));
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(vgx_carve(c, c->h_pinned, vgx_part(stage, 2 * kChunk)));
   EventPair ev;
-  if ((rc = ev.init(c)) != VGX_OK) return rc;
+  VGX_TRY(ev.init(c));
   const uint64_t chunks = (n + kChunk - 1) / kChunk;
   for (uint64_t k = 0; k <= chunks; ++k) {
     if (k < chunks) {   // enqueue chunk k, then drain chunk k - 1 while it runs
@@ -772,40 +770,39 @@ int copy_d2h_chunked(vgx_ctx* c, uint8_t* h, const uint8_t* d, uint64_t n) {
 // ------------------------------------------------------------------ C-ABI
 extern "C" int vgx_collection_scan(const uint8_t* bytes, uint64_t n, int max_submaps, vgx_collection_entry* out,
                                    int* n_submaps) {
-  if (!n_submaps || max_submaps < 0 || (max_submaps > 0 && !out)) return VGX_ERR_INVALID;
-  *n_submaps = 0;
-  CollLayout L;
-  std::string err;
-  if (!parse_stream(bytes, n, false, &L, &err)) return VGX_ERR_INVALID;
-  if (L.submaps.size() > (size_t)INT32_MAX) return VGX_ERR_INVALID;
-  *n_submaps = (int)L.submaps.size();
-  if (L.submaps.size() > (size_t)max_submaps) return VGX_ERR_CAPACITY;
-  for (size_t i = 0; i < L.submaps.size(); ++i) {
-    const CollSubmapRef& s = L.submaps[i];
-    out[i].id = s.id;
-    out[i].num_blocks = s.n_blocks;
-    out[i].voxel_size = (float)L.voxel_size;
-    out[i].voxels_per_side = (int32_t)L.vps;
-    for (int k = 0; k < 7; ++k) out[i].T_M_S[k] = s.T[k];
-  }
-  return VGX_OK;
+  return vgx_entry_noctx([&] {
+    if (!n_submaps || max_submaps < 0 || (max_submaps > 0 && !out)) return VGX_ERR_INVALID;
+    *n_submaps = 0;
+    CollLayout L;
+    std::string err;
+    if (!parse_stream(bytes, n, false, &L, &err)) return VGX_ERR_INVALID;
+    if (L.submaps.size() > (size_t)INT32_MAX) return VGX_ERR_INVALID;
+    *n_submaps = (int)L.submaps.size();
+    if (L.submaps.size() > (size_t)max_submaps) return VGX_ERR_CAPACITY;
+    for (size_t i = 0; i < L.submaps.size(); ++i) {
+      const CollSubmapRef& s = L.submaps[i];
+      out[i].id = s.id;
+      out[i].num_blocks = s.n_blocks;
+      out[i].voxel_size = (float)L.voxel_size;
+      out[i].voxels_per_side = (int32_t)L.vps;
+      for (int k = 0; k < 7; ++k) out[i].T_M_S[k] = s.T[k];
+    }
+    return VGX_OK;
+  });
 }
 
 // Decodes a parsed stream into new submaps, one per entry of L.submaps under the entry's id, then runs the
-// upload path (block hash, registration view, block-index rules, grid) on each.  `what` prefixes errors.
+// upload path (block hash, registration view, block-index rules, grid) on each.
 // keep_colour: every submap gets a colour channel for the decode, and keeps it iff a colour word is non-zero
 // (a colourless file loaded with the flag pays a transient 4 B per voxel and its clearing: whether a word is
 // non-zero is only known once the varints are decoded, which is the decode pass itself).
-static int decode_layout(vgx_ctx* c, const char* what, const CollLayout& L, const uint8_t* bytes, uint64_t n,
-                         bool keep_colour) {
-  VGX_CUDA(c, cudaSetDevice(c->device));
+static int decode_layout(vgx_ctx* c, const CollLayout& L, const uint8_t* bytes, uint64_t n, bool keep_colour) {
   const int vpb = (int)(L.vps * L.vps * L.vps);
   CollBlockRef* d_regions;
   int *d_err, *d_any;   // d_any: one flag per submap
   uint8_t* d_bytes;
-  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_regions, L.blocks.size()), vgx_part(d_err, 1),
-                     vgx_part(d_any, keep_colour ? L.submaps.size() : 0), vgx_part(d_bytes, (size_t)n));
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_regions, L.blocks.size()), vgx_part(d_err, 1),
+                    vgx_part(d_any, keep_colour ? L.submaps.size() : 0), vgx_part(d_bytes, (size_t)n)));
   if (keep_colour && !L.submaps.empty())
     VGX_CUDA(c, cudaMemsetAsync(d_any, 0, sizeof(int) * L.submaps.size(), c->stream));
   {
@@ -814,26 +811,20 @@ static int decode_layout(vgx_ctx* c, const char* what, const CollLayout& L, cons
       VGX_CUDA(c, cudaMemcpyAsync(d_regions, L.blocks.data(), L.blocks.size() * sizeof(CollBlockRef),
                                   cudaMemcpyHostToDevice, c->stream));
     VGX_CUDA(c, cudaMemsetAsync(d_err, 0, sizeof(int), c->stream));
-    rc = copy_h2d_chunked(c, d_bytes, bytes, n);
-    if (rc != VGX_OK) return rc;
+    VGX_TRY(copy_h2d_chunked(c, d_bytes, bytes, n));
   }
   for (size_t k = 0; k < L.submaps.size(); ++k) {
     const CollSubmapRef& s = L.submaps[k];
     VgxSubmap* sm = nullptr;
-    rc = vgx_submap_alloc(c, s.id, (float)L.voxel_size, (int)L.vps, (int)s.n_blocks, true, &sm);
-    if (rc != VGX_OK) return rc;
+    VGX_TRY(vgx_submap_alloc(c, s.id, (float)L.voxel_size, (int)L.vps, (int)s.n_blocks, true, &sm));
     sm->n_blocks = (int)s.n_blocks;
     sm->finished = true;
     if (s.n_blocks == 0) continue;
-    if (keep_colour && (rc = vgx_submap_ensure_colour(c, sm)) != VGX_OK) return rc;
+    if (keep_colour) VGX_TRY(vgx_submap_ensure_colour(c, sm));
     {
       VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
-      const cudaError_t e = cudaMemcpyAsync(sm->d_block_idx.get(), L.block_idx.data() + 3 * s.first_block,
-                                            sizeof(int32_t) * 3 * s.n_blocks, cudaMemcpyHostToDevice, c->stream);
-      if (e != cudaSuccess) {
-        c->set_error(std::string(what) + ": " + cudaGetErrorString(e));
-        return VGX_ERR_CUDA;
-      }
+      VGX_CUDA(c, cudaMemcpyAsync(sm->d_block_idx.get(), L.block_idx.data() + 3 * s.first_block,
+                                  sizeof(int32_t) * 3 * s.n_blocks, cudaMemcpyHostToDevice, c->stream));
     }
     VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
     collection_decode_kernel<<<s.n_blocks, COLL_THREADS, 0, c->stream>>>(
@@ -842,17 +833,13 @@ static int decode_layout(vgx_ctx* c, const char* what, const CollLayout& L, cons
   }
   int h_err = 0;
   std::vector<int> h_any(keep_colour ? L.submaps.size() : 0);
-  cudaError_t e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaMemcpyAsync(&h_err, d_err, sizeof(int), cudaMemcpyDeviceToHost, c->stream);
-  if (e == cudaSuccess && !h_any.empty())
-    e = cudaMemcpyAsync(h_any.data(), d_any, sizeof(int) * h_any.size(), cudaMemcpyDeviceToHost, c->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-  if (e != cudaSuccess) {
-    c->set_error(std::string(what) + ": " + cudaGetErrorString(e));
-    return VGX_ERR_CUDA;
-  }
+  VGX_CUDA(c, cudaGetLastError());
+  VGX_CUDA(c, cudaMemcpyAsync(&h_err, d_err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  if (!h_any.empty())
+    VGX_CUDA(c, cudaMemcpyAsync(h_any.data(), d_any, sizeof(int) * h_any.size(), cudaMemcpyDeviceToHost, c->stream));
+  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   if (h_err) {
-    c->set_error(std::string(what) + ": voxel_data: " +
+    c->set_error(std::string("voxel_data: ") +
                  ((h_err & COLL_ERR_TAG) ? "unexpected tag; " : "") +
                  ((h_err & COLL_ERR_VARINT) ? "varint longer than 5 bytes, above 32 bits or truncated; " : "") +
                  ((h_err & COLL_ERR_COUNT) ? "not 3 vps^3 values; " : "") +
@@ -863,174 +850,170 @@ static int decode_layout(vgx_ctx* c, const char* what, const CollLayout& L, cons
     VgxSubmap* sm = c->find(L.submaps[k].id);
     if (keep_colour && !h_any[k]) sm->d_rgba.reset();   // all words zero: a colour-free submap (synchronised above)
     VgxLaunchScope scope(c, VGX_SLOT_COLL_UPLOAD, 0);
-    rc = vgx_submap_upload_finish(c, sm, what);
-    if (rc != VGX_OK) return rc;
+    VGX_TRY(vgx_submap_upload_finish(c, sm));
   }
   return VGX_OK;
 }
 
 // decode_layout for ids none of which exists yet: on failure no submap of L is left
-static int load_layout(vgx_ctx* c, const char* what, const CollLayout& L, const uint8_t* bytes, uint64_t n,
-                       bool keep_colour) {
-  const int rc = decode_layout(c, what, L, bytes, n, keep_colour);
+static int load_layout(vgx_ctx* c, const CollLayout& L, const uint8_t* bytes, uint64_t n, bool keep_colour) {
+  const int rc = decode_layout(c, L, bytes, n, keep_colour);
   if (rc != VGX_OK)
     for (const CollSubmapRef& s : L.submaps) vgx_submap_drop(c, s.id);
   return rc;
 }
 
 extern "C" int vgx_collection_load_ex(vgx_ctx* c, const uint8_t* bytes, uint64_t n, int flags, int* n_submaps) {
-  if (!c) return VGX_ERR_INVALID;
-  if (n_submaps) *n_submaps = 0;
-  if (flags & ~VGX_COLLECTION_KEEP_COLOUR) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_collection_load: unknown flag");
-  CollLayout L;
-  std::string err;
-  if (!parse_stream(bytes, n, false, &L, &err)) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_collection_load: " + err);
-  for (const CollSubmapRef& s : L.submaps)
-    if (c->find(s.id))
-      VGX_FAIL(c, VGX_ERR_INVALID, "vgx_collection_load: submap " + std::to_string(s.id) + " already exists");
-  const int rc = load_layout(c, "vgx_collection_load", L, bytes, n, (flags & VGX_COLLECTION_KEEP_COLOUR) != 0);
-  if (rc == VGX_OK && n_submaps) *n_submaps = (int)L.submaps.size();
-  return rc;
+  return vgx_entry(c, __func__, [&] {
+    if (n_submaps) *n_submaps = 0;
+    if (flags & ~VGX_COLLECTION_KEEP_COLOUR) VGX_FAIL(c, VGX_ERR_INVALID, "unknown flag");
+    CollLayout L;
+    std::string err;
+    if (!parse_stream(bytes, n, false, &L, &err)) VGX_FAIL(c, VGX_ERR_INVALID, err);
+    for (const CollSubmapRef& s : L.submaps)
+      if (c->submaps.count(s.id))
+        VGX_FAIL(c, VGX_ERR_INVALID, "submap " + std::to_string(s.id) + " already exists");
+    const int rc = load_layout(c, L, bytes, n, (flags & VGX_COLLECTION_KEEP_COLOUR) != 0);
+    if (rc == VGX_OK && n_submaps) *n_submaps = (int)L.submaps.size();
+    return rc;
+  });
 }
 
 extern "C" int vgx_collection_load(vgx_ctx* c, const uint8_t* bytes, uint64_t n, int* n_submaps) {
-  return vgx_collection_load_ex(c, bytes, n, 0, n_submaps);
+  return vgx_entry(c, __func__, [&] { return vgx_collection_load_ex(c, bytes, n, 0, n_submaps); });
 }
 
 extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const float* T_M_S, uint8_t* out,
                                    uint64_t capacity, uint64_t* size) {
-  if (!c) return VGX_ERR_INVALID;
-  if (n < 0 || !size || (n > 0 && (!ids || !T_M_S)))
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_collection_save: invalid argument");
-  *size = 0;
-  std::vector<int> order((size_t)n);
-  for (int i = 0; i < n; ++i) order[i] = i;
-  std::sort(order.begin(), order.end(), [&](int a, int b) { return ids[a] < ids[b]; });   // cblox: std::map order
-  std::vector<VgxSubmap*> subs;
-  for (int k = 0; k < n; ++k) {
-    const uint32_t id = ids[order[k]];
-    if (k > 0 && ids[order[k - 1]] == id) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_collection_save: repeated submap id");
-    VgxSubmap* s = c->find(id);
-    if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_collection_save: unknown submap " + std::to_string(id));
-    if (!subs.empty() && (s->voxel_size != subs[0]->voxel_size || s->vps != subs[0]->vps))
-      VGX_FAIL(c, VGX_ERR_INVALID, "vgx_collection_save: a collection has one voxel size and voxels_per_side");
-    subs.push_back(s);
-  }
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // n_blocks of an active submap is final after its integration
-  const double voxel_size = subs.empty() ? 0.0 : (double)subs[0]->voxel_size;
-  const int vps = subs.empty() ? 16 : subs[0]->vps;
-  const uint32_t hdr = block_header_bytes(vps);
-  size_t total_blocks = 0;
-  for (VgxSubmap* s : subs) total_blocks += (size_t)s->n_blocks;
-  // scratch: [payload sizes | block offsets | block messages]
-  uint32_t* d_sizes;
-  uint64_t* d_offs;
-  uint8_t* d_msgs;
-  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_sizes, total_blocks), vgx_part(d_offs, total_blocks));
-  if (rc != VGX_OK) return rc;
-  CollEncodeArgs a{};
-  a.vps = vps;
-  a.header_bytes = hdr;
-  size_t first = 0;
-  for (VgxSubmap* s : subs) {
-    if (s->n_blocks > 0) {
-      a.dw = s->d_dw.get();
-      a.rgba = s->d_rgba.get();
-      a.block_idx = s->d_block_idx.get();
-      a.vox_per_block = s->vox_per_block;
-      a.out_sizes = d_sizes + first;
-      VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
-      collection_encode_kernel<false><<<s->n_blocks, COLL_THREADS, 0, c->stream>>>(a);
+  return vgx_entry(c, __func__, [&] {
+    if (n < 0 || !size || (n > 0 && (!ids || !T_M_S))) VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
+    *size = 0;
+    std::vector<int> order((size_t)n);
+    for (int i = 0; i < n; ++i) order[i] = i;
+    std::sort(order.begin(), order.end(), [&](int a, int b) { return ids[a] < ids[b]; });   // cblox: std::map order
+    std::vector<VgxSubmap*> subs;
+    for (int k = 0; k < n; ++k) {
+      const uint32_t id = ids[order[k]];
+      if (k > 0 && ids[order[k - 1]] == id) VGX_FAIL(c, VGX_ERR_INVALID, "repeated submap id");
+      VgxSubmap* s;
+      VGX_TRY(vgx_submap_get(c, id, &s));
+      if (!subs.empty() && (s->voxel_size != subs[0]->voxel_size || s->vps != subs[0]->vps))
+        VGX_FAIL(c, VGX_ERR_INVALID, "a collection has one voxel size and voxels_per_side");
+      subs.push_back(s);
     }
-    first += (size_t)s->n_blocks;
-  }
-  VGX_CUDA(c, cudaGetLastError());
-  std::vector<uint32_t> sizes(total_blocks);
-  if (total_blocks)
-    VGX_CUDA(c, cudaMemcpyAsync(sizes.data(), d_sizes, total_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost,
-                                c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  // layout: header, then per submap its SubmapProto and its blocks; block messages are contiguous per
-  // submap in the device buffer
-  std::vector<std::vector<uint8_t>> framing((size_t)n + 1);
-  put_delimited(framing[0], collection_header(voxel_size, (uint32_t)vps, (uint32_t)n));
-  std::vector<uint64_t> offsets(total_blocks), span((size_t)n);
-  uint64_t total = framing[0].size(), dev_bytes = 0;
-  first = 0;
-  for (int k = 0; k < n; ++k) {
-    VgxSubmap* s = subs[k];
-    put_delimited(framing[k + 1], submap_message(s->id, (uint32_t)s->n_blocks, T_M_S + 7 * (size_t)order[k]));
-    const uint64_t start = dev_bytes;
-    for (int b = 0; b < s->n_blocks; ++b) {
-      const uint64_t msg = (uint64_t)hdr + sizes[first + b];
-      offsets[first + b] = dev_bytes;
-      dev_bytes += varint_len(msg) + msg;
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // n_blocks of an active submap is final after its integration
+    const double voxel_size = subs.empty() ? 0.0 : (double)subs[0]->voxel_size;
+    const int vps = subs.empty() ? 16 : subs[0]->vps;
+    const uint32_t hdr = block_header_bytes(vps);
+    size_t total_blocks = 0;
+    for (VgxSubmap* s : subs) total_blocks += (size_t)s->n_blocks;
+    // scratch: [payload sizes | block offsets | block messages]
+    uint32_t* d_sizes;
+    uint64_t* d_offs;
+    uint8_t* d_msgs;
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_sizes, total_blocks), vgx_part(d_offs, total_blocks)));
+    CollEncodeArgs a{};
+    a.vps = vps;
+    a.header_bytes = hdr;
+    size_t first = 0;
+    for (VgxSubmap* s : subs) {
+      if (s->n_blocks > 0) {
+        a.dw = s->d_dw.get();
+        a.rgba = s->d_rgba.get();
+        a.block_idx = s->d_block_idx.get();
+        a.vox_per_block = s->vox_per_block;
+        a.out_sizes = d_sizes + first;
+        VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
+        collection_encode_kernel<false><<<s->n_blocks, COLL_THREADS, 0, c->stream>>>(a);
+      }
+      first += (size_t)s->n_blocks;
     }
-    span[k] = dev_bytes - start;
-    total += framing[k + 1].size() + span[k];
-    first += (size_t)s->n_blocks;
-  }
-  *size = total;
-  if (!out) return VGX_OK;
-  if (capacity < total) VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_collection_save: capacity too small");
-  // the second carve of d_scratch may move it: the sizes are re-sent
-  rc = vgx_carve(c, c->d_scratch, vgx_part(d_sizes, total_blocks), vgx_part(d_offs, total_blocks),
-                 vgx_part(d_msgs, (size_t)dev_bytes));
-  if (rc != VGX_OK) return rc;
-  if (total_blocks) {
+    VGX_CUDA(c, cudaGetLastError());
+    std::vector<uint32_t> sizes(total_blocks);
+    if (total_blocks)
+      VGX_CUDA(c, cudaMemcpyAsync(sizes.data(), d_sizes, total_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost,
+                                  c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    // layout: header, then per submap its SubmapProto and its blocks; block messages are contiguous per
+    // submap in the device buffer
+    std::vector<std::vector<uint8_t>> framing((size_t)n + 1);
+    put_delimited(framing[0], collection_header(voxel_size, (uint32_t)vps, (uint32_t)n));
+    std::vector<uint64_t> offsets(total_blocks), span((size_t)n);
+    uint64_t total = framing[0].size(), dev_bytes = 0;
+    first = 0;
+    for (int k = 0; k < n; ++k) {
+      VgxSubmap* s = subs[k];
+      put_delimited(framing[k + 1], submap_message(s->id, (uint32_t)s->n_blocks, T_M_S + 7 * (size_t)order[k]));
+      const uint64_t start = dev_bytes;
+      for (int b = 0; b < s->n_blocks; ++b) {
+        const uint64_t msg = (uint64_t)hdr + sizes[first + b];
+        offsets[first + b] = dev_bytes;
+        dev_bytes += varint_len(msg) + msg;
+      }
+      span[k] = dev_bytes - start;
+      total += framing[k + 1].size() + span[k];
+      first += (size_t)s->n_blocks;
+    }
+    *size = total;
+    if (!out) return VGX_OK;
+    if (capacity < total) VGX_FAIL(c, VGX_ERR_CAPACITY, "capacity too small");
+    // the second carve of d_scratch may move it: the sizes are re-sent
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_sizes, total_blocks), vgx_part(d_offs, total_blocks),
+                      vgx_part(d_msgs, (size_t)dev_bytes)));
+    if (total_blocks) {
+      VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
+      VGX_CUDA(c, cudaMemcpyAsync(d_sizes, sizes.data(), total_blocks * sizeof(uint32_t), cudaMemcpyHostToDevice,
+                                  c->stream));
+      VGX_CUDA(c, cudaMemcpyAsync(d_offs, offsets.data(), total_blocks * sizeof(uint64_t), cudaMemcpyHostToDevice,
+                                  c->stream));
+    }
+    a.dst = d_msgs;
+    first = 0;
+    for (VgxSubmap* s : subs) {
+      if (s->n_blocks > 0) {
+        a.dw = s->d_dw.get();
+        a.rgba = s->d_rgba.get();
+        a.block_idx = s->d_block_idx.get();
+        a.vox_per_block = s->vox_per_block;
+        a.voxel_size = s->voxel_size;
+        a.block_size = s->block_size;
+        a.sizes = d_sizes + first;
+        a.offsets = d_offs + first;
+        VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
+        collection_encode_kernel<true><<<s->n_blocks, COLL_THREADS, 0, c->stream>>>(a);
+      }
+      first += (size_t)s->n_blocks;
+    }
+    VGX_CUDA(c, cudaGetLastError());
     VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
-    VGX_CUDA(c, cudaMemcpyAsync(d_sizes, sizes.data(), total_blocks * sizeof(uint32_t), cudaMemcpyHostToDevice,
-                                c->stream));
-    VGX_CUDA(c, cudaMemcpyAsync(d_offs, offsets.data(), total_blocks * sizeof(uint64_t), cudaMemcpyHostToDevice,
-                                c->stream));
-  }
-  a.dst = d_msgs;
-  first = 0;
-  for (VgxSubmap* s : subs) {
-    if (s->n_blocks > 0) {
-      a.dw = s->d_dw.get();
-      a.rgba = s->d_rgba.get();
-      a.block_idx = s->d_block_idx.get();
-      a.vox_per_block = s->vox_per_block;
-      a.voxel_size = s->voxel_size;
-      a.block_size = s->block_size;
-      a.sizes = d_sizes + first;
-      a.offsets = d_offs + first;
-      VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
-      collection_encode_kernel<true><<<s->n_blocks, COLL_THREADS, 0, c->stream>>>(a);
+    uint8_t* o = out;
+    uint64_t dev_off = 0;
+    memcpy(o, framing[0].data(), framing[0].size());
+    o += framing[0].size();
+    for (int k = 0; k < n; ++k) {
+      memcpy(o, framing[k + 1].data(), framing[k + 1].size());
+      o += framing[k + 1].size();
+      VGX_TRY(copy_d2h_chunked(c, o, d_msgs + dev_off, span[k]));
+      o += span[k];
+      dev_off += span[k];
     }
-    first += (size_t)s->n_blocks;
-  }
-  VGX_CUDA(c, cudaGetLastError());
-  VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
-  uint8_t* o = out;
-  uint64_t dev_off = 0;
-  memcpy(o, framing[0].data(), framing[0].size());
-  o += framing[0].size();
-  for (int k = 0; k < n; ++k) {
-    memcpy(o, framing[k + 1].data(), framing[k + 1].size());
-    o += framing[k + 1].size();
-    rc = copy_d2h_chunked(c, o, d_msgs + dev_off, span[k]);
-    if (rc != VGX_OK) return rc;
-    o += span[k];
-    dev_off += span[k];
-  }
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  return VGX_OK;
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_layer_load(vgx_ctx* c, uint32_t id, const uint8_t* bytes, uint64_t n, int* n_blocks) {
-  if (!c) return VGX_ERR_INVALID;
-  if (n_blocks) *n_blocks = 0;
-  CollLayout L;
-  std::string err;
-  if (!parse_stream(bytes, n, true, &L, &err)) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_layer_load: " + err);
-  if (c->find(id)) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_layer_load: submap " + std::to_string(id) + " already exists");
-  // the layer is the single submap entry; a repeated block index is refused by the upload path
-  // (voxblox BlockMergingStrategy::kProhibit)
-  L.submaps[0].id = id;
-  const int rc = load_layout(c, "vgx_layer_load", L, bytes, n, false);
-  if (rc == VGX_OK && n_blocks) *n_blocks = (int)L.submaps[0].n_blocks;
-  return rc;
+  return vgx_entry(c, __func__, [&] {
+    if (n_blocks) *n_blocks = 0;
+    CollLayout L;
+    std::string err;
+    if (!parse_stream(bytes, n, true, &L, &err)) VGX_FAIL(c, VGX_ERR_INVALID, err);
+    if (c->submaps.count(id)) VGX_FAIL(c, VGX_ERR_INVALID, "submap " + std::to_string(id) + " already exists");
+    // the layer is the single submap entry; a repeated block index is refused by the upload path
+    // (voxblox BlockMergingStrategy::kProhibit)
+    L.submaps[0].id = id;
+    const int rc = load_layout(c, L, bytes, n, false);
+    if (rc == VGX_OK && n_blocks) *n_blocks = (int)L.submaps[0].n_blocks;
+    return rc;
+  });
 }

@@ -109,87 +109,82 @@ extern "C" void vgx_esdf_config_default(vgx_esdf_config* c) {
 }
 
 extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_config* cfg, int* sweeps_out) {
-  if (!c) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_generate_esdf: unknown submap");
-  if (!s->finished) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_generate_esdf: submap is not finished");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  vgx_esdf_config dc;
-  vgx_esdf_config_default(&dc);
-  if (cfg) dc = *cfg;
-  if (!(dc.max_distance_m > 0) || !(dc.min_distance_m >= 0))
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_generate_esdf: invalid distances");
-  vgx_graph_invalidate_registration(c);
-  s->d_esdf.reset();
-  s->d_view_esdf.reset();
-  const size_t nvox = (size_t)s->n_blocks * s->vox_per_block;
-  if (sweeps_out) *sweeps_out = 0;
-  if (nvox == 0) return s->d_view_esdf.alloc(c, 32, "ESDF registration view");
-  EsdfParams P;
-  P.voxel_size = s->voxel_size;
-  P.max_distance = dc.max_distance_m; P.default_distance = dc.default_distance_m;
-  P.min_distance = dc.min_distance_m; P.min_weight = dc.min_weight;
-  P.vps = s->vps;
-  P.sh = s->sh;
-  P.n_blocks = s->n_blocks;
-  cudaStream_t st = c->stream;
-  int rc = s->d_esdf.alloc(c, sizeof(float2) * nvox, "ESDF bricks");
-  if (rc != VGX_OK) return rc;
-  unsigned char* d_fixed;
-  int *d_nb, *d_changed;
-  rc = vgx_carve(c, c->d_work, vgx_part(d_fixed, nvox), vgx_part(d_nb, (size_t)27 * s->n_blocks),
-                 vgx_part(d_changed, 1));
-  if (rc != VGX_OK) return rc;
-  const unsigned grid = (unsigned)((nvox + 255) / 256);
-  esdf_init_kernel<<<grid, 256, 0, st>>>(P, s->d_dw.get(), s->d_esdf.get(), d_fixed);
-  esdf_neighbours_kernel<<<(27 * s->n_blocks + 127) / 128, 128, 0, st>>>(s->hash(), s->d_block_idx.get(), s->n_blocks,
-                                                                          d_nb);
-  c->launches += 2;
-  // relax to convergence: the flag is read back every other sweep
-  int sweeps = 0;
-  const int max_sweeps = 4 * (int)ceilf(dc.max_distance_m / s->voxel_size) + 16;
-  for (;;) {
-    VGX_CUDA(c, cudaMemsetAsync(d_changed, 0, sizeof(int), st));
-    for (int k = 0; k < 2; ++k) {
-      esdf_sweep_kernel<<<grid, 256, 0, st>>>(P, s->d_esdf.get(), d_fixed, d_nb, d_changed);
-      c->launches++;
-      ++sweeps;
+  return vgx_entry(c, __func__, [&] {
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s, VgxNeed::finished));
+    vgx_esdf_config dc;
+    vgx_esdf_config_default(&dc);
+    if (cfg) dc = *cfg;
+    if (!(dc.max_distance_m > 0) || !(dc.min_distance_m >= 0))
+      VGX_FAIL(c, VGX_ERR_INVALID, "invalid distances");
+    vgx_graph_invalidate_registration(c);
+    s->d_esdf.reset();
+    s->d_view_esdf.reset();
+    const size_t nvox = (size_t)s->n_blocks * s->vox_per_block;
+    if (sweeps_out) *sweeps_out = 0;
+    if (nvox == 0) return s->d_view_esdf.alloc(c, 32, "ESDF registration view");
+    EsdfParams P;
+    P.voxel_size = s->voxel_size;
+    P.max_distance = dc.max_distance_m; P.default_distance = dc.default_distance_m;
+    P.min_distance = dc.min_distance_m; P.min_weight = dc.min_weight;
+    P.vps = s->vps;
+    P.sh = s->sh;
+    P.n_blocks = s->n_blocks;
+    cudaStream_t st = c->stream;
+    VGX_TRY(s->d_esdf.alloc(c, sizeof(float2) * nvox, "ESDF bricks"));
+    unsigned char* d_fixed;
+    int *d_nb, *d_changed;
+    VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_fixed, nvox), vgx_part(d_nb, (size_t)27 * s->n_blocks),
+                      vgx_part(d_changed, 1)));
+    const unsigned grid = (unsigned)((nvox + 255) / 256);
+    esdf_init_kernel<<<grid, 256, 0, st>>>(P, s->d_dw.get(), s->d_esdf.get(), d_fixed);
+    esdf_neighbours_kernel<<<(27 * s->n_blocks + 127) / 128, 128, 0, st>>>(s->hash(), s->d_block_idx.get(), s->n_blocks,
+                                                                            d_nb);
+    c->launches += 2;
+    // relax to convergence: the flag is read back every other sweep
+    int sweeps = 0;
+    const int max_sweeps = 4 * (int)ceilf(dc.max_distance_m / s->voxel_size) + 16;
+    for (;;) {
+      VGX_CUDA(c, cudaMemsetAsync(d_changed, 0, sizeof(int), st));
+      for (int k = 0; k < 2; ++k) {
+        esdf_sweep_kernel<<<grid, 256, 0, st>>>(P, s->d_esdf.get(), d_fixed, d_nb, d_changed);
+        c->launches++;
+        ++sweeps;
+      }
+      int changed = 0;
+      VGX_CUDA(c, cudaMemcpyAsync(&changed, d_changed, sizeof(int), cudaMemcpyDeviceToHost, st));
+      VGX_CUDA(c, cudaStreamSynchronize(st));
+      if (!changed) break;
+      if (sweeps > max_sweeps) VGX_FAIL(c, VGX_ERR_INVALID, "relaxation did not converge");
     }
-    int changed = 0;
-    VGX_CUDA(c, cudaMemcpyAsync(&changed, d_changed, sizeof(int), cudaMemcpyDeviceToHost, st));
+    VGX_CUDA(c, cudaGetLastError());
+    if (sweeps_out) *sweeps_out = sweeps;
+    // registration view of the ESDF layer (observed <=> weight 1), same octet layout as the TSDF view
+    VGX_TRY(s->d_view_esdf.alloc(c, sizeof(float) * 8 * nvox, "ESDF registration view"));
+    VGX_TRY(vgx_submap_build_view(c, s, s->d_esdf.get(), s->d_view_esdf.get()));
     VGX_CUDA(c, cudaStreamSynchronize(st));
-    if (!changed) break;
-    if (sweeps > max_sweeps) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_generate_esdf: relaxation did not converge");
-  }
-  VGX_CUDA(c, cudaGetLastError());
-  if (sweeps_out) *sweeps_out = sweeps;
-  // registration view of the ESDF layer (observed <=> weight 1), same octet layout as the TSDF view
-  rc = s->d_view_esdf.alloc(c, sizeof(float) * 8 * nvox, "ESDF registration view");
-  if (rc != VGX_OK) return rc;
-  rc = vgx_submap_build_view(c, s, s->d_esdf.get(), s->d_view_esdf.get());
-  if (rc != VGX_OK) return rc;
-  VGX_CUDA(c, cudaStreamSynchronize(st));
-  return VGX_OK;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_download_esdf(vgx_ctx* c, uint32_t id, int max_blocks, float* distance,
                                         float* observed, int* n_out) {
-  if (!c) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_download_esdf: unknown submap");
-  if (!s->d_esdf.get() && s->n_blocks > 0) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_download_esdf: no ESDF generated");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  const int n = s->n_blocks;
-  if (n_out) *n_out = n;
-  if (n > max_blocks) VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_submap_download_esdf: max_blocks too small");
-  if (n == 0) return VGX_OK;
-  const size_t nvox = (size_t)n * s->vox_per_block;
-  std::vector<float2> h(nvox);
-  VGX_CUDA(c, cudaMemcpyAsync(h.data(), s->d_esdf.get(), sizeof(float2) * nvox, cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  for (size_t i = 0; i < nvox; ++i) {
-    if (distance) distance[i] = h[i].x;
-    if (observed) observed[i] = h[i].y;
-  }
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    if (!s->d_esdf.get() && s->n_blocks > 0) VGX_FAIL(c, VGX_ERR_INVALID, "no ESDF generated");
+    const int n = s->n_blocks;
+    if (n_out) *n_out = n;
+    if (n > max_blocks) VGX_FAIL(c, VGX_ERR_CAPACITY, "max_blocks too small");
+    if (n == 0) return VGX_OK;
+    const size_t nvox = (size_t)n * s->vox_per_block;
+    std::vector<float2> h(nvox);
+    VGX_CUDA(c, cudaMemcpyAsync(h.data(), s->d_esdf.get(), sizeof(float2) * nvox, cudaMemcpyDeviceToHost, c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    for (size_t i = 0; i < nvox; ++i) {
+      if (distance) distance[i] = h[i].x;
+      if (observed) observed[i] = h[i].y;
+    }
+    return VGX_OK;
+  });
 }

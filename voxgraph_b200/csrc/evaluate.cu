@@ -132,10 +132,10 @@ rmse_total_kernel(const RmsePartial* __restrict__ part, int n, RmsePartial* __re
 // ------------------------------------------------------------------ host
 static int rmse_layer(vgx_ctx* c, VgxSubmap* s, int which, const char* name, RmseLayer* L) {
   if (which != VGX_LAYER_TSDF && which != VGX_LAYER_ESDF)
-    VGX_FAIL(c, VGX_ERR_INVALID, std::string("vgx_evaluate_layers_rmse: unknown layer selector for the ") + name);
-  if (!s->finished) VGX_FAIL(c, VGX_ERR_INVALID, std::string("vgx_evaluate_layers_rmse: the ") + name + " is not finished");
+    VGX_FAIL(c, VGX_ERR_INVALID, std::string("unknown layer selector for the ") + name);
+  if (!s->finished) VGX_FAIL(c, VGX_ERR_INVALID, std::string("the ") + name + " is not finished");
   if (which == VGX_LAYER_ESDF && !s->d_view_esdf.get())
-    VGX_FAIL(c, VGX_ERR_INVALID, std::string("vgx_evaluate_layers_rmse: the ") + name + " has no ESDF");
+    VGX_FAIL(c, VGX_ERR_INVALID, std::string("the ") + name + " has no ESDF");
   L->hash = s->hash();
   L->dw = which == VGX_LAYER_ESDF ? s->d_esdf.get() : s->d_dw.get();
   L->block_idx = s->d_block_idx.get();
@@ -146,50 +146,48 @@ static int rmse_layer(vgx_ctx* c, VgxSubmap* s, int which, const char* name, Rms
 
 extern "C" int vgx_evaluate_layers_rmse(vgx_ctx* c, uint32_t gt_id, int gt_layer, uint32_t test_id, int test_layer,
                                         vgx_voxel_evaluation_details* out) {
-  if (!c) return VGX_ERR_INVALID;
-  if (!out) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_evaluate_layers_rmse: invalid argument");
-  memset(out, 0, sizeof(*out));
-  VgxSubmap* g = c->find(gt_id);
-  VgxSubmap* t = c->find(test_id);
-  if (!g || !t) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_evaluate_layers_rmse: unknown submap");
-  if (g->voxel_size != t->voxel_size || g->vps != t->vps)
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_evaluate_layers_rmse: the layers differ in voxel size or voxels_per_side");
-  RmseLayer G, T;
-  int rc = rmse_layer(c, g, gt_layer, "ground truth", &G);
-  if (rc == VGX_OK) rc = rmse_layer(c, t, test_layer, "test layer", &T);
-  if (rc != VGX_OK) return rc;
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  const size_t n_part = (size_t)G.n_blocks + (size_t)T.n_blocks;
-  if (n_part > (size_t)INT32_MAX) VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_evaluate_layers_rmse: too many blocks");
-  RmsePartial total;
-  memset(&total, 0, sizeof(total));
-  if (n_part > 0) {
-    RmsePartial* d_part;
-    rc = vgx_carve(c, c->d_work, vgx_part(d_part, n_part + 1));
-    if (rc != VGX_OK) return rc;
-    cudaStream_t st = c->stream;
-    const int threads = std::min(RMSE_THREADS, g->vox_per_block);
-    {
-      VgxLaunchScope scope(c, VGX_SLOT_EVAL);
-      rmse_block_kernel<<<(unsigned)n_part, threads, 0, st>>>(G, T, g->vox_per_block, d_part);
+  return vgx_entry(c, __func__, [&] {
+    if (!out) VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
+    memset(out, 0, sizeof(*out));
+    VgxSubmap *g, *t;
+    VGX_TRY(vgx_submap_get(c, gt_id, &g));
+    VGX_TRY(vgx_submap_get(c, test_id, &t));
+    if (g->voxel_size != t->voxel_size || g->vps != t->vps)
+      VGX_FAIL(c, VGX_ERR_INVALID, "the layers differ in voxel size or voxels_per_side");
+    RmseLayer G, T;
+    VGX_TRY(rmse_layer(c, g, gt_layer, "ground truth", &G));
+    VGX_TRY(rmse_layer(c, t, test_layer, "test layer", &T));
+    const size_t n_part = (size_t)G.n_blocks + (size_t)T.n_blocks;
+    if (n_part > (size_t)INT32_MAX) VGX_FAIL(c, VGX_ERR_CAPACITY, "too many blocks");
+    RmsePartial total;
+    memset(&total, 0, sizeof(total));
+    if (n_part > 0) {
+      RmsePartial* d_part;
+      VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_part, n_part + 1)));
+      cudaStream_t st = c->stream;
+      const int threads = std::min(RMSE_THREADS, g->vox_per_block);
+      {
+        VgxLaunchScope scope(c, VGX_SLOT_EVAL);
+        rmse_block_kernel<<<(unsigned)n_part, threads, 0, st>>>(G, T, g->vox_per_block, d_part);
+      }
+      VGX_CUDA(c, cudaGetLastError());
+      {
+        VgxLaunchScope scope(c, VGX_SLOT_EVAL);
+        rmse_total_kernel<<<1, RMSE_THREADS, 0, st>>>(d_part, (int)n_part, d_part + n_part);
+      }
+      VGX_CUDA(c, cudaGetLastError());
+      VGX_CUDA(c, cudaMemcpyAsync(&total, d_part + n_part, sizeof(RmsePartial), cudaMemcpyDeviceToHost, st));
+      VGX_CUDA(c, cudaStreamSynchronize(st));
     }
-    VGX_CUDA(c, cudaGetLastError());
-    {
-      VgxLaunchScope scope(c, VGX_SLOT_EVAL);
-      rmse_total_kernel<<<1, RMSE_THREADS, 0, st>>>(d_part, (int)n_part, d_part + n_part);
-    }
-    VGX_CUDA(c, cudaGetLastError());
-    VGX_CUDA(c, cudaMemcpyAsync(&total, d_part + n_part, sizeof(RmsePartial), cudaMemcpyDeviceToHost, st));
-    VGX_CUDA(c, cudaStreamSynchronize(st));
-  }
-  out->rmse = (float)sqrt(total.sum / (double)total.n_eval);
-  out->max_error = total.max_error;
-  out->min_error = 0.0f;
-  out->num_evaluated_voxels = total.n_eval;
-  out->num_ignored_voxels = total.n_ign;
-  out->num_overlapping_voxels = total.n_ovl;
-  out->num_non_overlapping_voxels = total.n_non;
-  return VGX_OK;
+    out->rmse = (float)sqrt(total.sum / (double)total.n_eval);
+    out->max_error = total.max_error;
+    out->min_error = 0.0f;
+    out->num_evaluated_voxels = total.n_eval;
+    out->num_ignored_voxels = total.n_ign;
+    out->num_overlapping_voxels = total.n_ovl;
+    out->num_non_overlapping_voxels = total.n_non;
+    return VGX_OK;
+  });
 }
 
 // ------------------------------------------------------------------ MapEvaluation::evaluate
@@ -210,9 +208,8 @@ static void eval_exp_xyzyaw(const double pose[4], float T[7]) {
 // the projected map: view, ESDF (defaults), relevant voxels with the reference's registration filter
 // (voxgraph_submap.h:26-30), the registration points of the alignment's reference side
 static int eval_finish_projected(vgx_ctx* c, uint32_t id) {
-  int rc = vgx_submap_finish(c, id);
-  if (rc == VGX_OK) rc = vgx_submap_generate_esdf(c, id, nullptr, nullptr);
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(vgx_submap_finish(c, id));
+  VGX_TRY(vgx_submap_generate_esdf(c, id, nullptr, nullptr));
   vgx_registration_filter f;
   f.min_voxel_weight = 1.0;
   f.max_voxel_distance = 0.3;
@@ -222,8 +219,8 @@ static int eval_finish_projected(vgx_ctx* c, uint32_t id) {
 
 // the ground truth (the alignment's reading side): view and ESDF (defaults)
 static int eval_finish_gt(vgx_ctx* c, uint32_t id) {
-  const int rc = vgx_submap_finish(c, id);
-  return rc == VGX_OK ? vgx_submap_generate_esdf(c, id, nullptr, nullptr) : rc;
+  VGX_TRY(vgx_submap_finish(c, id));
+  return vgx_submap_generate_esdf(c, id, nullptr, nullptr);
 }
 
 // MapEvaluation::alignSubmapAtoSubmapB on a private pose graph (the context's graph is set aside)
@@ -273,39 +270,37 @@ static int eval_align(vgx_ctx* c, uint32_t projected, uint32_t gt, double pose[4
 
 extern "C" int vgx_map_evaluate(vgx_ctx* c, uint32_t gt_id, int n, const uint32_t* ids, const float* T_M_S,
                                 vgx_map_evaluation* out) {
-  if (!c) return VGX_ERR_INVALID;
-  if (!out || n < 1 || !ids || !T_M_S) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_map_evaluate: invalid argument");
-  memset(out, 0, sizeof(*out));
-  VgxSubmap* g = c->find(gt_id);
-  if (!g) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_map_evaluate: unknown ground truth " + std::to_string(gt_id));
-  for (int k = 0; k < n; ++k) {
-    if (ids[k] == gt_id) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_map_evaluate: the ground truth is one of the submaps");
-    const VgxSubmap* s = c->find(ids[k]);
-    if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_map_evaluate: unknown submap " + std::to_string(ids[k]));
-    if (s->voxel_size != g->voxel_size || s->vps != g->vps)   // map_evaluation.cpp:66 CHECK_EQ
-      VGX_FAIL(c, VGX_ERR_INVALID,
-               "vgx_map_evaluate: the ground truth and the submaps differ in voxel size or voxels_per_side");
-  }
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  // 1. the projected map, in a scratch submap freed on every exit
-  const uint32_t pid = vgx_scratch_id(c);
-  int rc = vgx_project_map(c, n, ids, T_M_S, pid, nullptr);
-  if (rc != VGX_OK) return rc;
-  // 2.-3. finish both
-  rc = eval_finish_projected(c, pid);
-  if (rc == VGX_OK) rc = eval_finish_gt(c, gt_id);
-  // 4. align the ground truth (reading, free) to the projected map (reference, constant)
-  if (rc == VGX_OK) rc = eval_align(c, pid, gt_id, out->aligned_pose, &out->summary);
-  // 5. move the ground truth into the map's frame and finish it again
-  if (rc == VGX_OK) {
-    eval_exp_xyzyaw(out->aligned_pose, out->T_projected_map__ground_truth);
-    ov_inverse(out->T_projected_map__ground_truth, out->T_ground_truth__reading);
-    rc = vgx_submap_transform(c, gt_id, out->T_projected_map__ground_truth);
-  }
-  if (rc == VGX_OK) rc = eval_finish_gt(c, gt_id);
-  // 6. RMSE of the projected map's ESDF against the ground truth's
-  if (rc == VGX_OK) rc = vgx_evaluate_layers_rmse(c, gt_id, VGX_LAYER_ESDF, pid, VGX_LAYER_ESDF, &out->details);
-  // 7.
-  vgx_submap_drop(c, pid);
-  return rc;
+  return vgx_entry(c, __func__, [&] {
+    if (!out || n < 1 || !ids || !T_M_S) VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
+    memset(out, 0, sizeof(*out));
+    VgxSubmap *g, *s;
+    VGX_TRY(vgx_submap_get(c, gt_id, &g));
+    for (int k = 0; k < n; ++k) {
+      if (ids[k] == gt_id) VGX_FAIL(c, VGX_ERR_INVALID, "the ground truth is one of the submaps");
+      VGX_TRY(vgx_submap_get(c, ids[k], &s));
+      if (s->voxel_size != g->voxel_size || s->vps != g->vps)   // map_evaluation.cpp:66 CHECK_EQ
+        VGX_FAIL(c, VGX_ERR_INVALID,
+                 "the ground truth and the submaps differ in voxel size or voxels_per_side");
+    }
+    // 1. the projected map, in a scratch submap freed on every exit
+    const uint32_t pid = vgx_scratch_id(c);
+    VGX_TRY(vgx_project_map(c, n, ids, T_M_S, pid, nullptr));
+    // 2.-3. finish both
+    int rc = eval_finish_projected(c, pid);
+    if (rc == VGX_OK) rc = eval_finish_gt(c, gt_id);
+    // 4. align the ground truth (reading, free) to the projected map (reference, constant)
+    if (rc == VGX_OK) rc = eval_align(c, pid, gt_id, out->aligned_pose, &out->summary);
+    // 5. move the ground truth into the map's frame and finish it again
+    if (rc == VGX_OK) {
+      eval_exp_xyzyaw(out->aligned_pose, out->T_projected_map__ground_truth);
+      ov_inverse(out->T_projected_map__ground_truth, out->T_ground_truth__reading);
+      rc = vgx_submap_transform(c, gt_id, out->T_projected_map__ground_truth);
+    }
+    if (rc == VGX_OK) rc = eval_finish_gt(c, gt_id);
+    // 6. RMSE of the projected map's ESDF against the ground truth's
+    if (rc == VGX_OK) rc = vgx_evaluate_layers_rmse(c, gt_id, VGX_LAYER_ESDF, pid, VGX_LAYER_ESDF, &out->details);
+    // 7.
+    vgx_submap_drop(c, pid);
+    return rc;
+  });
 }

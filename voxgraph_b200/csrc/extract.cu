@@ -334,16 +334,11 @@ static int install_points(vgx_ctx* c, VgxSubmap* s, int type, VgxBuffer<float>&&
   }
   std::vector<float> w((size_t)n);
   float* d_w;
-  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_w, (size_t)n));
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_w, (size_t)n)));
   gather_weights_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(d_pts.get(), n, d_w);
   c->launches++;
-  cudaError_t e = cudaMemcpyAsync(w.data(), d_w, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, c->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-  if (e != cudaSuccess) {
-    c->set_error(std::string("registration point extraction: ") + cudaGetErrorString(e));
-    return VGX_ERR_CUDA;
-  }
+  VGX_CUDA(c, cudaMemcpyAsync(w.data(), d_w, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   p.cumulative_w.resize((size_t)n);
   double sum = 0;
   for (int i = 0; i < n; ++i) { sum += (double)w[i]; p.cumulative_w[i] = sum; }
@@ -355,8 +350,7 @@ static int install_points(vgx_ctx* c, VgxSubmap* s, int type, VgxBuffer<float>&&
 
 static int alloc_points(vgx_ctx* c, int n, VgxBuffer<float>& out) {
   const size_t units = ((size_t)std::max(n, 1) + VGX_PT_UNIT - 1) / VGX_PT_UNIT;
-  const int rc = out.alloc(c, units * VGX_PT_UNIT_FLOATS * sizeof(float), "registration points");
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(out.alloc(c, units * VGX_PT_UNIT_FLOATS * sizeof(float), "registration points"));
   VGX_CUDA(c, cudaMemsetAsync(out.get(), 0, units * VGX_PT_UNIT_FLOATS * sizeof(float), c->stream));
   return VGX_OK;
 }
@@ -369,181 +363,173 @@ extern "C" void vgx_registration_filter_default(vgx_registration_filter* f) {
 }
 
 extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_registration_filter* filter) {
-  if (!c) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_extract_points: unknown submap");
-  if (!s->finished) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_extract_points: submap is not finished");
-  vgx_registration_filter f;
-  vgx_registration_filter_default(&f);
-  if (filter) f = *filter;
-  if (f.use_esdf_distance && !s->d_esdf.get() && s->n_blocks > 0)
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_extract_points: use_esdf_distance needs the submap's ESDF "
-                                 "(vgx_submap_generate_esdf first, as finishSubmap does)");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  vgx_graph_invalidate_registration(c);
-  const LayerDev L = layer_of(s);
-  const size_t nvox = (size_t)s->n_blocks * s->vox_per_block;
-  s->surface_obb_valid = false;
-  s->iso_blocks.clear();
-  s->d_iso_idx.reset();
-  s->n_iso = 0;
-  s->points_extracted = true;
-  if (nvox == 0) {
-    int rc = install_points(c, s, VGX_POINTS_VOXELS, VgxBuffer<float>(), 0);
-    if (rc == VGX_OK) rc = install_points(c, s, VGX_POINTS_ISOSURFACE, VgxBuffer<float>(), 0);
-    return rc;
-  }
-  if (nvox >= 0xFFFFFFFFull / 12) VGX_FAIL(c, VGX_ERR_CAPACITY, "submap too large for 32-bit candidate indices");
-  cudaStream_t st = c->stream;
-  unsigned *d_counts, *d_offsets, *d_tmp, *d_flags;
-  float* d_obb;
-  int rc = vgx_carve(c, c->d_work, vgx_part(d_counts, nvox + 1), vgx_part(d_offsets, nvox + 1),
-                     vgx_part(d_tmp, vgx_scan_tmp_count(nvox * 12)), vgx_part(d_obb, 6),
-                     vgx_part(d_flags, (size_t)s->n_blocks));
-  if (rc != VGX_OK) return rc;
-  const unsigned grid256 = (unsigned)((nvox + 255) / 256), grid128 = (unsigned)((nvox + 127) / 128);
+  return vgx_entry(c, __func__, [&] {
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s, VgxNeed::finished));
+    vgx_registration_filter f;
+    vgx_registration_filter_default(&f);
+    if (filter) f = *filter;
+    if (f.use_esdf_distance && !s->d_esdf.get() && s->n_blocks > 0)
+      VGX_FAIL(c, VGX_ERR_INVALID, "use_esdf_distance needs the submap's ESDF "
+                                   "(vgx_submap_generate_esdf first, as finishSubmap does)");
+    vgx_graph_invalidate_registration(c);
+    const LayerDev L = layer_of(s);
+    const size_t nvox = (size_t)s->n_blocks * s->vox_per_block;
+    s->surface_obb_valid = false;
+    s->iso_blocks.clear();
+    s->d_iso_idx.reset();
+    s->n_iso = 0;
+    s->points_extracted = true;
+    if (nvox == 0) {
+      VGX_TRY(install_points(c, s, VGX_POINTS_VOXELS, VgxBuffer<float>(), 0));
+      return install_points(c, s, VGX_POINTS_ISOSURFACE, VgxBuffer<float>(), 0);
+    }
+    if (nvox >= 0xFFFFFFFFull / 12) VGX_FAIL(c, VGX_ERR_CAPACITY, "submap too large for 32-bit candidate indices");
+    cudaStream_t st = c->stream;
+    unsigned *d_counts, *d_offsets, *d_tmp, *d_flags;
+    float* d_obb;
+    VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_counts, nvox + 1), vgx_part(d_offsets, nvox + 1),
+                      vgx_part(d_tmp, vgx_scan_tmp_count(nvox * 12)), vgx_part(d_obb, 6),
+                      vgx_part(d_flags, (size_t)s->n_blocks)));
+    const unsigned grid256 = (unsigned)((nvox + 255) / 256), grid128 = (unsigned)((nvox + 127) / 128);
 
-  // ---- relevant voxels + surface OBB
-  {
-    const float inf = INFINITY;
-    const float init[6] = {inf, inf, inf, -inf, -inf, -inf};
-    VGX_CUDA(c, cudaMemcpyAsync(d_obb, init, sizeof(init), cudaMemcpyHostToDevice, st));
-    relevant_count_kernel<<<grid256, 256, 0, st>>>(L, f.min_voxel_weight, f.max_voxel_distance, d_counts);
-    c->launches++;
-    rc = vgx_exclusive_scan_u32(c, d_counts, d_offsets, nvox, d_tmp);
-    if (rc != VGX_OK) return rc;
-    unsigned total = 0;
-    VGX_CUDA(c, cudaMemcpyAsync(&total, d_offsets + nvox, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-    VGX_CUDA(c, cudaStreamSynchronize(st));
-    VgxBuffer<float> d_pts;
-    rc = alloc_points(c, (int)total, d_pts);
-    if (rc != VGX_OK) return rc;
-    relevant_emit_kernel<<<grid256, 256, 0, st>>>(L, d_counts, d_offsets, f.use_esdf_distance ? s->d_esdf.get() : nullptr,
-                                                 d_pts.get(), d_obb);
-    c->launches++;
-    VGX_CUDA(c, cudaGetLastError());
-    float obb[6];
-    VGX_CUDA(c, cudaMemcpyAsync(obb, d_obb, sizeof(obb), cudaMemcpyDeviceToHost, st));
-    VGX_CUDA(c, cudaStreamSynchronize(st));
-    for (int a = 0; a < 3; ++a) { s->surface_obb_min[a] = obb[a]; s->surface_obb_max[a] = obb[3 + a]; }
-    s->surface_obb_valid = total > 0;
-    rc = install_points(c, s, VGX_POINTS_VOXELS, std::move(d_pts), (int)total);
-    if (rc != VGX_OK) return rc;
-  }
-  // ---- isosurface vertices
-  {
-    const float min_weight = (float)f.min_voxel_weight;                 // cpp:211-212
-    const float threshold = (float)(0.5 * (double)s->voxel_size);       // cpp:220
-    const double threshold_inv = 1.0 / (double)threshold;               // createConnectedMesh
-    iso_count_kernel<<<grid128, 128, 0, st>>>(L, min_weight, d_counts);
-    c->launches++;
-    rc = vgx_exclusive_scan_u32(c, d_counts, d_offsets, nvox, d_tmp);
-    if (rc != VGX_OK) return rc;
-    unsigned M = 0;
-    VGX_CUDA(c, cudaMemcpyAsync(&M, d_offsets + nvox, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-    VGX_CUDA(c, cudaStreamSynchronize(st));
-    unsigned kept = 0;
-    VgxBuffer<float> d_pts;
-    if (M > 0) {
-      size_t tsize = 1024;
-      while (tsize < 2 * (size_t)M) tsize <<= 1;
-      IsoBucket* d_table;
-      float* d_cand;
-      unsigned long long* d_key;
-      unsigned *d_keep, *d_koff, *d_tmp2;
-      float2* d_cdw;
-      rc = vgx_carve(c, c->d_work2, vgx_part(d_table, tsize), vgx_part(d_cand, (size_t)M * 3), vgx_part(d_key, M),
-                     vgx_part(d_keep, (size_t)M + 1), vgx_part(d_koff, (size_t)M + 1), vgx_part(d_cdw, M),
-                     vgx_part(d_tmp2, vgx_scan_tmp_count(M)));
-      if (rc != VGX_OK) return rc;
-      iso_table_clear_kernel<<<(unsigned)((tsize + 255) / 256), 256, 0, st>>>(d_table, tsize);
-      iso_emit_kernel<<<grid128, 128, 0, st>>>(L, min_weight, threshold_inv, d_counts, d_offsets, d_cand, d_key,
-                                              d_table, tsize - 1);
-      iso_select_kernel<<<(M + 127) / 128, 128, 0, st>>>(L, d_cand, d_key, d_table, tsize - 1, M, d_keep, d_cdw);
-      c->launches += 3;
-      rc = vgx_exclusive_scan_u32(c, d_keep, d_koff, M, d_tmp2);
-      if (rc != VGX_OK) return rc;
-      VGX_CUDA(c, cudaMemcpyAsync(&kept, d_koff + M, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    // ---- relevant voxels + surface OBB
+    {
+      const float inf = INFINITY;
+      const float init[6] = {inf, inf, inf, -inf, -inf, -inf};
+      VGX_CUDA(c, cudaMemcpyAsync(d_obb, init, sizeof(init), cudaMemcpyHostToDevice, st));
+      relevant_count_kernel<<<grid256, 256, 0, st>>>(L, f.min_voxel_weight, f.max_voxel_distance, d_counts);
+      c->launches++;
+      VGX_TRY(vgx_exclusive_scan_u32(c, d_counts, d_offsets, nvox, d_tmp));
+      unsigned total = 0;
+      VGX_CUDA(c, cudaMemcpyAsync(&total, d_offsets + nvox, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
       VGX_CUDA(c, cudaStreamSynchronize(st));
-      rc = alloc_points(c, (int)kept, d_pts);
-      if (rc != VGX_OK) return rc;
-      VGX_CUDA(c, cudaMemsetAsync(d_flags, 0, sizeof(unsigned) * (size_t)s->n_blocks, st));
-      iso_compact_kernel<<<(M + 127) / 128, 128, 0, st>>>(L, d_cand, d_cdw, d_keep, d_koff, M, d_pts.get(), d_flags);
+      VgxBuffer<float> d_pts;
+      VGX_TRY(alloc_points(c, (int)total, d_pts));
+      relevant_emit_kernel<<<grid256, 256, 0, st>>>(L, d_counts, d_offsets, f.use_esdf_distance ? s->d_esdf.get() : nullptr,
+                                                   d_pts.get(), d_obb);
       c->launches++;
       VGX_CUDA(c, cudaGetLastError());
-      // isosurface block list (slots, ascending) for overlapsWith
-      std::vector<unsigned> flags((size_t)s->n_blocks);
-      VGX_CUDA(c, cudaMemcpyAsync(flags.data(), d_flags, sizeof(unsigned) * (size_t)s->n_blocks,
-                                  cudaMemcpyDeviceToHost, st));
+      float obb[6];
+      VGX_CUDA(c, cudaMemcpyAsync(obb, d_obb, sizeof(obb), cudaMemcpyDeviceToHost, st));
       VGX_CUDA(c, cudaStreamSynchronize(st));
-      for (int b = 0; b < s->n_blocks; ++b)
-        if (flags[b]) s->iso_blocks.push_back(b);
-      if (!s->iso_blocks.empty()) {
-        std::vector<int32_t> bidx(3 * (size_t)s->n_blocks), iso(3 * s->iso_blocks.size());
-        VGX_CUDA(c, cudaMemcpyAsync(bidx.data(), s->d_block_idx.get(), sizeof(int32_t) * bidx.size(),
+      for (int a = 0; a < 3; ++a) { s->surface_obb_min[a] = obb[a]; s->surface_obb_max[a] = obb[3 + a]; }
+      s->surface_obb_valid = total > 0;
+      VGX_TRY(install_points(c, s, VGX_POINTS_VOXELS, std::move(d_pts), (int)total));
+    }
+    // ---- isosurface vertices
+    {
+      const float min_weight = (float)f.min_voxel_weight;                 // cpp:211-212
+      const float threshold = (float)(0.5 * (double)s->voxel_size);       // cpp:220
+      const double threshold_inv = 1.0 / (double)threshold;               // createConnectedMesh
+      iso_count_kernel<<<grid128, 128, 0, st>>>(L, min_weight, d_counts);
+      c->launches++;
+      VGX_TRY(vgx_exclusive_scan_u32(c, d_counts, d_offsets, nvox, d_tmp));
+      unsigned M = 0;
+      VGX_CUDA(c, cudaMemcpyAsync(&M, d_offsets + nvox, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+      VGX_CUDA(c, cudaStreamSynchronize(st));
+      unsigned kept = 0;
+      VgxBuffer<float> d_pts;
+      if (M > 0) {
+        size_t tsize = 1024;
+        while (tsize < 2 * (size_t)M) tsize <<= 1;
+        IsoBucket* d_table;
+        float* d_cand;
+        unsigned long long* d_key;
+        unsigned *d_keep, *d_koff, *d_tmp2;
+        float2* d_cdw;
+        VGX_TRY(vgx_carve(c, c->d_work2, vgx_part(d_table, tsize), vgx_part(d_cand, (size_t)M * 3), vgx_part(d_key, M),
+                          vgx_part(d_keep, (size_t)M + 1), vgx_part(d_koff, (size_t)M + 1), vgx_part(d_cdw, M),
+                          vgx_part(d_tmp2, vgx_scan_tmp_count(M))));
+        iso_table_clear_kernel<<<(unsigned)((tsize + 255) / 256), 256, 0, st>>>(d_table, tsize);
+        iso_emit_kernel<<<grid128, 128, 0, st>>>(L, min_weight, threshold_inv, d_counts, d_offsets, d_cand, d_key,
+                                                d_table, tsize - 1);
+        iso_select_kernel<<<(M + 127) / 128, 128, 0, st>>>(L, d_cand, d_key, d_table, tsize - 1, M, d_keep, d_cdw);
+        c->launches += 3;
+        VGX_TRY(vgx_exclusive_scan_u32(c, d_keep, d_koff, M, d_tmp2));
+        VGX_CUDA(c, cudaMemcpyAsync(&kept, d_koff + M, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+        VGX_CUDA(c, cudaStreamSynchronize(st));
+        VGX_TRY(alloc_points(c, (int)kept, d_pts));
+        VGX_CUDA(c, cudaMemsetAsync(d_flags, 0, sizeof(unsigned) * (size_t)s->n_blocks, st));
+        iso_compact_kernel<<<(M + 127) / 128, 128, 0, st>>>(L, d_cand, d_cdw, d_keep, d_koff, M, d_pts.get(), d_flags);
+        c->launches++;
+        VGX_CUDA(c, cudaGetLastError());
+        // isosurface block list (slots, ascending) for overlapsWith
+        std::vector<unsigned> flags((size_t)s->n_blocks);
+        VGX_CUDA(c, cudaMemcpyAsync(flags.data(), d_flags, sizeof(unsigned) * (size_t)s->n_blocks,
                                     cudaMemcpyDeviceToHost, st));
         VGX_CUDA(c, cudaStreamSynchronize(st));
-        for (size_t k = 0; k < s->iso_blocks.size(); ++k)
-          for (int a = 0; a < 3; ++a) iso[3 * k + a] = bidx[3 * (size_t)s->iso_blocks[k] + a];
-        rc = s->d_iso_idx.alloc(c, sizeof(int32_t) * iso.size(), "isosurface block list");
-        if (rc != VGX_OK) return rc;
-        VGX_CUDA(c, cudaMemcpyAsync(s->d_iso_idx.get(), iso.data(), sizeof(int32_t) * iso.size(),
-                                    cudaMemcpyHostToDevice, st));
-        VGX_CUDA(c, cudaStreamSynchronize(st));
-        s->n_iso = (int)s->iso_blocks.size();
+        for (int b = 0; b < s->n_blocks; ++b)
+          if (flags[b]) s->iso_blocks.push_back(b);
+        if (!s->iso_blocks.empty()) {
+          std::vector<int32_t> bidx(3 * (size_t)s->n_blocks), iso(3 * s->iso_blocks.size());
+          VGX_CUDA(c, cudaMemcpyAsync(bidx.data(), s->d_block_idx.get(), sizeof(int32_t) * bidx.size(),
+                                      cudaMemcpyDeviceToHost, st));
+          VGX_CUDA(c, cudaStreamSynchronize(st));
+          for (size_t k = 0; k < s->iso_blocks.size(); ++k)
+            for (int a = 0; a < 3; ++a) iso[3 * k + a] = bidx[3 * (size_t)s->iso_blocks[k] + a];
+          VGX_TRY(s->d_iso_idx.alloc(c, sizeof(int32_t) * iso.size(), "isosurface block list"));
+          VGX_CUDA(c, cudaMemcpyAsync(s->d_iso_idx.get(), iso.data(), sizeof(int32_t) * iso.size(),
+                                      cudaMemcpyHostToDevice, st));
+          VGX_CUDA(c, cudaStreamSynchronize(st));
+          s->n_iso = (int)s->iso_blocks.size();
+        }
+      } else {
+        VGX_TRY(alloc_points(c, 0, d_pts));
       }
-    } else {
-      rc = alloc_points(c, 0, d_pts);
-      if (rc != VGX_OK) return rc;
+      VGX_TRY(install_points(c, s, VGX_POINTS_ISOSURFACE, std::move(d_pts), (int)kept));
     }
-    rc = install_points(c, s, VGX_POINTS_ISOSURFACE, std::move(d_pts), (int)kept);
-    if (rc != VGX_OK) return rc;
-  }
-  return VGX_OK;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_finish_ex(vgx_ctx* c, uint32_t id, const vgx_registration_filter* filter) {
-  int rc = vgx_submap_finish(c, id);
-  if (rc != VGX_OK) return rc;
-  return vgx_submap_extract_points(c, id, filter);
+  return vgx_entry(c, __func__, [&] {
+    VGX_TRY(vgx_submap_finish(c, id));
+    return vgx_submap_extract_points(c, id, filter);
+  });
 }
 
 extern "C" int vgx_submap_num_points(vgx_ctx* c, uint32_t id, int type, int* n) {
-  if (!c || !n || type < 0 || type > 1) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_num_points: unknown submap");
-  *n = s->points[type].n;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!n || type < 0 || type > 1) return VGX_ERR_INVALID;
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    *n = s->points[type].n;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_download_points(vgx_ctx* c, uint32_t id, int type, int max_n, float* xyz,
                                           float* distance, float* weight, int* n_out) {
-  if (!c || type < 0 || type > 1) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_download_points: unknown submap");
-  const VgxPoints& p = s->points[type];
-  if (n_out) *n_out = p.n;
-  if (p.n > max_n) VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_submap_download_points: max_n too small");
-  if (p.n == 0) return VGX_OK;
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  const size_t n = (size_t)p.n;
-  float *d_xyz, *d_d, *d_w;
-  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_xyz, 3 * n), vgx_part(d_d, n), vgx_part(d_w, n));
-  if (rc != VGX_OK) return rc;
-  unpack_points_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(p.data.get(), p.n, d_xyz, d_d, d_w);
-  c->launches++;
-  if (xyz) VGX_CUDA(c, cudaMemcpyAsync(xyz, d_xyz, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-  if (distance) VGX_CUDA(c, cudaMemcpyAsync(distance, d_d, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-  if (weight) VGX_CUDA(c, cudaMemcpyAsync(weight, d_w, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (type < 0 || type > 1) return VGX_ERR_INVALID;
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    const VgxPoints& p = s->points[type];
+    if (n_out) *n_out = p.n;
+    if (p.n > max_n) VGX_FAIL(c, VGX_ERR_CAPACITY, "max_n too small");
+    if (p.n == 0) return VGX_OK;
+    const size_t n = (size_t)p.n;
+    float *d_xyz, *d_d, *d_w;
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_xyz, 3 * n), vgx_part(d_d, n), vgx_part(d_w, n)));
+    unpack_points_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(p.data.get(), p.n, d_xyz, d_d, d_w);
+    c->launches++;
+    if (xyz) VGX_CUDA(c, cudaMemcpyAsync(xyz, d_xyz, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    if (distance) VGX_CUDA(c, cudaMemcpyAsync(distance, d_d, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    if (weight) VGX_CUDA(c, cudaMemcpyAsync(weight, d_w, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_surface_obb(vgx_ctx* c, uint32_t id, float obb_min[3], float obb_max[3]) {
-  if (!c || !obb_min || !obb_max) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_surface_obb: unknown submap");
-  if (!s->surface_obb_valid) return VGX_ZERO_WEIGHT;  // no voxel qualifies: the box stays +-inf
-  for (int a = 0; a < 3; ++a) { obb_min[a] = s->surface_obb_min[a]; obb_max[a] = s->surface_obb_max[a]; }
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!obb_min || !obb_max) return VGX_ERR_INVALID;
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    if (!s->surface_obb_valid) return VGX_ZERO_WEIGHT;  // no voxel qualifies: the box stays +-inf
+    for (int a = 0; a < 3; ++a) { obb_min[a] = s->surface_obb_min[a]; obb_max[a] = s->surface_obb_max[a]; }
+    return VGX_OK;
+  });
 }

@@ -12,7 +12,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <new>
 #include <numeric>
 
 #include "graph.h"
@@ -35,9 +34,7 @@ void vgx_graph_invalidate_registration(vgx_ctx* c) {
 }
 
 static VgxGraph* graph_of(vgx_ctx* c) {
-  if (!c->graph) {
-    c->graph = new (std::nothrow) VgxGraph();
-  }
+  if (!c->graph) c->graph = new VgxGraph();
   return c->graph;
 }
 
@@ -301,29 +298,30 @@ assemble_exchange_kernel(const double* __restrict__ csum, const VgxRelEdge* __re
 // ------------------------------------------------------------------ sharding (host only)
 extern "C" int vgx_shard_constraints(int nranks, int n, const int32_t* num_residuals,
                                      const uint32_t* locality_keys, int32_t* owner) {
-  if (nranks < 1 || n < 0 || (n > 0 && (!num_residuals || !owner))) return VGX_ERR_INVALID;
-  std::vector<int> order(n);
-  std::iota(order.begin(), order.end(), 0);
-  if (locality_keys)
-    std::stable_sort(order.begin(), order.end(),
-                     [&](int a, int b) { return locality_keys[a] < locality_keys[b]; });
-  int64_t total = 0;
-  for (int i = 0; i < n; ++i) total += std::max(num_residuals[i], 0);
-  int64_t before = 0;
-  for (int i : order) {
-    const int64_t cnt = std::max(num_residuals[i], 0);
-    // rank whose share [r * total / nranks, (r + 1) * total / nranks) holds the midpoint
-    int r = total > 0 ? (int)(((2 * before + cnt) * nranks) / (2 * total)) : 0;
-    owner[i] = std::min(std::max(r, 0), nranks - 1);
-    before += cnt;
-  }
-  return VGX_OK;
+  return vgx_entry_noctx([&] {
+    if (nranks < 1 || n < 0 || (n > 0 && (!num_residuals || !owner))) return VGX_ERR_INVALID;
+    std::vector<int> order(n);
+    std::iota(order.begin(), order.end(), 0);
+    if (locality_keys)
+      std::stable_sort(order.begin(), order.end(),
+                       [&](int a, int b) { return locality_keys[a] < locality_keys[b]; });
+    int64_t total = 0;
+    for (int i = 0; i < n; ++i) total += std::max(num_residuals[i], 0);
+    int64_t before = 0;
+    for (int i : order) {
+      const int64_t cnt = std::max(num_residuals[i], 0);
+      // rank whose share [r * total / nranks, (r + 1) * total / nranks) holds the midpoint
+      int r = total > 0 ? (int)(((2 * before + cnt) * nranks) / (2 * total)) : 0;
+      owner[i] = std::min(std::max(r, 0), nranks - 1);
+      before += cnt;
+    }
+    return VGX_OK;
+  });
 }
 
 // ------------------------------------------------------------------ table construction
 
 static int build_tables(vgx_ctx* c, VgxGraph* g) {
-  VGX_CUDA(c, cudaSetDevice(c->device));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   g->dev = VgxGraphTables();
   const int N = g->N;
@@ -337,8 +335,7 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
   g->sample_override.resize(P);
   for (int i = 0; i < P; ++i) {
     bool sampled = false;
-    int rc = vgx_fill_constraint(c, g->reg_ref[i], g->reg_read[i], &g->reg_cfgs[i], &all[i], &sampled);
-    if (rc != VGX_OK) return rc;
+    VGX_TRY(vgx_fill_constraint(c, g->reg_ref[i], g->reg_read[i], &g->reg_cfgs[i], &all[i], &sampled));
     auto ia = g->index.find(g->reg_ref[i]);
     auto ib = g->index.find(g->reg_read[i]);
     if (ia == g->index.end() || ib == g->index.end())
@@ -355,7 +352,7 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
       if ((int)g->sample_override[i].size() == all[i].n) {
         g->samples[i] = g->sample_override[i];
         for (int32_t v : g->samples[i])
-          if (v < 0 || v >= p.n) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_graph_set_sample_indices: index out of range");
+          if (v < 0 || v >= p.n) VGX_FAIL(c, VGX_ERR_INVALID, "sample index out of range");
       } else {
         g->samples[i].resize(all[i].n);
         vgx_points_draw(p, all[i].n, g->samples[i].data());
@@ -383,9 +380,8 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
     for (int k = 0; k < g->n_local; ++k)
       if (is_sampled[g->local[k]]) { units += ((size_t)cons[k].n + 31) / 32; nidx += (size_t)cons[k].n; }
     if (units > 0) {
-      int rc = g->dev.d_sample_pts.alloc(c, units * VGX_PT_UNIT_FLOATS * sizeof(float), "registration sample points");
-      if (rc == VGX_OK) rc = g->dev.d_sample_idx.alloc(c, nidx * sizeof(int32_t), "registration sample points");
-      if (rc != VGX_OK) return rc;
+      VGX_TRY(g->dev.d_sample_pts.alloc(c, units * VGX_PT_UNIT_FLOATS * sizeof(float), "registration sample points"));
+      VGX_TRY(g->dev.d_sample_idx.alloc(c, nidx * sizeof(int32_t), "registration sample points"));
       size_t uo = 0, io = 0;
       for (int k = 0; k < g->n_local; ++k) {
         const int i = g->local[k];
@@ -631,8 +627,7 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
     cudaLaunchKernelEx(&L.cfg, reg_csum_kernel, sums, g->n_local, g->dev.d_csum.get(), skip);
   }
   if (p2p) {
-    int rc = vgx_p2p_begin(c, g->packed_len, &push, &gat);
-    if (rc != VGX_OK) return rc;
+    VGX_TRY(vgx_p2p_begin(c, g->packed_len, &push, &gat));
   }
   if (p2p && c->p2p_fused && g->packed_len < (size_t)INT_MAX) {
     // one launch: assemble + push -> signal -> wait -> local reduce (grid fully co-resident)
@@ -670,14 +665,10 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
 }
 
 int prepare(vgx_ctx* c, VgxGraph** out) {
-  if (!c) return VGX_ERR_INVALID;
   VgxGraph* g = graph_of(c);
-  if (!g) return VGX_ERR_NOMEM;
   if (g->N == 0) VGX_FAIL(c, VGX_ERR_INVALID, "pose graph has no nodes");
-  VGX_CUDA(c, cudaSetDevice(c->device));
   if (g->dirty) {
-    int rc = build_tables(c, g);
-    if (rc != VGX_OK) return rc;
+    VGX_TRY(build_tables(c, g));
   }
   *out = g;
   return VGX_OK;
@@ -686,86 +677,88 @@ int prepare(vgx_ctx* c, VgxGraph** out) {
 // ------------------------------------------------------------------ C-ABI: b2
 extern "C" int vgx_graph_set_nodes(vgx_ctx* c, int n, const uint32_t* ids, const double* xyzyaw,
                                    const uint8_t* constant) {
-  if (!c || n < 0 || (n > 0 && (!ids || !xyzyaw))) return VGX_ERR_INVALID;
-  VgxGraph* g = graph_of(c);
-  if (!g) return VGX_ERR_NOMEM;
-  std::map<uint32_t, int> index;
-  for (int i = 0; i < n; ++i) {
-    if (index.count(ids[i])) VGX_FAIL(c, VGX_ERR_INVALID, "duplicate submap id in node list");
-    index[ids[i]] = i;
-  }
-  g->N = n;
-  g->ids.assign(ids, ids + n);
-  g->x.assign(xyzyaw, xyzyaw + 4 * (size_t)n);
-  g->constant.assign(n, 0);
-  if (constant)
-    for (int i = 0; i < n; ++i) g->constant[i] = constant[i] ? 1 : 0;
-  g->index.swap(index);
-  g->rel.clear();
-  g->reg_ref.clear();
-  g->reg_read.clear();
-  g->reg_cfgs.clear();
-  g->sample_override.clear();
-  g->dirty = true;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (n < 0 || (n > 0 && (!ids || !xyzyaw))) return VGX_ERR_INVALID;
+    VgxGraph* g = graph_of(c);
+    std::map<uint32_t, int> index;
+    for (int i = 0; i < n; ++i) {
+      if (index.count(ids[i])) VGX_FAIL(c, VGX_ERR_INVALID, "duplicate submap id in node list");
+      index[ids[i]] = i;
+    }
+    g->N = n;
+    g->ids.assign(ids, ids + n);
+    g->x.assign(xyzyaw, xyzyaw + 4 * (size_t)n);
+    g->constant.assign(n, 0);
+    if (constant)
+      for (int i = 0; i < n; ++i) g->constant[i] = constant[i] ? 1 : 0;
+    g->index.swap(index);
+    g->rel.clear();
+    g->reg_ref.clear();
+    g->reg_read.clear();
+    g->reg_cfgs.clear();
+    g->sample_override.clear();
+    g->dirty = true;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_graph_set_poses(vgx_ctx* c, const double* xyzyaw) {
-  if (!c || !xyzyaw) return VGX_ERR_INVALID;
-  VgxGraph* g = graph_of(c);
-  if (!g || g->N == 0) VGX_FAIL(c, VGX_ERR_INVALID, "pose graph has no nodes");
-  g->x.assign(xyzyaw, xyzyaw + 4 * (size_t)g->N);
-  if (!g->dirty) {
-    VGX_CUDA(c, cudaSetDevice(c->device));
-    // stage through pinned memory so the copy is a true async H2D
-    double* h;
-    int rc = vgx_carve(c, c->h_pinned, vgx_part(h, 4 * (size_t)g->N));
-    if (rc != VGX_OK) return rc;
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    memcpy(h, xyzyaw, sizeof(double) * 4 * g->N);
-    VGX_CUDA(c, cudaMemcpyAsync(g->dev.d_x.get(), h, sizeof(double) * 4 * g->N, cudaMemcpyHostToDevice, c->stream));
-  }
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!xyzyaw) return VGX_ERR_INVALID;
+    VgxGraph* g = graph_of(c);
+    if (g->N == 0) VGX_FAIL(c, VGX_ERR_INVALID, "pose graph has no nodes");
+    g->x.assign(xyzyaw, xyzyaw + 4 * (size_t)g->N);
+    if (!g->dirty) {
+      // stage through pinned memory so the copy is a true async H2D
+      double* h;
+      VGX_TRY(vgx_carve(c, c->h_pinned, vgx_part(h, 4 * (size_t)g->N)));
+      VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+      memcpy(h, xyzyaw, sizeof(double) * 4 * g->N);
+      VGX_CUDA(c, cudaMemcpyAsync(g->dev.d_x.get(), h, sizeof(double) * 4 * g->N, cudaMemcpyHostToDevice, c->stream));
+    }
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_graph_get_poses(vgx_ctx* c, double* xyzyaw) {
-  if (!c || !xyzyaw) return VGX_ERR_INVALID;
-  VgxGraph* g = graph_of(c);
-  if (!g) return VGX_ERR_NOMEM;
-  memcpy(xyzyaw, g->x.data(), sizeof(double) * 4 * g->N);
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!xyzyaw) return VGX_ERR_INVALID;
+    VgxGraph* g = graph_of(c);
+    memcpy(xyzyaw, g->x.data(), sizeof(double) * 4 * g->N);
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_graph_set_relative_edges(vgx_ctx* c, int m, const uint32_t* ids_a,
                                             const uint32_t* ids_b, const double* t_obs,
                                             const double* sqrt_info) {
-  if (!c || m < 0 || (m > 0 && (!ids_a || !ids_b || !t_obs || !sqrt_info))) return VGX_ERR_INVALID;
-  VgxGraph* g = graph_of(c);
-  if (!g) return VGX_ERR_NOMEM;
-  std::vector<VgxRelEdge> rel(m);
-  for (int i = 0; i < m; ++i) {
-    auto ia = g->index.find(ids_a[i]);
-    auto ib = g->index.find(ids_b[i]);
-    if (ia == g->index.end() || ib == g->index.end())
-      VGX_FAIL(c, VGX_ERR_NOT_FOUND, "relative-pose edge references a submap without a node");
-    if (ia->second == ib->second) VGX_FAIL(c, VGX_ERR_INVALID, "relative-pose edge from a node to itself");
-    rel[i].a = ia->second;
-    rel[i].b = ib->second;
-    rel[i].t_obs[0] = t_obs[4 * i]; rel[i].t_obs[1] = t_obs[4 * i + 1]; rel[i].t_obs[2] = t_obs[4 * i + 2];
-    rel[i].yaw_obs = t_obs[4 * i + 3];
-    memcpy(rel[i].L, sqrt_info + 16 * (size_t)i, sizeof(double) * 16);
-  }
-  g->rel.swap(rel);
-  g->dirty = true;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (m < 0 || (m > 0 && (!ids_a || !ids_b || !t_obs || !sqrt_info))) return VGX_ERR_INVALID;
+    VgxGraph* g = graph_of(c);
+    std::vector<VgxRelEdge> rel(m);
+    for (int i = 0; i < m; ++i) {
+      auto ia = g->index.find(ids_a[i]);
+      auto ib = g->index.find(ids_b[i]);
+      if (ia == g->index.end() || ib == g->index.end())
+        VGX_FAIL(c, VGX_ERR_NOT_FOUND, "relative-pose edge references a submap without a node");
+      if (ia->second == ib->second) VGX_FAIL(c, VGX_ERR_INVALID, "relative-pose edge from a node to itself");
+      rel[i].a = ia->second;
+      rel[i].b = ib->second;
+      rel[i].t_obs[0] = t_obs[4 * i]; rel[i].t_obs[1] = t_obs[4 * i + 1]; rel[i].t_obs[2] = t_obs[4 * i + 2];
+      rel[i].yaw_obs = t_obs[4 * i + 3];
+      memcpy(rel[i].L, sqrt_info + 16 * (size_t)i, sizeof(double) * 16);
+    }
+    g->rel.swap(rel);
+    g->dirty = true;
+    return VGX_OK;
+  });
 }
 
 static int set_registration(vgx_ctx* c, int p, const uint32_t* ref_ids, const uint32_t* read_ids,
                             const vgx_reg_config* cfgs, bool per_constraint) {
-  if (!c || p < 0 || (p > 0 && (!ref_ids || !read_ids))) return VGX_ERR_INVALID;
+  if (p < 0 || (p > 0 && (!ref_ids || !read_ids))) return VGX_ERR_INVALID;
   if (per_constraint && p > 0 && !cfgs) return VGX_ERR_INVALID;
   VgxGraph* g = graph_of(c);
-  if (!g) return VGX_ERR_NOMEM;
   for (int i = 0; i < p; ++i) {
     if (ref_ids[i] == read_ids[i]) VGX_FAIL(c, VGX_ERR_INVALID, "cannot constrain a submap to itself");
     if (!g->index.count(ref_ids[i]) || !g->index.count(read_ids[i]))
@@ -785,115 +778,115 @@ static int set_registration(vgx_ctx* c, int p, const uint32_t* ref_ids, const ui
 extern "C" int vgx_graph_set_registration_constraints(vgx_ctx* c, int p, const uint32_t* ref_ids,
                                                       const uint32_t* read_ids,
                                                       const vgx_reg_config* cfg) {
-  return set_registration(c, p, ref_ids, read_ids, cfg, false);
+  return vgx_entry(c, __func__, [&] { return set_registration(c, p, ref_ids, read_ids, cfg, false); });
 }
 
 extern "C" int vgx_graph_set_registration_constraints_v(vgx_ctx* c, int p, const uint32_t* ref_ids,
                                                         const uint32_t* read_ids,
                                                         const vgx_reg_config* cfgs) {
-  return set_registration(c, p, ref_ids, read_ids, cfgs, true);
+  return vgx_entry(c, __func__, [&] { return set_registration(c, p, ref_ids, read_ids, cfgs, true); });
 }
 
 extern "C" int vgx_graph_set_sample_indices(vgx_ctx* c, int constraint, int n, const int32_t* indices) {
-  if (!c) return VGX_ERR_INVALID;
-  VgxGraph* g = graph_of(c);
-  if (!g) return VGX_ERR_NOMEM;
-  if (constraint < 0 || constraint >= (int)g->reg_ref.size() || n < 0 || (n > 0 && !indices))
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_graph_set_sample_indices: invalid argument");
-  if (g->reg_cfgs[constraint].sampling_ratio == -1.0f)
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_graph_set_sample_indices: the constraint is not in sampling mode");
-  g->sample_override.resize(g->reg_ref.size());
-  g->sample_override[constraint].assign(indices, indices + n);
-  g->dirty = true;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    VgxGraph* g = graph_of(c);
+    if (constraint < 0 || constraint >= (int)g->reg_ref.size() || n < 0 || (n > 0 && !indices))
+      VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
+    if (g->reg_cfgs[constraint].sampling_ratio == -1.0f)
+      VGX_FAIL(c, VGX_ERR_INVALID, "the constraint is not in sampling mode");
+    g->sample_override.resize(g->reg_ref.size());
+    g->sample_override[constraint].assign(indices, indices + n);
+    g->dirty = true;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_graph_num_registration_residuals(vgx_ctx* c, int64_t* local, int64_t* global) {
-  VgxGraph* g = nullptr;
-  int rc = prepare(c, &g);
-  if (rc != VGX_OK) return rc;
-  if (local) *local = g->residuals_local;
-  if (global) *global = g->residuals_global;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    VgxGraph* g = nullptr;
+    VGX_TRY(prepare(c, &g));
+    if (local) *local = g->residuals_local;
+    if (global) *global = g->residuals_global;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_graph_get_sample_indices(vgx_ctx* c, int constraint, int max_n, int32_t* indices, int* n) {
-  VgxGraph* g = nullptr;
-  int rc = prepare(c, &g);
-  if (rc != VGX_OK) return rc;
-  if (constraint < 0 || constraint >= (int)g->samples.size())
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_graph_get_sample_indices: invalid constraint index");
-  const std::vector<int32_t>& v = g->samples[constraint];
-  if (n) *n = (int)v.size();
-  if ((int)v.size() > max_n) VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_graph_get_sample_indices: max_n too small");
-  if (indices && !v.empty()) memcpy(indices, v.data(), sizeof(int32_t) * v.size());
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    VgxGraph* g = nullptr;
+    VGX_TRY(prepare(c, &g));
+    if (constraint < 0 || constraint >= (int)g->samples.size())
+      VGX_FAIL(c, VGX_ERR_INVALID, "invalid constraint index");
+    const std::vector<int32_t>& v = g->samples[constraint];
+    if (n) *n = (int)v.size();
+    if ((int)v.size() > max_n) VGX_FAIL(c, VGX_ERR_CAPACITY, "max_n too small");
+    if (indices && !v.empty()) memcpy(indices, v.data(), sizeof(int32_t) * v.size());
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_graph_eval_async(vgx_ctx* c, int exclude_registration) {
-  VgxGraph* g = nullptr;
-  int rc = prepare(c, &g);
-  if (rc != VGX_OK) return rc;
-  return eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, exclude_registration != 0);
+  return vgx_entry(c, __func__, [&] {
+    VgxGraph* g = nullptr;
+    VGX_TRY(prepare(c, &g));
+    return eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, exclude_registration != 0);
+  });
 }
 
 extern "C" int vgx_graph_eval(vgx_ctx* c, int exclude_registration, double* cost, double* gradient,
                               double* H) {
-  VgxGraph* g = nullptr;
-  int rc = prepare(c, &g);
-  if (rc != VGX_OK) return rc;
-  rc = eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, exclude_registration != 0);
-  if (rc != VGX_OK) return rc;
-  double* h;
-  rc = vgx_carve(c, c->h_pinned, vgx_part(h, g->packed_len));
-  if (rc != VGX_OK) return rc;
-  VGX_CUDA(c, cudaMemcpyAsync(h, g->dev.d_packed[0].get(), sizeof(double) * g->packed_len, cudaMemcpyDeviceToHost,
-                              c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  const int N = g->N, dim = 4 * N;
-  if (cost) *cost = h[0];
-  if (gradient) memcpy(gradient, h + PACK_HDR, sizeof(double) * dim);
-  if (H) {
-    memset(H, 0, sizeof(double) * (size_t)dim * dim);
-    const double* D = h + PACK_HDR + dim;
-    const double* O = D + 16 * (size_t)N;
-    for (int i = 0; i < N; ++i)
-      for (int r = 0; r < 4; ++r)
-        for (int q = 0; q < 4; ++q) H[(size_t)(4 * i + r) * dim + 4 * i + q] = D[16 * (size_t)i + 4 * r + q];
-    const std::vector<int>& bn = g->block_nodes;
-    for (int b = 0; b < g->E; ++b) {
-      const int i = bn[2 * b], j = bn[2 * b + 1];
-      for (int r = 0; r < 4; ++r)
-        for (int q = 0; q < 4; ++q) {
-          const double v = O[16 * (size_t)b + 4 * r + q];
-          H[(size_t)(4 * i + r) * dim + 4 * j + q] = v;
-          H[(size_t)(4 * j + q) * dim + 4 * i + r] = v;
-        }
+  return vgx_entry(c, __func__, [&] {
+    VgxGraph* g = nullptr;
+    VGX_TRY(prepare(c, &g));
+    VGX_TRY(eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, exclude_registration != 0));
+    double* h;
+    VGX_TRY(vgx_carve(c, c->h_pinned, vgx_part(h, g->packed_len)));
+    VGX_CUDA(c, cudaMemcpyAsync(h, g->dev.d_packed[0].get(), sizeof(double) * g->packed_len, cudaMemcpyDeviceToHost,
+                                c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    const int N = g->N, dim = 4 * N;
+    if (cost) *cost = h[0];
+    if (gradient) memcpy(gradient, h + PACK_HDR, sizeof(double) * dim);
+    if (H) {
+      memset(H, 0, sizeof(double) * (size_t)dim * dim);
+      const double* D = h + PACK_HDR + dim;
+      const double* O = D + 16 * (size_t)N;
+      for (int i = 0; i < N; ++i)
+        for (int r = 0; r < 4; ++r)
+          for (int q = 0; q < 4; ++q) H[(size_t)(4 * i + r) * dim + 4 * i + q] = D[16 * (size_t)i + 4 * r + q];
+      const std::vector<int>& bn = g->block_nodes;
+      for (int b = 0; b < g->E; ++b) {
+        const int i = bn[2 * b], j = bn[2 * b + 1];
+        for (int r = 0; r < 4; ++r)
+          for (int q = 0; q < 4; ++q) {
+            const double v = O[16 * (size_t)b + 4 * r + q];
+            H[(size_t)(4 * i + r) * dim + 4 * j + q] = v;
+            H[(size_t)(4 * j + q) * dim + 4 * i + r] = v;
+          }
+      }
     }
-  }
-  if (c->nranks > 1) {
-    rc = vgx_p2p_check(c);
-    if (rc != VGX_OK) return rc;
-  }
-  if (!exclude_registration && g->zero_weight) return VGX_ZERO_WEIGHT;
-  return VGX_OK;
+    if (c->nranks > 1) {
+      VGX_TRY(vgx_p2p_check(c));
+    }
+    if (!exclude_registration && g->zero_weight) return VGX_ZERO_WEIGHT;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_graph_registration_costs(vgx_ctx* c, double* per_constraint) {
-  VgxGraph* g = nullptr;
-  int rc = prepare(c, &g);
-  if (rc != VGX_OK) return rc;
-  if (!per_constraint) return VGX_ERR_INVALID;
-  rc = eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[1].get(), false, false);
-  if (rc != VGX_OK) return rc;
-  const int P = (int)g->reg_ref.size();
-  std::vector<double> cs((size_t)g->n_local * VGX_REG_NSTRIDE + 1);
-  if (g->n_local > 0)
-    VGX_CUDA(c, cudaMemcpyAsync(cs.data(), g->dev.d_csum.get(), sizeof(double) * VGX_REG_NSTRIDE * g->n_local,
-                                cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  for (int i = 0; i < P; ++i) per_constraint[i] = 0.0;
-  for (int k = 0; k < g->n_local; ++k) per_constraint[g->local[k]] = cs[(size_t)k * VGX_REG_NSTRIDE + 20];
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    VgxGraph* g = nullptr;
+    VGX_TRY(prepare(c, &g));
+    if (!per_constraint) return VGX_ERR_INVALID;
+    VGX_TRY(eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[1].get(), false, false));
+    const int P = (int)g->reg_ref.size();
+    std::vector<double> cs((size_t)g->n_local * VGX_REG_NSTRIDE + 1);
+    if (g->n_local > 0)
+      VGX_CUDA(c, cudaMemcpyAsync(cs.data(), g->dev.d_csum.get(), sizeof(double) * VGX_REG_NSTRIDE * g->n_local,
+                                  cudaMemcpyDeviceToHost, c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    for (int i = 0; i < P; ++i) per_constraint[i] = 0.0;
+    for (int k = 0; k < g->n_local; ++k) per_constraint[g->local[k]] = cs[(size_t)k * VGX_REG_NSTRIDE + 20];
+    return VGX_OK;
+  });
 }
-

@@ -164,7 +164,7 @@ int ensure_table(vgx_ctx* c) {
     ok = build_table(&table);
     built = true;
   }
-  if (!ok) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_mesh_build: the face-walk rule failed to build its table");
+  if (!ok) VGX_FAIL(c, VGX_ERR_INVALID, "the face-walk rule failed to build its table");
   VGX_CUDA(c, cudaMemcpyToSymbolAsync(c_mesh_ntri, table.ntri, sizeof(table.ntri), 0, cudaMemcpyHostToDevice, c->stream));
   VGX_CUDA(c, cudaMemcpyToSymbolAsync(c_mesh_tri, table.tri, sizeof(table.tri), 0, cudaMemcpyHostToDevice, c->stream));
   VGX_CUDA(c, cudaMemcpyToSymbolAsync(c_mesh_edge, table.edge, sizeof(table.edge), 0, cudaMemcpyHostToDevice, c->stream));
@@ -428,11 +428,10 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
   cudaStream_t st = c->stream;
   unsigned *d_cnt, *d_toff, *d_flag, *d_voff, *d_tmp, *d_offs;
   MeshJob* d_jobs;
-  int rc = vgx_carve(c, c->d_work, vgx_part(d_cnt, n_vox + 1), vgx_part(d_toff, n_vox + 1),
-                     vgx_part(d_flag, n_vox + 1), vgx_part(d_voff, n_vox + 1),
-                     vgx_part(d_tmp, vgx_scan_tmp_count(n_vox)), vgx_part(d_jobs, (size_t)nj),
-                     vgx_part(d_offs, 2 * ((size_t)nj + 1)));
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_cnt, n_vox + 1), vgx_part(d_toff, n_vox + 1),
+                    vgx_part(d_flag, n_vox + 1), vgx_part(d_voff, n_vox + 1),
+                    vgx_part(d_tmp, vgx_scan_tmp_count(n_vox)), vgx_part(d_jobs, (size_t)nj),
+                    vgx_part(d_offs, 2 * ((size_t)nj + 1))));
   VGX_CUDA(c, cudaMemcpyAsync(d_jobs, jobs.data(), (size_t)nj * sizeof(MeshJob), cudaMemcpyHostToDevice, st));
   VGX_CUDA(c, cudaMemsetAsync(d_flag, 0, n_vox * sizeof(unsigned), st));
   const unsigned g128 = (unsigned)((n_vox + 127) / 128), g256 = (unsigned)((n_vox + 255) / 256);
@@ -442,20 +441,18 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
   }
   {
     VgxLaunchScope scope(c, VGX_SLOT_MESH, 0);
-    rc = vgx_exclusive_scan_u32(c, d_cnt, d_toff, n_vox, d_tmp);
     c->prof[VGX_SLOT_MESH].launches += 3;
+    VGX_TRY(vgx_exclusive_scan_u32(c, d_cnt, d_toff, n_vox, d_tmp));
   }
-  if (rc != VGX_OK) return rc;
   {
     VgxLaunchScope scope(c, VGX_SLOT_MESH);
     mesh_popc_kernel<<<g256, 256, 0, st>>>(d_flag, n_vox, d_cnt);
   }
   {
     VgxLaunchScope scope(c, VGX_SLOT_MESH, 0);
-    rc = vgx_exclusive_scan_u32(c, d_cnt, d_voff, n_vox, d_tmp);
     c->prof[VGX_SLOT_MESH].launches += 3;
+    VGX_TRY(vgx_exclusive_scan_u32(c, d_cnt, d_voff, n_vox, d_tmp));
   }
-  if (rc != VGX_OK) return rc;
   {
     VgxLaunchScope scope(c, VGX_SLOT_MESH);
     mesh_offsets_kernel<<<(nj + 1 + 127) / 128, 128, 0, st>>>(d_jobs, nj, n_vox, d_toff, d_voff, d_offs);
@@ -467,21 +464,18 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
   const size_t vbase = (size_t)c->mesh_nv, tbase = (size_t)c->mesh_nt;
   const size_t nv = vbase + offs[2 * (size_t)nj + 1], nt = tbase + offs[2 * (size_t)nj];
   if (nv > (size_t)INT32_MAX || nt > (size_t)INT32_MAX)
-    VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_mesh_build: more than 2^31 - 1 vertices or triangles");
+    VGX_FAIL(c, VGX_ERR_CAPACITY, "more than 2^31 - 1 vertices or triangles");
   for (int k = 0; k < nj; ++k) {
     toff.push_back((int64_t)(tbase + offs[2 * (size_t)k]));
     voff.push_back((int64_t)(vbase + offs[2 * (size_t)k + 1]));
   }
-  rc = c->d_mesh_xyz.grow_keep(c, 3 * sizeof(float) * std::max(nv, (size_t)1), 3 * sizeof(float) * vbase,
-                                "mesh vertices");
-  if (rc != VGX_OK) return rc;
-  rc = c->d_mesh_tri.grow_keep(c, 3 * sizeof(uint32_t) * std::max(nt, (size_t)1), 3 * sizeof(uint32_t) * tbase,
-                               "mesh triangles");
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(c->d_mesh_xyz.grow_keep(c, 3 * sizeof(float) * std::max(nv, (size_t)1), 3 * sizeof(float) * vbase,
+                                  "mesh vertices"));
+  VGX_TRY(c->d_mesh_tri.grow_keep(c, 3 * sizeof(uint32_t) * std::max(nt, (size_t)1), 3 * sizeof(uint32_t) * tbase,
+                                  "mesh triangles"));
   if (coloured) {
-    rc = c->d_mesh_rgba.grow_keep(c, sizeof(uint32_t) * std::max(nv, (size_t)1), sizeof(uint32_t) * vbase,
-                                  "mesh vertex colours");
-    if (rc != VGX_OK) return rc;
+    VGX_TRY(c->d_mesh_rgba.grow_keep(c, sizeof(uint32_t) * std::max(nv, (size_t)1), sizeof(uint32_t) * vbase,
+                                     "mesh vertex colours"));
   }
   {
     VgxLaunchScope scope(c, VGX_SLOT_MESH);
@@ -507,13 +501,9 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
 static int mesh_build(vgx_ctx* c, int n, const uint32_t* ids, const float* T_M_S, const vgx_mesh_config& f,
                       std::vector<int64_t>& voff, std::vector<int64_t>& toff) {
   std::vector<VgxSubmap*> subs((size_t)n);
-  for (int k = 0; k < n; ++k) {
-    subs[k] = c->find(ids[k]);
-    if (!subs[k]) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_mesh_build: unknown submap " + std::to_string(ids[k]));
-  }
+  for (int k = 0; k < n; ++k) VGX_TRY(vgx_submap_get(c, ids[k], &subs[k]));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // n_blocks of an active submap is final after its integration
-  int rc = ensure_table(c);
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(ensure_table(c));
   // the build carries vertex colours iff one of its submaps has a colour channel
   bool coloured = false;
   for (int k = 0; k < n; ++k) {
@@ -527,9 +517,8 @@ static int mesh_build(vgx_ctx* c, int n, const uint32_t* ids, const float* T_M_S
     if (k == n || (!jobs.empty() && n_vox + sv > VGX_MESH_BATCH_VOXELS)) {   // run the batch so far
       if (n_vox > 0) {
         if (n_vox > (size_t)0xFFFFFFFFu / 5)
-          VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_mesh_build: a submap too large for 32-bit triangle counts");
-        rc = mesh_batch(c, jobs, n_vox, f.min_weight, coloured, voff, toff);
-        if (rc != VGX_OK) return rc;
+          VGX_FAIL(c, VGX_ERR_CAPACITY, "a submap too large for 32-bit triangle counts");
+        VGX_TRY(mesh_batch(c, jobs, n_vox, f.min_weight, coloured, voff, toff));
       } else {
         for (size_t j = 0; j < jobs.size(); ++j) {
           voff.push_back(c->mesh_nv);
@@ -556,114 +545,113 @@ static int mesh_build(vgx_ctx* c, int n, const uint32_t* ids, const float* T_M_S
 
 extern "C" int vgx_mesh_build(vgx_ctx* c, int n, const uint32_t* ids, const float* T_M_S,
                               const vgx_mesh_config* cfg, int64_t* vertex_offsets, int64_t* triangle_offsets) {
-  if (!c) return VGX_ERR_INVALID;
-  if (n < 0 || (n > 0 && !ids)) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_mesh_build: invalid argument");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  vgx_mesh_free(c);
-  vgx_mesh_config f;
-  vgx_mesh_config_default(&f);
-  if (cfg) f = *cfg;
-  std::vector<int64_t> voff, toff;
-  const int rc = mesh_build(c, n, ids, T_M_S, f, voff, toff);
-  if (rc != VGX_OK) {
+  return vgx_entry(c, __func__, [&] {
+    if (n < 0 || (n > 0 && !ids)) VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
     vgx_mesh_free(c);
-    voff.assign((size_t)n + 1, 0);
-    toff.assign((size_t)n + 1, 0);
-  } else {
-    c->mesh_ids.assign(ids, ids + n);
-    c->mesh_voff = voff;
-  }
-  if (vertex_offsets) memcpy(vertex_offsets, voff.data(), voff.size() * sizeof(int64_t));
-  if (triangle_offsets) memcpy(triangle_offsets, toff.data(), toff.size() * sizeof(int64_t));
-  return rc;
+    vgx_mesh_config f;
+    vgx_mesh_config_default(&f);
+    if (cfg) f = *cfg;
+    std::vector<int64_t> voff, toff;
+    const int rc = mesh_build(c, n, ids, T_M_S, f, voff, toff);
+    if (rc != VGX_OK) {
+      vgx_mesh_free(c);
+      voff.assign((size_t)n + 1, 0);
+      toff.assign((size_t)n + 1, 0);
+    } else {
+      c->mesh_ids.assign(ids, ids + n);
+      c->mesh_voff = voff;
+    }
+    if (vertex_offsets) memcpy(vertex_offsets, voff.data(), voff.size() * sizeof(int64_t));
+    if (triangle_offsets) memcpy(triangle_offsets, toff.data(), toff.size() * sizeof(int64_t));
+    return rc;
+  });
 }
 
 extern "C" int vgx_mesh_download(vgx_ctx* c, int64_t max_vertices, float* xyz, int64_t max_triangles,
                                  uint32_t* triangles, int64_t* n_vertices, int64_t* n_triangles) {
-  if (!c) return VGX_ERR_INVALID;
-  if (n_vertices) *n_vertices = c->mesh_nv;
-  if (n_triangles) *n_triangles = c->mesh_nt;
-  if ((xyz && c->mesh_nv > max_vertices) || (triangles && c->mesh_nt > max_triangles))
-    VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_mesh_download: output too small");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  if (xyz && c->mesh_nv)
-    VGX_CUDA(c, cudaMemcpyAsync(xyz, c->d_mesh_xyz.get(), 3 * sizeof(float) * (size_t)c->mesh_nv, cudaMemcpyDeviceToHost,
-                                c->stream));
-  if (triangles && c->mesh_nt)
-    VGX_CUDA(c, cudaMemcpyAsync(triangles, c->d_mesh_tri.get(), 3 * sizeof(uint32_t) * (size_t)c->mesh_nt,
-                                cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (n_vertices) *n_vertices = c->mesh_nv;
+    if (n_triangles) *n_triangles = c->mesh_nt;
+    if ((xyz && c->mesh_nv > max_vertices) || (triangles && c->mesh_nt > max_triangles))
+      VGX_FAIL(c, VGX_ERR_CAPACITY, "output too small");
+    if (xyz && c->mesh_nv)
+      VGX_CUDA(c, cudaMemcpyAsync(xyz, c->d_mesh_xyz.get(), 3 * sizeof(float) * (size_t)c->mesh_nv, cudaMemcpyDeviceToHost,
+                                  c->stream));
+    if (triangles && c->mesh_nt)
+      VGX_CUDA(c, cudaMemcpyAsync(triangles, c->d_mesh_tri.get(), 3 * sizeof(uint32_t) * (size_t)c->mesh_nt,
+                                  cudaMemcpyDeviceToHost, c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_mesh_download_colours(vgx_ctx* c, int64_t max_vertices, uint32_t* rgba, int64_t* n_vertices) {
-  if (!c) return VGX_ERR_INVALID;
-  if (n_vertices) *n_vertices = c->mesh_nv;
-  if (!rgba || c->mesh_nv == 0) return VGX_OK;
-  if (c->mesh_nv > max_vertices) VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_mesh_download_colours: output too small");
-  if (!c->d_mesh_rgba.get()) {   // no submap of the build has a colour channel
-    memset(rgba, 0, sizeof(uint32_t) * (size_t)c->mesh_nv);
+  return vgx_entry(c, __func__, [&] {
+    if (n_vertices) *n_vertices = c->mesh_nv;
+    if (!rgba || c->mesh_nv == 0) return VGX_OK;
+    if (c->mesh_nv > max_vertices) VGX_FAIL(c, VGX_ERR_CAPACITY, "output too small");
+    if (!c->d_mesh_rgba.get()) {   // no submap of the build has a colour channel
+      memset(rgba, 0, sizeof(uint32_t) * (size_t)c->mesh_nv);
+      return VGX_OK;
+    }
+    VGX_CUDA(c, cudaMemcpyAsync(rgba, c->d_mesh_rgba.get(), sizeof(uint32_t) * (size_t)c->mesh_nv, cudaMemcpyDeviceToHost,
+                                c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
     return VGX_OK;
-  }
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  VGX_CUDA(c, cudaMemcpyAsync(rgba, c->d_mesh_rgba.get(), sizeof(uint32_t) * (size_t)c->mesh_nv, cudaMemcpyDeviceToHost,
-                              c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  return VGX_OK;
+  });
 }
 
 extern "C" int vgx_mesh_ply(vgx_ctx* c, const uint8_t* rgba, uint8_t* out, uint64_t capacity, uint64_t* size) {
-  return vgx_mesh_ply_ex(c, rgba, 0, out, capacity, size);
+  return vgx_entry(c, __func__, [&] { return vgx_mesh_ply_ex(c, rgba, 0, out, capacity, size); });
 }
 
 extern "C" int vgx_mesh_ply_ex(vgx_ctx* c, const uint8_t* rgba, int voxel_colours, uint8_t* out, uint64_t capacity,
                                uint64_t* size) {
-  if (!c) return VGX_ERR_INVALID;
-  if (!size) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_mesh_ply: invalid argument");
-  char hdr[512];
-  const int hn = snprintf(hdr, sizeof(hdr),
-                          "ply\nformat binary_little_endian 1.0\nelement vertex %lld\nproperty float x\n"
-                          "property float y\nproperty float z\nproperty uchar red\nproperty uchar green\n"
-                          "property uchar blue\nproperty uchar alpha\nelement face %lld\n"
-                          "property list uchar int vertex_indices\nend_header\n",
-                          (long long)c->mesh_nv, (long long)c->mesh_nt);
-  const uint64_t body = 16 * (uint64_t)c->mesh_nv + 13 * (uint64_t)c->mesh_nt;
-  *size = (uint64_t)hn + body;
-  if (!out) return VGX_OK;
-  if (capacity < *size) VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_mesh_ply: capacity too small");
-  memcpy(out, hdr, (size_t)hn);
-  if (body == 0) return VGX_OK;
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  const int ns = (int)c->mesh_ids.size();
-  std::vector<uint32_t> col((size_t)ns);
-  for (int k = 0; k < ns; ++k) {
-    uint8_t q[4];
-    if (rgba) memcpy(q, rgba + 4 * (size_t)k, 4); else rainbow(c->mesh_ids[k], q);
-    col[k] = (uint32_t)q[0] | ((uint32_t)q[1] << 8) | ((uint32_t)q[2] << 16) | ((uint32_t)q[3] << 24);
-  }
-  const bool voxel = voxel_colours && c->d_mesh_rgba.get();
-  std::vector<uint32_t> use((size_t)ns, 0u);
-  for (int k = 0; voxel && k < ns; ++k) use[k] = c->mesh_has_colour[k];
-  uint8_t* d_body;
-  int64_t* d_voff;
-  uint32_t *d_col, *d_use;
-  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_body, (size_t)body), vgx_part(d_voff, c->mesh_voff.size()),
-                     vgx_part(d_col, col.size()), vgx_part(d_use, voxel ? use.size() : 0));
-  if (rc != VGX_OK) return rc;
-  if (voxel)
-    VGX_CUDA(c, cudaMemcpyAsync(d_use, use.data(), use.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-  VGX_CUDA(c, cudaMemcpyAsync(d_voff, c->mesh_voff.data(), c->mesh_voff.size() * sizeof(int64_t),
-                              cudaMemcpyHostToDevice, c->stream));
-  VGX_CUDA(c, cudaMemcpyAsync(d_col, col.data(), col.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-  const int64_t recs = c->mesh_nv + c->mesh_nt;
-  {
-    VgxLaunchScope scope(c, VGX_SLOT_MESH);
-    mesh_ply_kernel<<<(unsigned)((recs + 255) / 256), 256, 0, c->stream>>>(c->d_mesh_xyz.get(), c->d_mesh_tri.get(), c->mesh_nv,
-                                                                          c->mesh_nt, d_voff, ns, d_col,
-                                                                          voxel ? c->d_mesh_rgba.get() : nullptr, d_use, d_body);
-  }
-  VGX_CUDA(c, cudaGetLastError());
-  VGX_CUDA(c, cudaMemcpyAsync(out + hn, d_body, (size_t)body, cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!size) VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
+    char hdr[512];
+    const int hn = snprintf(hdr, sizeof(hdr),
+                            "ply\nformat binary_little_endian 1.0\nelement vertex %lld\nproperty float x\n"
+                            "property float y\nproperty float z\nproperty uchar red\nproperty uchar green\n"
+                            "property uchar blue\nproperty uchar alpha\nelement face %lld\n"
+                            "property list uchar int vertex_indices\nend_header\n",
+                            (long long)c->mesh_nv, (long long)c->mesh_nt);
+    const uint64_t body = 16 * (uint64_t)c->mesh_nv + 13 * (uint64_t)c->mesh_nt;
+    *size = (uint64_t)hn + body;
+    if (!out) return VGX_OK;
+    if (capacity < *size) VGX_FAIL(c, VGX_ERR_CAPACITY, "capacity too small");
+    memcpy(out, hdr, (size_t)hn);
+    if (body == 0) return VGX_OK;
+    const int ns = (int)c->mesh_ids.size();
+    std::vector<uint32_t> col((size_t)ns);
+    for (int k = 0; k < ns; ++k) {
+      uint8_t q[4];
+      if (rgba) memcpy(q, rgba + 4 * (size_t)k, 4); else rainbow(c->mesh_ids[k], q);
+      col[k] = (uint32_t)q[0] | ((uint32_t)q[1] << 8) | ((uint32_t)q[2] << 16) | ((uint32_t)q[3] << 24);
+    }
+    const bool voxel = voxel_colours && c->d_mesh_rgba.get();
+    std::vector<uint32_t> use((size_t)ns, 0u);
+    for (int k = 0; voxel && k < ns; ++k) use[k] = c->mesh_has_colour[k];
+    uint8_t* d_body;
+    int64_t* d_voff;
+    uint32_t *d_col, *d_use;
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_body, (size_t)body), vgx_part(d_voff, c->mesh_voff.size()),
+                      vgx_part(d_col, col.size()), vgx_part(d_use, voxel ? use.size() : 0)));
+    if (voxel)
+      VGX_CUDA(c, cudaMemcpyAsync(d_use, use.data(), use.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    VGX_CUDA(c, cudaMemcpyAsync(d_voff, c->mesh_voff.data(), c->mesh_voff.size() * sizeof(int64_t),
+                                cudaMemcpyHostToDevice, c->stream));
+    VGX_CUDA(c, cudaMemcpyAsync(d_col, col.data(), col.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    const int64_t recs = c->mesh_nv + c->mesh_nt;
+    {
+      VgxLaunchScope scope(c, VGX_SLOT_MESH);
+      mesh_ply_kernel<<<(unsigned)((recs + 255) / 256), 256, 0, c->stream>>>(c->d_mesh_xyz.get(), c->d_mesh_tri.get(), c->mesh_nv,
+                                                                            c->mesh_nt, d_voff, ns, d_col,
+                                                                            voxel ? c->d_mesh_rgba.get() : nullptr, d_use, d_body);
+    }
+    VGX_CUDA(c, cudaGetLastError());
+    VGX_CUDA(c, cudaMemcpyAsync(out + hn, d_body, (size_t)body, cudaMemcpyDeviceToHost, c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    return VGX_OK;
+  });
 }

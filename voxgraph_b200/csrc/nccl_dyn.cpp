@@ -49,44 +49,48 @@ static bool nccl_load(std::string* err) {
 }
 
 extern "C" int vgx_comm_unique_id(uint8_t id[128]) {
-  if (!id) return VGX_ERR_INVALID;
-  if (!nccl_load(nullptr)) return VGX_ERR_NCCL;
-  ncclUniqueId u;
-  if (g_nccl.GetUniqueId(&u) != 0) return VGX_ERR_NCCL;
-  memcpy(id, u.internal, 128);
-  return VGX_OK;
+  return vgx_entry_noctx([&] {
+    if (!id) return VGX_ERR_INVALID;
+    if (!nccl_load(nullptr)) return VGX_ERR_NCCL;
+    ncclUniqueId u;
+    if (g_nccl.GetUniqueId(&u) != 0) return VGX_ERR_NCCL;
+    memcpy(id, u.internal, 128);
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_comm_init(vgx_ctx* c, int nranks, int rank, const uint8_t id[128]) {
-  if (!c || !id || nranks < 1 || rank < 0 || rank >= nranks) return VGX_ERR_INVALID;
-  std::string err;
-  if (!nccl_load(&err)) VGX_FAIL(c, VGX_ERR_NCCL, err);
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  vgx_comm_destroy(c);
-  ncclUniqueId u;
-  memcpy(u.internal, id, 128);
-  ncclComm_t comm = nullptr;
-  ncclResult_t r = g_nccl.CommInitRank(&comm, nranks, u, rank);
-  if (r != 0)
-    VGX_FAIL(c, VGX_ERR_NCCL, std::string("ncclCommInitRank: ") +
-                                  (g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "error"));
-  c->nccl_comm = comm;
-  c->nranks = nranks;
-  c->rank = rank;
-  vgx_graph_invalidate_registration(c);
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!id || nranks < 1 || rank < 0 || rank >= nranks) return VGX_ERR_INVALID;
+    std::string err;
+    if (!nccl_load(&err)) VGX_FAIL(c, VGX_ERR_NCCL, err);
+    vgx_comm_destroy(c);
+    ncclUniqueId u;
+    memcpy(u.internal, id, 128);
+    ncclComm_t comm = nullptr;
+    ncclResult_t r = g_nccl.CommInitRank(&comm, nranks, u, rank);
+    if (r != 0)
+      VGX_FAIL(c, VGX_ERR_NCCL, std::string("ncclCommInitRank: ") +
+                                    (g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "error"));
+    c->nccl_comm = comm;
+    c->nranks = nranks;
+    c->rank = rank;
+    vgx_graph_invalidate_registration(c);
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_comm_destroy(vgx_ctx* c) {
-  if (!c) return VGX_ERR_INVALID;
-  if (c->nccl_comm && g_nccl.handle) {
-    cudaStreamSynchronize(c->stream);
-    g_nccl.CommDestroy((ncclComm_t)c->nccl_comm);
-  }
-  c->nccl_comm = nullptr;
-  c->nranks = 1;
-  c->rank = 0;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (c->nccl_comm && g_nccl.handle) {
+      cudaStreamSynchronize(c->stream);
+      g_nccl.CommDestroy((ncclComm_t)c->nccl_comm);
+    }
+    c->nccl_comm = nullptr;
+    c->nranks = 1;
+    c->rank = 0;
+    return VGX_OK;
+  });
 }
 
 int vgx_nccl_allreduce_sum_f64(vgx_ctx* c, double* d_buf, size_t count) {

@@ -64,83 +64,82 @@ overlap_pairs_kernel(const OverlapJob* __restrict__ jobs, int* __restrict__ flag
 
 extern "C" int vgx_find_overlapping_pairs(vgx_ctx* c, int n, const uint32_t* ids, const float* poses,
                                           int max_pairs, uint32_t* pairs, int* n_pairs) {
-  if (!c || n < 0 || (n > 0 && (!ids || !poses)) || !n_pairs || max_pairs < 0 || (max_pairs > 0 && !pairs))
-    return VGX_ERR_INVALID;
-  *n_pairs = 0;
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  std::vector<VgxSubmap*> sm(n);
-  std::vector<float> amin(3 * (size_t)n), amax(3 * (size_t)n);
-  for (int i = 0; i < n; ++i) {
-    sm[i] = c->find(ids[i]);
-    if (!sm[i]) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_find_overlapping_pairs: unknown submap");
-    if (!sm[i]->finished || !sm[i]->points_extracted)
-      VGX_FAIL(c, VGX_ERR_INVALID, "vgx_find_overlapping_pairs: run vgx_submap_extract_points / "
-                                   "vgx_submap_finish_ex on every submap first (surface OBB + isosurface blocks)");
-    // getMissionFrameSurfaceAabb = getAabbFromObbAndPose(surface OBB, pose): an OBB that was never
-    // updated stays (+inf, -inf) and so does the AABB, which then fails every interval test
-    float* mn = &amin[3 * (size_t)i];
-    float* mx = &amax[3 * (size_t)i];
-    for (int a = 0; a < 3; ++a) { mn[a] = INFINITY; mx[a] = -INFINITY; }
-    const float* T = poses + 7 * (size_t)i;
-    const float omin[3] = {sm[i]->surface_obb_valid ? sm[i]->surface_obb_min[0] : INFINITY,
-                           sm[i]->surface_obb_valid ? sm[i]->surface_obb_min[1] : INFINITY,
-                           sm[i]->surface_obb_valid ? sm[i]->surface_obb_min[2] : INFINITY};
-    const float omax[3] = {sm[i]->surface_obb_valid ? sm[i]->surface_obb_max[0] : -INFINITY,
-                           sm[i]->surface_obb_valid ? sm[i]->surface_obb_max[1] : -INFINITY,
-                           sm[i]->surface_obb_valid ? sm[i]->surface_obb_max[2] : -INFINITY};
-    for (unsigned k = 0; k < 8; ++k) {
-      // getCornerCoordinates: bit set -> min, clear -> max
-      const float corner[3] = {(k & 1) ? omin[0] : omax[0], (k & 2) ? omin[1] : omax[1],
-                               (k & 4) ? omin[2] : omax[2]};
-      float m[3];
-      ov_transform(T, corner, m);
-      for (int a = 0; a < 3; ++a) {
-        if (m[a] < mn[a]) mn[a] = m[a];   // cwiseMin / cwiseMax (NaN never replaces)
-        if (m[a] > mx[a]) mx[a] = m[a];
+  return vgx_entry(c, __func__, [&] {
+    if (n < 0 || (n > 0 && (!ids || !poses)) || !n_pairs || max_pairs < 0 || (max_pairs > 0 && !pairs))
+      return VGX_ERR_INVALID;
+    *n_pairs = 0;
+    std::vector<VgxSubmap*> sm(n);
+    std::vector<float> amin(3 * (size_t)n), amax(3 * (size_t)n);
+    for (int i = 0; i < n; ++i) {
+      VGX_TRY(vgx_submap_get(c, ids[i], &sm[i]));
+      if (!sm[i]->finished || !sm[i]->points_extracted)
+        VGX_FAIL(c, VGX_ERR_INVALID, "run vgx_submap_extract_points / "
+                                     "vgx_submap_finish_ex on every submap first (surface OBB + isosurface blocks)");
+      // getMissionFrameSurfaceAabb = getAabbFromObbAndPose(surface OBB, pose): an OBB that was never
+      // updated stays (+inf, -inf) and so does the AABB, which then fails every interval test
+      float* mn = &amin[3 * (size_t)i];
+      float* mx = &amax[3 * (size_t)i];
+      for (int a = 0; a < 3; ++a) { mn[a] = INFINITY; mx[a] = -INFINITY; }
+      const float* T = poses + 7 * (size_t)i;
+      const float omin[3] = {sm[i]->surface_obb_valid ? sm[i]->surface_obb_min[0] : INFINITY,
+                             sm[i]->surface_obb_valid ? sm[i]->surface_obb_min[1] : INFINITY,
+                             sm[i]->surface_obb_valid ? sm[i]->surface_obb_min[2] : INFINITY};
+      const float omax[3] = {sm[i]->surface_obb_valid ? sm[i]->surface_obb_max[0] : -INFINITY,
+                             sm[i]->surface_obb_valid ? sm[i]->surface_obb_max[1] : -INFINITY,
+                             sm[i]->surface_obb_valid ? sm[i]->surface_obb_max[2] : -INFINITY};
+      for (unsigned k = 0; k < 8; ++k) {
+        // getCornerCoordinates: bit set -> min, clear -> max
+        const float corner[3] = {(k & 1) ? omin[0] : omax[0], (k & 2) ? omin[1] : omax[1],
+                                 (k & 4) ? omin[2] : omax[2]};
+        float m[3];
+        ov_transform(T, corner, m);
+        for (int a = 0; a < 3; ++a) {
+          if (m[a] < mn[a]) mn[a] = m[a];   // cwiseMin / cwiseMax (NaN never replaces)
+          if (m[a] > mx[a]) mx[a] = m[a];
+        }
       }
     }
-  }
-  // pose_graph_interface.cpp:115-146: every i against the subsequent j
-  std::vector<OverlapJob> jobs;
-  std::vector<std::pair<int, int>> cand;
-  for (int i = 0; i < n; ++i) {
-    for (int j = i + 1; j < n; ++j) {
-      bool sep = false;
-      for (int a = 0; a < 3; ++a)   // cpp:251-256
-        if (amax[3 * (size_t)i + a] < amin[3 * (size_t)j + a] || amin[3 * (size_t)i + a] > amax[3 * (size_t)j + a]) sep = true;
-      if (sep || sm[i]->n_iso == 0) continue;
-      OverlapJob J;
-      J.other_hash = sm[j]->hash();
-      J.iso_idx = sm[i]->d_iso_idx.get();
-      J.n_iso = sm[i]->n_iso;
-      J.block_size = sm[i]->block_size;
-      J.other_block_size_inv = sm[j]->block_size_inv;
-      float inv[7];
-      ov_inverse(poses + 7 * (size_t)j, inv);              // cpp:261-262
-      ov_compose(inv, poses + 7 * (size_t)i, J.T);
-      jobs.push_back(J);
-      cand.emplace_back(i, j);
+    // pose_graph_interface.cpp:115-146: every i against the subsequent j
+    std::vector<OverlapJob> jobs;
+    std::vector<std::pair<int, int>> cand;
+    for (int i = 0; i < n; ++i) {
+      for (int j = i + 1; j < n; ++j) {
+        bool sep = false;
+        for (int a = 0; a < 3; ++a)   // cpp:251-256
+          if (amax[3 * (size_t)i + a] < amin[3 * (size_t)j + a] || amin[3 * (size_t)i + a] > amax[3 * (size_t)j + a]) sep = true;
+        if (sep || sm[i]->n_iso == 0) continue;
+        OverlapJob J;
+        J.other_hash = sm[j]->hash();
+        J.iso_idx = sm[i]->d_iso_idx.get();
+        J.n_iso = sm[i]->n_iso;
+        J.block_size = sm[i]->block_size;
+        J.other_block_size_inv = sm[j]->block_size_inv;
+        float inv[7];
+        ov_inverse(poses + 7 * (size_t)j, inv);              // cpp:261-262
+        ov_compose(inv, poses + 7 * (size_t)i, J.T);
+        jobs.push_back(J);
+        cand.emplace_back(i, j);
+      }
     }
-  }
-  if (jobs.empty()) return VGX_OK;
-  OverlapJob* d_jobs;
-  int* d_flags;
-  int rc = vgx_carve(c, c->d_scratch, vgx_part(d_jobs, jobs.size()), vgx_part(d_flags, jobs.size()));
-  if (rc != VGX_OK) return rc;
-  VGX_CUDA(c, cudaMemcpyAsync(d_jobs, jobs.data(), jobs.size() * sizeof(OverlapJob), cudaMemcpyHostToDevice, c->stream));
-  overlap_pairs_kernel<<<(unsigned)jobs.size(), 128, 0, c->stream>>>(d_jobs, d_flags);
-  c->launches++;
-  VGX_CUDA(c, cudaGetLastError());
-  std::vector<int> flags(jobs.size());
-  VGX_CUDA(c, cudaMemcpyAsync(flags.data(), d_flags, jobs.size() * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  int np = 0;
-  for (size_t k = 0; k < jobs.size(); ++k) {
-    if (!flags[k]) continue;
-    if (np < max_pairs) { pairs[2 * np] = ids[cand[k].first]; pairs[2 * np + 1] = ids[cand[k].second]; }
-    ++np;
-  }
-  *n_pairs = np;
-  if (np > max_pairs) VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_find_overlapping_pairs: max_pairs too small");
-  return VGX_OK;
+    if (jobs.empty()) return VGX_OK;
+    OverlapJob* d_jobs;
+    int* d_flags;
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_jobs, jobs.size()), vgx_part(d_flags, jobs.size())));
+    VGX_CUDA(c, cudaMemcpyAsync(d_jobs, jobs.data(), jobs.size() * sizeof(OverlapJob), cudaMemcpyHostToDevice, c->stream));
+    overlap_pairs_kernel<<<(unsigned)jobs.size(), 128, 0, c->stream>>>(d_jobs, d_flags);
+    c->launches++;
+    VGX_CUDA(c, cudaGetLastError());
+    std::vector<int> flags(jobs.size());
+    VGX_CUDA(c, cudaMemcpyAsync(flags.data(), d_flags, jobs.size() * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    int np = 0;
+    for (size_t k = 0; k < jobs.size(); ++k) {
+      if (!flags[k]) continue;
+      if (np < max_pairs) { pairs[2 * np] = ids[cand[k].first]; pairs[2 * np + 1] = ids[cand[k].second]; }
+      ++np;
+    }
+    *n_pairs = np;
+    if (np > max_pairs) VGX_FAIL(c, VGX_ERR_CAPACITY, "max_pairs too small");
+    return VGX_OK;
+  });
 }

@@ -35,55 +35,57 @@ void vgx_p2p_free(vgx_ctx* c) {
 }
 
 extern "C" int vgx_comm_p2p_export(vgx_ctx* c, uint64_t capacity_doubles, uint8_t handle[64]) {
-  if (!c || !handle || capacity_doubles == 0) return VGX_ERR_INVALID;
-  static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  vgx_p2p_free(c);
-  const size_t cap = ((size_t)capacity_doubles + 31) & ~(size_t)31;
-  // the rank count is not known yet: room for the 8 source ranks of one node, two parities
-  const size_t bytes = P2P_FLAG_BYTES + 2 * (size_t)P2P_MAX_RANKS * cap * P2P_ELEM_BYTES;
-  VGX_CUDA(c, cudaMalloc(&c->p2p_base, bytes));
-  VGX_CUDA(c, cudaMemset(c->p2p_base, 0, bytes));
-  cudaIpcMemHandle_t h;
-  VGX_CUDA(c, cudaIpcGetMemHandle(&h, c->p2p_base));
-  memcpy(handle, &h, 64);
-  c->p2p_cap = cap;
-  c->p2p_epoch = 0;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!handle || capacity_doubles == 0) return VGX_ERR_INVALID;
+    static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
+    vgx_p2p_free(c);
+    const size_t cap = ((size_t)capacity_doubles + 31) & ~(size_t)31;
+    // the rank count is not known yet: room for the 8 source ranks of one node, two parities
+    const size_t bytes = P2P_FLAG_BYTES + 2 * (size_t)P2P_MAX_RANKS * cap * P2P_ELEM_BYTES;
+    VGX_CUDA(c, cudaMalloc(&c->p2p_base, bytes));
+    VGX_CUDA(c, cudaMemset(c->p2p_base, 0, bytes));
+    cudaIpcMemHandle_t h;
+    VGX_CUDA(c, cudaIpcGetMemHandle(&h, c->p2p_base));
+    memcpy(handle, &h, 64);
+    c->p2p_cap = cap;
+    c->p2p_epoch = 0;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_comm_p2p_import(vgx_ctx* c, int nranks, int rank, const uint8_t* handles) {
-  if (!c || !handles || nranks < 1 || nranks > P2P_MAX_RANKS || rank < 0 || rank >= nranks) return VGX_ERR_INVALID;
-  if (!c->p2p_base) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_comm_p2p_import: call vgx_comm_p2p_export first");
-  if (c->nccl_comm && (c->nranks != nranks || c->rank != rank))
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_comm_p2p_import: rank layout differs from vgx_comm_init");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  for (int r = 0; r < nranks; ++r) {
-    if (r == rank) { c->p2p_peer[r] = c->p2p_base; continue; }
-    cudaIpcMemHandle_t h;
-    memcpy(&h, handles + 64 * (size_t)r, 64);
-    void* p = nullptr;
-    VGX_CUDA(c, cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
-    c->p2p_peer[r] = p;
-  }
-  c->nranks = nranks;
-  c->rank = rank;
-  c->p2p_ready = true;
-  {
-    // one launch (assemble + push + wait + reduce) by default; VGX_P2P_FUSED=0 selects two launches
-    const char* f = getenv("VGX_P2P_FUSED");
-    c->p2p_fused = !(f && f[0] == '0');
-    // a rank that lags (first-launch module load, table builds, uploads) must not look dead:
-    // generous default, VGX_P2P_TIMEOUT_S overrides; callers barrier before the first exchange
-    const char* t = getenv("VGX_P2P_TIMEOUT_S");
-    double secs = t ? atof(t) : 30.0;
-    if (!(secs > 0)) secs = 30.0;
-    int khz = 1965000;
-    cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, c->device);
-    c->p2p_timeout_cycles = (long long)(secs * 1e3 * (double)khz);
-  }
-  vgx_graph_invalidate_registration(c);
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!handles || nranks < 1 || nranks > P2P_MAX_RANKS || rank < 0 || rank >= nranks) return VGX_ERR_INVALID;
+    if (!c->p2p_base) VGX_FAIL(c, VGX_ERR_INVALID, "call vgx_comm_p2p_export first");
+    if (c->nccl_comm && (c->nranks != nranks || c->rank != rank))
+      VGX_FAIL(c, VGX_ERR_INVALID, "rank layout differs from vgx_comm_init");
+    for (int r = 0; r < nranks; ++r) {
+      if (r == rank) { c->p2p_peer[r] = c->p2p_base; continue; }
+      cudaIpcMemHandle_t h;
+      memcpy(&h, handles + 64 * (size_t)r, 64);
+      void* p = nullptr;
+      VGX_CUDA(c, cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
+      c->p2p_peer[r] = p;
+    }
+    c->nranks = nranks;
+    c->rank = rank;
+    c->p2p_ready = true;
+    {
+      // one launch (assemble + push + wait + reduce) by default; VGX_P2P_FUSED=0 selects two launches
+      const char* f = getenv("VGX_P2P_FUSED");
+      c->p2p_fused = !(f && f[0] == '0');
+      // a rank that lags (first-launch module load, table builds, uploads) must not look dead:
+      // generous default, VGX_P2P_TIMEOUT_S overrides; callers barrier before the first exchange
+      const char* t = getenv("VGX_P2P_TIMEOUT_S");
+      double secs = t ? atof(t) : 30.0;
+      if (!(secs > 0)) secs = 30.0;
+      int khz = 1965000;
+      cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, c->device);
+      c->p2p_timeout_cycles = (long long)(secs * 1e3 * (double)khz);
+    }
+    vgx_graph_invalidate_registration(c);
+    return VGX_OK;
+  });
 }
 
 int vgx_p2p_check(vgx_ctx* c) {
@@ -136,21 +138,22 @@ int vgx_p2p_gather(vgx_ctx* c, const VgxP2PGather& gat, double* d_out, size_t co
 }
 
 extern "C" int vgx_comm_suspend(vgx_ctx* c, int on) {
-  if (!c) return VGX_ERR_INVALID;
-  if (on) {
-    if (c->saved_nranks == 0) {
-      c->saved_nranks = c->nranks;
-      c->saved_rank = c->rank;
-      c->nranks = 1;
-      c->rank = 0;
+  return vgx_entry(c, __func__, [&] {
+    if (on) {
+      if (c->saved_nranks == 0) {
+        c->saved_nranks = c->nranks;
+        c->saved_rank = c->rank;
+        c->nranks = 1;
+        c->rank = 0;
+        vgx_graph_invalidate_registration(c);
+      }
+    } else if (c->saved_nranks != 0) {
+      c->nranks = c->saved_nranks;
+      c->rank = c->saved_rank;
+      c->saved_nranks = 0;
+      c->saved_rank = 0;
       vgx_graph_invalidate_registration(c);
     }
-  } else if (c->saved_nranks != 0) {
-    c->nranks = c->saved_nranks;
-    c->rank = c->saved_rank;
-    c->saved_nranks = 0;
-    c->saved_rank = 0;
-    vgx_graph_invalidate_registration(c);
-  }
-  return VGX_OK;
+    return VGX_OK;
+  });
 }

@@ -330,7 +330,7 @@ static int launch_fold(vgx_ctx* c, int vps, unsigned n_keys, const ProjSrc* d_sr
     case 16: PROJ_FOLD(16, true, 256)
     case 32: PROJ_FOLD(128, false, 256)
 #undef PROJ_FOLD
-    default: VGX_FAIL(c, VGX_ERR_INVALID, "vgx_project_map: unsupported voxels_per_side");
+    default: VGX_FAIL(c, VGX_ERR_INVALID, "unsupported voxels_per_side");
   }
   VGX_CUDA(c, cudaGetLastError());
   return VGX_OK;
@@ -354,8 +354,8 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
   }
   const size_t per_block = transform ? 9 : 8;   // candidate pairs per input block
   if (n_in > (size_t)INT32_MAX / per_block)
-    VGX_FAIL(c, VGX_ERR_CAPACITY, transform ? "vgx_submap_transform: more than 2^31 / 9 input blocks"
-                                            : "vgx_project_map: more than 2^28 input blocks");
+    VGX_FAIL(c, VGX_ERR_CAPACITY, transform ? "more than 2^31 / 9 input blocks"
+                                            : "more than 2^28 input blocks");
   const size_t P = per_block * n_in;
   cudaStream_t st = c->stream;
   unsigned n_keys = 0, n_out = 0;
@@ -375,12 +375,11 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
   ProjSrc* d_src;
   int* d_ctl;
   char* d_sort_tmp;
-  int rc = vgx_carve(c, c->d_work, vgx_part(keys_a, P + 1), vgx_part(keys_b, P + 1), vgx_part(ranks_a, P + 1),
-                     vgx_part(ranks_b, P + 1), vgx_part(pair_head, P + 1), vgx_part(key_head, P + 1),
-                     vgx_part(pair_pos, P + 1), vgx_part(key_pos, P + 1), vgx_part(useg, P + 1),
-                     vgx_part(scan_tmp, vgx_scan_tmp_count(P + 1)), vgx_part(d_src, (size_t)ns), vgx_part(d_ctl, 1),
-                     vgx_part(d_sort_tmp, sort_tmp));
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(vgx_carve(c, c->d_work, vgx_part(keys_a, P + 1), vgx_part(keys_b, P + 1), vgx_part(ranks_a, P + 1),
+                    vgx_part(ranks_b, P + 1), vgx_part(pair_head, P + 1), vgx_part(key_head, P + 1),
+                    vgx_part(pair_pos, P + 1), vgx_part(key_pos, P + 1), vgx_part(useg, P + 1),
+                    vgx_part(scan_tmp, vgx_scan_tmp_count(P + 1)), vgx_part(d_src, (size_t)ns), vgx_part(d_ctl, 1),
+                    vgx_part(d_sort_tmp, sort_tmp)));
   if (P > 0) {
     VGX_CUDA(c, cudaMemcpyAsync(d_src, h.data(), sizeof(ProjSrc) * (size_t)ns, cudaMemcpyHostToDevice, st));
     VGX_CUDA(c, cudaMemsetAsync(d_ctl, 0, sizeof(int), st));
@@ -404,11 +403,10 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
     VGX_CUDA(c, cudaGetLastError());
     {
       VgxLaunchScope scope(c, VGX_SLOT_PROJECT, 0);
-      rc = vgx_exclusive_scan_u32(c, pair_head, pair_pos, P, scan_tmp);
-      if (rc == VGX_OK) rc = vgx_exclusive_scan_u32(c, key_head, key_pos, P, scan_tmp);
       c->prof[VGX_SLOT_PROJECT].launches += 6;
+      VGX_TRY(vgx_exclusive_scan_u32(c, pair_head, pair_pos, P, scan_tmp));
+      VGX_TRY(vgx_exclusive_scan_u32(c, key_head, key_pos, P, scan_tmp));
     }
-    if (rc != VGX_OK) return rc;
     {
       VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
       project_scatter_kernel<<<gp, 256, 0, st>>>(keys_b, ranks_b, P, pair_head, key_head, pair_pos, key_pos, keys_a,
@@ -420,9 +418,9 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
     VGX_CUDA(c, cudaMemcpyAsync(&ctl[1], key_pos + P, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     VGX_CUDA(c, cudaStreamSynchronize(st));
     if (ctl[0] & 2)
-      VGX_FAIL(c, VGX_ERR_INVALID, "vgx_project_map: a projected block index lies outside the accepted range");
+      VGX_FAIL(c, VGX_ERR_INVALID, "a projected block index lies outside the accepted range");
     if (ctl[0] & 4)
-      VGX_FAIL(c, VGX_ERR_INVALID, "vgx_project_map: more than two candidate samples on an axis");
+      VGX_FAIL(c, VGX_ERR_INVALID, "more than two candidate samples on an axis");
     n_keys = (unsigned)ctl[1];
   }
   unsigned* keep = pair_head;
@@ -436,16 +434,14 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
     VGX_CUDA(c, cudaGetLastError());
     {
       VgxLaunchScope scope(c, VGX_SLOT_PROJECT, 0);
-      rc = vgx_exclusive_scan_u32(c, keep, slot, n_keys, scan_tmp);
       c->prof[VGX_SLOT_PROJECT].launches += 3;
+      VGX_TRY(vgx_exclusive_scan_u32(c, keep, slot, n_keys, scan_tmp));
     }
-    if (rc != VGX_OK) return rc;
     VGX_CUDA(c, cudaMemcpyAsync(&n_out, slot + n_keys, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
     VGX_CUDA(c, cudaStreamSynchronize(st));
   }
   VgxSubmap* s = nullptr;
-  rc = vgx_submap_alloc(c, out_id, g0.voxel_size, g0.vps, (int)n_out, true, &s);
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(vgx_submap_alloc(c, out_id, g0.voxel_size, g0.vps, (int)n_out, true, &s));
   s->n_blocks = (int)n_out;
   s->finished = true;
   if (n_out > 0 && transform) {
@@ -458,70 +454,67 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
   } else if (n_out > 0) {
     bool coloured = false;
     for (const VgxSubmap* in : subs) coloured = coloured || in->d_rgba.get();
-    if (coloured && (rc = vgx_submap_ensure_colour(c, s)) != VGX_OK) return rc;
+    if (coloured) VGX_TRY(vgx_submap_ensure_colour(c, s));
     {
       VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
-      rc = launch_fold(c, g0.vps, n_keys, d_src, keys_a, ranks_a, useg, slot, s);
+      VGX_TRY(launch_fold(c, g0.vps, n_keys, d_src, keys_a, ranks_a, useg, slot, s));
     }
-    if (rc != VGX_OK) return rc;
   }
-  rc = vgx_submap_upload_finish(c, s, "vgx_project_map");
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(vgx_submap_upload_finish(c, s));
   *n_out_blocks = (int)n_out;
   return VGX_OK;
 }
 
 extern "C" int vgx_project_map(vgx_ctx* c, int n, const uint32_t* ids, const float* T_M_S, uint32_t out_id,
                                int* n_blocks) {
-  if (!c) return VGX_ERR_INVALID;
-  if (n_blocks) *n_blocks = 0;
-  if (n < 1 || !ids || !T_M_S) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_project_map: invalid argument");
-  std::vector<std::pair<uint32_t, int>> order;   // (id, row of ids / T_M_S)
-  for (int k = 0; k < n; ++k) {
-    if (ids[k] == out_id) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_project_map: out_id is one of the inputs");
-    order.emplace_back(ids[k], k);
-  }
-  std::sort(order.begin(), order.end());
-  for (int k = 1; k < n; ++k)
-    if (order[k].first == order[k - 1].first)
-      VGX_FAIL(c, VGX_ERR_INVALID, "vgx_project_map: repeated submap " + std::to_string(order[k].first));
-  std::vector<VgxSubmap*> subs((size_t)n);
-  std::vector<const float*> poses((size_t)n);
-  for (int r = 0; r < n; ++r) {
-    subs[r] = c->find(order[r].first);
-    if (!subs[r]) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_project_map: unknown submap " + std::to_string(order[r].first));
-    poses[r] = T_M_S + 7 * (size_t)order[r].second;
-  }
-  if (c->find(out_id)) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_project_map: out_id already exists");
-  for (int r = 1; r < n; ++r)
-    if (subs[r]->voxel_size != subs[0]->voxel_size || subs[r]->vps != subs[0]->vps)
-      VGX_FAIL(c, VGX_ERR_INVALID, "vgx_project_map: the submaps differ in voxel size or voxels_per_side");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // n_blocks of an active submap is final after its integration
-  int nb = 0;
-  const int rc = project(c, subs, poses, out_id, &nb);
-  if (rc != VGX_OK) {
-    vgx_submap_drop(c, out_id);   // a failure after the allocation leaves a half-built submap
-    return rc;
-  }
-  if (n_blocks) *n_blocks = nb;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (n_blocks) *n_blocks = 0;
+    if (n < 1 || !ids || !T_M_S) VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
+    std::vector<std::pair<uint32_t, int>> order;   // (id, row of ids / T_M_S)
+    for (int k = 0; k < n; ++k) {
+      if (ids[k] == out_id) VGX_FAIL(c, VGX_ERR_INVALID, "out_id is one of the inputs");
+      order.emplace_back(ids[k], k);
+    }
+    std::sort(order.begin(), order.end());
+    for (int k = 1; k < n; ++k)
+      if (order[k].first == order[k - 1].first)
+        VGX_FAIL(c, VGX_ERR_INVALID, "repeated submap " + std::to_string(order[k].first));
+    std::vector<VgxSubmap*> subs((size_t)n);
+    std::vector<const float*> poses((size_t)n);
+    for (int r = 0; r < n; ++r) {
+      VGX_TRY(vgx_submap_get(c, order[r].first, &subs[r]));
+      poses[r] = T_M_S + 7 * (size_t)order[r].second;
+    }
+    if (c->submaps.count(out_id)) VGX_FAIL(c, VGX_ERR_INVALID, "out_id already exists");
+    for (int r = 1; r < n; ++r)
+      if (subs[r]->voxel_size != subs[0]->voxel_size || subs[r]->vps != subs[0]->vps)
+        VGX_FAIL(c, VGX_ERR_INVALID, "the submaps differ in voxel size or voxels_per_side");
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // n_blocks of an active submap is final after its integration
+    int nb = 0;
+    const int rc = project(c, subs, poses, out_id, &nb);
+    if (rc != VGX_OK) {
+      vgx_submap_drop(c, out_id);   // a failure after the allocation leaves a half-built submap
+      return rc;
+    }
+    if (n_blocks) *n_blocks = nb;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_transform(vgx_ctx* c, uint32_t id, const float* T_new_old) {
-  if (!c) return VGX_ERR_INVALID;
-  if (!T_new_old) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_transform: invalid argument");
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_transform: unknown submap " + std::to_string(id));
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // n_blocks of an active submap is final after its integration
-  // the result is built in a scratch submap next to the old copy, then takes the submap's id
-  const uint32_t tmp = vgx_scratch_id(c);
-  int nb = 0;
-  const int rc = project(c, {s}, {T_new_old}, tmp, &nb, true);
-  if (rc != VGX_OK) {
-    vgx_submap_drop(c, tmp);
-    return rc;
-  }
-  return vgx_submap_move(c, tmp, id);
+  return vgx_entry(c, __func__, [&] {
+    if (!T_new_old) VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // n_blocks of an active submap is final after its integration
+    // the result is built in a scratch submap next to the old copy, then takes the submap's id
+    const uint32_t tmp = vgx_scratch_id(c);
+    int nb = 0;
+    const int rc = project(c, {s}, {T_new_old}, tmp, &nb, true);
+    if (rc != VGX_OK) {
+      vgx_submap_drop(c, tmp);
+      return rc;
+    }
+    return vgx_submap_move(c, tmp, id);
+  });
 }

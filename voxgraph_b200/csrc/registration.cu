@@ -555,9 +555,9 @@ int vgx_fill_constraint(vgx_ctx* c, uint32_t ref_id, uint32_t read_id, const vgx
   if (cfg->sampling_ratio != -1.0f && !(cfg->sampling_ratio >= 0.0f))
     VGX_FAIL(c, VGX_ERR_INVALID, "sampling_ratio must be -1 (all points) or >= 0");
   if (ref_id == read_id) VGX_FAIL(c, VGX_ERR_INVALID, "cannot constrain a submap to itself");
-  VgxSubmap* ref = c->find(ref_id);
-  VgxSubmap* rd = c->find(read_id);
-  if (!ref || !rd) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "registration constraint: unknown submap");
+  VgxSubmap *ref, *rd;
+  VGX_TRY(vgx_submap_get(c, ref_id, &ref));
+  VGX_TRY(vgx_submap_get(c, read_id, &rd));
   if (!rd->finished || !rd->d_view.get())
     VGX_FAIL(c, VGX_ERR_INVALID, "registration constraint: reading submap is not finished");
   if (cfg->use_esdf_distance && !rd->d_view_esdf.get())
@@ -598,64 +598,64 @@ extern "C" void vgx_reg_config_default(vgx_reg_config* cfg) {
 }
 
 extern "C" int vgx_reg_num_residuals(vgx_ctx* c, uint32_t ref_id, const vgx_reg_config* cfg, int* n) {
-  if (!c || !cfg || !n) return VGX_ERR_INVALID;
-  VgxSubmap* ref = c->find(ref_id);
-  if (!ref) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_reg_num_residuals: unknown submap");
-  if (cfg->registration_point_type < 0 || cfg->registration_point_type > 1) return VGX_ERR_INVALID;
-  if (cfg->sampling_ratio != -1.0f && !(cfg->sampling_ratio >= 0.0f)) return VGX_ERR_INVALID;
-  *n = reg_num_residuals(ref->points[cfg->registration_point_type], cfg);
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!cfg || !n) return VGX_ERR_INVALID;
+    VgxSubmap* ref;
+    VGX_TRY(vgx_submap_get(c, ref_id, &ref));
+    if (cfg->registration_point_type < 0 || cfg->registration_point_type > 1) return VGX_ERR_INVALID;
+    if (cfg->sampling_ratio != -1.0f && !(cfg->sampling_ratio >= 0.0f)) return VGX_ERR_INVALID;
+    *n = reg_num_residuals(ref->points[cfg->registration_point_type], cfg);
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_reg_eval_emit(vgx_ctx* c, uint32_t ref_id, uint32_t read_id,
                                  const vgx_reg_config* cfg, const double ref_pose[4],
                                  const double read_pose[4], double* residuals, double* jac_ref,
                                  double* jac_read) {
-  if (!c || !ref_pose || !read_pose || !residuals) return VGX_ERR_INVALID;
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  RegConstraintDev C;
-  bool sampled = false;
-  int rc = vgx_fill_constraint(c, ref_id, read_id, cfg, &C, &sampled);
-  if (rc != VGX_OK) return rc;
-  if (C.n == 0) return VGX_ZERO_WEIGHT;  // summed weight 0 -> Evaluate returns false
-  if (C.factor == 0.0) return VGX_ZERO_WEIGHT;
-  const size_t K = (size_t)C.n;
-  const size_t Kp = (K + 3) & ~(size_t)3;  // keep the Jacobian blocks 32-byte aligned
-  const size_t units = (K + 31) / 32;
-  // scratch: residuals and both Jacobians (9 x Kp) | (sampling mode) the drawn points and their indices
-  double* d_r;
-  float* d_pts;
-  int32_t* d_idx;
-  rc = vgx_carve(c, c->d_scratch, vgx_part(d_r, 9 * Kp), vgx_part(d_pts, sampled ? units * VGX_PT_UNIT_FLOATS : 0),
-                 vgx_part(d_idx, sampled ? Kp : 0));
-  if (rc != VGX_OK) return rc;
-  if (sampled) {
-    // cpp:118-122: every Evaluate draws its points anew from the reference submap's sampler
-    VgxPoints& p = c->find(ref_id)->points[cfg->registration_point_type];
-    int32_t* h_idx;
-    rc = vgx_carve(c, c->h_pinned, vgx_part(h_idx, Kp));
-    if (rc != VGX_OK) return rc;
+  return vgx_entry(c, __func__, [&] {
+    if (!ref_pose || !read_pose || !residuals) return VGX_ERR_INVALID;
+    RegConstraintDev C;
+    bool sampled = false;
+    VGX_TRY(vgx_fill_constraint(c, ref_id, read_id, cfg, &C, &sampled));
+    if (C.n == 0) return VGX_ZERO_WEIGHT;  // summed weight 0 -> Evaluate returns false
+    if (C.factor == 0.0) return VGX_ZERO_WEIGHT;
+    const size_t K = (size_t)C.n;
+    const size_t Kp = (K + 3) & ~(size_t)3;  // keep the Jacobian blocks 32-byte aligned
+    const size_t units = (K + 31) / 32;
+    // scratch: residuals and both Jacobians (9 x Kp) | (sampling mode) the drawn points and their indices
+    double* d_r;
+    float* d_pts;
+    int32_t* d_idx;
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_r, 9 * Kp), vgx_part(d_pts, sampled ? units * VGX_PT_UNIT_FLOATS : 0),
+                      vgx_part(d_idx, sampled ? Kp : 0)));
+    if (sampled) {
+      // cpp:118-122: every Evaluate draws its points anew from the reference submap's sampler
+      VgxPoints& p = c->submaps.at(ref_id)->points[cfg->registration_point_type];
+      int32_t* h_idx;
+      VGX_TRY(vgx_carve(c, c->h_pinned, vgx_part(h_idx, Kp)));
+      VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+      vgx_points_draw(p, (int)K, h_idx);
+      VGX_CUDA(c, cudaMemcpyAsync(d_idx, h_idx, K * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+      vgx_launch_reg_gather_samples(c->stream, p.data.get(), d_idx, (int)K, d_pts);
+      c->launches++;
+      C.pts = d_pts;
+    }
+    RegPoseConst P;
+    vgx_reg_pose_setup<TrigHostLibm>(ref_pose, read_pose, P);
+    double* d_jr = jac_ref ? d_r + Kp : nullptr;
+    double* d_je = jac_read ? d_r + 5 * Kp : nullptr;
+    {
+      VgxLaunchScope scope(c, VGX_SLOT_REG_EMIT);
+      reg_emit_kernel<<<(unsigned)((K + 255) / 256), 256, 0, c->stream>>>(C, P, d_r, d_jr, d_je);
+    }
+    VGX_CUDA(c, cudaGetLastError());
+    VGX_CUDA(c, cudaMemcpyAsync(residuals, d_r, K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    if (jac_ref)
+      VGX_CUDA(c, cudaMemcpyAsync(jac_ref, d_jr, 4 * K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    if (jac_read)
+      VGX_CUDA(c, cudaMemcpyAsync(jac_read, d_je, 4 * K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
     VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    vgx_points_draw(p, (int)K, h_idx);
-    VGX_CUDA(c, cudaMemcpyAsync(d_idx, h_idx, K * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-    vgx_launch_reg_gather_samples(c->stream, p.data.get(), d_idx, (int)K, d_pts);
-    c->launches++;
-    C.pts = d_pts;
-  }
-  RegPoseConst P;
-  vgx_reg_pose_setup<TrigHostLibm>(ref_pose, read_pose, P);
-  double* d_jr = jac_ref ? d_r + Kp : nullptr;
-  double* d_je = jac_read ? d_r + 5 * Kp : nullptr;
-  {
-    VgxLaunchScope scope(c, VGX_SLOT_REG_EMIT);
-    reg_emit_kernel<<<(unsigned)((K + 255) / 256), 256, 0, c->stream>>>(C, P, d_r, d_jr, d_je);
-  }
-  VGX_CUDA(c, cudaGetLastError());
-  VGX_CUDA(c, cudaMemcpyAsync(residuals, d_r, K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  if (jac_ref)
-    VGX_CUDA(c, cudaMemcpyAsync(jac_ref, d_jr, 4 * K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  if (jac_read)
-    VGX_CUDA(c, cudaMemcpyAsync(jac_read, d_je, 4 * K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  return VGX_OK;
+    return VGX_OK;
+  });
 }

@@ -738,91 +738,89 @@ cov_column_kernel(const double* __restrict__ A, int n, const int* __restrict__ c
 
 extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids_a, const uint32_t* ids_b,
                                           double* cov) {
-  VgxGraph* g = nullptr;
-  int rc = prepare(c, &g);
-  if (rc != VGX_OK) return rc;
-  if (m < 0 || (m > 0 && (!ids_a || !ids_b || !cov))) return VGX_ERR_INVALID;
-  if (m == 0) return VGX_OK;
-  if (g->zero_weight) VGX_FAIL(c, VGX_ZERO_WEIGHT, "a registration constraint has zero summed weight (Evaluate == false)");
-  const int N = g->N, n = g->n_free;
-  const std::vector<int>& red = g->red;
-  // distinct columns: the 4 parameters of every second node that is free
-  std::vector<int> col_of(N, -1), cols;
-  std::vector<std::pair<int, int>> pr(m);
-  for (int k = 0; k < m; ++k) {
-    auto ia = g->index.find(ids_a[k]);
-    auto ib = g->index.find(ids_b[k]);
-    if (ia == g->index.end() || ib == g->index.end())
-      VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_graph_edge_covariances: graph contains no node for a requested submap");
-    pr[k] = {ia->second, ib->second};
-    const int b = ib->second;
-    if (red[b] >= 0 && col_of[b] < 0) {
-      col_of[b] = (int)cols.size();
-      for (int q = 0; q < 4; ++q) cols.push_back(red[b] + q);
+  return vgx_entry(c, __func__, [&] {
+    VgxGraph* g = nullptr;
+    VGX_TRY(prepare(c, &g));
+    if (m < 0 || (m > 0 && (!ids_a || !ids_b || !cov))) return VGX_ERR_INVALID;
+    if (m == 0) return VGX_OK;
+    if (g->zero_weight) VGX_FAIL(c, VGX_ZERO_WEIGHT, "a registration constraint has zero summed weight (Evaluate == false)");
+    const int N = g->N, n = g->n_free;
+    const std::vector<int>& red = g->red;
+    // distinct columns: the 4 parameters of every second node that is free
+    std::vector<int> col_of(N, -1), cols;
+    std::vector<std::pair<int, int>> pr(m);
+    for (int k = 0; k < m; ++k) {
+      auto ia = g->index.find(ids_a[k]);
+      auto ib = g->index.find(ids_b[k]);
+      if (ia == g->index.end() || ib == g->index.end())
+        VGX_FAIL(c, VGX_ERR_NOT_FOUND, "graph contains no node for a requested submap");
+      pr[k] = {ia->second, ib->second};
+      const int b = ib->second;
+      if (red[b] >= 0 && col_of[b] < 0) {
+        col_of[b] = (int)cols.size();
+        for (int q = 0; q < 4; ++q) cols.push_back(red[b] + q);
+      }
     }
-  }
-  for (int k = 0; k < 16 * m; ++k) cov[k] = 0.0;   // constant blocks: zero covariance
-  if (n == 0 || cols.empty()) return VGX_OK;
-  cudaStream_t st = c->stream;
-  rc = eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, false);
-  if (rc != VGX_OK) return rc;
-  const size_t M = (size_t)n + 1;
-  // scratch: requested column indices | X (ncols x n)
-  const size_t ncols = cols.size();
-  int* d_cols;
-  double* d_X;
-  rc = vgx_carve(c, c->d_scratch, vgx_part(d_cols, ncols), vgx_part(d_X, ncols * (size_t)n));
-  if (rc != VGX_OK) return rc;
-  size_t no_smem = 0;
-  int coop_grid = 0;
-  rc = chol_dispatch(c, n, false, &no_smem, &coop_grid);
-  if (rc != VGX_OK) return rc;
-  // J^T J is the LM system without Jacobi scaling or damping: with scaling off, a [0, inf] diagonal
-  // clamp and an infinite radius lm_build_kernel writes exactly H_ff (and the gradient as row n, which
-  // no column of L depends on), and lm_persist_kernel stores the unfactored diagonal H_kk in d_diag.
-  LmOpts lo;
-  memset(&lo, 0, sizeof(lo));
-  lo.min_lm_diagonal = 0.0;
-  lo.max_lm_diagonal = INFINITY;
-  lo.jacobi_scaling = 0;
-  LmState* init = g->h_state.get();   // pinned: the copy stays asynchronous (the stream is synchronised below)
-  memset(init, 0, sizeof(*init));
-  init->radius = INFINITY;
-  init->step_valid = 1;
-  VGX_CUDA(c, cudaMemsetAsync(g->dev.d_A.get(), 0, sizeof(double) * M * M, st));
-  VGX_CUDA(c, cudaMemcpyAsync(g->dev.d_state.get(), init, sizeof(*init), cudaMemcpyHostToDevice, st));
-  {
-    VgxLaunchScope s(c, VGX_SLOT_SOLVE, 3);
-    enqueue_lm_build(st, g, n, lo);
-    VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->dev.d_A.get(), n, g->dev.d_state.get(), g->dev.d_diag.get(),
-                                 VGX_COV_RANK_TOL));
-  }
-  VGX_CUDA(c, cudaGetLastError());
-  // inverse columns
-  VGX_CUDA(c, cudaMemcpyAsync(d_cols, cols.data(), sizeof(int) * ncols, cudaMemcpyHostToDevice, st));
-  if (sizeof(double) * (size_t)n > 48 * 1024)
-    VGX_CUDA(c, cudaFuncSetAttribute(cov_column_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)(sizeof(double) * (size_t)n)));
-  {
-    VgxLaunchScope s(c, VGX_SLOT_SOLVE);
-    cov_column_kernel<<<(unsigned)ncols, 256, sizeof(double) * (size_t)n, st>>>(g->dev.d_A.get(), n, d_cols, d_X);
-  }
-  VGX_CUDA(c, cudaGetLastError());
-  std::vector<double> X(ncols * (size_t)n);
-  LmState hs;
-  VGX_CUDA(c, cudaMemcpyAsync(X.data(), d_X, sizeof(double) * X.size(), cudaMemcpyDeviceToHost, st));
-  VGX_CUDA(c, cudaMemcpyAsync(&hs, g->dev.d_state.get(), sizeof(hs), cudaMemcpyDeviceToHost, st));
-  VGX_CUDA(c, cudaStreamSynchronize(st));
-  if (!hs.step_valid)   // a pivot failed the rank rule above (ceres::Covariance::Compute returns false)
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_graph_edge_covariances: J^T J is not positive definite (rank deficient)");
-  for (int k = 0; k < m; ++k) {
-    const int a = pr[k].first, b = pr[k].second;
-    if (red[a] < 0 || red[b] < 0) continue;
-    for (int r = 0; r < 4; ++r)
-      for (int q = 0; q < 4; ++q)
-        cov[16 * (size_t)k + 4 * r + q] = X[(size_t)(col_of[b] + q) * n + red[a] + r];
-  }
-  return VGX_OK;
+    for (int k = 0; k < 16 * m; ++k) cov[k] = 0.0;   // constant blocks: zero covariance
+    if (n == 0 || cols.empty()) return VGX_OK;
+    cudaStream_t st = c->stream;
+    VGX_TRY(eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, false));
+    const size_t M = (size_t)n + 1;
+    // scratch: requested column indices | X (ncols x n)
+    const size_t ncols = cols.size();
+    int* d_cols;
+    double* d_X;
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_cols, ncols), vgx_part(d_X, ncols * (size_t)n)));
+    size_t no_smem = 0;
+    int coop_grid = 0;
+    VGX_TRY(chol_dispatch(c, n, false, &no_smem, &coop_grid));
+    // J^T J is the LM system without Jacobi scaling or damping: with scaling off, a [0, inf] diagonal
+    // clamp and an infinite radius lm_build_kernel writes exactly H_ff (and the gradient as row n, which
+    // no column of L depends on), and lm_persist_kernel stores the unfactored diagonal H_kk in d_diag.
+    LmOpts lo;
+    memset(&lo, 0, sizeof(lo));
+    lo.min_lm_diagonal = 0.0;
+    lo.max_lm_diagonal = INFINITY;
+    lo.jacobi_scaling = 0;
+    LmState* init = g->h_state.get();   // pinned: the copy stays asynchronous (the stream is synchronised below)
+    memset(init, 0, sizeof(*init));
+    init->radius = INFINITY;
+    init->step_valid = 1;
+    VGX_CUDA(c, cudaMemsetAsync(g->dev.d_A.get(), 0, sizeof(double) * M * M, st));
+    VGX_CUDA(c, cudaMemcpyAsync(g->dev.d_state.get(), init, sizeof(*init), cudaMemcpyHostToDevice, st));
+    {
+      VgxLaunchScope s(c, VGX_SLOT_SOLVE, 3);
+      enqueue_lm_build(st, g, n, lo);
+      VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->dev.d_A.get(), n, g->dev.d_state.get(), g->dev.d_diag.get(),
+                                   VGX_COV_RANK_TOL));
+    }
+    VGX_CUDA(c, cudaGetLastError());
+    // inverse columns
+    VGX_CUDA(c, cudaMemcpyAsync(d_cols, cols.data(), sizeof(int) * ncols, cudaMemcpyHostToDevice, st));
+    if (sizeof(double) * (size_t)n > 48 * 1024)
+      VGX_CUDA(c, cudaFuncSetAttribute(cov_column_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)(sizeof(double) * (size_t)n)));
+    {
+      VgxLaunchScope s(c, VGX_SLOT_SOLVE);
+      cov_column_kernel<<<(unsigned)ncols, 256, sizeof(double) * (size_t)n, st>>>(g->dev.d_A.get(), n, d_cols, d_X);
+    }
+    VGX_CUDA(c, cudaGetLastError());
+    std::vector<double> X(ncols * (size_t)n);
+    LmState hs;
+    VGX_CUDA(c, cudaMemcpyAsync(X.data(), d_X, sizeof(double) * X.size(), cudaMemcpyDeviceToHost, st));
+    VGX_CUDA(c, cudaMemcpyAsync(&hs, g->dev.d_state.get(), sizeof(hs), cudaMemcpyDeviceToHost, st));
+    VGX_CUDA(c, cudaStreamSynchronize(st));
+    if (!hs.step_valid)   // a pivot failed the rank rule above (ceres::Covariance::Compute returns false)
+      VGX_FAIL(c, VGX_ERR_INVALID, "J^T J is not positive definite (rank deficient)");
+    for (int k = 0; k < m; ++k) {
+      const int a = pr[k].first, b = pr[k].second;
+      if (red[a] < 0 || red[b] < 0) continue;
+      for (int r = 0; r < 4; ++r)
+        for (int q = 0; q < 4; ++q)
+          cov[16 * (size_t)k + 4 * r + q] = X[(size_t)(col_of[b] + q) * n + red[a] + r];
+    }
+    return VGX_OK;
+  });
 }
 
 extern "C" void vgx_solver_options_default(vgx_solver_options* o) {
@@ -850,167 +848,164 @@ static double wall_s() {
 
 extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, double* xyzyaw_out,
                                vgx_solver_summary* summary) {
-  const double t0 = wall_s();
-  VgxGraph* g = nullptr;
-  int rc = prepare(c, &g);
-  if (rc != VGX_OK) return rc;
-  vgx_solver_options od;
-  vgx_solver_options_default(&od);
-  const vgx_solver_options* o = opts ? opts : &od;
-  const bool excl = o->exclude_registration != 0;
-  vgx_solver_summary S;
-  memset(&S, 0, sizeof(S));
-  const int N = g->N, n = g->n_free;
-  cudaStream_t st = c->stream;
-  if (!excl && g->zero_weight) {
-    S.termination = 6;
-    if (summary) *summary = S;
-    VGX_FAIL(c, VGX_ZERO_WEIGHT, "a registration constraint has zero summed weight (Evaluate == false)");
-  }
-  // dense Cholesky: whole system in shared memory when it fits (configs[0..1]), else the
-  // cooperative multi-CTA kernel
-  size_t smem_chol_bytes = 0;
-  int coop_grid = 0;
-  if (n > 0) {
-    rc = chol_dispatch(c, n, true, &smem_chol_bytes, &coop_grid);
-    if (rc != VGX_OK) return rc;
-  }
-  const bool use_smem_chol = smem_chol_bytes > 0;
+  return vgx_entry(c, __func__, [&] {
+    const double t0 = wall_s();
+    VgxGraph* g = nullptr;
+    VGX_TRY(prepare(c, &g));
+    vgx_solver_options od;
+    vgx_solver_options_default(&od);
+    const vgx_solver_options* o = opts ? opts : &od;
+    const bool excl = o->exclude_registration != 0;
+    vgx_solver_summary S;
+    memset(&S, 0, sizeof(S));
+    const int N = g->N, n = g->n_free;
+    cudaStream_t st = c->stream;
+    if (!excl && g->zero_weight) {
+      S.termination = 6;
+      if (summary) *summary = S;
+      VGX_FAIL(c, VGX_ZERO_WEIGHT, "a registration constraint has zero summed weight (Evaluate == false)");
+    }
+    // dense Cholesky: whole system in shared memory when it fits (configs[0..1]), else the
+    // cooperative multi-CTA kernel
+    size_t smem_chol_bytes = 0;
+    int coop_grid = 0;
+    if (n > 0) {
+      VGX_TRY(chol_dispatch(c, n, true, &smem_chol_bytes, &coop_grid));
+    }
+    const bool use_smem_chol = smem_chol_bytes > 0;
 
-  LmOpts lo;
-  lo.max_num_iterations = o->max_num_iterations;
-  lo.parameter_tolerance = o->parameter_tolerance;
-  lo.function_tolerance = o->function_tolerance;
-  lo.gradient_tolerance = o->gradient_tolerance;
-  lo.max_radius = o->max_trust_region_radius;
-  lo.min_radius = o->min_trust_region_radius;
-  lo.min_relative_decrease = o->min_relative_decrease;
-  lo.min_lm_diagonal = o->min_lm_diagonal;
-  lo.max_lm_diagonal = o->max_lm_diagonal;
-  lo.jacobi_scaling = o->jacobi_scaling;
+    LmOpts lo;
+    lo.max_num_iterations = o->max_num_iterations;
+    lo.parameter_tolerance = o->parameter_tolerance;
+    lo.function_tolerance = o->function_tolerance;
+    lo.gradient_tolerance = o->gradient_tolerance;
+    lo.max_radius = o->max_trust_region_radius;
+    lo.min_radius = o->min_trust_region_radius;
+    lo.min_relative_decrease = o->min_relative_decrease;
+    lo.min_lm_diagonal = o->min_lm_diagonal;
+    lo.max_lm_diagonal = o->max_lm_diagonal;
+    lo.jacobi_scaling = o->jacobi_scaling;
 
-  // Slot 0 of d_packed always holds the normal equations at the current poses, slot 1 the candidate's;
-  // an accepted step copies 1 -> 0 on the device, so an iteration is a fixed sequence of launches
-  // that needs nothing from the host.  The host therefore runs ONE ITERATION AHEAD: iteration k + 1
-  // is enqueued before the 144-byte outcome of iteration k has been read (on a second stream, from
-  // a snapshot the decide kernel writes); every kernel of an iteration returns at once when the
-  // solve has ended, so the speculative iteration after the last one is a row of empty launches
-  // that drain while the host already returns.  Multi-rank: no run-ahead (the ranks stay in step).
-  rc = eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, excl);
-  if (rc != VGX_OK) return rc;
-  {
-    VgxLaunchScope s(c, VGX_SLOT_SOLVE);
-    lm_init_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), N, g->dev.d_state.get(),
-                                      o->initial_trust_region_radius, lo);
-  }
-  VGX_CUDA(c, cudaMemcpyAsync(g->h_state.get(), g->dev.d_state.get(), sizeof(LmState), cudaMemcpyDeviceToHost, st));
-  VGX_CUDA(c, cudaStreamSynchronize(st));
-  S.initial_cost = g->h_state.get()->cost;
-  // Ceres checks the time budget before every iteration, the first included, and before the other
-  // tests (iterations, gradient, radius): a budget spent by now ends the solve with x untouched.
-  bool timed_out = c->nranks == 1 && wall_s() - t0 >= o->max_solver_time_s;
-  static const char* no_spec = getenv("VGX_LM_NO_RUNAHEAD");
-  const int ahead = (c->nranks == 1 && !(no_spec && no_spec[0] == '1')) ? 1 : 0;
-  // VGX_CHOL_DEBUG=1: phase cycle counts of the last shared-memory Cholesky, printed after the solve
-  static const char* chol_dbg_env = getenv("VGX_CHOL_DEBUG");
-  VgxBuffer<long long> chol_dbg;
-  if (chol_dbg_env && chol_dbg_env[0] == '1' && use_smem_chol)
-    chol_dbg.alloc(c, 8 * sizeof(long long), "VGX_CHOL_DEBUG");
-  long long* d_chol_dbg = chol_dbg.get();
-  const int* skip = &g->dev.d_state.get()->done;
-  auto enqueue_iteration = [&](int k) -> int {
+    // Slot 0 of d_packed always holds the normal equations at the current poses, slot 1 the candidate's;
+    // an accepted step copies 1 -> 0 on the device, so an iteration is a fixed sequence of launches
+    // that needs nothing from the host.  The host therefore runs ONE ITERATION AHEAD: iteration k + 1
+    // is enqueued before the 144-byte outcome of iteration k has been read (on a second stream, from
+    // a snapshot the decide kernel writes); every kernel of an iteration returns at once when the
+    // solve has ended, so the speculative iteration after the last one is a row of empty launches
+    // that drain while the host already returns.  Multi-rank: no run-ahead (the ranks stay in step).
+    VGX_TRY(eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, excl));
     {
-      VgxLaunchScope s(c, VGX_SLOT_SOLVE, 4);
-      if (!use_smem_chol)   // the shared-memory solver reads the written blocks only
-        VGX_CUDA(c, cudaMemsetAsync(g->dev.d_A.get(), 0, sizeof(double) * (size_t)(n + 1) * (n + 1), st));
-      enqueue_lm_build(st, g, n, lo);
-      if (use_smem_chol) {
-        chol_solve_smem_kernel<<<1, 512, smem_chol_bytes, st>>>(g->dev.d_A.get(), n, g->dev.d_step.get(),
-                                                                g->dev.d_state.get(), g->dev.d_red_offset.get(),
-                                                                g->dev.d_block_nodes.get(), N, g->E, d_chol_dbg);
-      } else {
-        // LM: sign test only (as Eigen's LLT in the reference)
-        VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->dev.d_A.get(), n, g->dev.d_state.get(), nullptr, 0.0));
+      VgxLaunchScope s(c, VGX_SLOT_SOLVE);
+      lm_init_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), N, g->dev.d_state.get(),
+                                        o->initial_trust_region_radius, lo);
+    }
+    VGX_CUDA(c, cudaMemcpyAsync(g->h_state.get(), g->dev.d_state.get(), sizeof(LmState), cudaMemcpyDeviceToHost, st));
+    VGX_CUDA(c, cudaStreamSynchronize(st));
+    S.initial_cost = g->h_state.get()->cost;
+    // Ceres checks the time budget before every iteration, the first included, and before the other
+    // tests (iterations, gradient, radius): a budget spent by now ends the solve with x untouched.
+    bool timed_out = c->nranks == 1 && wall_s() - t0 >= o->max_solver_time_s;
+    static const char* no_spec = getenv("VGX_LM_NO_RUNAHEAD");
+    const int ahead = (c->nranks == 1 && !(no_spec && no_spec[0] == '1')) ? 1 : 0;
+    // VGX_CHOL_DEBUG=1: phase cycle counts of the last shared-memory Cholesky, printed after the solve
+    static const char* chol_dbg_env = getenv("VGX_CHOL_DEBUG");
+    VgxBuffer<long long> chol_dbg;
+    if (chol_dbg_env && chol_dbg_env[0] == '1' && use_smem_chol)
+      chol_dbg.alloc(c, 8 * sizeof(long long), "VGX_CHOL_DEBUG");
+    long long* d_chol_dbg = chol_dbg.get();
+    const int* skip = &g->dev.d_state.get()->done;
+    auto enqueue_iteration = [&](int k) -> int {
+      {
+        VgxLaunchScope s(c, VGX_SLOT_SOLVE, 4);
+        if (!use_smem_chol)   // the shared-memory solver reads the written blocks only
+          VGX_CUDA(c, cudaMemsetAsync(g->dev.d_A.get(), 0, sizeof(double) * (size_t)(n + 1) * (n + 1), st));
+        enqueue_lm_build(st, g, n, lo);
+        if (use_smem_chol) {
+          chol_solve_smem_kernel<<<1, 512, smem_chol_bytes, st>>>(g->dev.d_A.get(), n, g->dev.d_step.get(),
+                                                                  g->dev.d_state.get(), g->dev.d_red_offset.get(),
+                                                                  g->dev.d_block_nodes.get(), N, g->E, d_chol_dbg);
+        } else {
+          // LM: sign test only (as Eigen's LLT in the reference)
+          VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->dev.d_A.get(), n, g->dev.d_state.get(), nullptr, 0.0));
+        }
+        lm_step_kernel<<<1, 1024, sizeof(double) * n, st>>>(g->dev.d_A.get(), n, N, g->dev.d_red_offset.get(),
+                                                           g->dev.d_scale.get(), g->dev.d_diag.get(), g->dev.d_gs.get(),
+                                                           g->dev.d_x.get(), g->dev.d_xc.get(), g->dev.d_step.get(),
+                                                           g->dev.d_state.get(),
+                                                           use_smem_chol ? g->dev.d_step.get() : nullptr);
       }
-      lm_step_kernel<<<1, 1024, sizeof(double) * n, st>>>(g->dev.d_A.get(), n, N, g->dev.d_red_offset.get(),
-                                                         g->dev.d_scale.get(), g->dev.d_diag.get(), g->dev.d_gs.get(),
-                                                         g->dev.d_x.get(), g->dev.d_xc.get(), g->dev.d_step.get(),
-                                                         g->dev.d_state.get(),
-                                                         use_smem_chol ? g->dev.d_step.get() : nullptr);
-    }
-    VGX_CUDA(c, cudaGetLastError());
-    // candidate evaluated with Jacobians so an accepted step needs no second pass
-    int rc2 = eval_enqueue(c, g, g->dev.d_xc.get(), g->dev.d_packed[1].get(), true, excl, skip);
-    if (rc2 != VGX_OK) return rc2;
-    {
-      VgxLaunchScope s(c, VGX_SLOT_SOLVE, 2);
-      lm_decide_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_packed[1].get(), g->dev.d_red_offset.get(),
-                                          N, g->dev.d_x.get(), g->dev.d_xc.get(), g->dev.d_state.get(), lo, 1,
-                                          g->dev.d_snap.get() + (k & 1));
-      lm_accept_kernel<<<std::max(1, std::min(64, (int)(g->packed_len / 2048))), 256, 0, st>>>(
-          g->dev.d_packed[1].get(), g->dev.d_packed[0].get(), g->packed_len, g->dev.d_state.get());
-    }
-    VGX_CUDA(c, cudaGetLastError());
-    // outcome of iteration k -> host, on the copy stream (the main stream keeps running ahead)
-    VGX_CUDA(c, cudaEventRecord(g->ev_iter[k & 1], st));
-    VGX_CUDA(c, cudaStreamWaitEvent(g->copy_stream, g->ev_iter[k & 1], 0));
-    VGX_CUDA(c, cudaMemcpyAsync(g->h_snap.get() + (k & 1), g->dev.d_snap.get() + (k & 1), sizeof(LmState),
-                                cudaMemcpyDeviceToHost, g->copy_stream));
-    VGX_CUDA(c, cudaEventRecord(g->ev_copy[k & 1], g->copy_stream));
-    return VGX_OK;
-  };
-  bool run = !timed_out && !g->h_state.get()->done && n > 0;
-  if (run) {
-    int enq = 0, k = 0;   // iterations enqueued / the one whose outcome is awaited
-    for (;;) {
-      while (enq <= k + ahead) {
-        // (single-rank only: ranks must take identical decisions or the exchange would hang)
-        if (enq > k && c->nranks == 1 && wall_s() - t0 >= o->max_solver_time_s) break;
-        rc = enqueue_iteration(enq);
-        if (rc != VGX_OK) return rc;
-        ++enq;
+      VGX_CUDA(c, cudaGetLastError());
+      // candidate evaluated with Jacobians so an accepted step needs no second pass
+      int rc2 = eval_enqueue(c, g, g->dev.d_xc.get(), g->dev.d_packed[1].get(), true, excl, skip);
+      if (rc2 != VGX_OK) return rc2;
+      {
+        VgxLaunchScope s(c, VGX_SLOT_SOLVE, 2);
+        lm_decide_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_packed[1].get(), g->dev.d_red_offset.get(),
+                                            N, g->dev.d_x.get(), g->dev.d_xc.get(), g->dev.d_state.get(), lo, 1,
+                                            g->dev.d_snap.get() + (k & 1));
+        lm_accept_kernel<<<std::max(1, std::min(64, (int)(g->packed_len / 2048))), 256, 0, st>>>(
+            g->dev.d_packed[1].get(), g->dev.d_packed[0].get(), g->packed_len, g->dev.d_state.get());
       }
-      VGX_CUDA(c, cudaEventSynchronize(g->ev_copy[k & 1]));
-      *g->h_state.get() = g->h_snap.get()[k & 1];
-      if (g->h_state.get()->done) break;
-      if (c->nranks == 1 && wall_s() - t0 >= o->max_solver_time_s) { timed_out = true; break; }
-      ++k;
-    }
-    if (timed_out) VGX_CUDA(c, cudaStreamSynchronize(st));   // iterations in flight still move x
-    // final poses: the main stream may still be draining the empty launches of the speculative
-    // iteration; the copy stream is ordered after the deciding iteration only
-    VGX_CUDA(c, cudaMemcpyAsync(g->h_x.get(), g->dev.d_x.get(), sizeof(double) * 4 * N, cudaMemcpyDeviceToHost,
-                                timed_out ? st : g->copy_stream));
-    VGX_CUDA(c, cudaStreamSynchronize(timed_out ? st : g->copy_stream));
-    if (timed_out) {
-      VGX_CUDA(c, cudaMemcpyAsync(g->h_state.get(), g->dev.d_state.get(), sizeof(LmState), cudaMemcpyDeviceToHost, st));
+      VGX_CUDA(c, cudaGetLastError());
+      // outcome of iteration k -> host, on the copy stream (the main stream keeps running ahead)
+      VGX_CUDA(c, cudaEventRecord(g->ev_iter[k & 1], st));
+      VGX_CUDA(c, cudaStreamWaitEvent(g->copy_stream, g->ev_iter[k & 1], 0));
+      VGX_CUDA(c, cudaMemcpyAsync(g->h_snap.get() + (k & 1), g->dev.d_snap.get() + (k & 1), sizeof(LmState),
+                                  cudaMemcpyDeviceToHost, g->copy_stream));
+      VGX_CUDA(c, cudaEventRecord(g->ev_copy[k & 1], g->copy_stream));
+      return VGX_OK;
+    };
+    bool run = !timed_out && !g->h_state.get()->done && n > 0;
+    if (run) {
+      int enq = 0, k = 0;   // iterations enqueued / the one whose outcome is awaited
+      for (;;) {
+        while (enq <= k + ahead) {
+          // (single-rank only: ranks must take identical decisions or the exchange would hang)
+          if (enq > k && c->nranks == 1 && wall_s() - t0 >= o->max_solver_time_s) break;
+          VGX_TRY(enqueue_iteration(enq));
+          ++enq;
+        }
+        VGX_CUDA(c, cudaEventSynchronize(g->ev_copy[k & 1]));
+        *g->h_state.get() = g->h_snap.get()[k & 1];
+        if (g->h_state.get()->done) break;
+        if (c->nranks == 1 && wall_s() - t0 >= o->max_solver_time_s) { timed_out = true; break; }
+        ++k;
+      }
+      if (timed_out) VGX_CUDA(c, cudaStreamSynchronize(st));   // iterations in flight still move x
+      // final poses: the main stream may still be draining the empty launches of the speculative
+      // iteration; the copy stream is ordered after the deciding iteration only
+      VGX_CUDA(c, cudaMemcpyAsync(g->h_x.get(), g->dev.d_x.get(), sizeof(double) * 4 * N, cudaMemcpyDeviceToHost,
+                                  timed_out ? st : g->copy_stream));
+      VGX_CUDA(c, cudaStreamSynchronize(timed_out ? st : g->copy_stream));
+      if (timed_out) {
+        VGX_CUDA(c, cudaMemcpyAsync(g->h_state.get(), g->dev.d_state.get(), sizeof(LmState), cudaMemcpyDeviceToHost, st));
+        VGX_CUDA(c, cudaStreamSynchronize(st));
+      }
+      memcpy(g->x.data(), g->h_x.get(), sizeof(double) * 4 * N);
+    } else {
+      VGX_CUDA(c, cudaMemcpyAsync(g->x.data(), g->dev.d_x.get(), sizeof(double) * 4 * N, cudaMemcpyDeviceToHost, st));
       VGX_CUDA(c, cudaStreamSynchronize(st));
     }
-    memcpy(g->x.data(), g->h_x.get(), sizeof(double) * 4 * N);
-  } else {
-    VGX_CUDA(c, cudaMemcpyAsync(g->x.data(), g->dev.d_x.get(), sizeof(double) * 4 * N, cudaMemcpyDeviceToHost, st));
-    VGX_CUDA(c, cudaStreamSynchronize(st));
-  }
-  if (n == 0) { g->h_state.get()->termination = 2; }
-  if (d_chol_dbg) {
-    long long h[5] = {0, 0, 0, 0, 0};
-    cudaStreamSynchronize(st);
-    cudaMemcpy(h, d_chol_dbg, sizeof(h), cudaMemcpyDeviceToHost);
-    fprintf(stderr, "[vgx] chol n=%d cycles: load %lld update %lld factor+solve %lld back %lld total %lld\n", n, h[0],
-            h[1], h[2], h[3], h[4]);
-  }
-  S.iterations = g->h_state.get()->iterations;
-  S.num_successful_steps = g->h_state.get()->successful;
-  S.num_residual_evals = g->h_state.get()->evals;
-  S.termination = timed_out ? 4 : g->h_state.get()->termination;
-  S.final_cost = g->h_state.get()->cost;
-  S.total_time_s = wall_s() - t0;
-  if (xyzyaw_out) memcpy(xyzyaw_out, g->x.data(), sizeof(double) * 4 * N);
-  if (summary) *summary = S;
-  if (c->nranks > 1) {
-    rc = vgx_p2p_check(c);
-    if (rc != VGX_OK) return rc;
-  }
-  if (S.termination == 6) VGX_FAIL(c, VGX_ERR_INVALID, "solver failure: too many consecutive invalid steps");
-  return VGX_OK;
+    if (n == 0) { g->h_state.get()->termination = 2; }
+    if (d_chol_dbg) {
+      long long h[5] = {0, 0, 0, 0, 0};
+      cudaStreamSynchronize(st);
+      cudaMemcpy(h, d_chol_dbg, sizeof(h), cudaMemcpyDeviceToHost);
+      fprintf(stderr, "[vgx] chol n=%d cycles: load %lld update %lld factor+solve %lld back %lld total %lld\n", n, h[0],
+              h[1], h[2], h[3], h[4]);
+    }
+    S.iterations = g->h_state.get()->iterations;
+    S.num_successful_steps = g->h_state.get()->successful;
+    S.num_residual_evals = g->h_state.get()->evals;
+    S.termination = timed_out ? 4 : g->h_state.get()->termination;
+    S.final_cost = g->h_state.get()->cost;
+    S.total_time_s = wall_s() - t0;
+    if (xyzyaw_out) memcpy(xyzyaw_out, g->x.data(), sizeof(double) * 4 * N);
+    if (summary) *summary = S;
+    if (c->nranks > 1) {
+      VGX_TRY(vgx_p2p_check(c));
+    }
+    if (S.termination == 6) VGX_FAIL(c, VGX_ERR_INVALID, "solver failure: too many consecutive invalid steps");
+    return VGX_OK;
+  });
 }

@@ -8,6 +8,8 @@
 
 #include <algorithm>
 #include <new>
+#include <stdexcept>
+#include <string>
 #include <vector>
 
 #include "vgx_internal.h"
@@ -20,64 +22,108 @@ extern "C" int vgx_device_count(void) {
 }
 
 extern "C" int vgx_ctx_create(int device, vgx_ctx** out) {
-  if (!out) return VGX_ERR_INVALID;
-  *out = nullptr;
-  int n = 0;
-  if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0 || device < 0 || device >= n)
-    return VGX_ERR_CUDA;  // no CPU fallback: the product path needs a GPU
-  if (cudaSetDevice(device) != cudaSuccess) return VGX_ERR_CUDA;
-  vgx_ctx* c = new (std::nothrow) vgx_ctx();
-  if (!c) return VGX_ERR_NOMEM;
-  c->device = device;
-  if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
-      cudaEventCreate(&c->ev0) != cudaSuccess || cudaEventCreate(&c->ev1) != cudaSuccess) {
-    delete c;
-    return VGX_ERR_CUDA;
-  }
-  *out = c;
-  return VGX_OK;
+  return vgx_entry_noctx([&] {
+    if (!out) return VGX_ERR_INVALID;
+    *out = nullptr;
+    int n = 0;
+    if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0 || device < 0 || device >= n)
+      return VGX_ERR_CUDA;  // no CPU fallback: the product path needs a GPU
+    if (cudaSetDevice(device) != cudaSuccess) return VGX_ERR_CUDA;
+    vgx_ctx* c = new vgx_ctx();
+    c->device = device;
+    if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreate(&c->ev0) != cudaSuccess || cudaEventCreate(&c->ev1) != cudaSuccess) {
+      delete c;
+      return VGX_ERR_CUDA;
+    }
+    *out = c;
+    return VGX_OK;
+  });
 }
 
 extern "C" void vgx_ctx_destroy(vgx_ctx* c) {
-  if (!c) return;
-  cudaSetDevice(c->device);
-  cudaStreamSynchronize(c->stream);
-  vgx_comm_destroy(c);
-  vgx_p2p_free(c);
-  vgx_graph_free(c);
-  for (auto& kv : c->submaps) delete kv.second;
-  cudaEventDestroy(c->ev0);
-  cudaEventDestroy(c->ev1);
-  cudaStreamDestroy(c->stream);
-  delete c;
+  vgx_entry_noctx([&] {
+    if (!c) return VGX_OK;
+    vgx_comm_destroy(c);   // as an entry point, it selects the context's device
+    cudaStreamSynchronize(c->stream);
+    vgx_p2p_free(c);
+    vgx_graph_free(c);
+    for (auto& kv : c->submaps) delete kv.second;
+    cudaEventDestroy(c->ev0);
+    cudaEventDestroy(c->ev1);
+    cudaStreamDestroy(c->stream);
+    delete c;
+    return VGX_OK;
+  });
 }
 
 extern "C" const char* vgx_last_error(const vgx_ctx* c) { return c ? c->error.c_str() : "null context"; }
 extern "C" void* vgx_ctx_stream(vgx_ctx* c) { return c ? (void*)c->stream : nullptr; }
 extern "C" int vgx_ctx_synchronize(vgx_ctx* c) {
-  if (!c) return VGX_ERR_INVALID;
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_profile_enable(vgx_ctx* c, int on) {
-  if (!c) return VGX_ERR_INVALID;
-  c->profile = on != 0;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    c->profile = on != 0;
+    return VGX_OK;
+  });
 }
 extern "C" int vgx_profile_reset(vgx_ctx* c) {
-  if (!c) return VGX_ERR_INVALID;
-  for (auto& p : c->prof) p = VgxProfileSlot();
-  c->launches = 0;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    for (auto& p : c->prof) p = VgxProfileSlot();
+    c->launches = 0;
+    return VGX_OK;
+  });
 }
 extern "C" int vgx_profile_get(vgx_ctx* c, int which, double* total_ms, int64_t* launches) {
-  if (!c || which < 0 || which >= VGX_PROFILE_SLOTS) return VGX_ERR_INVALID;
-  if (total_ms) *total_ms = c->prof[which].total_ms;
-  if (launches) *launches = c->prof[which].launches;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (which < 0 || which >= VGX_PROFILE_SLOTS) return VGX_ERR_INVALID;
+    if (total_ms) *total_ms = c->prof[which].total_ms;
+    if (launches) *launches = c->prof[which].launches;
+    return VGX_OK;
+  });
 }
 extern "C" int64_t vgx_launch_count(vgx_ctx* c) { return c ? c->launches : 0; }
+
+const char* vgx_status_name(int rc) {
+  static const char* const names[] = {"invalid argument", "CUDA error", "not found", "out of memory",
+                                      "NCCL error", "capacity exceeded"};   // VGX_ERR_INVALID ... VGX_ERR_CAPACITY
+  return rc <= VGX_ERR_INVALID && rc >= VGX_ERR_CAPACITY ? names[VGX_ERR_INVALID - rc] : "error";
+}
+
+int vgx_caught(vgx_ctx* c) noexcept {
+  int rc = VGX_ERR_NOMEM;
+  const char* what = "out of host memory";
+  try {
+    throw;
+  } catch (const std::bad_alloc&) {
+  } catch (const std::length_error&) {
+  } catch (const std::exception& e) {
+    rc = VGX_ERR_INVALID;
+    what = e.what();
+  } catch (...) {
+    rc = VGX_ERR_INVALID;
+    what = "unknown exception";
+  }
+  try {
+    if (c) c->set_error(what);
+  } catch (...) {   // no memory for the message either: the status alone tells
+  }
+  return rc;
+}
+
+int vgx_submap_get(vgx_ctx* c, uint32_t id, VgxSubmap** out, VgxNeed need) {
+  VgxSubmap* s = c->find(id);
+  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "unknown submap " + std::to_string(id));
+  if (need != VgxNeed::any && s->finished != (need == VgxNeed::finished))
+    VGX_FAIL(c, VGX_ERR_INVALID, "submap " + std::to_string(id) + (s->finished ? " is finished" : " is not finished"));
+  *out = s;
+  return VGX_OK;
+}
 
 // ------------------------------------------------------------------ kernels
 __global__ void hash_clear_kernel(VgxHashEntry* entries, uint32_t size) {
@@ -119,15 +165,13 @@ __global__ void hash_insert_kernel(VgxHash h, const int32_t* block_idx, int n, i
 
 // Reads back hash_insert_kernel's input flag of an upload (d_counters[2]); on a bad block list the
 // new submap is dropped and the upload fails.
-static int check_uploaded_blocks(vgx_ctx* c, VgxSubmap* s, const char* what) {
+static int check_uploaded_blocks(vgx_ctx* c, VgxSubmap* s) {
   int bad = 0;
   VGX_CUDA(c, cudaMemcpyAsync(&bad, s->d_counters.get() + 2, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   if (!bad) return VGX_OK;
   vgx_submap_drop(c, s->id);
-  c->set_error(std::string(what) + ((bad & 2) ? ": block index outside the accepted range"
-                                              : ": repeated block index"));
-  return VGX_ERR_INVALID;
+  VGX_FAIL(c, VGX_ERR_INVALID, (bad & 2) ? "block index outside the accepted range" : "repeated block index");
 }
 
 // (distance[], weight[]) -> interleaved float2 bricks.
@@ -213,14 +257,12 @@ int vgx_submap_build_grid(vgx_ctx* c, VgxSubmap* s) {
   for (int i = 0; i < n; ++i)
     grid[(size_t)(idx[3 * i + 2] - lo[2]) * dy * dx + (size_t)(idx[3 * i + 1] - lo[1]) * dx +
          (idx[3 * i] - lo[0])] = i;
-  int rc = s->d_grid.alloc(c, sizeof(int32_t) * cells, "dense block grid");
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(s->d_grid.alloc(c, sizeof(int32_t) * cells, "dense block grid"));
   VGX_CUDA(c, cudaMemcpyAsync(s->d_grid.get(), grid.data(), sizeof(int32_t) * cells, cudaMemcpyHostToDevice, c->stream));
   // 16-bit copy for the registration kernel's shared-memory grid (one bulk copy per tile)
   std::vector<uint16_t> g16(((size_t)cells + 7) & ~(size_t)7, 0xFFFF);
   for (long long k = 0; k < cells; ++k) g16[(size_t)k] = grid[(size_t)k] < 0 ? 0xFFFF : (uint16_t)grid[(size_t)k];
-  rc = s->d_grid16.alloc(c, sizeof(uint16_t) * g16.size(), "dense block grid");
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(s->d_grid16.alloc(c, sizeof(uint16_t) * g16.size(), "dense block grid"));
   VGX_CUDA(c, cudaMemcpyAsync(s->d_grid16.get(), g16.data(), sizeof(uint16_t) * g16.size(), cudaMemcpyHostToDevice, c->stream));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   for (int a = 0; a < 3; ++a) { s->grid_min[a] = lo[a]; s->grid_dim[a] = hi[a] - lo[a] + 1; }
@@ -259,7 +301,6 @@ int vgx_submap_alloc(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int cap
                         VgxSubmap** out) {
   if (!(voxel_size > 0) || vps < 2 || vps > 32 || (vps & (vps - 1)) != 0 || cap < 0)
     VGX_FAIL(c, VGX_ERR_INVALID, "invalid voxel_size / voxels_per_side / capacity");
-  VGX_CUDA(c, cudaSetDevice(c->device));
   VgxSubmap* old = c->find(id);
   if (old) {
     VGX_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -267,8 +308,7 @@ int vgx_submap_alloc(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int cap
     c->submaps.erase(id);
     vgx_graph_invalidate_registration(c);
   }
-  VgxSubmap* s = new (std::nothrow) VgxSubmap();
-  if (!s) return VGX_ERR_NOMEM;
+  VgxSubmap* s = new VgxSubmap();
   s->id = id;
   s->voxel_size = voxel_size;
   // voxblox Layer ctor: inverses by double division, stored as float
@@ -304,59 +344,57 @@ int vgx_submap_alloc(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int cap
 extern "C" int vgx_submap_upload(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int n_blocks,
                                  const int32_t* block_idx, const float* distance,
                                  const float* weight) {
-  if (!c) return VGX_ERR_INVALID;
-  if (n_blocks < 0 || (n_blocks > 0 && (!block_idx || !distance || !weight)))
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_upload: null input");
-  VgxSubmap* s = nullptr;
-  int rc = vgx_submap_alloc(c, id, voxel_size, vps, n_blocks, true, &s);
-  if (rc != VGX_OK) return rc;
-  s->n_blocks = n_blocks;
-  s->finished = true;
-  if (n_blocks == 0) return VGX_OK;
-  const size_t nvox = (size_t)n_blocks * s->vox_per_block;
-  float *tmp_d, *tmp_w;
-  rc = vgx_carve(c, c->d_scratch, vgx_part(tmp_d, nvox), vgx_part(tmp_w, nvox));
-  if (rc != VGX_OK) return rc;
-  VGX_CUDA(c, cudaMemcpyAsync(tmp_d, distance, nvox * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  VGX_CUDA(c, cudaMemcpyAsync(tmp_w, weight, nvox * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx.get(), block_idx, sizeof(int32_t) * 3 * n_blocks,
-                              cudaMemcpyHostToDevice, c->stream));
-  interleave_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(tmp_d, tmp_w, s->d_dw.get(), nvox);
-  c->launches++;
-  // synchronises: the host buffers are the caller's
-  return vgx_submap_upload_finish(c, s, "vgx_submap_upload");
+  return vgx_entry(c, __func__, [&] {
+    if (n_blocks < 0 || (n_blocks > 0 && (!block_idx || !distance || !weight)))
+      VGX_FAIL(c, VGX_ERR_INVALID, "null input");
+    VgxSubmap* s = nullptr;
+    VGX_TRY(vgx_submap_alloc(c, id, voxel_size, vps, n_blocks, true, &s));
+    s->n_blocks = n_blocks;
+    s->finished = true;
+    if (n_blocks == 0) return VGX_OK;
+    const size_t nvox = (size_t)n_blocks * s->vox_per_block;
+    float *tmp_d, *tmp_w;
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(tmp_d, nvox), vgx_part(tmp_w, nvox)));
+    VGX_CUDA(c, cudaMemcpyAsync(tmp_d, distance, nvox * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    VGX_CUDA(c, cudaMemcpyAsync(tmp_w, weight, nvox * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx.get(), block_idx, sizeof(int32_t) * 3 * n_blocks,
+                                cudaMemcpyHostToDevice, c->stream));
+    interleave_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(tmp_d, tmp_w, s->d_dw.get(), nvox);
+    c->launches++;
+    // synchronises: the host buffers are the caller's
+    return vgx_submap_upload_finish(c, s);
+  });
 }
 
 extern "C" int vgx_submap_peek_device(vgx_ctx* c, uint32_t id, const int32_t** d_block_idx,
                                       const float** d_dw, int* n_blocks) {
-  if (!c) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_peek_device: unknown submap");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // the caller reads the bricks on its own stream
-  if (d_block_idx) *d_block_idx = s->d_block_idx.get();
-  if (d_dw) *d_dw = reinterpret_cast<const float*>(s->d_dw.get());
-  if (n_blocks) *n_blocks = s->n_blocks;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // the caller reads the bricks on its own stream
+    if (d_block_idx) *d_block_idx = s->d_block_idx.get();
+    if (d_dw) *d_dw = reinterpret_cast<const float*>(s->d_dw.get());
+    if (n_blocks) *n_blocks = s->n_blocks;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_upload_device(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int n_blocks,
                                         const int32_t* d_block_idx, const float* d_dw) {
-  if (!c) return VGX_ERR_INVALID;
-  if (n_blocks < 0 || (n_blocks > 0 && (!d_block_idx || !d_dw)))
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_upload_device: null input");
-  VgxSubmap* s = nullptr;
-  int rc = vgx_submap_alloc(c, id, voxel_size, vps, n_blocks, true, &s);
-  if (rc != VGX_OK) return rc;
-  s->n_blocks = n_blocks;
-  s->finished = true;
-  if (n_blocks == 0) return VGX_OK;
-  const size_t nvox = (size_t)n_blocks * s->vox_per_block;
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx.get(), d_block_idx, sizeof(int32_t) * 3 * n_blocks,
-                              cudaMemcpyDeviceToDevice, c->stream));
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_dw.get(), d_dw, sizeof(float2) * nvox, cudaMemcpyDeviceToDevice, c->stream));
-  // synchronises: the source buffers are the caller's
-  return vgx_submap_upload_finish(c, s, "vgx_submap_upload_device");
+  return vgx_entry(c, __func__, [&] {
+    if (n_blocks < 0 || (n_blocks > 0 && (!d_block_idx || !d_dw))) VGX_FAIL(c, VGX_ERR_INVALID, "null input");
+    VgxSubmap* s = nullptr;
+    VGX_TRY(vgx_submap_alloc(c, id, voxel_size, vps, n_blocks, true, &s));
+    s->n_blocks = n_blocks;
+    s->finished = true;
+    if (n_blocks == 0) return VGX_OK;
+    const size_t nvox = (size_t)n_blocks * s->vox_per_block;
+    VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx.get(), d_block_idx, sizeof(int32_t) * 3 * n_blocks,
+                                cudaMemcpyDeviceToDevice, c->stream));
+    VGX_CUDA(c, cudaMemcpyAsync(s->d_dw.get(), d_dw, sizeof(float2) * nvox, cudaMemcpyDeviceToDevice, c->stream));
+    // synchronises: the source buffers are the caller's
+    return vgx_submap_upload_finish(c, s);
+  });
 }
 
 // ------------------------------------------------------------------ colour channel
@@ -364,55 +402,52 @@ int vgx_submap_ensure_colour(vgx_ctx* c, VgxSubmap* s) {
   if (s->d_rgba.get()) return VGX_OK;
   const size_t bytes = sizeof(uint32_t) * (size_t)s->cap_blocks * s->vox_per_block;
   VgxBuffer<uint32_t> q;
-  const int rc = q.alloc(c, bytes, "submap colour channel", VGX_ERR_NOMEM);
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(q.alloc(c, bytes, "submap colour channel", VGX_ERR_NOMEM));
   VGX_CUDA(c, cudaMemsetAsync(q.get(), 0, bytes, c->stream));
   s->d_rgba = std::move(q);
   return VGX_OK;
 }
 
 extern "C" int vgx_submap_has_colour(vgx_ctx* c, uint32_t id, int* has) {
-  if (!c || !has) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_has_colour: unknown submap");
-  *has = s->d_rgba.get() ? 1 : 0;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!has) return VGX_ERR_INVALID;
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    *has = s->d_rgba.get() ? 1 : 0;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_download_colour(vgx_ctx* c, uint32_t id, int max_blocks, uint32_t* rgba, int* n_out) {
-  if (!c) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_download_colour: unknown submap");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  const int n = s->n_blocks;
-  if (n_out) *n_out = n;
-  if (n > max_blocks) VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_submap_download_colour: max_blocks too small");
-  if (n == 0 || !rgba) return VGX_OK;
-  const size_t bytes = sizeof(uint32_t) * (size_t)n * s->vox_per_block;
-  if (!s->d_rgba.get()) {
-    memset(rgba, 0, bytes);
+  return vgx_entry(c, __func__, [&] {
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    const int n = s->n_blocks;
+    if (n_out) *n_out = n;
+    if (n > max_blocks) VGX_FAIL(c, VGX_ERR_CAPACITY, "max_blocks too small");
+    if (n == 0 || !rgba) return VGX_OK;
+    const size_t bytes = sizeof(uint32_t) * (size_t)n * s->vox_per_block;
+    if (!s->d_rgba.get()) {
+      memset(rgba, 0, bytes);
+      return VGX_OK;
+    }
+    VGX_CUDA(c, cudaMemcpyAsync(rgba, s->d_rgba.get(), bytes, cudaMemcpyDeviceToHost, c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
     return VGX_OK;
-  }
-  VGX_CUDA(c, cudaMemcpyAsync(rgba, s->d_rgba.get(), bytes, cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  return VGX_OK;
+  });
 }
 
 // the channel of submap id from n_blocks x vps^3 words in host or device memory; the submap keeps its
 // previous channel (or none) when anything fails
-static int upload_colour(vgx_ctx* c, uint32_t id, int n_blocks, const uint32_t* rgba, cudaMemcpyKind kind,
-                         const char* what) {
-  if (!c) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, std::string(what) + ": unknown submap");
-  if (n_blocks != s->n_blocks) VGX_FAIL(c, VGX_ERR_INVALID, std::string(what) + ": n_blocks differs from the submap's");
-  if (n_blocks > 0 && !rgba) VGX_FAIL(c, VGX_ERR_INVALID, std::string(what) + ": null input");
-  VGX_CUDA(c, cudaSetDevice(c->device));
+static int upload_colour(vgx_ctx* c, uint32_t id, int n_blocks, const uint32_t* rgba, cudaMemcpyKind kind) {
+  VgxSubmap* s;
+  VGX_TRY(vgx_submap_get(c, id, &s));
+  if (n_blocks != s->n_blocks) VGX_FAIL(c, VGX_ERR_INVALID, "n_blocks differs from the submap's");
+  if (n_blocks > 0 && !rgba) VGX_FAIL(c, VGX_ERR_INVALID, "null input");
   const size_t cap_bytes = sizeof(uint32_t) * (size_t)s->cap_blocks * s->vox_per_block;
   const size_t bytes = sizeof(uint32_t) * (size_t)n_blocks * s->vox_per_block;
   VgxBuffer<uint32_t> q;
-  const int rc = q.alloc(c, cap_bytes, what, VGX_ERR_NOMEM);
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(q.alloc(c, cap_bytes, "colour channel", VGX_ERR_NOMEM));
   VGX_CUDA(c, cudaMemsetAsync(q.get(), 0, cap_bytes, c->stream));
   if (bytes) VGX_CUDA(c, cudaMemcpyAsync(q.get(), rgba, bytes, kind, c->stream));
   // synchronises: the source is the caller's, and the stream may still read the old channel
@@ -422,90 +457,84 @@ static int upload_colour(vgx_ctx* c, uint32_t id, int n_blocks, const uint32_t* 
 }
 
 extern "C" int vgx_submap_upload_colour(vgx_ctx* c, uint32_t id, int n_blocks, const uint32_t* rgba) {
-  return upload_colour(c, id, n_blocks, rgba, cudaMemcpyHostToDevice, "vgx_submap_upload_colour");
+  return vgx_entry(c, __func__, [&] { return upload_colour(c, id, n_blocks, rgba, cudaMemcpyHostToDevice); });
 }
 
 extern "C" int vgx_submap_peek_device_colour(vgx_ctx* c, uint32_t id, const uint32_t** d_rgba) {
-  if (!c || !d_rgba) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_peek_device_colour: unknown submap");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // the caller reads the channel on its own stream
-  *d_rgba = s->d_rgba.get();
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!d_rgba) return VGX_ERR_INVALID;
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // the caller reads the channel on its own stream
+    *d_rgba = s->d_rgba.get();
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_upload_device_colour(vgx_ctx* c, uint32_t id, int n_blocks, const uint32_t* d_rgba) {
-  return upload_colour(c, id, n_blocks, d_rgba, cudaMemcpyDeviceToDevice, "vgx_submap_upload_device_colour");
+  return vgx_entry(c, __func__, [&] { return upload_colour(c, id, n_blocks, d_rgba, cudaMemcpyDeviceToDevice); });
 }
 
-int vgx_submap_upload_finish(vgx_ctx* c, VgxSubmap* s, const char* what) {
+int vgx_submap_upload_finish(vgx_ctx* c, VgxSubmap* s) {
   if (s->n_blocks == 0) return VGX_OK;
   VGX_CUDA(c, cudaMemcpyAsync(s->d_counters.get(), &s->n_blocks, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   hash_insert_kernel<<<(s->n_blocks + 127) / 128, 128, 0, c->stream>>>(s->hash(), s->d_block_idx.get(), s->n_blocks,
                                                                        s->d_counters.get() + 2);
   c->launches++;
-  int rc = vgx_submap_build_view(c, s, s->d_dw.get(), s->d_view.get());
-  if (rc != VGX_OK) return rc;
-  rc = check_uploaded_blocks(c, s, what);
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(vgx_submap_build_view(c, s, s->d_dw.get(), s->d_view.get()));
+  VGX_TRY(check_uploaded_blocks(c, s));
   return vgx_submap_build_grid(c, s);
 }
 
 extern "C" int vgx_submap_create(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int capacity) {
-  if (!c) return VGX_ERR_INVALID;
-  if (capacity <= 0) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_create: capacity must be > 0");
-  VgxSubmap* s = nullptr;
-  int rc = vgx_submap_alloc(c, id, voxel_size, vps, capacity, false, &s);
-  if (rc != VGX_OK) return rc;
-  // new voxblox blocks are zero-initialised (distance 0, weight 0)
-  VGX_CUDA(c, cudaMemsetAsync(s->d_dw.get(), 0, sizeof(float2) * (size_t)capacity * s->vox_per_block,
-                              c->stream));
-  s->finished = false;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (capacity <= 0) VGX_FAIL(c, VGX_ERR_INVALID, "capacity must be > 0");
+    VgxSubmap* s = nullptr;
+    VGX_TRY(vgx_submap_alloc(c, id, voxel_size, vps, capacity, false, &s));
+    // new voxblox blocks are zero-initialised (distance 0, weight 0)
+    VGX_CUDA(c, cudaMemsetAsync(s->d_dw.get(), 0, sizeof(float2) * (size_t)capacity * s->vox_per_block,
+                                c->stream));
+    s->finished = false;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_finish(vgx_ctx* c, uint32_t id) {
-  if (!c) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_finish: unknown submap");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  // the layer is frozen from here on: the view only needs the blocks that exist, not the
-  // integration capacity (128 KiB per brick)
-  const size_t used = (size_t)s->n_blocks * s->vox_per_block;
-  if (!s->d_view.get()) {
-    const int rc = s->d_view.alloc(c, sizeof(float) * 8 * (used > 0 ? used : 1), "registration view");
-    if (rc != VGX_OK) return rc;
-  }
-  const int rc = vgx_submap_build_view(c, s, s->d_dw.get(), s->d_view.get());
-  if (rc != VGX_OK) return rc;
-  s->finished = true;
-  vgx_graph_invalidate_registration(c);
-  return vgx_submap_build_grid(c, s);
+  return vgx_entry(c, __func__, [&] {
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    // the layer is frozen from here on: the view only needs the blocks that exist, not the
+    // integration capacity (128 KiB per brick)
+    const size_t used = (size_t)s->n_blocks * s->vox_per_block;
+    if (!s->d_view.get()) {
+      VGX_TRY(s->d_view.alloc(c, sizeof(float) * 8 * (used > 0 ? used : 1), "registration view"));
+    }
+    VGX_TRY(vgx_submap_build_view(c, s, s->d_dw.get(), s->d_view.get()));
+    s->finished = true;
+    vgx_graph_invalidate_registration(c);
+    return vgx_submap_build_grid(c, s);
+  });
 }
 
 extern "C" int vgx_submap_free(vgx_ctx* c, uint32_t id) {
-  if (!c) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_free: unknown submap");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  delete s;
-  c->submaps.erase(id);
-  vgx_graph_invalidate_registration(c);
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    delete s;
+    c->submaps.erase(id);
+    vgx_graph_invalidate_registration(c);
+    return VGX_OK;
+  });
 }
 
 void vgx_submap_drop(vgx_ctx* c, uint32_t id) {
-  if (!c->find(id)) return;
-  const std::string msg = c->error;
-  vgx_submap_free(c, id);
-  c->set_error(msg);
+  if (c->find(id)) vgx_submap_free(c, id);
 }
 
 int vgx_submap_move(vgx_ctx* c, uint32_t from_id, uint32_t id) {
-  VgxSubmap* s = c->find(from_id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_move: unknown submap");
+  VgxSubmap* s;
+  VGX_TRY(vgx_submap_get(c, from_id, &s));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   VgxSubmap* old = c->find(id);
   delete old;
@@ -523,101 +552,97 @@ uint32_t vgx_scratch_id(vgx_ctx* c) {
 }
 
 extern "C" int vgx_submap_block_count(vgx_ctx* c, uint32_t id, int* n) {
-  if (!c || !n) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_block_count: unknown submap");
-  *n = s->n_blocks;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (!n) return VGX_ERR_INVALID;
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    *n = s->n_blocks;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_info(vgx_ctx* c, uint32_t id, float* voxel_size, int* vps, int* n_blocks,
                                int* finished) {
-  if (!c) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_info: unknown submap");
-  if (voxel_size) *voxel_size = s->voxel_size;
-  if (vps) *vps = s->vps;
-  if (n_blocks) *n_blocks = s->n_blocks;
-  if (finished) *finished = s->finished ? 1 : 0;
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    if (voxel_size) *voxel_size = s->voxel_size;
+    if (vps) *vps = s->vps;
+    if (n_blocks) *n_blocks = s->n_blocks;
+    if (finished) *finished = s->finished ? 1 : 0;
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_download(vgx_ctx* c, uint32_t id, int max_blocks, int32_t* block_idx,
                                    float* distance, float* weight, int* n_out) {
-  if (!c) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_download: unknown submap");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  const int n = s->n_blocks;
-  if (n_out) *n_out = n;
-  if (n > max_blocks) VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_submap_download: max_blocks too small");
-  if (n == 0) return VGX_OK;
-  const size_t nvox = (size_t)n * s->vox_per_block;
-  if (block_idx)
-    VGX_CUDA(c, cudaMemcpyAsync(block_idx, s->d_block_idx.get(), sizeof(int32_t) * 3 * n,
-                                cudaMemcpyDeviceToHost, c->stream));
-  if (distance || weight) {
-    float *tmp_d, *tmp_w;
-    int rc = vgx_carve(c, c->d_scratch, vgx_part(tmp_d, nvox), vgx_part(tmp_w, nvox));
-    if (rc != VGX_OK) return rc;
-    deinterleave_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(s->d_dw.get(), tmp_d, tmp_w, nvox);
-    c->launches++;
-    VGX_CUDA(c, cudaGetLastError());
-    if (distance)
-      VGX_CUDA(c, cudaMemcpyAsync(distance, tmp_d, nvox * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    if (weight)
-      VGX_CUDA(c, cudaMemcpyAsync(weight, tmp_w, nvox * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-  }
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    const int n = s->n_blocks;
+    if (n_out) *n_out = n;
+    if (n > max_blocks) VGX_FAIL(c, VGX_ERR_CAPACITY, "max_blocks too small");
+    if (n == 0) return VGX_OK;
+    const size_t nvox = (size_t)n * s->vox_per_block;
+    if (block_idx)
+      VGX_CUDA(c, cudaMemcpyAsync(block_idx, s->d_block_idx.get(), sizeof(int32_t) * 3 * n,
+                                  cudaMemcpyDeviceToHost, c->stream));
+    if (distance || weight) {
+      float *tmp_d, *tmp_w;
+      VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(tmp_d, nvox), vgx_part(tmp_w, nvox)));
+      deinterleave_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(s->d_dw.get(), tmp_d, tmp_w, nvox);
+      c->launches++;
+      VGX_CUDA(c, cudaGetLastError());
+      if (distance)
+        VGX_CUDA(c, cudaMemcpyAsync(distance, tmp_d, nvox * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+      if (weight)
+        VGX_CUDA(c, cudaMemcpyAsync(weight, tmp_w, nvox * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    }
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    return VGX_OK;
+  });
 }
 
 extern "C" int vgx_submap_upload_points(vgx_ctx* c, uint32_t id, int type, int n, const float* xyz,
                                         const float* distance, const float* weight) {
-  if (!c) return VGX_ERR_INVALID;
-  if (type < 0 || type > 1 || n < 0 || (n > 0 && (!xyz || !distance || !weight)))
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_upload_points: invalid argument");
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_upload_points: unknown submap");
-  VGX_CUDA(c, cudaSetDevice(c->device));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  VgxPoints& p = s->points[type];
-  p = VgxPoints();
-  vgx_graph_invalidate_registration(c);
-  if (n == 0) return VGX_OK;
-  // unit-major AoSoA staging on the host (pinned): unit u = {x[32], y[32], z[32], d[32], w[32]}
-  const size_t units = ((size_t)n + VGX_PT_UNIT - 1) / VGX_PT_UNIT;
-  const size_t floats = units * VGX_PT_UNIT_FLOATS;
-  float* h;
-  int rc = vgx_carve(c, c->h_pinned, vgx_part(h, floats));
-  if (rc != VGX_OK) return rc;
-  memset(h, 0, floats * sizeof(float));
-  double sum_w = 0;
-  std::vector<double> cumulative((size_t)n);
-  for (int i = 0; i < n; ++i) {
-    float* u = h + vgx_pt_index((size_t)i, 0);
-    u[0] = xyz[3 * (size_t)i];
-    u[32] = xyz[3 * (size_t)i + 1];
-    u[64] = xyz[3 * (size_t)i + 2];
-    u[96] = distance[i];
-    u[128] = weight[i];
-    sum_w += (double)weight[i];  // cpp:124, in point order
-    cumulative[i] = sum_w;       // WeightedSampler::addItem (weighted_sampler_inl.h:6-17)
-  }
-  VgxBuffer<float> d;
-  rc = d.alloc(c, floats * sizeof(float), "points upload");
-  if (rc != VGX_OK) return rc;
-  cudaError_t e = cudaMemcpyAsync(d.get(), h, floats * sizeof(float), cudaMemcpyHostToDevice, c->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-  if (e != cudaSuccess) {
-    c->set_error(std::string("points upload: ") + cudaGetErrorString(e));
-    return VGX_ERR_CUDA;
-  }
-  p.n = n;
-  p.data = std::move(d);
-  p.sum_w = sum_w;
-  p.cumulative_w.swap(cumulative);
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (type < 0 || type > 1 || n < 0 || (n > 0 && (!xyz || !distance || !weight)))
+      VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    VgxPoints& p = s->points[type];
+    p = VgxPoints();
+    vgx_graph_invalidate_registration(c);
+    if (n == 0) return VGX_OK;
+    // unit-major AoSoA staging on the host (pinned): unit u = {x[32], y[32], z[32], d[32], w[32]}
+    const size_t units = ((size_t)n + VGX_PT_UNIT - 1) / VGX_PT_UNIT;
+    const size_t floats = units * VGX_PT_UNIT_FLOATS;
+    float* h;
+    VGX_TRY(vgx_carve(c, c->h_pinned, vgx_part(h, floats)));
+    memset(h, 0, floats * sizeof(float));
+    double sum_w = 0;
+    std::vector<double> cumulative((size_t)n);
+    for (int i = 0; i < n; ++i) {
+      float* u = h + vgx_pt_index((size_t)i, 0);
+      u[0] = xyz[3 * (size_t)i];
+      u[32] = xyz[3 * (size_t)i + 1];
+      u[64] = xyz[3 * (size_t)i + 2];
+      u[96] = distance[i];
+      u[128] = weight[i];
+      sum_w += (double)weight[i];  // cpp:124, in point order
+      cumulative[i] = sum_w;       // WeightedSampler::addItem (weighted_sampler_inl.h:6-17)
+    }
+    VgxBuffer<float> d;
+    VGX_TRY(d.alloc(c, floats * sizeof(float), "points upload"));
+    VGX_CUDA(c, cudaMemcpyAsync(d.get(), h, floats * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    p.n = n;
+    p.data = std::move(d);
+    p.sum_w = sum_w;
+    p.cumulative_w.swap(cumulative);
+    return VGX_OK;
+  });
 }
 
 // ------------------------------------------------------------------ WeightedSampler
@@ -639,13 +664,13 @@ void vgx_points_draw(VgxPoints& p, int count, int32_t* idx) {
 }
 
 extern "C" int vgx_submap_draw_samples(vgx_ctx* c, uint32_t id, int type, int n, int32_t* indices) {
-  if (!c) return VGX_ERR_INVALID;
-  if (type < 0 || type > 1 || n < 0 || (n > 0 && !indices))
-    VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_draw_samples: invalid argument");
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_submap_draw_samples: unknown submap");
-  VgxPoints& p = s->points[type];
-  if (p.n == 0) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_submap_draw_samples: the submap has no registration points");
-  vgx_points_draw(p, n, indices);
-  return VGX_OK;
+  return vgx_entry(c, __func__, [&] {
+    if (type < 0 || type > 1 || n < 0 || (n > 0 && !indices)) VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
+    VgxSubmap* s;
+    VGX_TRY(vgx_submap_get(c, id, &s));
+    VgxPoints& p = s->points[type];
+    if (p.n == 0) VGX_FAIL(c, VGX_ERR_INVALID, "the submap has no registration points");
+    vgx_points_draw(p, n, indices);
+    return VGX_OK;
+  });
 }

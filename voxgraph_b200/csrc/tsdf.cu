@@ -686,10 +686,9 @@ static int tsdf_sort_and_apply(vgx_ctx* c, VgxSubmap* s, const TsdfParams& P, co
   unsigned *k_in, *k_out, *d_nlong, *d_heads;
   Tuple *v_in, *v_out;
   char* d_sort_tmp;
-  const int rc = vgx_carve(c, c->d_work2, vgx_part(k_in, total), vgx_part(k_out, total), vgx_part(v_in, total),
-                           vgx_part(v_out, total), vgx_part(d_nlong, 64),
-                           vgx_part(d_heads, (size_t)total / VGX_TSDF_LONG_SEGMENT + 2), vgx_part(d_sort_tmp, sort_tmp));
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(vgx_carve(c, c->d_work2, vgx_part(k_in, total), vgx_part(k_out, total), vgx_part(v_in, total),
+                    vgx_part(v_out, total), vgx_part(d_nlong, 64),
+                    vgx_part(d_heads, (size_t)total / VGX_TSDF_LONG_SEGMENT + 2), vgx_part(d_sort_tmp, sort_tmp)));
   uint32_t* d_rgba = kColour ? s->d_rgba.get() : nullptr;
   VgxLaunchScope scope(c, VGX_SLOT_TSDF_INTEGRATE, 4);
   VGX_CUDA(c, cudaMemsetAsync(d_nlong, 0, 256, stream));
@@ -710,15 +709,11 @@ static int tsdf_sort_and_apply(vgx_ctx* c, VgxSubmap* s, const TsdfParams& P, co
 
 int vgx_tsdf_check(vgx_ctx* c, uint32_t id, const float T_G_C[7], const vgx_tsdf_config* cfg, VgxSubmap** out,
                    vgx_tsdf_config* resolved) {
-  if (!c || !T_G_C) return VGX_ERR_INVALID;
-  VgxSubmap* s = c->find(id);
-  if (!s) VGX_FAIL(c, VGX_ERR_NOT_FOUND, "vgx_tsdf_integrate: unknown submap");
-  if (s->finished) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_tsdf_integrate: submap is finished");
-  VGX_CUDA(c, cudaSetDevice(c->device));
+  if (!T_G_C) return VGX_ERR_INVALID;
+  VGX_TRY(vgx_submap_get(c, id, out, VgxNeed::active));
   vgx_tsdf_config_default(resolved);
   if (cfg) *resolved = *cfg;
-  if (resolved->mode != 0 && resolved->mode != 1) VGX_FAIL(c, VGX_ERR_INVALID, "vgx_tsdf_integrate: invalid mode");
-  *out = s;
+  if (resolved->mode != 0 && resolved->mode != 1) VGX_FAIL(c, VGX_ERR_INVALID, "invalid mode");
   return VGX_OK;
 }
 
@@ -741,7 +736,7 @@ int vgx_tsdf_integrate_resident(vgx_ctx* c, VgxSubmap* s, const float T_G_C[7], 
   int rc;
   // the first coloured scan gives the submap its colour channel, once its scratch is in place; a call that
   // fails later (block capacity) or whose points are all rejected still leaves the channel, all zero
-  if (rgba && (rc = vgx_submap_ensure_colour(c, s)) != VGX_OK) return rc;
+  if (rgba) VGX_TRY(vgx_submap_ensure_colour(c, s));
   const size_t set_bytes = sizeof(unsigned long long) << 20;
   unsigned long long* d_obs = d_start + (1u << 20);
   cudaStream_t stream = c->stream;
@@ -756,22 +751,19 @@ int vgx_tsdf_integrate_resident(vgx_ctx* c, VgxSubmap* s, const float T_G_C[7], 
                                                     s->cap_blocks);
     }
     unsigned *d_counts, *d_offsets, *d_scan_tmp;
-    rc = vgx_carve(c, c->d_work, vgx_part(d_counts, (size_t)n + 2), vgx_part(d_offsets, (size_t)n + 2),
-                   vgx_part(d_scan_tmp, vgx_scan_tmp_count((size_t)n)));
-    if (rc != VGX_OK) return rc;
+    VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_counts, (size_t)n + 2), vgx_part(d_offsets, (size_t)n + 2),
+                      vgx_part(d_scan_tmp, vgx_scan_tmp_count((size_t)n))));
     unsigned total = 0;
     {
       VgxLaunchScope scope(c, VGX_SLOT_TSDF_INTEGRATE, 1);
       tsdf_count_kernel<<<grid, 128, 0, stream>>>(P, d_pts, d_counts);
-      rc = vgx_exclusive_scan_u32(c, d_counts, d_offsets, (size_t)n, d_scan_tmp);   // hand-written, 3 launches
-      if (rc != VGX_OK) return rc;
+      VGX_TRY(vgx_exclusive_scan_u32(c, d_counts, d_offsets, (size_t)n, d_scan_tmp));   // hand-written, 3 launches
     }
     VGX_CUDA(c, cudaMemcpyAsync(&total, d_offsets + n, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
     VGX_CUDA(c, cudaStreamSynchronize(stream));
     if (total > 0) {
-      rc = rgba ? tsdf_sort_and_apply<true>(c, s, P, d_pts, d_ray_rgba, d_offsets, total, d_stats)
-                : tsdf_sort_and_apply<false>(c, s, P, d_pts, nullptr, d_offsets, total, d_stats);
-      if (rc != VGX_OK) return rc;
+      VGX_TRY(rgba ? tsdf_sort_and_apply<true>(c, s, P, d_pts, d_ray_rgba, d_offsets, total, d_stats)
+                                               : tsdf_sort_and_apply<false>(c, s, P, d_pts, nullptr, d_offsets, total, d_stats));
     }
   } else {
     // ---- Fast scheduling: one kernel, blocks allocated on demand
@@ -806,7 +798,7 @@ int vgx_tsdf_integrate_resident(vgx_ctx* c, VgxSubmap* s, const float T_G_C[7], 
     cudaMemcpyAsync(s->d_counters.get(), fixed, sizeof(fixed), cudaMemcpyHostToDevice, stream);
     vgx_submap_rebuild_hash(c, s);
     cudaStreamSynchronize(stream);
-    VGX_FAIL(c, VGX_ERR_CAPACITY, "vgx_tsdf_integrate: submap block capacity exhausted");
+    VGX_FAIL(c, VGX_ERR_CAPACITY, "submap block capacity exhausted");
   }
   return VGX_OK;
 }
@@ -814,54 +806,54 @@ int vgx_tsdf_integrate_resident(vgx_ctx* c, VgxSubmap* s, const float T_G_C[7], 
 extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7], int n,
                                   const float* points_C, const uint8_t* rgba,
                                   const vgx_tsdf_config* cfg, vgx_tsdf_stats* stats) {
-  if (!c || !T_G_C || n < 0 || (n > 0 && !points_C)) return VGX_ERR_INVALID;
-  VgxSubmap* s;
-  vgx_tsdf_config rcfg;
-  int rc = vgx_tsdf_check(c, id, T_G_C, cfg, &s, &rcfg);
-  if (rc != VGX_OK) return rc;
-  if (n == 0) {
-    if (stats) memset(stats, 0, sizeof(*stats));
-    return VGX_OK;
-  }
-  // scratch: points | stats (cleared as 256 bytes) | (fast) two 2^20-entry approximate sets | ray colours
-  float* d_pts;
-  unsigned long long *d_stats, *d_start;
-  uint32_t* d_ray_rgba;   // r, g, b, a bytes per point, as the caller has them
-  rc = vgx_carve(c, c->d_scratch, vgx_part(d_pts, 3 * (size_t)n), vgx_part(d_stats, VGX_TSDF_STAT_WORDS),
-                 vgx_part(d_start, vgx_tsdf_set_words(rcfg)), vgx_part(d_ray_rgba, rgba ? (size_t)n : 0));
-  if (rc != VGX_OK) return rc;
-  cudaStream_t stream = c->stream;
-  VGX_CUDA(c, cudaMemcpyAsync(d_pts, points_C, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice, stream));
-  if (rgba) VGX_CUDA(c, cudaMemcpyAsync(d_ray_rgba, rgba, 4 * (size_t)n, cudaMemcpyHostToDevice, stream));
-  VGX_CUDA(c, cudaMemsetAsync(d_stats, 0, sizeof(unsigned long long) * VGX_TSDF_STAT_WORDS, stream));
-  return vgx_tsdf_integrate_resident(c, s, T_G_C, rcfg, n, d_pts, rgba ? d_ray_rgba : nullptr, d_stats, d_start, stats,
-                                     nullptr);
+  return vgx_entry(c, __func__, [&] {
+    if (!T_G_C || n < 0 || (n > 0 && !points_C)) return VGX_ERR_INVALID;
+    VgxSubmap* s;
+    vgx_tsdf_config rcfg;
+    VGX_TRY(vgx_tsdf_check(c, id, T_G_C, cfg, &s, &rcfg));
+    if (n == 0) {
+      if (stats) memset(stats, 0, sizeof(*stats));
+      return VGX_OK;
+    }
+    // scratch: points | stats (cleared as 256 bytes) | (fast) two 2^20-entry approximate sets | ray colours
+    float* d_pts;
+    unsigned long long *d_stats, *d_start;
+    uint32_t* d_ray_rgba;   // r, g, b, a bytes per point, as the caller has them
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_pts, 3 * (size_t)n), vgx_part(d_stats, VGX_TSDF_STAT_WORDS),
+                      vgx_part(d_start, vgx_tsdf_set_words(rcfg)), vgx_part(d_ray_rgba, rgba ? (size_t)n : 0)));
+    cudaStream_t stream = c->stream;
+    VGX_CUDA(c, cudaMemcpyAsync(d_pts, points_C, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice, stream));
+    if (rgba) VGX_CUDA(c, cudaMemcpyAsync(d_ray_rgba, rgba, 4 * (size_t)n, cudaMemcpyHostToDevice, stream));
+    VGX_CUDA(c, cudaMemsetAsync(d_stats, 0, sizeof(unsigned long long) * VGX_TSDF_STAT_WORDS, stream));
+    return vgx_tsdf_integrate_resident(c, s, T_G_C, rcfg, n, d_pts, rgba ? d_ray_rgba : nullptr, d_stats, d_start, stats,
+                                       nullptr);
+  });
 }
 
 extern "C" int vgx_tsdf_integrate_device(vgx_ctx* c, uint32_t id, const float T_G_C[7], int n,
                                          const float* d_points_C, const uint32_t* d_rgba,
                                          const vgx_tsdf_config* cfg, vgx_tsdf_stats* stats) {
-  if (!c || !T_G_C || n < 0 || (n > 0 && !d_points_C)) return VGX_ERR_INVALID;
-  VgxSubmap* s;
-  vgx_tsdf_config rcfg;
-  int rc = vgx_tsdf_check(c, id, T_G_C, cfg, &s, &rcfg);
-  if (rc != VGX_OK) return rc;
-  if (n == 0) {
-    if (stats) memset(stats, 0, sizeof(*stats));
-    return VGX_OK;
-  }
-  // the kernels dereference these: refuse host memory and memory of another GPU before any launch
-  for (const void* p : {(const void*)d_points_C, (const void*)d_rgba}) {
-    if (!p) continue;
-    cudaPointerAttributes at;
-    VGX_CUDA(c, cudaPointerGetAttributes(&at, p));
-    const bool device = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
-    if (!device || (at.type == cudaMemoryTypeDevice && at.device != c->device))
-      VGX_FAIL(c, VGX_ERR_INVALID, "vgx_tsdf_integrate_device: not device memory of this context's GPU");
-  }
-  unsigned long long *d_stats, *d_start;
-  rc = vgx_carve(c, c->d_scratch, vgx_part(d_stats, VGX_TSDF_STAT_WORDS), vgx_part(d_start, vgx_tsdf_set_words(rcfg)));
-  if (rc != VGX_OK) return rc;
-  VGX_CUDA(c, cudaMemsetAsync(d_stats, 0, sizeof(unsigned long long) * VGX_TSDF_STAT_WORDS, c->stream));
-  return vgx_tsdf_integrate_resident(c, s, T_G_C, rcfg, n, d_points_C, d_rgba, d_stats, d_start, stats, nullptr);
+  return vgx_entry(c, __func__, [&] {
+    if (!T_G_C || n < 0 || (n > 0 && !d_points_C)) return VGX_ERR_INVALID;
+    VgxSubmap* s;
+    vgx_tsdf_config rcfg;
+    VGX_TRY(vgx_tsdf_check(c, id, T_G_C, cfg, &s, &rcfg));
+    if (n == 0) {
+      if (stats) memset(stats, 0, sizeof(*stats));
+      return VGX_OK;
+    }
+    // the kernels dereference these: refuse host memory and memory of another GPU before any launch
+    for (const void* p : {(const void*)d_points_C, (const void*)d_rgba}) {
+      if (!p) continue;
+      cudaPointerAttributes at;
+      VGX_CUDA(c, cudaPointerGetAttributes(&at, p));
+      const bool device = at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged;
+      if (!device || (at.type == cudaMemoryTypeDevice && at.device != c->device))
+        VGX_FAIL(c, VGX_ERR_INVALID, "not device memory of this context's GPU");
+    }
+    unsigned long long *d_stats, *d_start;
+    VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_stats, VGX_TSDF_STAT_WORDS), vgx_part(d_start, vgx_tsdf_set_words(rcfg))));
+    VGX_CUDA(c, cudaMemsetAsync(d_stats, 0, sizeof(unsigned long long) * VGX_TSDF_STAT_WORDS, c->stream));
+    return vgx_tsdf_integrate_resident(c, s, T_G_C, rcfg, n, d_points_C, d_rgba, d_stats, d_start, stats, nullptr);
+  });
 }

@@ -13,6 +13,7 @@
 #include "voxgraph_b200.h"
 
 // ------------------------------------------------------------------ error handling
+// Both set the context's message through vgx_ctx::set_error, which prefixes the entry point's name.
 #define VGX_CUDA(ctx, expr)                                                            \
   do {                                                                                 \
     cudaError_t _e = (expr);                                                           \
@@ -26,6 +27,13 @@
   do {                           \
     (ctx)->set_error(msg);       \
     return (code);               \
+  } while (0)
+
+// returns the status of a call that did not return VGX_OK (its message is already set)
+#define VGX_TRY(expr)              \
+  do {                             \
+    const int _rc = (expr);        \
+    if (_rc != VGX_OK) return _rc; \
   } while (0)
 
 // ------------------------------------------------------------------ memory owner
@@ -254,13 +262,61 @@ struct vgx_ctx {
   std::vector<uint32_t> mesh_ids;     // the submaps of the build, in build order
   std::vector<int64_t> mesh_voff;     // their first vertices (+ the total)
   bool mesh_table_ready = false;      // triangle table in this device's constant memory
+  // the entry point the caller called, while it runs (vgx_entry); nullptr between calls
+  const char* entry = nullptr;
 
-  void set_error(const std::string& e) { error = e; }
+  void set_error(const std::string& e) { error = std::string(entry ? entry : "voxgraph_b200") + ": " + e; }
   VgxSubmap* find(uint32_t id) {
     auto it = submaps.find(id);
     return it == submaps.end() ? nullptr : it->second;
   }
 };
+
+// ------------------------------------------------------------------ C-ABI guard
+// Every extern "C" entry point with a context runs its body through vgx_entry.  The outermost call on a
+// context records its name, clears the message, selects the context's device and runs the body inside
+// try: std::bad_alloc and std::length_error become VGX_ERR_NOMEM, any other exception VGX_ERR_INVALID with
+// its what().  A failure the body left without a message reads "<name>: <status>"; VGX_OK leaves the
+// message empty.  An entry point called from inside another one only runs its body, so its messages name
+// the outer call and its exceptions reach the outer guard.  A null context is VGX_ERR_INVALID.
+int vgx_caught(vgx_ctx* c) noexcept;   // the status (and message, with c) of the exception being handled
+const char* vgx_status_name(int rc);
+
+template <class F>
+int vgx_entry(vgx_ctx* c, const char* name, F&& body) {
+  if (!c) return VGX_ERR_INVALID;
+  if (c->entry) return body();
+  c->entry = name;
+  int rc;
+  try {
+    c->error.clear();
+    rc = [&] {
+      VGX_CUDA(c, cudaSetDevice(c->device));
+      return body();
+    }();
+    if (rc == VGX_OK) c->error.clear();
+    else if (rc < 0 && c->error.empty()) c->set_error(vgx_status_name(rc));
+  } catch (...) {
+    rc = vgx_caught(c);
+  }
+  c->entry = nullptr;
+  return rc;
+}
+
+// the same for the entry points without a context: exceptions become a status, with no message
+template <class F>
+int vgx_entry_noctx(F&& body) noexcept {
+  try {
+    return body();
+  } catch (...) {
+    return vgx_caught(nullptr);
+  }
+}
+
+// The submap `id`: VGX_ERR_NOT_FOUND ("unknown submap <id>") when the context has none, VGX_ERR_INVALID
+// when it is not finished (need = finished) or is finished (need = active).
+enum class VgxNeed { any, finished, active };
+int vgx_submap_get(vgx_ctx* c, uint32_t id, VgxSubmap** out, VgxNeed need = VgxNeed::any);
 
 template <class T>
 int VgxBuffer<T>::alloc(vgx_ctx* c, size_t bytes, const char* what, int nomem) {
@@ -280,8 +336,7 @@ template <class T>
 int VgxBuffer<T>::grow_keep(vgx_ctx* c, size_t need, size_t used, const char* what) {
   if (need <= bytes_) return VGX_OK;
   VgxBuffer q(kind_);
-  const int rc = q.alloc(c, need + need / 4, what);
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(q.alloc(c, need + need / 4, what));
   if (used) {
     VGX_CUDA(c, cudaMemcpyAsync(q.p_, p_, used, cudaMemcpyDefault, c->stream));
     VGX_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -305,8 +360,7 @@ static inline size_t vgx_part_span(size_t bytes) { return (bytes + 255) & ~(size
 // 256-byte aligned), growing the arena to the total first; no CUDA call when it is large enough.
 template <class... T>
 int vgx_carve(vgx_ctx* c, VgxBuffer<>& arena, VgxPart<T>... parts) {
-  const int rc = arena.grow(c, (vgx_part_span(parts.bytes) + ...), "scratch arena");
-  if (rc != VGX_OK) return rc;
+  VGX_TRY(arena.grow(c, (vgx_part_span(parts.bytes) + ...), "scratch arena"));
   char* at = arena.get();
   ((parts.at = reinterpret_cast<T*>(at), at += vgx_part_span(parts.bytes)), ...);
   return VGX_OK;
@@ -339,7 +393,7 @@ int vgx_submap_alloc(vgx_ctx* ctx, uint32_t submap_id, float voxel_size, int vps
 // the rest of an upload once s->n_blocks block indices and bricks are in place on the device: block
 // hash, registration view, the upload rules (a bad block list drops the submap: VGX_ERR_INVALID) and
 // the dense grid.  Synchronises.
-int vgx_submap_upload_finish(vgx_ctx* ctx, VgxSubmap* s, const char* what);
+int vgx_submap_upload_finish(vgx_ctx* ctx, VgxSubmap* s);
 // gives the submap its colour channel if it has none: cap_blocks x vps^3 words, zero (voxblox Color())
 int vgx_submap_ensure_colour(vgx_ctx* ctx, VgxSubmap* s);
 // frees submap_id if it exists and keeps the error message of the failure that leads to the drop
@@ -358,8 +412,8 @@ int vgx_exclusive_scan_u32(vgx_ctx* c, const unsigned* d_in, unsigned* d_out, si
 size_t vgx_scan_tmp_count(size_t n);
 // TSDF integration over points that are already in device memory (tsdf.cu): the core behind
 // vgx_tsdf_integrate, vgx_tsdf_integrate_device and vgx_tsdf_integrate_cloud.
-//   check:    the argument rules the three share (unknown / finished submap, mode) -> the submap and the
-//             configuration with defaults filled in.
+//   check:    the argument rules the three share (null pose, unknown / finished submap, mode) -> the submap
+//             and the configuration with defaults filled in.
 //   resident: integrates the n point slots d_pts (a slot with a non-finite coordinate is skipped and not
 //             counted) with ray colours d_ray_rgba (r, g, b, a bytes per slot, or NULL), ends in the one
 //             synchronising copy that brings the statistics back.  The caller lays out, in d_scratch,
