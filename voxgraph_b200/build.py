@@ -28,6 +28,7 @@ SOURCES = [
     ("solve.cu", []),
     ("p2p.cu", []),
     ("nccl_dyn.cpp", []),
+    ("graph_plan.cpp", []),
 ]
 
 

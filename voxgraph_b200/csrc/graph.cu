@@ -300,35 +300,135 @@ extern "C" int vgx_shard_constraints(int nranks, int n, const int32_t* num_resid
                                      const uint32_t* locality_keys, int32_t* owner) {
   return vgx_entry_noctx([&] {
     if (nranks < 1 || n < 0 || (n > 0 && (!num_residuals || !owner))) return VGX_ERR_INVALID;
-    std::vector<int> order(n);
-    std::iota(order.begin(), order.end(), 0);
-    if (locality_keys)
-      std::stable_sort(order.begin(), order.end(),
-                       [&](int a, int b) { return locality_keys[a] < locality_keys[b]; });
-    int64_t total = 0;
-    for (int i = 0; i < n; ++i) total += std::max(num_residuals[i], 0);
-    int64_t before = 0;
-    for (int i : order) {
-      const int64_t cnt = std::max(num_residuals[i], 0);
-      // rank whose share [r * total / nranks, (r + 1) * total / nranks) holds the midpoint
-      int r = total > 0 ? (int)(((2 * before + cnt) * nranks) / (2 * total)) : 0;
-      owner[i] = std::min(std::max(r, 0), nranks - 1);
-      before += cnt;
-    }
+    vgx_partition_constraints(nranks, n, num_residuals, locality_keys, owner);
     return VGX_OK;
   });
 }
 
 // ------------------------------------------------------------------ table construction
+// A build collects the constraints, plans the layout (graph_plan.cpp) and uploads the plan.
+
+// d <- n elements of T (at least 8 bytes: an empty table has an address too)
+template <class T>
+static int table_alloc(vgx_ctx* c, VgxBuffer<T>& d, size_t n) {
+  return d.alloc(c, std::max<size_t>(sizeof(T) * n, 8), "graph table build", VGX_ERR_NOMEM);
+}
+
+// d <- a copy of v
+template <class T>
+static int table_upload(vgx_ctx* c, VgxBuffer<T>& d, const std::vector<T>& v) {
+  VGX_TRY(table_alloc(c, d, std::max<size_t>(v.size(), 1)));
+  if (!v.empty())
+    VGX_CUDA(c, cudaMemcpyAsync(d.get(), v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice, c->stream));
+  return VGX_OK;
+}
+
+// The device tables of `plan`; all[i] is the descriptor of constraint i, is_sampled[i] whether its points are the
+// draws in g->samples[i].  Every buffer is t's, so a failure leaves nothing behind.
+static int upload_tables(vgx_ctx* c, VgxGraph* g, const VgxGraphPlan& plan, const std::vector<RegConstraintDev>& all,
+                         const std::vector<uint8_t>& is_sampled, int sms, VgxGraphTables& t) {
+  cudaStream_t st = c->stream;
+  const int N = g->N, n_local = plan.n_local(), n_tiles = plan.n_tiles(), n = plan.n_free;
+  std::vector<RegConstraintDev> cons(n_local);
+  for (int k = 0; k < n_local; ++k) cons[k] = all[plan.local[k]];
+  // gather the drawn points of the local sampled blocks into their own unit-major buffers
+  size_t units = 0, nidx = 0;
+  for (int k = 0; k < n_local; ++k)
+    if (is_sampled[plan.local[k]]) { units += ((size_t)cons[k].n + 31) / 32; nidx += (size_t)cons[k].n; }
+  if (units > 0) {
+    VGX_TRY(t.d_sample_pts.alloc(c, units * VGX_PT_UNIT_FLOATS * sizeof(float), "registration sample points"));
+    VGX_TRY(t.d_sample_idx.alloc(c, nidx * sizeof(int32_t), "registration sample points"));
+    size_t uo = 0, io = 0;
+    for (int k = 0; k < n_local; ++k) {
+      const int i = plan.local[k];
+      if (!is_sampled[i]) continue;
+      const VgxPoints& p = c->find(g->reg_ref[i])->points[g->reg_cfgs[i].registration_point_type];
+      VGX_CUDA(c, cudaMemcpyAsync(t.d_sample_idx.get() + io, g->samples[i].data(), sizeof(int32_t) * cons[k].n,
+                                  cudaMemcpyHostToDevice, st));
+      float* dst = t.d_sample_pts.get() + uo * VGX_PT_UNIT_FLOATS;
+      vgx_launch_reg_gather_samples(st, p.data.get(), t.d_sample_idx.get() + io, cons[k].n, dst);
+      c->launches++;
+      cons[k].pts = dst;
+      uo += ((size_t)cons[k].n + 31) / 32;
+      io += (size_t)cons[k].n;
+    }
+    VGX_CUDA(c, cudaStreamSynchronize(st));  // g->samples[] are pageable host vectors
+  }
+  // what the CTA of a tile needs to start its bulk copies without a dependent load
+  std::vector<RegTile> tiles(n_tiles);
+  for (int j = 0; j < n_tiles; ++j) {
+    const VgxPlanTile& pt = plan.tiles[j];
+    const RegConstraintDev& cc = cons[pt.constraint];
+    tiles[j].constraint = pt.constraint;
+    tiles[j].unit0 = pt.unit0;
+    tiles[j].count = pt.count;
+    tiles[j].grid_bytes = pt.grid_bytes;
+    tiles[j].pts = cc.pts + (size_t)(pt.first / VGX_REG_UNIT) * VGX_PT_UNIT_FLOATS;
+    tiles[j].grid16 = cc.grid16;
+  }
+  std::vector<int> ident(n_tiles), zero(n_tiles, 0);
+  std::iota(ident.begin(), ident.end(), 0);
+  VGX_TRY(table_upload(c, t.d_cons, cons));
+  VGX_TRY(table_upload(c, t.d_tiles, tiles));
+  VGX_TRY(table_upload(c, t.d_tile_begin, plan.tile_begin));
+  VGX_TRY(table_upload(c, t.d_tile_order, ident));
+  VGX_TRY(table_upload(c, t.d_tile_cost, zero));
+  VGX_TRY(table_upload(c, t.d_rel, g->rel));
+  VGX_TRY(table_upload(c, t.d_csr_begin, plan.csr_begin));
+  VGX_TRY(table_upload(c, t.d_csr_items, plan.items));
+  VGX_TRY(table_upload(c, t.d_block_mask, plan.block_mask));
+  VGX_TRY(table_upload(c, t.d_block_nodes, plan.block_nodes));
+  VGX_TRY(table_upload(c, t.d_red_offset, plan.red));
+  VGX_TRY(table_upload(c, t.d_x, g->x));
+  VGX_TRY(table_alloc(c, t.d_unit_bounds, plan.n_units));
+  if (n_tiles > 0) {
+    vgx_launch_reg_unit_bounds(st, t.d_tiles.get(), n_tiles, t.d_unit_bounds.get());
+    c->launches++;
+    VGX_CUDA(c, cudaGetLastError());
+  }
+  VGX_TRY(table_alloc(c, t.d_poses, n_local));
+  VGX_TRY(table_alloc(c, t.d_partials, VGX_REG_NSTRIDE * (size_t)n_tiles));
+  VGX_TRY(table_alloc(c, t.d_csum, VGX_REG_NSTRIDE * (size_t)n_local));
+  VGX_TRY(table_alloc(c, t.d_xc, 4 * (size_t)N));
+  VGX_TRY(table_alloc(c, t.d_packed[0], plan.packed_len));
+  VGX_TRY(table_alloc(c, t.d_packed[1], plan.packed_len));
+  VGX_TRY(table_alloc(c, t.d_A, (size_t)(n + 1) * (n + 1)));
+  VGX_TRY(table_alloc(c, t.d_scale, n));
+  VGX_TRY(table_alloc(c, t.d_diag, n));
+  VGX_TRY(table_alloc(c, t.d_gs, n));
+  VGX_TRY(table_alloc(c, t.d_step, n));
+  VGX_TRY(table_alloc(c, t.d_state, 1));
+  const char* what = "graph table build";
+  if (!g->h_state.get()) VGX_TRY(g->h_state.alloc(c, sizeof(LmState), what, VGX_ERR_NOMEM));
+  VGX_TRY(table_alloc(c, t.d_snap, 2));
+  if (!g->h_snap.get()) VGX_TRY(g->h_snap.alloc(c, 2 * sizeof(LmState), what, VGX_ERR_NOMEM));
+  if (g->h_x.bytes() < sizeof(double) * 4 * (size_t)N)
+    VGX_TRY(g->h_x.alloc(c, sizeof(double) * 4 * (size_t)std::max(2 * N, 64), what, VGX_ERR_NOMEM));
+  if (!g->copy_stream) {
+    VGX_CUDA(c, cudaStreamCreateWithFlags(&g->copy_stream, cudaStreamNonBlocking));
+    for (int k = 0; k < 2; ++k) {
+      VGX_CUDA(c, cudaEventCreateWithFlags(&g->ev_iter[k], cudaEventDisableTiming));
+      VGX_CUDA(c, cudaEventCreateWithFlags(&g->ev_copy[k], cudaEventDisableTiming));
+    }
+  }
+  VGX_CUDA(c, cudaStreamSynchronize(st));
+  // the fused assembly and exchange spins on its peers, so its grid must be co-resident as a whole
+  int per_sm = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, assemble_exchange_kernel, 128, 0) != cudaSuccess)
+    per_sm = 1;
+  t.exchange_grid = std::min(N + plan.E + 1, std::max(1, sms * std::max(per_sm, 1)));
+  return VGX_OK;
+}
 
 static int build_tables(vgx_ctx* c, VgxGraph* g) {
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  g->dev = VgxGraphTables();
-  const int N = g->N;
+  g->dev = VgxGraphTables();   // before the new tables are allocated: a rebuild needs no more device memory
+  // ---- collect: the descriptors, nodes and sampling draws of all constraints, and their partition over ranks
   const int P = (int)g->reg_ref.size();
-  // ---- shard registration constraints over ranks: greedy by descending point count
   std::vector<RegConstraintDev> all(P);
+  std::vector<VgxPlanConstraint> facts(P);
   std::vector<uint8_t> is_sampled(P, 0);
+  std::vector<int32_t> counts(P), owner(P, 0);
   g->zero_weight = false;
   g->residuals_global = 0;
   g->samples.assign(P, std::vector<int32_t>());
@@ -358,224 +458,24 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
         vgx_points_draw(p, all[i].n, g->samples[i].data());
       }
     }
+    const RegConstraintDev& cc = all[i];
+    facts[i] = {cc.n, cc.ref_node, cc.read_node, cc.gd0 * cc.gd1 * cc.gd2, cc.grid16 != nullptr};
+    counts[i] = cc.n;
   }
-  std::vector<int32_t> owner(P, 0), counts(P, 0);
-  for (int i = 0; i < P; ++i) counts[i] = all[i].n;
-  vgx_shard_constraints(c->nranks, P, counts.data(), g->reg_read.data(), owner.data());
-  g->local.clear();
-  std::vector<RegConstraintDev> cons;
-  std::vector<RegTile> tiles;
-  std::vector<int> tile_begin;
-  g->residuals_local = 0;
-  for (int i = 0; i < P; ++i) {
-    if (owner[i] != c->rank) continue;
-    g->local.push_back(i);
-    cons.push_back(all[i]);
-    g->residuals_local += all[i].n;
-  }
-  g->n_local = (int)cons.size();
-  // gather the drawn points of the local sampled blocks into their own unit-major buffers
-  {
-    size_t units = 0, nidx = 0;
-    for (int k = 0; k < g->n_local; ++k)
-      if (is_sampled[g->local[k]]) { units += ((size_t)cons[k].n + 31) / 32; nidx += (size_t)cons[k].n; }
-    if (units > 0) {
-      VGX_TRY(g->dev.d_sample_pts.alloc(c, units * VGX_PT_UNIT_FLOATS * sizeof(float), "registration sample points"));
-      VGX_TRY(g->dev.d_sample_idx.alloc(c, nidx * sizeof(int32_t), "registration sample points"));
-      size_t uo = 0, io = 0;
-      for (int k = 0; k < g->n_local; ++k) {
-        const int i = g->local[k];
-        if (!is_sampled[i]) continue;
-        const VgxPoints& p = c->find(g->reg_ref[i])->points[g->reg_cfgs[i].registration_point_type];
-        VGX_CUDA(c, cudaMemcpyAsync(g->dev.d_sample_idx.get() + io, g->samples[i].data(), sizeof(int32_t) * cons[k].n,
-                                    cudaMemcpyHostToDevice, c->stream));
-        float* dst = g->dev.d_sample_pts.get() + uo * VGX_PT_UNIT_FLOATS;
-        vgx_launch_reg_gather_samples(c->stream, p.data.get(), g->dev.d_sample_idx.get() + io, cons[k].n, dst);
-        c->launches++;
-        cons[k].pts = dst;
-        uo += ((size_t)cons[k].n + 31) / 32;
-        io += (size_t)cons[k].n;
-      }
-      VGX_CUDA(c, cudaStreamSynchronize(c->stream));  // g->samples[] are pageable host vectors
-    }
-  }
-  // Scheduling of the reduce kernel.  The cost of a unit varies ~4x with the share of its points
-  // that land in the reading submap, so a static equal cut of the units over the resident CTAs
-  // leaves SMs idle while the hit-heavy ones finish (measured: max SM busy time 16 % above the
-  // mean).  Instead each residual block is cut into fixed tiles of hw_units 32-point units, ONE CTA
-  // PER TILE, dealt to the SMs by the hardware block scheduler as resident CTAs retire (dynamic
-  // balancing at no instruction cost; the per-CTA set-up latency hides behind the other resident
-  // CTAs).  Tiles never straddle constraints and start on a unit boundary (128-byte aligned SoA
-  // slices for TMA).
-  g->grid_capacity = 0;
-  for (const auto& cc : cons)
-    if (cc.grid) g->grid_capacity = std::max(g->grid_capacity, (cc.gd0 * cc.gd1 * cc.gd2 + 7) & ~7);  // 16-byte multiple
+  vgx_partition_constraints(c->nranks, P, counts.data(), g->reg_read.data(), owner.data());
+  // ---- plan
+  std::vector<int2> rel(g->rel.size());
+  for (size_t e = 0; e < rel.size(); ++e) rel[e] = make_int2(g->rel[e].a, g->rel[e].b);
   int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
-  const int slots = std::max(sms, 1) * VGX_REG_TILE_SLOTS_PER_SM;
-  int64_t U = 0;  // total units
-  for (const auto& cc : cons) U += (cc.n + VGX_REG_UNIT - 1) / VGX_REG_UNIT;
-  // Tile size: at most VGX_REG_HW_TILE_UNITS units, fewer when the problem is small, so that there
-  // are at least ~2 tiles per CTA slot (a 3-pair streaming graph still fills the machine).  The slots
-  // are a fixed count per SM, not the resident CTAs, so that the tiles do not follow the occupancy.
-  // The environment variable of the same name forces a size (n >= 1; tests use it for shapes the
-  // formula never produces).
-  int hw_units = (int)std::min<int64_t>(VGX_REG_HW_TILE_UNITS,
-                                        std::max<int64_t>(4, (U + 2 * (int64_t)slots - 1) / (2 * (int64_t)slots)));
-  if (const char* env = getenv("VGX_REG_HW_TILE_UNITS"))
-    if (atoi(env) >= 1) hw_units = atoi(env);
-  g->evals_since_order = -1;
-  const int tile_pts = hw_units * VGX_REG_UNIT;
-  for (int k = 0; k < g->n_local; ++k) {
-    tile_begin.push_back((int)tiles.size());
-    for (int s0 = 0; s0 < cons[k].n; s0 += tile_pts) {
-      RegTile t;
-      t.constraint = k; t.count = std::min(tile_pts, cons[k].n - s0);
-      t.pts = cons[k].pts + (size_t)(s0 / VGX_REG_UNIT) * VGX_PT_UNIT_FLOATS;
-      tiles.push_back(t);
-    }
-  }
-  tile_begin.push_back((int)tiles.size());
-  g->n_tiles = (int)tiles.size();
-  int n_units = 0;   // units of all tiles = entries of the unit-bound table
-  for (auto& t : tiles) {   // what the CTA needs to start its bulk copies without a dependent load
-    const RegConstraintDev& cc = cons[t.constraint];
-    const int cells = cc.gd0 * cc.gd1 * cc.gd2;
-    t.unit0 = n_units;
-    n_units += (t.count + VGX_REG_UNIT - 1) / VGX_REG_UNIT;
-    t.grid16 = cc.grid16;
-    t.grid_bytes = (cc.grid16 && cells > 0) ? (int)((((size_t)cells + 7) & ~(size_t)7) * sizeof(uint16_t)) : 0;
-  }
-  g->n_rel_local = (c->rank == 0) ? (int)g->rel.size() : 0;
-
-  // ---- off-diagonal block index over ALL edges (identical on every rank)
-  std::map<std::pair<int, int>, int> block_of;
-  std::vector<int>& block_nodes = g->block_nodes;
-  block_nodes.clear();
-  auto block_id = [&](int a, int b) {
-    std::pair<int, int> key(std::min(a, b), std::max(a, b));
-    auto it = block_of.find(key);
-    if (it != block_of.end()) return it->second;
-    int id = (int)block_of.size();
-    block_of[key] = id;
-    block_nodes.push_back(key.first);
-    block_nodes.push_back(key.second);
-    return id;
-  };
-  for (const auto& e : g->rel) block_id(e.a, e.b);
-  for (int i = 0; i < P; ++i) block_id(all[i].ref_node, all[i].read_node);
-  g->E = (int)block_of.size();
-
-  // ---- CSR of contributions per output block (local blocks only)
-  std::vector<std::vector<int2>> lists(N + g->E);
-  auto add_items = [&](int blk, int a, int b) {
-    lists[a].push_back(make_int2(blk, 0));
-    lists[b].push_back(make_int2(blk, 1));
-    const int ob = N + block_id(a, b);
-    lists[ob].push_back(make_int2(blk, a < b ? 2 : 3));
-  };
-  for (int e = 0; e < g->n_rel_local; ++e) add_items(-(e + 1), g->rel[e].a, g->rel[e].b);
-  for (int k = 0; k < g->n_local; ++k) add_items(k, cons[k].ref_node, cons[k].read_node);
-  // which ranks have items for an output block (every rank computes the same table: the partition
-  // of the constraints is global knowledge; relative edges live on rank 0)
-  std::vector<unsigned char> block_mask(N + g->E, 0);
-  for (const auto& e : g->rel) {
-    block_mask[e.a] |= 1; block_mask[e.b] |= 1;
-    block_mask[N + block_id(e.a, e.b)] |= 1;
-  }
-  for (int i = 0; i < P; ++i) {
-    const unsigned char bit = (unsigned char)(1u << owner[i]);
-    block_mask[all[i].ref_node] |= bit; block_mask[all[i].read_node] |= bit;
-    block_mask[N + block_id(all[i].ref_node, all[i].read_node)] |= bit;
-  }
-  std::vector<int> csr_begin(N + g->E + 1, 0);
-  std::vector<int4> items;   // a registration item carries its constraint's tile range
-  for (int ob = 0; ob < N + g->E; ++ob) {
-    csr_begin[ob] = (int)items.size();
-    for (const int2& it : lists[ob])
-      items.push_back(it.x >= 0 ? make_int4(it.x, it.y, tile_begin[it.x], tile_begin[it.x + 1])
-                                : make_int4(it.x, it.y, 0, 0));
-  }
-  csr_begin[N + g->E] = (int)items.size();
-
-  // ---- reduced offsets
-  std::vector<int>& red = g->red;
-  red.assign(N, -1);
-  int n = 0;
-  for (int i = 0; i < N; ++i)
-    if (!g->constant[i]) { red[i] = n; n += 4; }
-  g->n_free = n;
-  g->packed_len = PACK_HDR + 20 * (size_t)N + 16 * (size_t)g->E;
-
-  // every failure here reads "graph table build: <CUDA error>"; out of memory is VGX_ERR_NOMEM
-  const char* what = "graph table build";
-  VgxGraphTables& t = g->dev;
-  cudaStream_t st = c->stream;
-  int rc = VGX_OK;
-  auto check = [&](cudaError_t e) {
-    if (rc != VGX_OK || e == cudaSuccess) return;
-    c->set_error(std::string(what) + ": " + cudaGetErrorString(e));
-    rc = e == cudaErrorMemoryAllocation ? VGX_ERR_NOMEM : VGX_ERR_CUDA;
-  };
-  auto dmalloc = [&](auto& d, size_t bytes) {
-    if (rc == VGX_OK) rc = d.alloc(c, std::max<size_t>(bytes, 8), what, VGX_ERR_NOMEM);
-  };
-  auto upload = [&](auto& d, const auto& v) {
-    dmalloc(d, sizeof(v[0]) * std::max<size_t>(v.size(), 1));
-    if (rc == VGX_OK && !v.empty())
-      check(cudaMemcpyAsync(d.get(), v.data(), sizeof(v[0]) * v.size(), cudaMemcpyHostToDevice, st));
-  };
-  upload(t.d_cons, cons);
-  upload(t.d_tiles, tiles);
-  upload(t.d_tile_begin, tile_begin);
-  {
-    std::vector<int> ident(tiles.size()), zero(tiles.size(), 0);
-    std::iota(ident.begin(), ident.end(), 0);
-    upload(t.d_tile_order, ident);
-    upload(t.d_tile_cost, zero);
-  }
-  upload(t.d_rel, g->rel);
-  upload(t.d_csr_begin, csr_begin);
-  upload(t.d_csr_items, items);
-  upload(t.d_block_mask, block_mask);
-  upload(t.d_block_nodes, block_nodes);
-  upload(t.d_red_offset, red);
-  upload(t.d_x, g->x);
-  dmalloc(t.d_unit_bounds, sizeof(float4) * (size_t)n_units);
-  if (rc == VGX_OK && g->n_tiles > 0) {
-    vgx_launch_reg_unit_bounds(st, t.d_tiles.get(), g->n_tiles, t.d_unit_bounds.get());
-    c->launches++;
-    check(cudaGetLastError());
-  }
-  dmalloc(t.d_poses, sizeof(RegPoseConst) * g->n_local);
-  dmalloc(t.d_partials, sizeof(double) * VGX_REG_NSTRIDE * (size_t)g->n_tiles);
-  dmalloc(t.d_csum, sizeof(double) * VGX_REG_NSTRIDE * (size_t)g->n_local);
-  dmalloc(t.d_xc, sizeof(double) * 4 * N);
-  dmalloc(t.d_packed[0], sizeof(double) * g->packed_len);
-  dmalloc(t.d_packed[1], sizeof(double) * g->packed_len);
-  dmalloc(t.d_A, sizeof(double) * (size_t)(n + 1) * (n + 1));
-  dmalloc(t.d_scale, sizeof(double) * n);
-  dmalloc(t.d_diag, sizeof(double) * n);
-  dmalloc(t.d_gs, sizeof(double) * n);
-  dmalloc(t.d_step, sizeof(double) * n);
-  dmalloc(t.d_state, sizeof(LmState));
-  if (rc == VGX_OK && !g->h_state.get()) rc = g->h_state.alloc(c, sizeof(LmState), what, VGX_ERR_NOMEM);
-  dmalloc(t.d_snap, 2 * sizeof(LmState));
-  if (rc == VGX_OK && !g->h_snap.get()) rc = g->h_snap.alloc(c, 2 * sizeof(LmState), what, VGX_ERR_NOMEM);
-  if (rc == VGX_OK && g->h_x.bytes() < sizeof(double) * 4 * (size_t)N)
-    rc = g->h_x.alloc(c, sizeof(double) * 4 * (size_t)std::max(2 * N, 64), what, VGX_ERR_NOMEM);
-  if (rc == VGX_OK && !g->copy_stream) {
-    check(cudaStreamCreateWithFlags(&g->copy_stream, cudaStreamNonBlocking));
-    for (int k = 0; k < 2 && rc == VGX_OK; ++k) {
-      check(cudaEventCreateWithFlags(&g->ev_iter[k], cudaEventDisableTiming));
-      check(cudaEventCreateWithFlags(&g->ev_copy[k], cudaEventDisableTiming));
-    }
-  }
-  if (rc == VGX_OK) check(cudaStreamSynchronize(st));
-  if (rc != VGX_OK) {
-    g->dev = VgxGraphTables();
-    return rc;
-  }
+  const char* tile_units = getenv("VGX_REG_HW_TILE_UNITS");
+  VgxGraphPlan plan = vgx_graph_plan(facts, owner, rel, g->N, g->constant, c->rank, sms,
+                                     tile_units ? atoi(tile_units) : 0);
+  // ---- upload
+  VgxGraphTables t;
+  VGX_TRY(upload_tables(c, g, plan, all, is_sampled, sms, t));
+  g->plan = std::move(plan);
+  g->dev = std::move(t);
   g->dirty = false;
   return VGX_OK;
 }
@@ -584,27 +484,29 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
 int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, bool jacobian, bool exclude_reg,
                  const int* skip) {
   cudaStream_t st = c->stream;
-  const bool do_reg = !exclude_reg && g->n_local > 0;
+  const VgxGraphPlan& plan = g->plan;
+  VgxGraphTables& dev = g->dev;
+  const bool do_reg = !exclude_reg && plan.n_local() > 0;
   if (do_reg) {
     // refresh the longest-first tile order from the cost measured by the previous evaluation: before
     // the second evaluation on new tables, then every 32nd (the poses move little inside a solve)
-    if (g->n_tiles > 1 && (g->evals_since_order == -2 || g->evals_since_order >= 32)) {
+    if (plan.n_tiles() > 1 && (dev.evals_since_order == -2 || dev.evals_since_order >= 32)) {
       VgxLaunchScope s(c, VGX_SLOT_OTHER);
-      vgx_launch_reg_order(st, g->dev.d_tile_cost.get(), g->n_tiles, g->dev.d_tile_order.get());
-      g->evals_since_order = 0;
+      vgx_launch_reg_order(st, dev.d_tile_cost.get(), plan.n_tiles(), dev.d_tile_order.get());
+      dev.evals_since_order = 0;
     }
-    if (g->evals_since_order >= 0) ++g->evals_since_order;
+    if (dev.evals_since_order >= 0) ++dev.evals_since_order;
     {
       VgxLaunchScope s(c, VGX_SLOT_REG_POSE_SETUP);
-      vgx_launch_reg_pose_setup(st, g->dev.d_cons.get(), d_x, g->dev.d_poses.get(), g->n_local, skip);
+      vgx_launch_reg_pose_setup(st, dev.d_cons.get(), d_x, dev.d_poses.get(), plan.n_local(), skip);
     }
     {
       VgxLaunchScope s(c, VGX_SLOT_REG_REDUCE);
-      vgx_launch_reg_reduce(st, g->dev.d_cons.get(), g->dev.d_poses.get(), g->dev.d_tiles.get(), g->n_tiles,
-                            g->dev.d_tile_order.get(), g->dev.d_tile_cost.get(), g->dev.d_partials.get(),
-                            g->grid_capacity, g->dev.d_unit_bounds.get(), jacobian, skip);
+      vgx_launch_reg_reduce(st, dev.d_cons.get(), dev.d_poses.get(), dev.d_tiles.get(), plan.n_tiles(),
+                            dev.d_tile_order.get(), dev.d_tile_cost.get(), dev.d_partials.get(), plan.grid_capacity,
+                            dev.d_unit_bounds.get(), jacobian, skip);
     }
-    if (g->evals_since_order < 0) g->evals_since_order = -2;   // a cost has been measured now
+    if (dev.evals_since_order < 0) dev.evals_since_order = -2;   // a cost has been measured now
   }
   // multi-rank peer path: the assembly pushes this rank's partial into every rank's region
   const bool p2p = c->nranks > 1 && c->p2p_ready;
@@ -620,48 +522,39 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
   const int excl = do_reg ? 0 : 1;
   if (do_reg) {
     RegSums sums;
-    sums.partials = g->dev.d_partials.get(); sums.tile_begin = g->dev.d_tile_begin.get();
-    sums.cons = g->dev.d_cons.get();
+    sums.partials = dev.d_partials.get(); sums.tile_begin = dev.d_tile_begin.get();
+    sums.cons = dev.d_cons.get();
     VgxLaunchScope s(c, VGX_SLOT_REG_SUMS);
-    L.cfg.gridDim = dim3((unsigned)((g->n_local + 3) / 4));
-    cudaLaunchKernelEx(&L.cfg, reg_csum_kernel, sums, g->n_local, g->dev.d_csum.get(), skip);
+    L.cfg.gridDim = dim3((unsigned)((plan.n_local() + 3) / 4));
+    cudaLaunchKernelEx(&L.cfg, reg_csum_kernel, sums, plan.n_local(), dev.d_csum.get(), skip);
   }
   if (p2p) {
-    VGX_TRY(vgx_p2p_begin(c, g->packed_len, &push, &gat));
+    VGX_TRY(vgx_p2p_begin(c, plan.packed_len, &push, &gat));
   }
-  if (p2p && c->p2p_fused && g->packed_len < (size_t)INT_MAX) {
+  if (p2p && c->p2p_fused && plan.packed_len < (size_t)INT_MAX) {
     // one launch: assemble + push -> signal -> wait -> local reduce (grid fully co-resident)
-    static int resident = 0;
-    if (resident == 0) {
-      int sms = 0, per_sm = 0;
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device);
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, assemble_exchange_kernel, 128, 0) != cudaSuccess)
-        per_sm = 1;
-      resident = std::max(1, sms * std::max(per_sm, 1));
-    }
-    const int grid = std::min(g->N + g->E + 1, resident);
     {
       VgxLaunchScope s(c, VGX_SLOT_ASSEMBLY);
-      L.cfg.gridDim = dim3((unsigned)grid);
-      cudaLaunchKernelEx(&L.cfg, assemble_exchange_kernel, (const double*)g->dev.d_csum.get(),
-                         (const VgxRelEdge*)g->dev.d_rel.get(), d_x, (const int*)g->dev.d_csr_begin.get(),
-                         (const int4*)g->dev.d_csr_items.get(), push, g->N, g->E, g->n_local,
-                         g->n_rel_local, excl, gat, d_packed, (int)g->packed_len, skip,
-                         (const unsigned char*)g->dev.d_block_mask.get());
+      L.cfg.gridDim = dim3((unsigned)dev.exchange_grid);
+      cudaLaunchKernelEx(&L.cfg, assemble_exchange_kernel, (const double*)dev.d_csum.get(),
+                         (const VgxRelEdge*)dev.d_rel.get(), d_x, (const int*)dev.d_csr_begin.get(),
+                         (const int4*)dev.d_csr_items.get(), push, g->N, plan.E, plan.n_local(), plan.n_rel_local,
+                         excl, gat, d_packed, (int)plan.packed_len, skip,
+                         (const unsigned char*)dev.d_block_mask.get());
     }
     VGX_CUDA(c, cudaGetLastError());
     return VGX_OK;
   }
   {
     VgxLaunchScope s(c, VGX_SLOT_ASSEMBLY);
-    L.cfg.gridDim = dim3((unsigned)(g->N + g->E + 1));
-    cudaLaunchKernelEx(&L.cfg, assemble_kernel, (const double*)g->dev.d_csum.get(),
-                       (const VgxRelEdge*)g->dev.d_rel.get(), d_x, (const int*)g->dev.d_csr_begin.get(),
-                       (const int4*)g->dev.d_csr_items.get(), push, g->N, g->E, g->n_local, g->n_rel_local, excl, skip);
+    L.cfg.gridDim = dim3((unsigned)(g->N + plan.E + 1));
+    cudaLaunchKernelEx(&L.cfg, assemble_kernel, (const double*)dev.d_csum.get(), (const VgxRelEdge*)dev.d_rel.get(),
+                       d_x, (const int*)dev.d_csr_begin.get(), (const int4*)dev.d_csr_items.get(), push, g->N, plan.E,
+                       plan.n_local(), plan.n_rel_local, excl, skip);
   }
   VGX_CUDA(c, cudaGetLastError());
-  if (p2p) return vgx_p2p_gather(c, gat, d_packed, g->packed_len, g->dev.d_block_mask.get(), g->N);
-  return vgx_nccl_allreduce_sum_f64(c, d_packed, g->packed_len);
+  if (p2p) return vgx_p2p_gather(c, gat, d_packed, plan.packed_len, dev.d_block_mask.get(), g->N);
+  return vgx_nccl_allreduce_sum_f64(c, d_packed, plan.packed_len);
 }
 
 int prepare(vgx_ctx* c, VgxGraph** out) {
@@ -805,7 +698,7 @@ extern "C" int vgx_graph_num_registration_residuals(vgx_ctx* c, int64_t* local, 
   return vgx_entry(c, __func__, [&] {
     VgxGraph* g = nullptr;
     VGX_TRY(prepare(c, &g));
-    if (local) *local = g->residuals_local;
+    if (local) *local = g->plan.residuals_local;
     if (global) *global = g->residuals_global;
     return VGX_OK;
   });
@@ -840,9 +733,9 @@ extern "C" int vgx_graph_eval(vgx_ctx* c, int exclude_registration, double* cost
     VGX_TRY(prepare(c, &g));
     VGX_TRY(eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, exclude_registration != 0));
     double* h;
-    VGX_TRY(vgx_carve(c, c->h_pinned, vgx_part(h, g->packed_len)));
-    VGX_CUDA(c, cudaMemcpyAsync(h, g->dev.d_packed[0].get(), sizeof(double) * g->packed_len, cudaMemcpyDeviceToHost,
-                                c->stream));
+    VGX_TRY(vgx_carve(c, c->h_pinned, vgx_part(h, g->plan.packed_len)));
+    VGX_CUDA(c, cudaMemcpyAsync(h, g->dev.d_packed[0].get(), sizeof(double) * g->plan.packed_len,
+                                cudaMemcpyDeviceToHost, c->stream));
     VGX_CUDA(c, cudaStreamSynchronize(c->stream));
     const int N = g->N, dim = 4 * N;
     if (cost) *cost = h[0];
@@ -854,8 +747,8 @@ extern "C" int vgx_graph_eval(vgx_ctx* c, int exclude_registration, double* cost
       for (int i = 0; i < N; ++i)
         for (int r = 0; r < 4; ++r)
           for (int q = 0; q < 4; ++q) H[(size_t)(4 * i + r) * dim + 4 * i + q] = D[16 * (size_t)i + 4 * r + q];
-      const std::vector<int>& bn = g->block_nodes;
-      for (int b = 0; b < g->E; ++b) {
+      const std::vector<int>& bn = g->plan.block_nodes;
+      for (int b = 0; b < g->plan.E; ++b) {
         const int i = bn[2 * b], j = bn[2 * b + 1];
         for (int r = 0; r < 4; ++r)
           for (int q = 0; q < 4; ++q) {
@@ -879,14 +772,14 @@ extern "C" int vgx_graph_registration_costs(vgx_ctx* c, double* per_constraint) 
     VGX_TRY(prepare(c, &g));
     if (!per_constraint) return VGX_ERR_INVALID;
     VGX_TRY(eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[1].get(), false, false));
-    const int P = (int)g->reg_ref.size();
-    std::vector<double> cs((size_t)g->n_local * VGX_REG_NSTRIDE + 1);
-    if (g->n_local > 0)
-      VGX_CUDA(c, cudaMemcpyAsync(cs.data(), g->dev.d_csum.get(), sizeof(double) * VGX_REG_NSTRIDE * g->n_local,
+    const int P = (int)g->reg_ref.size(), n_local = g->plan.n_local();
+    std::vector<double> cs((size_t)n_local * VGX_REG_NSTRIDE + 1);
+    if (n_local > 0)
+      VGX_CUDA(c, cudaMemcpyAsync(cs.data(), g->dev.d_csum.get(), sizeof(double) * VGX_REG_NSTRIDE * n_local,
                                   cudaMemcpyDeviceToHost, c->stream));
     VGX_CUDA(c, cudaStreamSynchronize(c->stream));
     for (int i = 0; i < P; ++i) per_constraint[i] = 0.0;
-    for (int k = 0; k < g->n_local; ++k) per_constraint[g->local[k]] = cs[(size_t)k * VGX_REG_NSTRIDE + 20];
+    for (int k = 0; k < n_local; ++k) per_constraint[g->plan.local[k]] = cs[(size_t)k * VGX_REG_NSTRIDE + 20];
     return VGX_OK;
   });
 }

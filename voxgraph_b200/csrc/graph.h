@@ -1,13 +1,8 @@
 // Pose-graph state shared by the evaluation pipeline (graph.cu) and the dense solver (solve.cu).
 #pragma once
 
+#include "graph_plan.h"
 #include "registration_kernels.h"
-
-// Packed normal equations, the output of one evaluation (doubles):
-//   [PACK_HDR header: [0] cost, [1..3] reserved | 4 N gradient, node-major |
-//    16 N diagonal 4x4 blocks, row-major, node order |
-//    16 E off-diagonal 4x4 blocks, row-major: rows node block_nodes[2b] (the smaller index), cols block_nodes[2b + 1]]
-#define PACK_HDR 4
 
 struct LmState {
   double radius, decrease_factor;
@@ -18,7 +13,8 @@ struct LmState {
   int termination, done, accepted, step_valid, scale_ready;
 };
 
-// The device buffers of one table build: all of them are released when the tables are rebuilt.
+// The device buffers of one table build, and the state that belongs to them: all of it is released when the
+// tables are rebuilt.
 struct VgxGraphTables {
   VgxBuffer<RegConstraintDev> d_cons;
   VgxBuffer<RegPoseConst> d_poses;
@@ -47,6 +43,8 @@ struct VgxGraphTables {
   VgxBuffer<LmState> d_snap;    // [2] outcome of iteration k (written by lm_decide), parity k & 1
   VgxBuffer<float> d_sample_pts;   // gathered unit-major points of the local sampled blocks
   VgxBuffer<int32_t> d_sample_idx;
+  int evals_since_order = -1;   // -1: no cost measured yet since the tables were built
+  int exchange_grid = 0;        // CTAs of the fused assembly and exchange: all co-resident on this device
 };
 
 struct VgxGraph {
@@ -62,19 +60,10 @@ struct VgxGraph {
   std::vector<std::vector<int32_t>> sample_override; // vgx_graph_set_sample_indices
   bool dirty = true;
 
-  // derived
-  std::vector<int> local;  // global indices of this rank's registration constraints
-  std::vector<int> block_nodes;  // E x 2 (host copy)
-  std::vector<int> red;    // N: reduced offset or -1 (host copy of d_red_offset)
-  int n_local = 0, n_tiles = 0, n_rel_local = 0, grid_capacity = 0;
-  int E = 0;               // off-diagonal blocks
-  int n_free = 0;          // reduced dimension 4 * (non-constant nodes)
-  int64_t residuals_local = 0, residuals_global = 0;
-  bool zero_weight = false;
-  size_t packed_len = 0;
-  int evals_since_order = -1;   // -1: no cost measured yet since the tables were built
-
-  // device
+  // derived, by the table build
+  bool zero_weight = false;       // some registration constraint has no points or zero weight
+  int64_t residuals_global = 0;
+  VgxGraphPlan plan;              // the layout, host copy
   VgxGraphTables dev;
   // pinned; they outlive the tables: a page-locked allocation costs ~0.2 ms
   VgxBuffer<LmState> h_state{VgxMem::pinned};

@@ -1,6 +1,7 @@
 // Host-visible declarations of the registration kernels (registration.cu).
 #pragma once
 
+#include "graph_plan.h"   // the tile constants
 #include "vgx_internal.h"
 
 struct RegConstraintDev;
@@ -8,12 +9,7 @@ struct RegPoseConst;
 
 #define VGX_REG_THREADS 128        // 4 warps per CTA, each with its own TMA ring + software pipeline
 #define VGX_REG_MIN_BLOCKS 8       // resident CTAs per SM the register budget is sized for (64 registers)
-#define VGX_REG_TILE_SLOTS_PER_SM 7  // CTA slots per SM the tile size is cut for (graph.cu).  A fixed count,
-                                     // not the resident one: the tiles, and with them the last bits of every
-                                     // sum, do not follow the occupancy (7 CTAs per SM when the rule was set)
 #define VGX_REG_RING 4             // point-slice ring slots per warp (units in flight = RING - 1)
-#define VGX_REG_HW_TILE_UNITS 64   // largest tile, in units (graph.cu makes them smaller on small problems)
-#define VGX_REG_UNIT 32            // points per unit = one warp iteration; tiles are cut on unit boundaries
 #define VGX_REG_NSUM 21            // 15 (upper 5x5) + 5 (gradient) + 1 (cost)
 #define VGX_REG_NSTRIDE 24
 

@@ -671,10 +671,10 @@ static cudaError_t launch_chol_coop(cudaStream_t st, int grid, double* A, int n,
 // lm_build_kernel + lm_persist_kernel on the normal equations in d_packed[0]
 static void enqueue_lm_build(cudaStream_t st, VgxGraph* g, int n, const LmOpts& lo) {
   const int N = g->N;
-  const int nthreads = std::max(16 * (N + g->E), 4 * N);
+  const int nthreads = std::max(16 * (N + g->plan.E), 4 * N);
   lm_build_kernel<<<std::min(296, (nthreads + 255) / 256), 256, 0, st>>>(
-      g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), g->dev.d_block_nodes.get(), N, g->E, n, g->dev.d_A.get(),
-      g->dev.d_scale.get(), g->dev.d_diag.get(), g->dev.d_gs.get(), g->dev.d_state.get(), lo);
+      g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), g->dev.d_block_nodes.get(), N, g->plan.E, n,
+      g->dev.d_A.get(), g->dev.d_scale.get(), g->dev.d_diag.get(), g->dev.d_gs.get(), g->dev.d_state.get(), lo);
   lm_persist_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), N, g->dev.d_scale.get(),
                                        g->dev.d_diag.get(), g->dev.d_state.get(), lo);
 }
@@ -744,8 +744,8 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
     if (m < 0 || (m > 0 && (!ids_a || !ids_b || !cov))) return VGX_ERR_INVALID;
     if (m == 0) return VGX_OK;
     if (g->zero_weight) VGX_FAIL(c, VGX_ZERO_WEIGHT, "a registration constraint has zero summed weight (Evaluate == false)");
-    const int N = g->N, n = g->n_free;
-    const std::vector<int>& red = g->red;
+    const int N = g->N, n = g->plan.n_free;
+    const std::vector<int>& red = g->plan.red;
     // distinct columns: the 4 parameters of every second node that is free
     std::vector<int> col_of(N, -1), cols;
     std::vector<std::pair<int, int>> pr(m);
@@ -858,7 +858,7 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
     const bool excl = o->exclude_registration != 0;
     vgx_solver_summary S;
     memset(&S, 0, sizeof(S));
-    const int N = g->N, n = g->n_free;
+    const int N = g->N, n = g->plan.n_free;
     cudaStream_t st = c->stream;
     if (!excl && g->zero_weight) {
       S.termination = 6;
@@ -923,7 +923,7 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
         if (use_smem_chol) {
           chol_solve_smem_kernel<<<1, 512, smem_chol_bytes, st>>>(g->dev.d_A.get(), n, g->dev.d_step.get(),
                                                                   g->dev.d_state.get(), g->dev.d_red_offset.get(),
-                                                                  g->dev.d_block_nodes.get(), N, g->E, d_chol_dbg);
+                                                                  g->dev.d_block_nodes.get(), N, g->plan.E, d_chol_dbg);
         } else {
           // LM: sign test only (as Eigen's LLT in the reference)
           VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->dev.d_A.get(), n, g->dev.d_state.get(), nullptr, 0.0));
@@ -943,8 +943,8 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
         lm_decide_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_packed[1].get(), g->dev.d_red_offset.get(),
                                             N, g->dev.d_x.get(), g->dev.d_xc.get(), g->dev.d_state.get(), lo, 1,
                                             g->dev.d_snap.get() + (k & 1));
-        lm_accept_kernel<<<std::max(1, std::min(64, (int)(g->packed_len / 2048))), 256, 0, st>>>(
-            g->dev.d_packed[1].get(), g->dev.d_packed[0].get(), g->packed_len, g->dev.d_state.get());
+        lm_accept_kernel<<<std::max(1, std::min(64, (int)(g->plan.packed_len / 2048))), 256, 0, st>>>(
+            g->dev.d_packed[1].get(), g->dev.d_packed[0].get(), g->plan.packed_len, g->dev.d_state.get());
       }
       VGX_CUDA(c, cudaGetLastError());
       // outcome of iteration k -> host, on the copy stream (the main stream keeps running ahead)
