@@ -50,6 +50,18 @@ __device__ __forceinline__ void dmma_8x8x4(double& d0, double& d1, double a, dou
                : "d"(a), "d"(b));
 }
 
+// Half of an octet through the read-only path, marked evict-first in L2.  The gathers are what the kernel spends
+// its HBM bandwidth on (asking L2 to fetch 128 or 256 bytes around each sector made a config 2 step 7 and 12 %
+// slower); the reading submap's view is far larger than L2 and its sectors are rarely met again before
+// they would be evicted, while the point units, block grids and descriptors are re-read by every tile of
+// their constraints.  Evict-first keeps the gathers from pushing those out.
+__device__ __forceinline__ float4 ldg_evict_first(const float4* p, uint64_t policy) {
+  float4 v;
+  asm volatile("ld.global.nc.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(policy));
+  return v;
+}
+
 #define VGX_STAGE_STRIDE 36  // doubles per component row (32 points + pad: 2-way = optimal for 8 B)
 
 // ---- TMA (1-D bulk copy) + mbarrier primitives, sm_90a PTX
@@ -270,16 +282,24 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
   }
   mbar_wait(tbar, 0);   // descriptor, pose block and grid have landed
   if (threadIdx.x == 0) s_clk0 = clock64();
+  // The tile's constants are read from shared memory once, here, into locals whose address is never
+  // taken.  Every ring wait below keeps its "memory" clobber, because it is what orders the reads of a
+  // ring slot after the bulk copy that filled it; but a clobber reaches only memory, so these values
+  // are not reloaded per unit.  They are the same for the whole CTA, and ptxas holds them in uniform
+  // registers, which the 64-register budget of __launch_bounds__ does not count.
+  const RegConstraintDev C = s_C;
   const RegPoseConst P = s_P;
-  const bool gram_always = s_C.no_corr != 0.0;  // r = w * no_correspondence_cost without a match
+  const bool gram_always = C.no_corr != 0.0;  // r = w * no_correspondence_cost without a match
   if (may_cull) {
-    live = __ballot_sync(0xffffffffu, lane < my_units && (gram_always || reg_unit_may_hit(s_C, P, s_grid, bnd)));
+    live = __ballot_sync(0xffffffffu, lane < my_units && (gram_always || reg_unit_may_hit(C, P, s_grid, bnd)));
     n_live = __popc(live);
 #pragma unroll
     for (int j = 0; j < kRing - 1; ++j)
       if (j < n_live) issue(it + j);
   }
   double d0 = 0.0, d1 = 0.0;
+  uint64_t octet_policy;
+  asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(octet_policy));
 
   // a lane without a correspondence carries an all-NaN octet
   struct Pipe { float4 lo, hi; float ox, oy, oz; };
@@ -291,7 +311,7 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
     const bool ok = vgx_octet_ok(d);
     if (gram_always || __any_sync(0xffffffffu, ok)) {
       const float xi = sp[0], yi = sp[32], dist = sp[96], w = sp[128];
-      const RegPointResult Q = vgx_reg_math<kJacobian>(s_C, P, xi, yi, dist, w, ok, d, R.ox, R.oy, R.oz);
+      const RegPointResult Q = vgx_reg_math<kJacobian>(C, P, xi, yi, dist, w, ok, d, R.ox, R.oy, R.oz);
       if (kJacobian) {
         stage_w[0 * VGX_STAGE_STRIDE] = (double)Q.jr[0];
         stage_w[1 * VGX_STAGE_STRIDE] = (double)Q.jr[1];
@@ -300,9 +320,11 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
         stage_w[4 * VGX_STAGE_STRIDE] = (double)Q.je3;
         stage_w[5 * VGX_STAGE_STRIDE] = Q.r;
         __syncwarp();
+        // lanes of groups 6 and 7 feed rows 6 and 7 of A with a copy of row 0: those rows reach only row
+        // and column 6 and 7 of the Gram matrix, which the epilogue never reads
 #pragma unroll
         for (int t4 = 0; t4 < 8; ++t4) {
-          const double a = (grp < 6) ? stage_r[4 * t4] : 0.0;
+          const double a = stage_r[4 * t4];
           dmma_8x8x4(d0, d1, a, a);
         }
       } else {
@@ -314,8 +336,16 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
 
   // The tile's pipeline, instantiated once per lookup path (use_grid is uniform across the CTA):
   // kGrid, the reading submap's block grid staged in shared memory, or its hash in global memory.
-  auto run_tile = [&](auto path) {
+  // kShift > 0 fixes the reading submap's brick at 2^kShift voxels per side, so that the voxel clamp,
+  // the block wrap and the octet address fold to constants; 0 reads the brick size from the descriptor.
+  auto run_tile = [&](auto path, auto brick) {
     constexpr bool kGrid = decltype(path)::value;
+    constexpr int kShift = decltype(brick)::value;
+    RegConstraintDev K = C;
+    if constexpr (kShift > 0) {
+      K.vps = 1 << kShift;
+      K.vps_shift = kShift;
+    }
     // stage A: everything up to the ISSUE of the octet load
     auto stage_a = [&](uint32_t seq, Pipe& R) {
       const uint32_t slot = seq % kRing;
@@ -328,32 +358,32 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
       R.hi = R.lo;
       R.ox = R.oy = R.oz = 0.f;
       int b0, b1, b2;
-      vgx_block_index(s_C, p0, p1, p2, b0, b1, b2);
+      vgx_block_index(K, p0, p1, p2, b0, b1, b2);
       RegLocate L;
       int slot_b;
       if constexpr (kGrid) {
         // getVoxelsAndQVector fails right away when the block that contains pos does not exist;
         // overlapping submaps share only part of their surface and consecutive points are
         // spatially coherent: most warps miss with all 32 lanes and skip the rest of the unit
-        const int slot_c = vgx_grid_slot(s_C, s_grid, b0, b1, b2);
+        const int slot_c = vgx_grid_slot(K, s_grid, b0, b1, b2);
         if (!__any_sync(0xffffffffu, slot_c >= 0)) return;
-        vgx_locate_in_block(s_C, p0, p1, p2, b0, b1, b2, L);
+        vgx_locate_in_block(K, p0, p1, p2, b0, b1, b2, L);
         // the base corner lies in another block only when it moved into a lower neighbour
         const bool moved = (L.b0 != b0) | (L.b1 != b1) | (L.b2 != b2);
-        const int slot_m = moved ? vgx_grid_slot(s_C, s_grid, L.b0, L.b1, L.b2) : slot_c;
+        const int slot_m = moved ? vgx_grid_slot(K, s_grid, L.b0, L.b1, L.b2) : slot_c;
         slot_b = slot_c >= 0 ? slot_m : -1;
       } else {
         vgx_probe_range(b0, b1, b2);
-        vgx_locate_in_block(s_C, p0, p1, p2, b0, b1, b2, L);
-        RegProbe H = vgx_probe_start(s_C, L);
-        slot_b = vgx_resolve(s_C, H);
+        vgx_locate_in_block(K, p0, p1, p2, b0, b1, b2, L);
+        RegProbe H = vgx_probe_start(K, L);
+        slot_b = vgx_resolve(K, H);
       }
       R.ox = L.ox; R.oy = L.oy; R.oz = L.oz;
       if (slot_b >= 0) {
-        const float4* o = reinterpret_cast<const float4*>(s_C.view) +
-                          2 * (((size_t)slot_b << (3 * s_C.vps_shift)) + (size_t)L.lin);
+        const float4* o = reinterpret_cast<const float4*>(K.view) +
+                          2 * (((size_t)slot_b << (3 * K.vps_shift)) + (size_t)L.lin);
         // the whole 32-byte octet = one sector = two 128-bit loads (sm_90 has no 256-bit LDG)
-        R.lo = __ldg(o); R.hi = __ldg(o + 1);
+        R.lo = ldg_evict_first(o, octet_policy); R.hi = ldg_evict_first(o + 1, octet_policy);
       }
     };
     // two register sets alternate (loop unrolled by two): the in-flight octet is never copied
@@ -370,9 +400,11 @@ reg_reduce_kernel(const RegConstraintDev* __restrict__ constraints,
     }
     if (j < n_live) stage_b(it++, Ra);
   };
+  // 16 voxels per side: voxblox's default brick, which voxgraph and both bench workloads use
   if (n_live > 0) {
-    if (use_grid) run_tile(std::true_type());
-    else run_tile(std::false_type());
+    if (!use_grid) run_tile(std::false_type(), std::integral_constant<int, 0>());
+    else if (C.vps_shift == 4) run_tile(std::true_type(), std::integral_constant<int, 4>());
+    else run_tile(std::true_type(), std::integral_constant<int, 0>());
   }
   // ---- tile epilogue: warp Gram fragments -> 21 sums -> partials[tile]
   if (kJacobian) {
