@@ -50,12 +50,14 @@ const char* vgx_last_error(const vgx_ctx* ctx);
 void* vgx_ctx_stream(vgx_ctx* ctx);
 int vgx_ctx_synchronize(vgx_ctx* ctx);
 
-/* Kernel accounting: when enabled the library brackets each of its kernels with
- * CUDA events on the context stream and adds them to one slot, vgx_profile_get's `which`. */
+/* Kernel accounting: the library runs its kernels in regions, each of one slot (vgx_profile_get's `which`).
+ * A slot counts the launches inside its regions, a library sort counting as one launch; a launch outside
+ * every region counts in vgx_launch_count only.  When enabled the library also brackets each region with
+ * CUDA events on the context stream and adds its time to the slot. */
 enum VgxProfileSlotId {
   VGX_SLOT_REG_REDUCE = 0,       /* registration reduce kernel */
   VGX_SLOT_REG_EMIT = 1,         /* registration emit kernel */
-  VGX_SLOT_TSDF_INTEGRATE = 2,   /* TSDF integrate kernel */
+  VGX_SLOT_TSDF_INTEGRATE = 2,   /* TSDF integrate kernels (mode 0: count, scan, emit, sort and apply) */
   VGX_SLOT_TSDF_ALLOCATE = 3,    /* TSDF allocate kernel */
   VGX_SLOT_SOLVE = 4,            /* Cholesky / LM kernels */
   VGX_SLOT_OTHER = 5,            /* everything else */

@@ -15,6 +15,7 @@ import numpy as np
 import pytest
 
 import finish_exact as fx
+from collection_stream import field, varint
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 F32 = np.float32
@@ -52,6 +53,24 @@ def exists(ctx, sid):
     except api.VgxError as e:
         assert e.code == _lib.VGX_ERR_NOT_FOUND
         return False
+
+
+def layer_stream(vs, vps, idx, d, w, type_=b"tsdf", count=None, block_vps=None, trailing=b""):
+    """voxblox io::SaveLayer's stream: varint32 message count, LayerProto, one BlockProto per block (unpacked
+    voxel_data, colour 0)."""
+    bs = F32(vs) * F32(vps)
+    head = field(1, "d", float(vs)) + field(2, "v", int(vps)) + field(3, "L", type_)
+    body = b""
+    for b in range(len(idx)):
+        bvps = block_vps if (block_vps is not None and b == 0) else vps
+        blk = field(1, "v", int(bvps)) + field(2, "d", float(vs))
+        blk += b"".join(field(3 + a, "d", float(F32(idx[b][a]) * bs)) for a in range(3)) + field(6, "v", 1)
+        words = np.stack([np.asarray(d[b], F32).view(np.uint32), np.asarray(w[b], F32).view(np.uint32),
+                          np.zeros(vps ** 3, np.uint32)], -1).reshape(-1)
+        blk += b"".join(b"\x38" + varint(int(x)) for x in words)
+        body += varint(len(blk)) + blk
+    n = 1 + len(idx) if count is None else count
+    return varint(n) + varint(len(head)) + head + body + trailing
 
 
 def yaw_T(yaw, t=(0.0, 0.0, 0.0)):

@@ -17,9 +17,8 @@ import pytest
 import finish_exact as fx
 import rmse_exact as rx
 import transform_oracle as to
-from collection_stream import field, varint
 from finish_exact import MATRIX
-from support import IDENTITY, ctx, exists, poses_for, same_bits, yaw_T  # noqa: F401
+from support import IDENTITY, ctx, exists, layer_stream, poses_for, same_bits, yaw_T  # noqa: F401
 from voxgraph_b200 import _lib, synth
 
 pytestmark = pytest.mark.gpu
@@ -34,24 +33,6 @@ def _no_scratch(ctx):
 
 
 # ---------------------------------------------------------------- layer files
-def layer_stream(vs, vps, idx, d, w, type_=b"tsdf", count=None, block_vps=None, trailing=b""):
-    """voxblox io::SaveLayer's stream: varint32 message count, LayerProto, one BlockProto per block (unpacked
-    voxel_data, colour 0)."""
-    bs = F32(vs) * F32(vps)
-    head = field(1, "d", float(vs)) + field(2, "v", int(vps)) + field(3, "L", type_)
-    body = b""
-    for b in range(len(idx)):
-        bvps = block_vps if (block_vps is not None and b == 0) else vps
-        blk = field(1, "v", int(bvps)) + field(2, "d", float(vs))
-        blk += b"".join(field(3 + a, "d", float(F32(idx[b][a]) * bs)) for a in range(3)) + field(6, "v", 1)
-        words = np.stack([np.asarray(d[b], F32).view(np.uint32), np.asarray(w[b], F32).view(np.uint32),
-                          np.zeros(vps ** 3, np.uint32)], -1).reshape(-1)
-        blk += b"".join(b"\x38" + varint(int(x)) for x in words)
-        body += varint(len(blk)) + blk
-    n = 1 + len(idx) if count is None else count
-    return varint(n) + varint(len(head)) + head + body + trailing
-
-
 def _layer(seed=0, vs=0.1, vps=8, nan=True):
     lay = fx.layer((vs, vps), "box", ["tilted", "sphere", "plane", "noise"][seed % 4], seed=seed)
     d, w = lay[3].copy(), lay[4].copy()

@@ -82,14 +82,17 @@ def test_rank_threshold_separates_gauge_freedom_from_anchored_chains(oracle):
     assert worst_anchored >= tau * 1e3, worst_anchored
 
 
-def test_dispatch_sizes_follow_the_source():
+def test_dispatch_sizes_and_cooperative_launches_follow_the_source():
     """The GPU size lists straddle solve.cu's one dispatch: the last LM size solved in shared memory
     and the first on the cooperative grid.  The covariances always factor on the cooperative grid;
-    their sizes cross a CH_NB panel edge.  Moving a limit in solve.cu fails this until the sizes move."""
+    their sizes cross a CH_NB panel edge.  Moving a limit in solve.cu fails this until the sizes move.
+    chol_coop_kernel is launched in two places, both cooperative on the grid chol_dispatch sized."""
     src = _solve_src()
     assert len(re.findall(r"static int chol_dispatch\(", src)) == 1
     assert len(re.findall(r"cudaOccupancyMaxActiveBlocksPerMultiprocessor\(&per_sm, chol_coop_kernel,", src)) == 1
-    assert len(re.findall(r"cudaLaunchCooperativeKernel\(", src)) == 1
+    # the covariances' launch and the LM's
+    assert len(re.findall(r"vgx_launch\(c, chol_coop_kernel,", src)) == 2
+    assert len(re.findall(r"vgx_launch\(c, chol_coop_kernel, coop_grid, 256, 0, VgxLaunch::cooperative,", src)) == 2
     assert re.findall(r"chol_dispatch\(c, n, (true|false),", src) == ["false", "true"], \
         "the covariances (first) must not take the shared-memory solver, the LM (second) may"
     m = re.findall(r"const size_t smem_chol_bytes = sizeof\(double\) \* \(\(size_t\)\(n \+ 1\) \* \(n \+ 2\) / 2 \+ n \+ 2\);", src)

@@ -141,11 +141,9 @@ static int cloud_decode_launch(vgx_ctx* c, const vgx_cloud_layout& L, const uint
   P.stage_bytes = L.point_step <= CLOUD_STAGE_STEP ? 32 * L.point_step + 32 : 0;
   P.colour_max = colour_max;
   VGX_CUDA(c, cudaMemcpyAsync(d_raw, data, (size_t)L.height * L.row_step, cudaMemcpyHostToDevice, c->stream));
-  VgxLaunchScope scope(c, VGX_SLOT_CLOUD_DECODE);
-  cloud_decode_kernel<<<(P.n_warps + CLOUD_WARPS - 1) / CLOUD_WARPS, CLOUD_WARPS * 32, CLOUD_WARPS * (size_t)P.stage_bytes,
-                        c->stream>>>(P, d_raw, d_pts, d_rgba, d_flags, d_kept);
-  VGX_CUDA(c, cudaGetLastError());
-  return VGX_OK;
+  VgxProfileScope scope(c, VGX_SLOT_CLOUD_DECODE);
+  return vgx_launch(c, cloud_decode_kernel, (P.n_warps + CLOUD_WARPS - 1) / CLOUD_WARPS, CLOUD_WARPS * 32,
+                    CLOUD_WARPS * (size_t)P.stage_bytes, VgxLaunch::plain, P, d_raw, d_pts, d_rgba, d_flags, d_kept);
 }
 
 extern "C" int vgx_cloud_decode(vgx_ctx* c, const vgx_cloud_layout* L, const uint8_t* data, uint64_t n_bytes,
@@ -170,12 +168,11 @@ extern "C" int vgx_cloud_decode(vgx_ctx* c, const vgx_cloud_layout* L, const uin
     VGX_CUDA(c, cudaMemsetAsync(d_kept, 0, sizeof(*d_kept), stream));
     VGX_TRY(cloud_decode_launch(c, *L, data, colour_max, d_raw, d_pts, d_rgba, d_flags, d_kept));
     {
-      VgxLaunchScope scope(c, VGX_SLOT_CLOUD_DECODE);
+      VgxProfileScope scope(c, VGX_SLOT_CLOUD_DECODE);
       VGX_TRY(vgx_exclusive_scan_u32(c, d_flags, d_offsets, (size_t)n, d_scan_tmp));
-      cloud_compact_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(n, d_pts, d_rgba, d_flags, d_offsets, d_out_pts,
-                                                                            d_out_rgba);
+      VGX_TRY(vgx_launch(c, cloud_compact_kernel, (unsigned)((n + 255) / 256), 256, 0, VgxLaunch::plain, n, d_pts, d_rgba,
+                         d_flags, d_offsets, d_out_pts, d_out_rgba));
     }
-    VGX_CUDA(c, cudaGetLastError());
     unsigned kept = 0;
     VGX_CUDA(c, cudaMemcpyAsync(&kept, d_offsets + n, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
     VGX_CUDA(c, cudaStreamSynchronize(stream));

@@ -806,7 +806,7 @@ static int decode_layout(vgx_ctx* c, const CollLayout& L, const uint8_t* bytes, 
   if (keep_colour && !L.submaps.empty())
     VGX_CUDA(c, cudaMemsetAsync(d_any, 0, sizeof(int) * L.submaps.size(), c->stream));
   {
-    VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
+    VgxProfileScope copies(c, VGX_SLOT_COLL_COPY);
     if (!L.blocks.empty())
       VGX_CUDA(c, cudaMemcpyAsync(d_regions, L.blocks.data(), L.blocks.size() * sizeof(CollBlockRef),
                                   cudaMemcpyHostToDevice, c->stream));
@@ -822,18 +822,17 @@ static int decode_layout(vgx_ctx* c, const CollLayout& L, const uint8_t* bytes, 
     if (s.n_blocks == 0) continue;
     if (keep_colour) VGX_TRY(vgx_submap_ensure_colour(c, sm));
     {
-      VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
+      VgxProfileScope copies(c, VGX_SLOT_COLL_COPY);
       VGX_CUDA(c, cudaMemcpyAsync(sm->d_block_idx.get(), L.block_idx.data() + 3 * s.first_block,
                                   sizeof(int32_t) * 3 * s.n_blocks, cudaMemcpyHostToDevice, c->stream));
     }
-    VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
-    collection_decode_kernel<<<s.n_blocks, COLL_THREADS, 0, c->stream>>>(
-        d_bytes, d_regions + s.first_block, vpb, reinterpret_cast<float*>(sm->d_dw.get()), sm->d_rgba.get(),
-        keep_colour ? d_any + k : nullptr, d_err);
+    VgxProfileScope scope(c, VGX_SLOT_COLL_CODEC);
+    VGX_TRY(vgx_launch(c, collection_decode_kernel, s.n_blocks, COLL_THREADS, 0, VgxLaunch::plain, d_bytes,
+                       d_regions + s.first_block, vpb, reinterpret_cast<float*>(sm->d_dw.get()), sm->d_rgba.get(),
+                       keep_colour ? d_any + k : nullptr, d_err));
   }
   int h_err = 0;
   std::vector<int> h_any(keep_colour ? L.submaps.size() : 0);
-  VGX_CUDA(c, cudaGetLastError());
   VGX_CUDA(c, cudaMemcpyAsync(&h_err, d_err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   if (!h_any.empty())
     VGX_CUDA(c, cudaMemcpyAsync(h_any.data(), d_any, sizeof(int) * h_any.size(), cudaMemcpyDeviceToHost, c->stream));
@@ -849,7 +848,7 @@ static int decode_layout(vgx_ctx* c, const CollLayout& L, const uint8_t* bytes, 
   for (size_t k = 0; k < L.submaps.size(); ++k) {
     VgxSubmap* sm = c->find(L.submaps[k].id);
     if (keep_colour && !h_any[k]) sm->d_rgba.reset();   // all words zero: a colour-free submap (synchronised above)
-    VgxLaunchScope scope(c, VGX_SLOT_COLL_UPLOAD, 0);
+    VgxProfileScope scope(c, VGX_SLOT_COLL_UPLOAD);
     VGX_TRY(vgx_submap_upload_finish(c, sm));
   }
   return VGX_OK;
@@ -923,12 +922,11 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
         a.block_idx = s->d_block_idx.get();
         a.vox_per_block = s->vox_per_block;
         a.out_sizes = d_sizes + first;
-        VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
-        collection_encode_kernel<false><<<s->n_blocks, COLL_THREADS, 0, c->stream>>>(a);
+        VgxProfileScope scope(c, VGX_SLOT_COLL_CODEC);
+        VGX_TRY(vgx_launch(c, collection_encode_kernel<false>, s->n_blocks, COLL_THREADS, 0, VgxLaunch::plain, a));
       }
       first += (size_t)s->n_blocks;
     }
-    VGX_CUDA(c, cudaGetLastError());
     std::vector<uint32_t> sizes(total_blocks);
     if (total_blocks)
       VGX_CUDA(c, cudaMemcpyAsync(sizes.data(), d_sizes, total_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost,
@@ -961,7 +959,7 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
     VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_sizes, total_blocks), vgx_part(d_offs, total_blocks),
                       vgx_part(d_msgs, (size_t)dev_bytes)));
     if (total_blocks) {
-      VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
+      VgxProfileScope copies(c, VGX_SLOT_COLL_COPY);
       VGX_CUDA(c, cudaMemcpyAsync(d_sizes, sizes.data(), total_blocks * sizeof(uint32_t), cudaMemcpyHostToDevice,
                                   c->stream));
       VGX_CUDA(c, cudaMemcpyAsync(d_offs, offsets.data(), total_blocks * sizeof(uint64_t), cudaMemcpyHostToDevice,
@@ -979,13 +977,12 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
         a.block_size = s->block_size;
         a.sizes = d_sizes + first;
         a.offsets = d_offs + first;
-        VgxLaunchScope scope(c, VGX_SLOT_COLL_CODEC);
-        collection_encode_kernel<true><<<s->n_blocks, COLL_THREADS, 0, c->stream>>>(a);
+        VgxProfileScope scope(c, VGX_SLOT_COLL_CODEC);
+        VGX_TRY(vgx_launch(c, collection_encode_kernel<true>, s->n_blocks, COLL_THREADS, 0, VgxLaunch::plain, a));
       }
       first += (size_t)s->n_blocks;
     }
-    VGX_CUDA(c, cudaGetLastError());
-    VgxLaunchScope copies(c, VGX_SLOT_COLL_COPY, 0);
+    VgxProfileScope copies(c, VGX_SLOT_COLL_COPY);
     uint8_t* o = out;
     uint64_t dev_off = 0;
     memcpy(o, framing[0].data(), framing[0].size());

@@ -137,18 +137,17 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
     VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_fixed, nvox), vgx_part(d_nb, (size_t)27 * s->n_blocks),
                       vgx_part(d_changed, 1)));
     const unsigned grid = (unsigned)((nvox + 255) / 256);
-    esdf_init_kernel<<<grid, 256, 0, st>>>(P, s->d_dw.get(), s->d_esdf.get(), d_fixed);
-    esdf_neighbours_kernel<<<(27 * s->n_blocks + 127) / 128, 128, 0, st>>>(s->hash(), s->d_block_idx.get(), s->n_blocks,
-                                                                            d_nb);
-    c->launches += 2;
+    VGX_TRY(vgx_launch(c, esdf_init_kernel, grid, 256, 0, VgxLaunch::plain, P, s->d_dw.get(), s->d_esdf.get(), d_fixed));
+    VGX_TRY(vgx_launch(c, esdf_neighbours_kernel, (27 * s->n_blocks + 127) / 128, 128, 0, VgxLaunch::plain, s->hash(),
+                       s->d_block_idx.get(), s->n_blocks, d_nb));
     // relax to convergence: the flag is read back every other sweep
     int sweeps = 0;
     const int max_sweeps = 4 * (int)ceilf(dc.max_distance_m / s->voxel_size) + 16;
     for (;;) {
       VGX_CUDA(c, cudaMemsetAsync(d_changed, 0, sizeof(int), st));
       for (int k = 0; k < 2; ++k) {
-        esdf_sweep_kernel<<<grid, 256, 0, st>>>(P, s->d_esdf.get(), d_fixed, d_nb, d_changed);
-        c->launches++;
+        VGX_TRY(vgx_launch(c, esdf_sweep_kernel, grid, 256, 0, VgxLaunch::plain, P, s->d_esdf.get(), d_fixed, d_nb,
+                           d_changed));
         ++sweeps;
       }
       int changed = 0;
@@ -157,7 +156,6 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
       if (!changed) break;
       if (sweeps > max_sweeps) VGX_FAIL(c, VGX_ERR_INVALID, "relaxation did not converge");
     }
-    VGX_CUDA(c, cudaGetLastError());
     if (sweeps_out) *sweeps_out = sweeps;
     // registration view of the ESDF layer (observed <=> weight 1), same octet layout as the TSDF view
     VGX_TRY(s->d_view_esdf.alloc(c, sizeof(float) * 8 * nvox, "ESDF registration view"));

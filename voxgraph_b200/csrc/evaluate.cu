@@ -167,15 +167,15 @@ extern "C" int vgx_evaluate_layers_rmse(vgx_ctx* c, uint32_t gt_id, int gt_layer
       cudaStream_t st = c->stream;
       const int threads = std::min(RMSE_THREADS, g->vox_per_block);
       {
-        VgxLaunchScope scope(c, VGX_SLOT_EVAL);
-        rmse_block_kernel<<<(unsigned)n_part, threads, 0, st>>>(G, T, g->vox_per_block, d_part);
+        VgxProfileScope scope(c, VGX_SLOT_EVAL);
+        VGX_TRY(vgx_launch(c, rmse_block_kernel, (unsigned)n_part, threads, 0, VgxLaunch::plain, G, T, g->vox_per_block,
+                           d_part));
       }
-      VGX_CUDA(c, cudaGetLastError());
       {
-        VgxLaunchScope scope(c, VGX_SLOT_EVAL);
-        rmse_total_kernel<<<1, RMSE_THREADS, 0, st>>>(d_part, (int)n_part, d_part + n_part);
+        VgxProfileScope scope(c, VGX_SLOT_EVAL);
+        VGX_TRY(vgx_launch(c, rmse_total_kernel, 1, RMSE_THREADS, 0, VgxLaunch::plain, d_part, (int)n_part,
+                           d_part + n_part));
       }
-      VGX_CUDA(c, cudaGetLastError());
       VGX_CUDA(c, cudaMemcpyAsync(&total, d_part + n_part, sizeof(RmsePartial), cudaMemcpyDeviceToHost, st));
       VGX_CUDA(c, cudaStreamSynchronize(st));
     }

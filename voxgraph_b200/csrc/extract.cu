@@ -124,12 +124,10 @@ int vgx_exclusive_scan_u32(vgx_ctx* c, const unsigned* d_in, unsigned* d_out, si
     return VGX_OK;
   }
   const size_t tiles = (n + SCAN_TILE - 1) / SCAN_TILE;
-  scan_tile_kernel<<<(unsigned)tiles, SCAN_THREADS, 0, c->stream>>>(d_in, d_out, d_tmp, n);
-  scan_sums_kernel<<<1, 1024, 0, c->stream>>>(d_tmp, tiles, d_tmp + tiles);
-  scan_add_kernel<<<(unsigned)tiles, SCAN_THREADS, 0, c->stream>>>(d_out, d_tmp, n, d_tmp + tiles);
-  c->launches += 3;
-  VGX_CUDA(c, cudaGetLastError());
-  return VGX_OK;
+  VGX_TRY(vgx_launch(c, scan_tile_kernel, (unsigned)tiles, SCAN_THREADS, 0, VgxLaunch::plain, d_in, d_out, d_tmp, n));
+  VGX_TRY(vgx_launch(c, scan_sums_kernel, 1, 1024, 0, VgxLaunch::plain, d_tmp, tiles, d_tmp + tiles));
+  return vgx_launch(c, scan_add_kernel, (unsigned)tiles, SCAN_THREADS, 0, VgxLaunch::plain, d_out, d_tmp, n,
+                    d_tmp + tiles);
 }
 size_t vgx_scan_tmp_count(size_t n) { return (n + SCAN_TILE - 1) / SCAN_TILE + 2; }
 
@@ -335,8 +333,7 @@ static int install_points(vgx_ctx* c, VgxSubmap* s, int type, VgxBuffer<float>&&
   std::vector<float> w((size_t)n);
   float* d_w;
   VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_w, (size_t)n)));
-  gather_weights_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(d_pts.get(), n, d_w);
-  c->launches++;
+  VGX_TRY(vgx_launch(c, gather_weights_kernel, (n + 255) / 256, 256, 0, VgxLaunch::plain, d_pts.get(), n, d_w));
   VGX_CUDA(c, cudaMemcpyAsync(w.data(), d_w, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
   VGX_CUDA(c, cudaStreamSynchronize(c->stream));
   p.cumulative_w.resize((size_t)n);
@@ -398,18 +395,16 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
       const float inf = INFINITY;
       const float init[6] = {inf, inf, inf, -inf, -inf, -inf};
       VGX_CUDA(c, cudaMemcpyAsync(d_obb, init, sizeof(init), cudaMemcpyHostToDevice, st));
-      relevant_count_kernel<<<grid256, 256, 0, st>>>(L, f.min_voxel_weight, f.max_voxel_distance, d_counts);
-      c->launches++;
+      VGX_TRY(vgx_launch(c, relevant_count_kernel, grid256, 256, 0, VgxLaunch::plain, L, f.min_voxel_weight,
+                         f.max_voxel_distance, d_counts));
       VGX_TRY(vgx_exclusive_scan_u32(c, d_counts, d_offsets, nvox, d_tmp));
       unsigned total = 0;
       VGX_CUDA(c, cudaMemcpyAsync(&total, d_offsets + nvox, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
       VGX_CUDA(c, cudaStreamSynchronize(st));
       VgxBuffer<float> d_pts;
       VGX_TRY(alloc_points(c, (int)total, d_pts));
-      relevant_emit_kernel<<<grid256, 256, 0, st>>>(L, d_counts, d_offsets, f.use_esdf_distance ? s->d_esdf.get() : nullptr,
-                                                   d_pts.get(), d_obb);
-      c->launches++;
-      VGX_CUDA(c, cudaGetLastError());
+      VGX_TRY(vgx_launch(c, relevant_emit_kernel, grid256, 256, 0, VgxLaunch::plain, L, d_counts, d_offsets,
+                         f.use_esdf_distance ? s->d_esdf.get() : nullptr, d_pts.get(), d_obb));
       float obb[6];
       VGX_CUDA(c, cudaMemcpyAsync(obb, d_obb, sizeof(obb), cudaMemcpyDeviceToHost, st));
       VGX_CUDA(c, cudaStreamSynchronize(st));
@@ -422,8 +417,7 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
       const float min_weight = (float)f.min_voxel_weight;                 // cpp:211-212
       const float threshold = (float)(0.5 * (double)s->voxel_size);       // cpp:220
       const double threshold_inv = 1.0 / (double)threshold;               // createConnectedMesh
-      iso_count_kernel<<<grid128, 128, 0, st>>>(L, min_weight, d_counts);
-      c->launches++;
+      VGX_TRY(vgx_launch(c, iso_count_kernel, grid128, 128, 0, VgxLaunch::plain, L, min_weight, d_counts));
       VGX_TRY(vgx_exclusive_scan_u32(c, d_counts, d_offsets, nvox, d_tmp));
       unsigned M = 0;
       VGX_CUDA(c, cudaMemcpyAsync(&M, d_offsets + nvox, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
@@ -441,19 +435,19 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
         VGX_TRY(vgx_carve(c, c->d_work2, vgx_part(d_table, tsize), vgx_part(d_cand, (size_t)M * 3), vgx_part(d_key, M),
                           vgx_part(d_keep, (size_t)M + 1), vgx_part(d_koff, (size_t)M + 1), vgx_part(d_cdw, M),
                           vgx_part(d_tmp2, vgx_scan_tmp_count(M))));
-        iso_table_clear_kernel<<<(unsigned)((tsize + 255) / 256), 256, 0, st>>>(d_table, tsize);
-        iso_emit_kernel<<<grid128, 128, 0, st>>>(L, min_weight, threshold_inv, d_counts, d_offsets, d_cand, d_key,
-                                                d_table, tsize - 1);
-        iso_select_kernel<<<(M + 127) / 128, 128, 0, st>>>(L, d_cand, d_key, d_table, tsize - 1, M, d_keep, d_cdw);
-        c->launches += 3;
+        VGX_TRY(vgx_launch(c, iso_table_clear_kernel, (unsigned)((tsize + 255) / 256), 256, 0, VgxLaunch::plain, d_table,
+                           tsize));
+        VGX_TRY(vgx_launch(c, iso_emit_kernel, grid128, 128, 0, VgxLaunch::plain, L, min_weight, threshold_inv, d_counts,
+                           d_offsets, d_cand, d_key, d_table, tsize - 1));
+        VGX_TRY(vgx_launch(c, iso_select_kernel, (M + 127) / 128, 128, 0, VgxLaunch::plain, L, d_cand, d_key, d_table,
+                           tsize - 1, M, d_keep, d_cdw));
         VGX_TRY(vgx_exclusive_scan_u32(c, d_keep, d_koff, M, d_tmp2));
         VGX_CUDA(c, cudaMemcpyAsync(&kept, d_koff + M, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
         VGX_CUDA(c, cudaStreamSynchronize(st));
         VGX_TRY(alloc_points(c, (int)kept, d_pts));
         VGX_CUDA(c, cudaMemsetAsync(d_flags, 0, sizeof(unsigned) * (size_t)s->n_blocks, st));
-        iso_compact_kernel<<<(M + 127) / 128, 128, 0, st>>>(L, d_cand, d_cdw, d_keep, d_koff, M, d_pts.get(), d_flags);
-        c->launches++;
-        VGX_CUDA(c, cudaGetLastError());
+        VGX_TRY(vgx_launch(c, iso_compact_kernel, (M + 127) / 128, 128, 0, VgxLaunch::plain, L, d_cand, d_cdw, d_keep,
+                           d_koff, M, d_pts.get(), d_flags));
         // isosurface block list (slots, ascending) for overlapsWith
         std::vector<unsigned> flags((size_t)s->n_blocks);
         VGX_CUDA(c, cudaMemcpyAsync(flags.data(), d_flags, sizeof(unsigned) * (size_t)s->n_blocks,
@@ -513,8 +507,8 @@ extern "C" int vgx_submap_download_points(vgx_ctx* c, uint32_t id, int type, int
     const size_t n = (size_t)p.n;
     float *d_xyz, *d_d, *d_w;
     VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_xyz, 3 * n), vgx_part(d_d, n), vgx_part(d_w, n)));
-    unpack_points_kernel<<<(unsigned)((n + 255) / 256), 256, 0, c->stream>>>(p.data.get(), p.n, d_xyz, d_d, d_w);
-    c->launches++;
+    VGX_TRY(vgx_launch(c, unpack_points_kernel, (unsigned)((n + 255) / 256), 256, 0, VgxLaunch::plain, p.data.get(), p.n,
+                       d_xyz, d_d, d_w));
     if (xyz) VGX_CUDA(c, cudaMemcpyAsync(xyz, d_xyz, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     if (distance) VGX_CUDA(c, cudaMemcpyAsync(distance, d_d, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     if (weight) VGX_CUDA(c, cudaMemcpyAsync(weight, d_w, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));

@@ -346,8 +346,7 @@ static int upload_tables(vgx_ctx* c, VgxGraph* g, const VgxGraphPlan& plan, cons
       VGX_CUDA(c, cudaMemcpyAsync(t.d_sample_idx.get() + io, g->samples[i].data(), sizeof(int32_t) * cons[k].n,
                                   cudaMemcpyHostToDevice, st));
       float* dst = t.d_sample_pts.get() + uo * VGX_PT_UNIT_FLOATS;
-      vgx_launch_reg_gather_samples(st, p.data.get(), t.d_sample_idx.get() + io, cons[k].n, dst);
-      c->launches++;
+      VGX_TRY(vgx_launch_reg_gather_samples(c, p.data.get(), t.d_sample_idx.get() + io, cons[k].n, dst));
       cons[k].pts = dst;
       uo += ((size_t)cons[k].n + 31) / 32;
       io += (size_t)cons[k].n;
@@ -381,11 +380,7 @@ static int upload_tables(vgx_ctx* c, VgxGraph* g, const VgxGraphPlan& plan, cons
   VGX_TRY(table_upload(c, t.d_red_offset, plan.red));
   VGX_TRY(table_upload(c, t.d_x, g->x));
   VGX_TRY(table_alloc(c, t.d_unit_bounds, plan.n_units));
-  if (n_tiles > 0) {
-    vgx_launch_reg_unit_bounds(st, t.d_tiles.get(), n_tiles, t.d_unit_bounds.get());
-    c->launches++;
-    VGX_CUDA(c, cudaGetLastError());
-  }
+  VGX_TRY(vgx_launch_reg_unit_bounds(c, t.d_tiles.get(), n_tiles, t.d_unit_bounds.get()));
   VGX_TRY(table_alloc(c, t.d_poses, n_local));
   VGX_TRY(table_alloc(c, t.d_partials, VGX_REG_NSTRIDE * (size_t)n_tiles));
   VGX_TRY(table_alloc(c, t.d_csum, VGX_REG_NSTRIDE * (size_t)n_local));
@@ -483,7 +478,6 @@ static int build_tables(vgx_ctx* c, VgxGraph* g) {
 // ------------------------------------------------------------------ evaluation pipeline
 int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, bool jacobian, bool exclude_reg,
                  const int* skip) {
-  cudaStream_t st = c->stream;
   const VgxGraphPlan& plan = g->plan;
   VgxGraphTables& dev = g->dev;
   const bool do_reg = !exclude_reg && plan.n_local() > 0;
@@ -491,20 +485,20 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
     // refresh the longest-first tile order from the cost measured by the previous evaluation: before
     // the second evaluation on new tables, then every 32nd (the poses move little inside a solve)
     if (plan.n_tiles() > 1 && (dev.evals_since_order == -2 || dev.evals_since_order >= 32)) {
-      VgxLaunchScope s(c, VGX_SLOT_OTHER);
-      vgx_launch_reg_order(st, dev.d_tile_cost.get(), plan.n_tiles(), dev.d_tile_order.get());
+      VgxProfileScope s(c, VGX_SLOT_OTHER);
+      VGX_TRY(vgx_launch_reg_order(c, dev.d_tile_cost.get(), plan.n_tiles(), dev.d_tile_order.get()));
       dev.evals_since_order = 0;
     }
     if (dev.evals_since_order >= 0) ++dev.evals_since_order;
     {
-      VgxLaunchScope s(c, VGX_SLOT_REG_POSE_SETUP);
-      vgx_launch_reg_pose_setup(st, dev.d_cons.get(), d_x, dev.d_poses.get(), plan.n_local(), skip);
+      VgxProfileScope s(c, VGX_SLOT_REG_POSE_SETUP);
+      VGX_TRY(vgx_launch_reg_pose_setup(c, dev.d_cons.get(), d_x, dev.d_poses.get(), plan.n_local(), skip));
     }
     {
-      VgxLaunchScope s(c, VGX_SLOT_REG_REDUCE);
-      vgx_launch_reg_reduce(st, dev.d_cons.get(), dev.d_poses.get(), dev.d_tiles.get(), plan.n_tiles(),
-                            dev.d_tile_order.get(), dev.d_tile_cost.get(), dev.d_partials.get(), plan.grid_capacity,
-                            dev.d_unit_bounds.get(), jacobian, skip);
+      VgxProfileScope s(c, VGX_SLOT_REG_REDUCE);
+      VGX_TRY(vgx_launch_reg_reduce(c, dev.d_cons.get(), dev.d_poses.get(), dev.d_tiles.get(), plan.n_tiles(),
+                                    dev.d_tile_order.get(), dev.d_tile_cost.get(), dev.d_partials.get(),
+                                    plan.grid_capacity, dev.d_unit_bounds.get(), jacobian, skip));
     }
     if (dev.evals_since_order < 0) dev.evals_since_order = -2;   // a cost has been measured now
   }
@@ -518,41 +512,34 @@ int eval_enqueue(vgx_ctx* c, VgxGraph* g, const double* d_x, double* d_packed, b
   push.dst[0] = d_packed;
   // the assembly kernels and the constraint-sum kernel are launched as programmatic dependents of
   // what precedes them on the stream
-  VgxPdlLaunch L(st, dim3(1), dim3(128));
   const int excl = do_reg ? 0 : 1;
   if (do_reg) {
     RegSums sums;
     sums.partials = dev.d_partials.get(); sums.tile_begin = dev.d_tile_begin.get();
     sums.cons = dev.d_cons.get();
-    VgxLaunchScope s(c, VGX_SLOT_REG_SUMS);
-    L.cfg.gridDim = dim3((unsigned)((plan.n_local() + 3) / 4));
-    cudaLaunchKernelEx(&L.cfg, reg_csum_kernel, sums, plan.n_local(), dev.d_csum.get(), skip);
+    VgxProfileScope s(c, VGX_SLOT_REG_SUMS);
+    VGX_TRY(vgx_launch(c, reg_csum_kernel, (unsigned)((plan.n_local() + 3) / 4), 128, 0, VgxLaunch::pdl, sums,
+                       plan.n_local(), dev.d_csum.get(), skip));
   }
   if (p2p) {
     VGX_TRY(vgx_p2p_begin(c, plan.packed_len, &push, &gat));
   }
   if (p2p && c->p2p_fused && plan.packed_len < (size_t)INT_MAX) {
     // one launch: assemble + push -> signal -> wait -> local reduce (grid fully co-resident)
-    {
-      VgxLaunchScope s(c, VGX_SLOT_ASSEMBLY);
-      L.cfg.gridDim = dim3((unsigned)dev.exchange_grid);
-      cudaLaunchKernelEx(&L.cfg, assemble_exchange_kernel, (const double*)dev.d_csum.get(),
-                         (const VgxRelEdge*)dev.d_rel.get(), d_x, (const int*)dev.d_csr_begin.get(),
-                         (const int4*)dev.d_csr_items.get(), push, g->N, plan.E, plan.n_local(), plan.n_rel_local,
-                         excl, gat, d_packed, (int)plan.packed_len, skip,
-                         (const unsigned char*)dev.d_block_mask.get());
-    }
-    VGX_CUDA(c, cudaGetLastError());
-    return VGX_OK;
+    VgxProfileScope s(c, VGX_SLOT_ASSEMBLY);
+    return vgx_launch(c, assemble_exchange_kernel, (unsigned)dev.exchange_grid, 128, 0, VgxLaunch::pdl,
+                      (const double*)dev.d_csum.get(), (const VgxRelEdge*)dev.d_rel.get(), d_x,
+                      (const int*)dev.d_csr_begin.get(), (const int4*)dev.d_csr_items.get(), push, g->N, plan.E,
+                      plan.n_local(), plan.n_rel_local, excl, gat, d_packed, (int)plan.packed_len, skip,
+                      (const unsigned char*)dev.d_block_mask.get());
   }
   {
-    VgxLaunchScope s(c, VGX_SLOT_ASSEMBLY);
-    L.cfg.gridDim = dim3((unsigned)(g->N + plan.E + 1));
-    cudaLaunchKernelEx(&L.cfg, assemble_kernel, (const double*)dev.d_csum.get(), (const VgxRelEdge*)dev.d_rel.get(),
-                       d_x, (const int*)dev.d_csr_begin.get(), (const int4*)dev.d_csr_items.get(), push, g->N, plan.E,
-                       plan.n_local(), plan.n_rel_local, excl, skip);
+    VgxProfileScope s(c, VGX_SLOT_ASSEMBLY);
+    VGX_TRY(vgx_launch(c, assemble_kernel, (unsigned)(g->N + plan.E + 1), 128, 0, VgxLaunch::pdl,
+                       (const double*)dev.d_csum.get(), (const VgxRelEdge*)dev.d_rel.get(), d_x,
+                       (const int*)dev.d_csr_begin.get(), (const int4*)dev.d_csr_items.get(), push, g->N, plan.E,
+                       plan.n_local(), plan.n_rel_local, excl, skip));
   }
-  VGX_CUDA(c, cudaGetLastError());
   if (p2p) return vgx_p2p_gather(c, gat, d_packed, plan.packed_len, dev.d_block_mask.get(), g->N);
   return vgx_nccl_allreduce_sum_f64(c, d_packed, plan.packed_len);
 }

@@ -436,28 +436,27 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
   VGX_CUDA(c, cudaMemsetAsync(d_flag, 0, n_vox * sizeof(unsigned), st));
   const unsigned g128 = (unsigned)((n_vox + 127) / 128), g256 = (unsigned)((n_vox + 255) / 256);
   {
-    VgxLaunchScope scope(c, VGX_SLOT_MESH);
-    mesh_count_kernel<<<g128, 128, 0, st>>>(d_jobs, nj, n_vox, min_weight, d_cnt, d_flag);
+    VgxProfileScope scope(c, VGX_SLOT_MESH);
+    VGX_TRY(vgx_launch(c, mesh_count_kernel, g128, 128, 0, VgxLaunch::plain, d_jobs, nj, n_vox, min_weight, d_cnt,
+                       d_flag));
   }
   {
-    VgxLaunchScope scope(c, VGX_SLOT_MESH, 0);
-    c->prof[VGX_SLOT_MESH].launches += 3;
+    VgxProfileScope scope(c, VGX_SLOT_MESH);
     VGX_TRY(vgx_exclusive_scan_u32(c, d_cnt, d_toff, n_vox, d_tmp));
   }
   {
-    VgxLaunchScope scope(c, VGX_SLOT_MESH);
-    mesh_popc_kernel<<<g256, 256, 0, st>>>(d_flag, n_vox, d_cnt);
+    VgxProfileScope scope(c, VGX_SLOT_MESH);
+    VGX_TRY(vgx_launch(c, mesh_popc_kernel, g256, 256, 0, VgxLaunch::plain, d_flag, n_vox, d_cnt));
   }
   {
-    VgxLaunchScope scope(c, VGX_SLOT_MESH, 0);
-    c->prof[VGX_SLOT_MESH].launches += 3;
+    VgxProfileScope scope(c, VGX_SLOT_MESH);
     VGX_TRY(vgx_exclusive_scan_u32(c, d_cnt, d_voff, n_vox, d_tmp));
   }
   {
-    VgxLaunchScope scope(c, VGX_SLOT_MESH);
-    mesh_offsets_kernel<<<(nj + 1 + 127) / 128, 128, 0, st>>>(d_jobs, nj, n_vox, d_toff, d_voff, d_offs);
+    VgxProfileScope scope(c, VGX_SLOT_MESH);
+    VGX_TRY(vgx_launch(c, mesh_offsets_kernel, (nj + 1 + 127) / 128, 128, 0, VgxLaunch::plain, d_jobs, nj, n_vox, d_toff,
+                       d_voff, d_offs));
   }
-  VGX_CUDA(c, cudaGetLastError());
   std::vector<unsigned> offs(2 * ((size_t)nj + 1));
   VGX_CUDA(c, cudaMemcpyAsync(offs.data(), d_offs, offs.size() * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
   VGX_CUDA(c, cudaStreamSynchronize(st));
@@ -478,20 +477,16 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
                                      "mesh vertex colours"));
   }
   {
-    VgxLaunchScope scope(c, VGX_SLOT_MESH);
-    if (coloured)
-      mesh_vertex_kernel<true><<<g128, 128, 0, st>>>(d_jobs, nj, n_vox, d_flag, d_voff, vbase, c->d_mesh_xyz.get(),
-                                                     c->d_mesh_rgba.get());
-    else
-      mesh_vertex_kernel<false><<<g128, 128, 0, st>>>(d_jobs, nj, n_vox, d_flag, d_voff, vbase, c->d_mesh_xyz.get(),
-                                                      nullptr);
+    VgxProfileScope scope(c, VGX_SLOT_MESH);
+    VGX_TRY(vgx_launch(c, coloured ? mesh_vertex_kernel<true> : mesh_vertex_kernel<false>, g128, 128, 0, VgxLaunch::plain,
+                       d_jobs, nj, n_vox, d_flag, d_voff, vbase, c->d_mesh_xyz.get(),
+                       coloured ? c->d_mesh_rgba.get() : nullptr));
   }
   {
-    VgxLaunchScope scope(c, VGX_SLOT_MESH);
-    mesh_triangle_kernel<<<g128, 128, 0, st>>>(d_jobs, nj, n_vox, min_weight, d_toff, d_flag, d_voff, vbase,
-                                               tbase, c->d_mesh_tri.get());
+    VgxProfileScope scope(c, VGX_SLOT_MESH);
+    VGX_TRY(vgx_launch(c, mesh_triangle_kernel, g128, 128, 0, VgxLaunch::plain, d_jobs, nj, n_vox, min_weight, d_toff,
+                       d_flag, d_voff, vbase, tbase, c->d_mesh_tri.get()));
   }
-  VGX_CUDA(c, cudaGetLastError());
   VGX_CUDA(c, cudaStreamSynchronize(st));   // the scratch is reused by the next batch
   c->mesh_nv = (int64_t)nv;
   c->mesh_nt = (int64_t)nt;
@@ -644,12 +639,11 @@ extern "C" int vgx_mesh_ply_ex(vgx_ctx* c, const uint8_t* rgba, int voxel_colour
     VGX_CUDA(c, cudaMemcpyAsync(d_col, col.data(), col.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
     const int64_t recs = c->mesh_nv + c->mesh_nt;
     {
-      VgxLaunchScope scope(c, VGX_SLOT_MESH);
-      mesh_ply_kernel<<<(unsigned)((recs + 255) / 256), 256, 0, c->stream>>>(c->d_mesh_xyz.get(), c->d_mesh_tri.get(), c->mesh_nv,
-                                                                            c->mesh_nt, d_voff, ns, d_col,
-                                                                            voxel ? c->d_mesh_rgba.get() : nullptr, d_use, d_body);
+      VgxProfileScope scope(c, VGX_SLOT_MESH);
+      VGX_TRY(vgx_launch(c, mesh_ply_kernel, (unsigned)((recs + 255) / 256), 256, 0, VgxLaunch::plain, c->d_mesh_xyz.get(),
+                         c->d_mesh_tri.get(), c->mesh_nv, c->mesh_nt, d_voff, ns, d_col,
+                         voxel ? c->d_mesh_rgba.get() : nullptr, d_use, d_body));
     }
-    VGX_CUDA(c, cudaGetLastError());
     VGX_CUDA(c, cudaMemcpyAsync(out + hn, d_body, (size_t)body, cudaMemcpyDeviceToHost, c->stream));
     VGX_CUDA(c, cudaStreamSynchronize(c->stream));
     return VGX_OK;

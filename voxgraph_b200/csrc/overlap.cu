@@ -126,9 +126,7 @@ extern "C" int vgx_find_overlapping_pairs(vgx_ctx* c, int n, const uint32_t* ids
     int* d_flags;
     VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_jobs, jobs.size()), vgx_part(d_flags, jobs.size())));
     VGX_CUDA(c, cudaMemcpyAsync(d_jobs, jobs.data(), jobs.size() * sizeof(OverlapJob), cudaMemcpyHostToDevice, c->stream));
-    overlap_pairs_kernel<<<(unsigned)jobs.size(), 128, 0, c->stream>>>(d_jobs, d_flags);
-    c->launches++;
-    VGX_CUDA(c, cudaGetLastError());
+    VGX_TRY(vgx_launch(c, overlap_pairs_kernel, (unsigned)jobs.size(), 128, 0, VgxLaunch::plain, d_jobs, d_flags));
     std::vector<int> flags(jobs.size());
     VGX_CUDA(c, cudaMemcpyAsync(flags.data(), d_flags, jobs.size() * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     VGX_CUDA(c, cudaStreamSynchronize(c->stream));

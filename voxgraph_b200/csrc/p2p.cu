@@ -128,13 +128,10 @@ int vgx_p2p_begin(vgx_ctx* c, size_t count, VgxP2PPush* push, VgxP2PGather* gat)
 
 int vgx_p2p_gather(vgx_ctx* c, const VgxP2PGather& gat, double* d_out, size_t count,
                    const unsigned char* d_block_mask, int N) {
-  {
-    VgxLaunchScope s(c, VGX_SLOT_OTHER);
-    const int blocks = (int)((count + 1023) / 1024) > 0 ? (int)((count + 1023) / 1024) : 1;
-    p2p_gather_kernel<<<blocks < 64 ? blocks : 64, 256, 0, c->stream>>>(gat, d_out, count, d_block_mask, N);
-  }
-  VGX_CUDA(c, cudaGetLastError());
-  return VGX_OK;
+  VgxProfileScope s(c, VGX_SLOT_OTHER);
+  const int blocks = (int)((count + 1023) / 1024) > 0 ? (int)((count + 1023) / 1024) : 1;
+  return vgx_launch(c, p2p_gather_kernel, blocks < 64 ? blocks : 64, 256, 0, VgxLaunch::plain, gat, d_out, count,
+                    d_block_mask, N);
 }
 
 extern "C" int vgx_comm_suspend(vgx_ctx* c, int on) {

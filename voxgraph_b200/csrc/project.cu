@@ -312,18 +312,12 @@ transform_fold_kernel(const ProjSrc* __restrict__ src, const uint64_t* __restric
 // ------------------------------------------------------------------ host
 static int launch_fold(vgx_ctx* c, int vps, unsigned n_keys, const ProjSrc* d_src, const uint64_t* ukey,
                        const uint32_t* urank, const uint32_t* useg, const unsigned* slot, VgxSubmap* s) {
-  cudaStream_t st = c->stream;
   uint32_t* rgba = s->d_rgba.get();   // the output has a channel iff an input has one
   switch (vps) {
-#define PROJ_FOLD(VPT, REGS, THREADS)                                                                           \
-  if (rgba)                                                                                                     \
-    project_fold_kernel<VPT, REGS, true><<<n_keys, THREADS, 0, st>>>(d_src, ukey, urank, useg, slot,             \
-                                                                     s->d_dw.get(), s->d_block_idx.get(), rgba); \
-  else                                                                                                          \
-    project_fold_kernel<VPT, REGS, false><<<n_keys, THREADS, 0, st>>>(d_src, ukey, urank, useg, slot,            \
-                                                                      s->d_dw.get(), s->d_block_idx.get(),       \
-                                                                      nullptr);                                  \
-  break;
+#define PROJ_FOLD(VPT, REGS, THREADS)                                                                              \
+  return vgx_launch(c, rgba ? project_fold_kernel<VPT, REGS, true> : project_fold_kernel<VPT, REGS, false>, n_keys, \
+                    THREADS, 0, VgxLaunch::plain, d_src, ukey, urank, useg, slot, s->d_dw.get(),                    \
+                    s->d_block_idx.get(), rgba);
     case 2: PROJ_FOLD(1, true, 8)
     case 4: PROJ_FOLD(1, true, 64)
     case 8: PROJ_FOLD(2, true, 256)
@@ -332,8 +326,6 @@ static int launch_fold(vgx_ctx* c, int vps, unsigned n_keys, const ProjSrc* d_sr
 #undef PROJ_FOLD
     default: VGX_FAIL(c, VGX_ERR_INVALID, "unsupported voxels_per_side");
   }
-  VGX_CUDA(c, cudaGetLastError());
-  return VGX_OK;
 }
 
 // subs / poses in rank (id) order; creates out_id on success.  transform (one submap, vgx_submap_transform):
@@ -384,35 +376,32 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
     VGX_CUDA(c, cudaMemcpyAsync(d_src, h.data(), sizeof(ProjSrc) * (size_t)ns, cudaMemcpyHostToDevice, st));
     VGX_CUDA(c, cudaMemsetAsync(d_ctl, 0, sizeof(int), st));
     {
-      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
-      project_candidate_kernel<<<(unsigned)((n_in + 127) / 128), 128, 0, st>>>(d_src, ns, (int)n_in, transform,
-                                                                            keys_a, ranks_a, d_ctl);
+      VgxProfileScope scope(c, VGX_SLOT_PROJECT);
+      VGX_TRY(vgx_launch(c, project_candidate_kernel, (unsigned)((n_in + 127) / 128), 128, 0, VgxLaunch::plain, d_src, ns,
+                         (int)n_in, transform, keys_a, ranks_a, d_ctl));
     }
-    VGX_CUDA(c, cudaGetLastError());
     {
-      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
+      VgxProfileScope scope(c, VGX_SLOT_PROJECT);
       VGX_CUDA(c, cub::DeviceRadixSort::SortPairs(d_sort_tmp, sort_tmp, (unsigned long long*)keys_a,
                                                   (unsigned long long*)keys_b, ranks_a, ranks_b, (int)P, 0,
                                                   PROJ_KEY_BITS, st));
+      vgx_count_launch(c);
     }
     const unsigned gp = (unsigned)((P + 255) / 256);
     {
-      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
-      project_flag_kernel<<<gp, 256, 0, st>>>(keys_b, ranks_b, P, pair_head, key_head);
+      VgxProfileScope scope(c, VGX_SLOT_PROJECT);
+      VGX_TRY(vgx_launch(c, project_flag_kernel, gp, 256, 0, VgxLaunch::plain, keys_b, ranks_b, P, pair_head, key_head));
     }
-    VGX_CUDA(c, cudaGetLastError());
     {
-      VgxLaunchScope scope(c, VGX_SLOT_PROJECT, 0);
-      c->prof[VGX_SLOT_PROJECT].launches += 6;
+      VgxProfileScope scope(c, VGX_SLOT_PROJECT);
       VGX_TRY(vgx_exclusive_scan_u32(c, pair_head, pair_pos, P, scan_tmp));
       VGX_TRY(vgx_exclusive_scan_u32(c, key_head, key_pos, P, scan_tmp));
     }
     {
-      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
-      project_scatter_kernel<<<gp, 256, 0, st>>>(keys_b, ranks_b, P, pair_head, key_head, pair_pos, key_pos, keys_a,
-                                                 ranks_a, useg);
+      VgxProfileScope scope(c, VGX_SLOT_PROJECT);
+      VGX_TRY(vgx_launch(c, project_scatter_kernel, gp, 256, 0, VgxLaunch::plain, keys_b, ranks_b, P, pair_head, key_head,
+                         pair_pos, key_pos, keys_a, ranks_a, useg));
     }
-    VGX_CUDA(c, cudaGetLastError());
     int ctl[2] = {0, 0};
     VGX_CUDA(c, cudaMemcpyAsync(&ctl[0], d_ctl, sizeof(int), cudaMemcpyDeviceToHost, st));
     VGX_CUDA(c, cudaMemcpyAsync(&ctl[1], key_pos + P, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
@@ -427,14 +416,12 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
   unsigned* slot = pair_pos;
   if (n_keys > 0) {
     {
-      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
-      project_occupancy_kernel<<<n_keys, std::min(PROJ_THREADS, g0.vox_per_block), 0, st>>>(d_src, keys_a, ranks_a,
-                                                                                            useg, transform, keep);
+      VgxProfileScope scope(c, VGX_SLOT_PROJECT);
+      VGX_TRY(vgx_launch(c, project_occupancy_kernel, n_keys, std::min(PROJ_THREADS, g0.vox_per_block), 0,
+                         VgxLaunch::plain, d_src, keys_a, ranks_a, useg, transform, keep));
     }
-    VGX_CUDA(c, cudaGetLastError());
     {
-      VgxLaunchScope scope(c, VGX_SLOT_PROJECT, 0);
-      c->prof[VGX_SLOT_PROJECT].launches += 3;
+      VgxProfileScope scope(c, VGX_SLOT_PROJECT);
       VGX_TRY(vgx_exclusive_scan_u32(c, keep, slot, n_keys, scan_tmp));
     }
     VGX_CUDA(c, cudaMemcpyAsync(&n_out, slot + n_keys, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
@@ -445,20 +432,15 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
   s->n_blocks = (int)n_out;
   s->finished = true;
   if (n_out > 0 && transform) {
-    {
-      VgxLaunchScope scope(c, VGX_SLOT_EVAL);
-      transform_fold_kernel<<<n_keys, std::min(PROJ_THREADS, g0.vox_per_block), 0, st>>>(d_src, keys_a, slot, s->d_dw.get(),
-                                                                                        s->d_block_idx.get());
-    }
-    VGX_CUDA(c, cudaGetLastError());
+    VgxProfileScope scope(c, VGX_SLOT_EVAL);
+    VGX_TRY(vgx_launch(c, transform_fold_kernel, n_keys, std::min(PROJ_THREADS, g0.vox_per_block), 0, VgxLaunch::plain,
+                       d_src, keys_a, slot, s->d_dw.get(), s->d_block_idx.get()));
   } else if (n_out > 0) {
     bool coloured = false;
     for (const VgxSubmap* in : subs) coloured = coloured || in->d_rgba.get();
     if (coloured) VGX_TRY(vgx_submap_ensure_colour(c, s));
-    {
-      VgxLaunchScope scope(c, VGX_SLOT_PROJECT);
-      VGX_TRY(launch_fold(c, g0.vps, n_keys, d_src, keys_a, ranks_a, useg, slot, s));
-    }
+    VgxProfileScope scope(c, VGX_SLOT_PROJECT);
+    VGX_TRY(launch_fold(c, g0.vps, n_keys, d_src, keys_a, ranks_a, useg, slot, s));
   }
   VGX_TRY(vgx_submap_upload_finish(c, s));
   *n_out_blocks = (int)n_out;

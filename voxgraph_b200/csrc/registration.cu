@@ -132,8 +132,9 @@ reg_unit_bounds_kernel(const RegTile* __restrict__ tiles, float4* __restrict__ b
   }
 }
 
-void vgx_launch_reg_unit_bounds(cudaStream_t st, const RegTile* tiles, int n_tiles, float4* bounds) {
-  if (n_tiles > 0) reg_unit_bounds_kernel<<<n_tiles, 128, 0, st>>>(tiles, bounds);
+int vgx_launch_reg_unit_bounds(vgx_ctx* c, const RegTile* tiles, int n_tiles, float4* bounds) {
+  if (n_tiles <= 0) return VGX_OK;
+  return vgx_launch(c, reg_unit_bounds_kernel, n_tiles, 128, 0, VgxLaunch::plain, tiles, bounds);
 }
 
 // May a point of the unit with bounding sphere b (reference frame) lie in an existing block?  One
@@ -478,8 +479,9 @@ reg_order_kernel(const int* __restrict__ cost, int n, int* __restrict__ order) {
     order[atomicAdd(&s_hist[1023 - min(1023, (int)((float)cost[i] * scale))], 1)] = i;
 }
 
-void vgx_launch_reg_order(cudaStream_t st, const int* tile_cost, int n_tiles, int* tile_order) {
-  if (n_tiles > 0) reg_order_kernel<<<1, 1024, 0, st>>>(tile_cost, n_tiles, tile_order);
+int vgx_launch_reg_order(vgx_ctx* c, const int* tile_cost, int n_tiles, int* tile_order) {
+  if (n_tiles <= 0) return VGX_OK;
+  return vgx_launch(c, reg_order_kernel, 1, 1024, 0, VgxLaunch::plain, tile_cost, n_tiles, tile_order);
 }
 
 // The pose blocks of one evaluation, one thread per constraint.  The kernel is a programmatic
@@ -529,27 +531,22 @@ __global__ void reg_pose_setup_kernel(const RegConstraintDev* __restrict__ const
 }
 
 // ------------------------------------------------------------------ launch helpers
-void vgx_launch_reg_pose_setup(cudaStream_t st, const RegConstraintDev* cons, const double* x,
-                               RegPoseConst* poses, int n, const int* skip) {
-  if (n <= 0) return;
-  VgxPdlLaunch L(st, dim3((unsigned)((n + 127) / 128)), dim3(128));
-  cudaLaunchKernelEx(&L.cfg, reg_pose_setup_kernel, cons, x, poses, n, skip);
+int vgx_launch_reg_pose_setup(vgx_ctx* c, const RegConstraintDev* cons, const double* x, RegPoseConst* poses, int n,
+                              const int* skip) {
+  if (n <= 0) return VGX_OK;
+  return vgx_launch(c, reg_pose_setup_kernel, (unsigned)((n + 127) / 128), 128, 0, VgxLaunch::pdl, cons, x, poses, n,
+                    skip);
 }
 
-void vgx_launch_reg_reduce(cudaStream_t st, const RegConstraintDev* cons, const RegPoseConst* poses,
-                           const RegTile* tiles, int n_tiles, const int* tile_order, int* tile_cost,
-                           double* partials, int grid_capacity, const float4* unit_bounds, bool jacobian,
-                           const int* skip) {
-  if (n_tiles <= 0) return;
+int vgx_launch_reg_reduce(vgx_ctx* c, const RegConstraintDev* cons, const RegPoseConst* poses, const RegTile* tiles,
+                          int n_tiles, const int* tile_order, int* tile_cost, double* partials, int grid_capacity,
+                          const float4* unit_bounds, bool jacobian, const int* skip) {
+  if (n_tiles <= 0) return VGX_OK;
   // its CTAs may start while the pose set-up kernel is still running; they block at
   // griddepcontrol.wait before touching the pose blocks
-  VgxPdlLaunch L(st, dim3((unsigned)n_tiles), dim3(VGX_REG_THREADS), sizeof(uint16_t) * (size_t)grid_capacity);
-  if (jacobian)
-    cudaLaunchKernelEx(&L.cfg, reg_reduce_kernel<true>, cons, poses, tiles, tile_order, tile_cost, partials,
-                       grid_capacity, unit_bounds, skip);
-  else
-    cudaLaunchKernelEx(&L.cfg, reg_reduce_kernel<false>, cons, poses, tiles, tile_order, tile_cost, partials,
-                       grid_capacity, unit_bounds, skip);
+  return vgx_launch(c, jacobian ? reg_reduce_kernel<true> : reg_reduce_kernel<false>, (unsigned)n_tiles,
+                    VGX_REG_THREADS, sizeof(uint16_t) * (size_t)grid_capacity, VgxLaunch::pdl, cons, poses, tiles,
+                    tile_order, tile_cost, partials, grid_capacity, unit_bounds, skip);
 }
 
 // cpp:45-55: num_residuals = int(sampling_ratio * size()) (float product) or size()
@@ -572,11 +569,10 @@ __global__ void reg_gather_samples_kernel(const float* __restrict__ src, const i
   dp[0] = x; dp[32] = y; dp[64] = z; dp[96] = d; dp[128] = w;
 }
 
-void vgx_launch_reg_gather_samples(cudaStream_t st, const float* src, const int32_t* d_idx, int n,
-                                   float* dst) {
-  if (n <= 0) return;
+int vgx_launch_reg_gather_samples(vgx_ctx* c, const float* src, const int32_t* d_idx, int n, float* dst) {
+  if (n <= 0) return VGX_OK;
   const int padded = (n + 31) & ~31;
-  reg_gather_samples_kernel<<<(padded + 255) / 256, 256, 0, st>>>(src, d_idx, n, dst);
+  return vgx_launch(c, reg_gather_samples_kernel, (padded + 255) / 256, 256, 0, VgxLaunch::plain, src, d_idx, n, dst);
 }
 
 int vgx_fill_constraint(vgx_ctx* c, uint32_t ref_id, uint32_t read_id, const vgx_reg_config* cfg,
@@ -669,8 +665,7 @@ extern "C" int vgx_reg_eval_emit(vgx_ctx* c, uint32_t ref_id, uint32_t read_id,
       VGX_CUDA(c, cudaStreamSynchronize(c->stream));
       vgx_points_draw(p, (int)K, h_idx);
       VGX_CUDA(c, cudaMemcpyAsync(d_idx, h_idx, K * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
-      vgx_launch_reg_gather_samples(c->stream, p.data.get(), d_idx, (int)K, d_pts);
-      c->launches++;
+      VGX_TRY(vgx_launch_reg_gather_samples(c, p.data.get(), d_idx, (int)K, d_pts));
       C.pts = d_pts;
     }
     RegPoseConst P;
@@ -678,10 +673,10 @@ extern "C" int vgx_reg_eval_emit(vgx_ctx* c, uint32_t ref_id, uint32_t read_id,
     double* d_jr = jac_ref ? d_r + Kp : nullptr;
     double* d_je = jac_read ? d_r + 5 * Kp : nullptr;
     {
-      VgxLaunchScope scope(c, VGX_SLOT_REG_EMIT);
-      reg_emit_kernel<<<(unsigned)((K + 255) / 256), 256, 0, c->stream>>>(C, P, d_r, d_jr, d_je);
+      VgxProfileScope scope(c, VGX_SLOT_REG_EMIT);
+      VGX_TRY(vgx_launch(c, reg_emit_kernel, (unsigned)((K + 255) / 256), 256, 0, VgxLaunch::plain, C, P, d_r, d_jr,
+                         d_je));
     }
-    VGX_CUDA(c, cudaGetLastError());
     VGX_CUDA(c, cudaMemcpyAsync(residuals, d_r, K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
     if (jac_ref)
       VGX_CUDA(c, cudaMemcpyAsync(jac_ref, d_jr, 4 * K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));

@@ -22,42 +22,21 @@ struct __align__(16) RegTile {   // 32 bytes: everything a CTA needs to start it
   const uint16_t* grid16;
 };
 
-// Launch configuration with programmatic stream serialisation: the kernel may be scheduled while the
-// one ahead of it on the stream is still running and waits for it at griddepcontrol.wait.  cfg points
-// at attr, so the object is not copied.
-struct VgxPdlLaunch {
-  cudaLaunchAttribute attr[1] = {};
-  cudaLaunchConfig_t cfg = {};
-  VgxPdlLaunch(cudaStream_t st, dim3 grid, dim3 block, size_t smem = 0) {
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-  }
-  VgxPdlLaunch(const VgxPdlLaunch&) = delete;
-  VgxPdlLaunch& operator=(const VgxPdlLaunch&) = delete;
-};
-
 // skip (device flag, may be null): when set, the kernel returns at once (an evaluation enqueued
 // ahead of a solve that has ended in the meantime)
-void vgx_launch_reg_pose_setup(cudaStream_t st, const RegConstraintDev* cons, const double* x,
-                               RegPoseConst* poses, int n, const int* skip = nullptr);
+int vgx_launch_reg_pose_setup(vgx_ctx* c, const RegConstraintDev* cons, const double* x, RegPoseConst* poses, int n,
+                              const int* skip = nullptr);
 // One CTA per tile, CTA b running tile tile_order[b] -> partials[tile][21] and tile_cost[tile]; the
 // consumer adds a constraint's tiles in tile order (graph.cu: reg_csum_kernel).  unit_bounds (may be
 // null: no culling): the table vgx_launch_reg_unit_bounds fills, indexed by RegTile::unit0 + unit.
-void vgx_launch_reg_reduce(cudaStream_t st, const RegConstraintDev* cons, const RegPoseConst* poses,
-                           const RegTile* tiles, int n_tiles, const int* tile_order, int* tile_cost,
-                           double* partials, int grid_capacity, const float4* unit_bounds, bool jacobian,
-                           const int* skip = nullptr);
+int vgx_launch_reg_reduce(vgx_ctx* c, const RegConstraintDev* cons, const RegPoseConst* poses, const RegTile* tiles,
+                          int n_tiles, const int* tile_order, int* tile_cost, double* partials, int grid_capacity,
+                          const float4* unit_bounds, bool jacobian, const int* skip = nullptr);
 // bounds[tile.unit0 + u] <- a sphere (centre xyz, radius w) around the points of unit u of every tile
 // that can contribute (radius +inf: the unit is never culled)
-void vgx_launch_reg_unit_bounds(cudaStream_t st, const RegTile* tiles, int n_tiles, float4* bounds);
+int vgx_launch_reg_unit_bounds(vgx_ctx* c, const RegTile* tiles, int n_tiles, float4* bounds);
 // tile_order <- tiles sorted by measured cost, most expensive first
-void vgx_launch_reg_order(cudaStream_t st, const int* tile_cost, int n_tiles, int* tile_order);
+int vgx_launch_reg_order(vgx_ctx* c, const int* tile_cost, int n_tiles, int* tile_order);
 // Fills the descriptor of one (reference -> reading) residual block.  Deterministic mode: pts / n /
 // factor describe all registration points.  Sampling mode (*sampled = true): n = int(ratio * K),
 // factor = 1 (all weights forced to 1) and pts is left null for the caller, who draws the
@@ -65,5 +44,4 @@ void vgx_launch_reg_order(cudaStream_t st, const int* tile_cost, int n_tiles, in
 int vgx_fill_constraint(vgx_ctx* c, uint32_t ref_id, uint32_t read_id, const vgx_reg_config* cfg,
                         RegConstraintDev* out, bool* sampled = nullptr);
 // dst (unit-major, ceil(n/32) units) <- the n points of src selected by d_idx, weight forced to 1
-void vgx_launch_reg_gather_samples(cudaStream_t st, const float* src, const int32_t* d_idx, int n,
-                                   float* dst);
+int vgx_launch_reg_gather_samples(vgx_ctx* c, const float* src, const int32_t* d_idx, int n, float* dst);

@@ -662,21 +662,16 @@ static int chol_dispatch(vgx_ctx* c, int n, bool smem_ok, size_t* smem_bytes, in
   return VGX_OK;
 }
 
-static cudaError_t launch_chol_coop(cudaStream_t st, int grid, double* A, int n, LmState* state,
-                                    const double* diag0, double rank_tol) {
-  void* args[] = {(void*)&A, (void*)&n, (void*)&state, (void*)&diag0, (void*)&rank_tol};
-  return cudaLaunchCooperativeKernel((void*)chol_coop_kernel, dim3(grid), dim3(256), args, 0, st);
-}
-
 // lm_build_kernel + lm_persist_kernel on the normal equations in d_packed[0]
-static void enqueue_lm_build(cudaStream_t st, VgxGraph* g, int n, const LmOpts& lo) {
+static int enqueue_lm_build(vgx_ctx* c, VgxGraph* g, int n, const LmOpts& lo) {
   const int N = g->N;
   const int nthreads = std::max(16 * (N + g->plan.E), 4 * N);
-  lm_build_kernel<<<std::min(296, (nthreads + 255) / 256), 256, 0, st>>>(
-      g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), g->dev.d_block_nodes.get(), N, g->plan.E, n,
-      g->dev.d_A.get(), g->dev.d_scale.get(), g->dev.d_diag.get(), g->dev.d_gs.get(), g->dev.d_state.get(), lo);
-  lm_persist_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), N, g->dev.d_scale.get(),
-                                       g->dev.d_diag.get(), g->dev.d_state.get(), lo);
+  VGX_TRY(vgx_launch(c, lm_build_kernel, std::min(296, (nthreads + 255) / 256), 256, 0, VgxLaunch::plain,
+                     g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), g->dev.d_block_nodes.get(), N, g->plan.E, n,
+                     g->dev.d_A.get(), g->dev.d_scale.get(), g->dev.d_diag.get(), g->dev.d_gs.get(),
+                     g->dev.d_state.get(), lo));
+  return vgx_launch(c, lm_persist_kernel, 1, 256, 0, VgxLaunch::plain, g->dev.d_packed[0].get(),
+                    g->dev.d_red_offset.get(), N, g->dev.d_scale.get(), g->dev.d_diag.get(), g->dev.d_state.get(), lo);
 }
 
 // ------------------------------------------------------------------ edge covariances
@@ -789,22 +784,21 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
     VGX_CUDA(c, cudaMemsetAsync(g->dev.d_A.get(), 0, sizeof(double) * M * M, st));
     VGX_CUDA(c, cudaMemcpyAsync(g->dev.d_state.get(), init, sizeof(*init), cudaMemcpyHostToDevice, st));
     {
-      VgxLaunchScope s(c, VGX_SLOT_SOLVE, 3);
-      enqueue_lm_build(st, g, n, lo);
-      VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->dev.d_A.get(), n, g->dev.d_state.get(), g->dev.d_diag.get(),
-                                   VGX_COV_RANK_TOL));
+      VgxProfileScope s(c, VGX_SLOT_SOLVE);
+      VGX_TRY(enqueue_lm_build(c, g, n, lo));
+      VGX_TRY(vgx_launch(c, chol_coop_kernel, coop_grid, 256, 0, VgxLaunch::cooperative, g->dev.d_A.get(), n,
+                         g->dev.d_state.get(), g->dev.d_diag.get(), VGX_COV_RANK_TOL));
     }
-    VGX_CUDA(c, cudaGetLastError());
     // inverse columns
     VGX_CUDA(c, cudaMemcpyAsync(d_cols, cols.data(), sizeof(int) * ncols, cudaMemcpyHostToDevice, st));
     if (sizeof(double) * (size_t)n > 48 * 1024)
       VGX_CUDA(c, cudaFuncSetAttribute(cov_column_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)(sizeof(double) * (size_t)n)));
     {
-      VgxLaunchScope s(c, VGX_SLOT_SOLVE);
-      cov_column_kernel<<<(unsigned)ncols, 256, sizeof(double) * (size_t)n, st>>>(g->dev.d_A.get(), n, d_cols, d_X);
+      VgxProfileScope s(c, VGX_SLOT_SOLVE);
+      VGX_TRY(vgx_launch(c, cov_column_kernel, (unsigned)ncols, 256, sizeof(double) * (size_t)n, VgxLaunch::plain,
+                         g->dev.d_A.get(), n, d_cols, d_X));
     }
-    VGX_CUDA(c, cudaGetLastError());
     std::vector<double> X(ncols * (size_t)n);
     LmState hs;
     VGX_CUDA(c, cudaMemcpyAsync(X.data(), d_X, sizeof(double) * X.size(), cudaMemcpyDeviceToHost, st));
@@ -895,9 +889,9 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
     // that drain while the host already returns.  Multi-rank: no run-ahead (the ranks stay in step).
     VGX_TRY(eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, excl));
     {
-      VgxLaunchScope s(c, VGX_SLOT_SOLVE);
-      lm_init_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_red_offset.get(), N, g->dev.d_state.get(),
-                                        o->initial_trust_region_radius, lo);
+      VgxProfileScope s(c, VGX_SLOT_SOLVE);
+      VGX_TRY(vgx_launch(c, lm_init_kernel, 1, 256, 0, VgxLaunch::plain, g->dev.d_packed[0].get(),
+                         g->dev.d_red_offset.get(), N, g->dev.d_state.get(), o->initial_trust_region_radius, lo));
     }
     VGX_CUDA(c, cudaMemcpyAsync(g->h_state.get(), g->dev.d_state.get(), sizeof(LmState), cudaMemcpyDeviceToHost, st));
     VGX_CUDA(c, cudaStreamSynchronize(st));
@@ -916,37 +910,36 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
     const int* skip = &g->dev.d_state.get()->done;
     auto enqueue_iteration = [&](int k) -> int {
       {
-        VgxLaunchScope s(c, VGX_SLOT_SOLVE, 4);
+        VgxProfileScope s(c, VGX_SLOT_SOLVE);
         if (!use_smem_chol)   // the shared-memory solver reads the written blocks only
           VGX_CUDA(c, cudaMemsetAsync(g->dev.d_A.get(), 0, sizeof(double) * (size_t)(n + 1) * (n + 1), st));
-        enqueue_lm_build(st, g, n, lo);
+        VGX_TRY(enqueue_lm_build(c, g, n, lo));
         if (use_smem_chol) {
-          chol_solve_smem_kernel<<<1, 512, smem_chol_bytes, st>>>(g->dev.d_A.get(), n, g->dev.d_step.get(),
-                                                                  g->dev.d_state.get(), g->dev.d_red_offset.get(),
-                                                                  g->dev.d_block_nodes.get(), N, g->plan.E, d_chol_dbg);
+          VGX_TRY(vgx_launch(c, chol_solve_smem_kernel, 1, 512, smem_chol_bytes, VgxLaunch::plain, g->dev.d_A.get(), n,
+                             g->dev.d_step.get(), g->dev.d_state.get(), g->dev.d_red_offset.get(),
+                             g->dev.d_block_nodes.get(), N, g->plan.E, d_chol_dbg));
         } else {
           // LM: sign test only (as Eigen's LLT in the reference)
-          VGX_CUDA(c, launch_chol_coop(st, coop_grid, g->dev.d_A.get(), n, g->dev.d_state.get(), nullptr, 0.0));
+          VGX_TRY(vgx_launch(c, chol_coop_kernel, coop_grid, 256, 0, VgxLaunch::cooperative, g->dev.d_A.get(), n,
+                             g->dev.d_state.get(), nullptr, 0.0));
         }
-        lm_step_kernel<<<1, 1024, sizeof(double) * n, st>>>(g->dev.d_A.get(), n, N, g->dev.d_red_offset.get(),
-                                                           g->dev.d_scale.get(), g->dev.d_diag.get(), g->dev.d_gs.get(),
-                                                           g->dev.d_x.get(), g->dev.d_xc.get(), g->dev.d_step.get(),
-                                                           g->dev.d_state.get(),
-                                                           use_smem_chol ? g->dev.d_step.get() : nullptr);
+        VGX_TRY(vgx_launch(c, lm_step_kernel, 1, 1024, sizeof(double) * n, VgxLaunch::plain, g->dev.d_A.get(), n, N,
+                           g->dev.d_red_offset.get(), g->dev.d_scale.get(), g->dev.d_diag.get(), g->dev.d_gs.get(),
+                           g->dev.d_x.get(), g->dev.d_xc.get(), g->dev.d_step.get(), g->dev.d_state.get(),
+                           use_smem_chol ? g->dev.d_step.get() : nullptr));
       }
-      VGX_CUDA(c, cudaGetLastError());
       // candidate evaluated with Jacobians so an accepted step needs no second pass
       int rc2 = eval_enqueue(c, g, g->dev.d_xc.get(), g->dev.d_packed[1].get(), true, excl, skip);
       if (rc2 != VGX_OK) return rc2;
       {
-        VgxLaunchScope s(c, VGX_SLOT_SOLVE, 2);
-        lm_decide_kernel<<<1, 256, 0, st>>>(g->dev.d_packed[0].get(), g->dev.d_packed[1].get(), g->dev.d_red_offset.get(),
-                                            N, g->dev.d_x.get(), g->dev.d_xc.get(), g->dev.d_state.get(), lo, 1,
-                                            g->dev.d_snap.get() + (k & 1));
-        lm_accept_kernel<<<std::max(1, std::min(64, (int)(g->plan.packed_len / 2048))), 256, 0, st>>>(
-            g->dev.d_packed[1].get(), g->dev.d_packed[0].get(), g->plan.packed_len, g->dev.d_state.get());
+        VgxProfileScope s(c, VGX_SLOT_SOLVE);
+        VGX_TRY(vgx_launch(c, lm_decide_kernel, 1, 256, 0, VgxLaunch::plain, g->dev.d_packed[0].get(),
+                           g->dev.d_packed[1].get(), g->dev.d_red_offset.get(), N, g->dev.d_x.get(), g->dev.d_xc.get(),
+                           g->dev.d_state.get(), lo, 1, g->dev.d_snap.get() + (k & 1)));
+        VGX_TRY(vgx_launch(c, lm_accept_kernel, std::max(1, std::min(64, (int)(g->plan.packed_len / 2048))), 256, 0,
+                           VgxLaunch::plain, g->dev.d_packed[1].get(), g->dev.d_packed[0].get(), g->plan.packed_len,
+                           g->dev.d_state.get()));
       }
-      VGX_CUDA(c, cudaGetLastError());
       // outcome of iteration k -> host, on the copy stream (the main stream keeps running ahead)
       VGX_CUDA(c, cudaEventRecord(g->ev_iter[k & 1], st));
       VGX_CUDA(c, cudaStreamWaitEvent(g->copy_stream, g->ev_iter[k & 1], 0));

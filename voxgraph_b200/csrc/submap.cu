@@ -74,8 +74,7 @@ extern "C" int vgx_profile_enable(vgx_ctx* c, int on) {
 }
 extern "C" int vgx_profile_reset(vgx_ctx* c) {
   return vgx_entry(c, __func__, [&] {
-    for (auto& p : c->prof) p = VgxProfileSlot();
-    c->launches = 0;
+    vgx_reset_counts(c);
     return VGX_OK;
   });
 }
@@ -272,22 +271,16 @@ int vgx_submap_build_grid(vgx_ctx* c, VgxSubmap* s) {
 int vgx_submap_build_view(vgx_ctx* c, VgxSubmap* s, const float2* bricks, float* view) {
   const size_t used = (size_t)s->n_blocks * s->vox_per_block;
   if (used == 0) return VGX_OK;
-  build_view_kernel<<<(unsigned)((used + 255) / 256), 256, 0, c->stream>>>(bricks, s->d_block_idx.get(), s->hash(), view,
-                                                                          s->n_blocks, s->vps, s->sh);
-  c->launches++;
-  VGX_CUDA(c, cudaGetLastError());
-  return VGX_OK;
+  return vgx_launch(c, build_view_kernel, (unsigned)((used + 255) / 256), 256, 0, VgxLaunch::plain, bricks,
+                    s->d_block_idx.get(), s->hash(), view, s->n_blocks, s->vps, s->sh);
 }
 
 int vgx_submap_rebuild_hash(vgx_ctx* c, VgxSubmap* s) {
   const uint32_t tsize = s->hash_mask + 1;
-  hash_clear_kernel<<<(tsize + 255) / 256, 256, 0, c->stream>>>(s->d_hash.get(), tsize);
-  if (s->n_blocks > 0)
-    hash_insert_kernel<<<(s->n_blocks + 127) / 128, 128, 0, c->stream>>>(s->hash(), s->d_block_idx.get(), s->n_blocks,
-                                                                         nullptr);
-  c->launches += 2;
-  VGX_CUDA(c, cudaGetLastError());
-  return VGX_OK;
+  VGX_TRY(vgx_launch(c, hash_clear_kernel, (tsize + 255) / 256, 256, 0, VgxLaunch::plain, s->d_hash.get(), tsize));
+  if (s->n_blocks == 0) return VGX_OK;
+  return vgx_launch(c, hash_insert_kernel, (s->n_blocks + 127) / 128, 128, 0, VgxLaunch::plain, s->hash(),
+                    s->d_block_idx.get(), s->n_blocks, nullptr);
 }
 
 // ------------------------------------------------------------------ submap management
@@ -329,12 +322,12 @@ int vgx_submap_alloc(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int cap
   if (rc == VGX_OK) rc = s->d_dw.alloc(c, sizeof(float2) * nvox, what, VGX_ERR_NOMEM);
   if (rc == VGX_OK && with_view) rc = s->d_view.alloc(c, sizeof(float) * 8 * nvox, what, VGX_ERR_NOMEM);
   if (rc == VGX_OK) rc = s->d_counters.alloc(c, sizeof(int) * 4, what, VGX_ERR_NOMEM);
+  if (rc == VGX_OK)
+    rc = vgx_launch(c, hash_clear_kernel, (tsize + 255) / 256, 256, 0, VgxLaunch::plain, s->d_hash.get(), tsize);
   if (rc != VGX_OK) {
     delete s;
     return rc;
   }
-  hash_clear_kernel<<<(tsize + 255) / 256, 256, 0, c->stream>>>(s->d_hash.get(), tsize);
-  c->launches++;
   VGX_CUDA(c, cudaMemsetAsync(s->d_counters.get(), 0, sizeof(int) * 4, c->stream));
   c->submaps[id] = s;
   *out = s;
@@ -359,8 +352,8 @@ extern "C" int vgx_submap_upload(vgx_ctx* c, uint32_t id, float voxel_size, int 
     VGX_CUDA(c, cudaMemcpyAsync(tmp_w, weight, nvox * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx.get(), block_idx, sizeof(int32_t) * 3 * n_blocks,
                                 cudaMemcpyHostToDevice, c->stream));
-    interleave_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(tmp_d, tmp_w, s->d_dw.get(), nvox);
-    c->launches++;
+    VGX_TRY(vgx_launch(c, interleave_kernel, (unsigned)((nvox + 255) / 256), 256, 0, VgxLaunch::plain, tmp_d, tmp_w,
+                       s->d_dw.get(), nvox));
     // synchronises: the host buffers are the caller's
     return vgx_submap_upload_finish(c, s);
   });
@@ -478,9 +471,8 @@ extern "C" int vgx_submap_upload_device_colour(vgx_ctx* c, uint32_t id, int n_bl
 int vgx_submap_upload_finish(vgx_ctx* c, VgxSubmap* s) {
   if (s->n_blocks == 0) return VGX_OK;
   VGX_CUDA(c, cudaMemcpyAsync(s->d_counters.get(), &s->n_blocks, sizeof(int), cudaMemcpyHostToDevice, c->stream));
-  hash_insert_kernel<<<(s->n_blocks + 127) / 128, 128, 0, c->stream>>>(s->hash(), s->d_block_idx.get(), s->n_blocks,
-                                                                       s->d_counters.get() + 2);
-  c->launches++;
+  VGX_TRY(vgx_launch(c, hash_insert_kernel, (s->n_blocks + 127) / 128, 128, 0, VgxLaunch::plain, s->hash(),
+                     s->d_block_idx.get(), s->n_blocks, s->d_counters.get() + 2));
   VGX_TRY(vgx_submap_build_view(c, s, s->d_dw.get(), s->d_view.get()));
   VGX_TRY(check_uploaded_blocks(c, s));
   return vgx_submap_build_grid(c, s);
@@ -590,9 +582,8 @@ extern "C" int vgx_submap_download(vgx_ctx* c, uint32_t id, int max_blocks, int3
     if (distance || weight) {
       float *tmp_d, *tmp_w;
       VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(tmp_d, nvox), vgx_part(tmp_w, nvox)));
-      deinterleave_kernel<<<(unsigned)((nvox + 255) / 256), 256, 0, c->stream>>>(s->d_dw.get(), tmp_d, tmp_w, nvox);
-      c->launches++;
-      VGX_CUDA(c, cudaGetLastError());
+      VGX_TRY(vgx_launch(c, deinterleave_kernel, (unsigned)((nvox + 255) / 256), 256, 0, VgxLaunch::plain,
+                         s->d_dw.get(), tmp_d, tmp_w, nvox));
       if (distance)
         VGX_CUDA(c, cudaMemcpyAsync(distance, tmp_d, nvox * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
       if (weight)

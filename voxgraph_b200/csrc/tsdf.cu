@@ -681,8 +681,8 @@ static int tsdf_sort_and_apply(vgx_ctx* c, VgxSubmap* s, const TsdfParams& P, co
   int end_bit = 1;
   while (end_bit < 32 && (1ull << end_bit) <= sent64) end_bit++;
   size_t sort_tmp = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (unsigned*)nullptr, (unsigned*)nullptr, (SortValue*)nullptr,
-                                  (SortValue*)nullptr, (int)total, 0, end_bit, stream);
+  VGX_CUDA(c, cub::DeviceRadixSort::SortPairs(nullptr, sort_tmp, (unsigned*)nullptr, (unsigned*)nullptr,
+                                              (SortValue*)nullptr, (SortValue*)nullptr, (int)total, 0, end_bit, stream));
   unsigned *k_in, *k_out, *d_nlong, *d_heads;
   Tuple *v_in, *v_out;
   char* d_sort_tmp;
@@ -690,21 +690,21 @@ static int tsdf_sort_and_apply(vgx_ctx* c, VgxSubmap* s, const TsdfParams& P, co
                     vgx_part(v_out, total), vgx_part(d_nlong, 64),
                     vgx_part(d_heads, (size_t)total / VGX_TSDF_LONG_SEGMENT + 2), vgx_part(d_sort_tmp, sort_tmp)));
   uint32_t* d_rgba = kColour ? s->d_rgba.get() : nullptr;
-  VgxLaunchScope scope(c, VGX_SLOT_TSDF_INTEGRATE, 4);
+  VgxProfileScope scope(c, VGX_SLOT_TSDF_INTEGRATE);
   VGX_CUDA(c, cudaMemsetAsync(d_nlong, 0, 256, stream));
-  tsdf_emit_kernel<kColour><<<grid, 128, 0, stream>>>(P, d_pts, d_ray_rgba, s->hash(), d_offsets, sentinel, k_in,
-                                                       v_in, d_stats);
-  cub::DeviceRadixSort::SortPairs(d_sort_tmp, sort_tmp, k_in, k_out, (SortValue*)v_in, (SortValue*)v_out, (int)total,
-                                  0, end_bit, stream);
-  tsdf_apply_kernel<kColour><<<(total + 255) / 256, 256, 0, stream>>>(
-      k_out, v_out, total, sentinel, s->d_dw.get(), d_rgba, P.cfg.default_truncation_distance, P.cfg.max_weight,
-      d_heads, d_nlong);
+  VGX_TRY(vgx_launch(c, tsdf_emit_kernel<kColour>, grid, 128, 0, VgxLaunch::plain, P, d_pts, d_ray_rgba, s->hash(),
+                     d_offsets, sentinel, k_in, v_in, d_stats));
+  VGX_CUDA(c, cub::DeviceRadixSort::SortPairs(d_sort_tmp, sort_tmp, k_in, k_out, (SortValue*)v_in, (SortValue*)v_out,
+                                              (int)total, 0, end_bit, stream));
+  vgx_count_launch(c);
+  VGX_TRY(vgx_launch(c, tsdf_apply_kernel<kColour>, (total + 255) / 256, 256, 0, VgxLaunch::plain, k_out, v_out, total,
+                     sentinel, s->d_dw.get(), d_rgba, P.cfg.default_truncation_distance, P.cfg.max_weight, d_heads,
+                     d_nlong));
   // at most total / 64 long segments; launch enough warps, the surplus exits
   const unsigned max_long = total / VGX_TSDF_LONG_SEGMENT + 1;
-  tsdf_apply_long_kernel<kColour><<<(max_long + 3) / 4, 128, 0, stream>>>(
-      k_out, v_out, total, s->d_dw.get(), d_rgba, P.cfg.default_truncation_distance, P.cfg.max_weight, d_heads,
-      d_nlong, d_stats + 3);
-  return VGX_OK;
+  return vgx_launch(c, tsdf_apply_long_kernel<kColour>, (max_long + 3) / 4, 128, 0, VgxLaunch::plain, k_out, v_out, total,
+                    s->d_dw.get(), d_rgba, P.cfg.default_truncation_distance, P.cfg.max_weight, d_heads, d_nlong,
+                    d_stats + 3);
 }
 
 int vgx_tsdf_check(vgx_ctx* c, uint32_t id, const float T_G_C[7], const vgx_tsdf_config* cfg, VgxSubmap** out,
@@ -746,17 +746,17 @@ int vgx_tsdf_integrate_resident(vgx_ctx* c, VgxSubmap* s, const float T_G_C[7], 
   if (P.cfg.mode == 0) {
     // ---- ray-ordered path: allocate -> count -> scan -> emit -> stable sort by voxel -> apply
     {
-      VgxLaunchScope scope(c, VGX_SLOT_TSDF_ALLOCATE);
-      tsdf_allocate_kernel<<<grid, 128, 0, stream>>>(P, d_pts, s->hash(), s->d_block_idx.get(), s->d_counters.get(),
-                                                    s->cap_blocks);
+      VgxProfileScope scope(c, VGX_SLOT_TSDF_ALLOCATE);
+      VGX_TRY(vgx_launch(c, tsdf_allocate_kernel, grid, 128, 0, VgxLaunch::plain, P, d_pts, s->hash(), s->d_block_idx.get(),
+                         s->d_counters.get(), s->cap_blocks));
     }
     unsigned *d_counts, *d_offsets, *d_scan_tmp;
     VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_counts, (size_t)n + 2), vgx_part(d_offsets, (size_t)n + 2),
                       vgx_part(d_scan_tmp, vgx_scan_tmp_count((size_t)n))));
     unsigned total = 0;
     {
-      VgxLaunchScope scope(c, VGX_SLOT_TSDF_INTEGRATE, 1);
-      tsdf_count_kernel<<<grid, 128, 0, stream>>>(P, d_pts, d_counts);
+      VgxProfileScope scope(c, VGX_SLOT_TSDF_INTEGRATE);
+      VGX_TRY(vgx_launch(c, tsdf_count_kernel, grid, 128, 0, VgxLaunch::plain, P, d_pts, d_counts));
       VGX_TRY(vgx_exclusive_scan_u32(c, d_counts, d_offsets, (size_t)n, d_scan_tmp));   // hand-written, 3 launches
     }
     VGX_CUDA(c, cudaMemcpyAsync(&total, d_offsets + n, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
@@ -767,17 +767,11 @@ int vgx_tsdf_integrate_resident(vgx_ctx* c, VgxSubmap* s, const float T_G_C[7], 
     }
   } else {
     // ---- Fast scheduling: one kernel, blocks allocated on demand
-    VgxLaunchScope scope(c, VGX_SLOT_TSDF_INTEGRATE);
-    if (rgba)
-      tsdf_integrate_kernel<true><<<grid, 128, 0, stream>>>(P, d_pts, d_ray_rgba, s->hash(), s->d_block_idx.get(),
-                                                           s->d_counters.get(), s->cap_blocks, s->d_dw.get(),
-                                                           s->d_rgba.get(), d_stats, d_start, d_obs);
-    else
-      tsdf_integrate_kernel<false><<<grid, 128, 0, stream>>>(P, d_pts, nullptr, s->hash(), s->d_block_idx.get(),
-                                                            s->d_counters.get(), s->cap_blocks, s->d_dw.get(),
-                                                            nullptr, d_stats, d_start, d_obs);
+    VgxProfileScope scope(c, VGX_SLOT_TSDF_INTEGRATE);
+    VGX_TRY(vgx_launch(c, rgba ? tsdf_integrate_kernel<true> : tsdf_integrate_kernel<false>, grid, 128, 0,
+                       VgxLaunch::plain, P, d_pts, d_ray_rgba, s->hash(), s->d_block_idx.get(), s->d_counters.get(),
+                       s->cap_blocks, s->d_dw.get(), rgba ? s->d_rgba.get() : nullptr, d_stats, d_start, d_obs));
   }
-  VGX_CUDA(c, cudaGetLastError());
   unsigned long long h_stats[VGX_TSDF_STAT_CALLER + 1];
   int h_counters[2];
   VGX_CUDA(c, cudaMemcpyAsync(h_stats, d_stats, sizeof(h_stats), cudaMemcpyDeviceToHost, stream));

@@ -231,6 +231,7 @@ struct vgx_ctx {
   bool profile = false;
   VgxProfileSlot prof[VGX_PROFILE_SLOTS];
   int64_t launches = 0;
+  int slot = -1;              // the slot of the innermost open VgxProfileScope, -1 outside every scope
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   // Scratch arenas.  They grow (discard-and-grow) and never shrink; a call lays its parts out in one
   // with vgx_carve, and the parts are valid until the next vgx_carve of the same arena.  A function
@@ -366,26 +367,79 @@ int vgx_carve(vgx_ctx* c, VgxBuffer<>& arena, VgxPart<T>... parts) {
   return VGX_OK;
 }
 
-// RAII-less helper to bracket kernel launches for accounting.
-struct VgxLaunchScope {
+// ------------------------------------------------------------------ kernel launches
+// The one place that counts launches and writes the profile slots.  A profile scope names the slot of the
+// launches inside it and, while profiling is enabled, times its region into that slot with two events on the
+// context's stream.  A launch outside every scope counts in the total only.
+struct VgxProfileScope {
   vgx_ctx* c;
-  int which;
-  VgxLaunchScope(vgx_ctx* ctx, int w, int n_launches = 1) : c(ctx), which(w) {
-    c->launches += n_launches;
-    c->prof[which].launches += n_launches;
+  int slot, outer;
+  VgxProfileScope(vgx_ctx* ctx, int s) : c(ctx), slot(s), outer(ctx->slot) {
+    c->slot = s;
     if (c->profile) cudaEventRecord(c->ev0, c->stream);
   }
-  ~VgxLaunchScope() {
+  ~VgxProfileScope() {
     if (c->profile) {
       cudaEventRecord(c->ev1, c->stream);
       cudaEventSynchronize(c->ev1);
       float ms = 0;
       cudaEventElapsedTime(&ms, c->ev0, c->ev1);
-      c->prof[which].total_ms += ms;
+      c->prof[slot].total_ms += ms;
     }
+    c->slot = outer;
   }
 };
 
+// one launch into the total and the open scope's slot; a library call that launches kernels of its own
+// (a cub sort) counts as one launch through this call
+static inline void vgx_count_launch(vgx_ctx* c) {
+  ++c->launches;
+  if (c->slot >= 0) ++c->prof[c->slot].launches;
+}
+
+// vgx_profile_reset: every slot and the total back to zero
+static inline void vgx_reset_counts(vgx_ctx* c) {
+  for (auto& p : c->prof) p = VgxProfileSlot();
+  c->launches = 0;
+}
+
+// plain: as <<<>>>.  pdl: programmatic stream serialisation, the kernel may be scheduled while the one
+// ahead of it on the stream is still running and waits for it at griddepcontrol.wait.  cooperative: the
+// grid is co-resident as a whole (grid-wide synchronisation).
+enum class VgxLaunch { plain, pdl, cooperative };
+
+// Every kernel of the library is launched here, on the context's stream, with its arguments converted
+// as <<<>>> converts them.  A launch that fails leaves no last error behind for a later check to find:
+// the message is set as VGX_CUDA sets it and the status is VGX_ERR_CUDA.
+template <class... P, class... A>
+int vgx_launch(vgx_ctx* c, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, VgxLaunch mode,
+               A&&... args) {
+  cudaLaunchAttribute attr = {};
+  if (mode == VgxLaunch::pdl) {
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr.val.programmaticStreamSerializationAllowed = 1;
+  } else if (mode == VgxLaunch::cooperative) {
+    attr.id = cudaLaunchAttributeCooperative;
+    attr.val.cooperative = 1;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = c->stream;
+  cfg.attrs = &attr;
+  cfg.numAttrs = mode == VgxLaunch::plain ? 0 : 1;
+  vgx_count_launch(c);
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    c->set_error(std::string("kernel launch: ") + cudaGetErrorString(e));
+    return VGX_ERR_CUDA;
+  }
+  return VGX_OK;
+}
+
+// ------------------------------------------------------------------ passes shared by the translation units
 int vgx_submap_build_grid(vgx_ctx* ctx, VgxSubmap* s);
 // a new, empty submap (replaces submap_id) with room for cap blocks; with_view: registration view storage
 int vgx_submap_alloc(vgx_ctx* ctx, uint32_t submap_id, float voxel_size, int vps, int cap, bool with_view,
