@@ -290,7 +290,7 @@ int vgx_mesh_ply_ex(vgx_ctx* ctx, const uint8_t* rgba, int voxel_colours, uint8_
 /* ------------------------------------------------------------------ projected global map */
 /* cblox SubmapCollection::getProjectedMap: every submap merged, at its pose, into one mission-frame TSDF
  * layer (voxblox mergeLayerAintoLayerB = transformLayer + the untransformed merge).  What
- * save_combined_mesh / publish_combined_mesh (cblox generateCombinedMesh: vgx_mesh_build on the result),
+ * save_combined_mesh / publish_combined_mesh (cblox generateCombinedMesh: vgx_mesh_build_combined below),
  * ProjectedMapServer and MapEvaluation consume.  The rule is restated from the published voxblox / cblox
  * sources and has not been checked against a compiled voxblox (see csrc/project.cu; the CPU restatement
  * tests/project_oracle.c pins it bit for bit):
@@ -321,6 +321,13 @@ int vgx_mesh_ply_ex(vgx_ctx* ctx, const uint8_t* rgba, int voxel_colours, uint8_
  * scratch. */
 int vgx_project_map(vgx_ctx* ctx, int n, const uint32_t* submap_ids, const float* T_M_S /* n x 7 */,
                     uint32_t out_id, int* n_blocks);
+/* cblox SubmapMesher::generateCombinedMesh: vgx_project_map of the n submaps at T_M_S (n x 7) into a scratch
+ * submap (the first unused id counting down from 2^32 - 2), vgx_mesh_build of that one submap with cfg (may be
+ * NULL: defaults), and the scratch submap freed on every exit, so the context's submaps are unchanged.  The mesh
+ * is left in the context's mesh buffer for vgx_mesh_download / vgx_mesh_ply_ex; SubmapVisuals::saveCombinedMesh
+ * is vgx_mesh_ply_ex with voxel_colours = 1 and one colour.  Errors are those of the two calls. */
+int vgx_mesh_build_combined(vgx_ctx* ctx, int n, const uint32_t* submap_ids, const float* T_M_S /* n x 7 */,
+                            const vgx_mesh_config* cfg);
 
 /* Registration points of a submap = WeightedSampler<RegistrationPoint> items
  * (include/voxgraph/frontend/submap_collection/registration_point.h:6-12).
@@ -502,9 +509,15 @@ int vgx_graph_set_nodes(vgx_ctx* ctx, int n, const uint32_t* submap_ids, const d
 int vgx_graph_set_poses(vgx_ctx* ctx, const double* xyzyaw);
 int vgx_graph_get_poses(vgx_ctx* ctx, double* xyzyaw);
 /* add{Relative,Absolute}PoseConstraint: m edges, observed [tx,ty,tz,yaw], sqrt-information
- * (lower LLT factor, row-major 4x4, constraint.cpp:8-14). */
+ * (vgx_sqrt_information of the edge's information matrix, row-major 4x4). */
 int vgx_graph_set_relative_edges(vgx_ctx* ctx, int m, const uint32_t* ids_a, const uint32_t* ids_b,
                                  const double* t_obs_xyzyaw, const double* sqrt_info);
+/* Host-only: the Constraint constructor's square-root information factor (constraint.cpp:4-38) of a
+ * row-major 4x4 information matrix.  allow_semi_definite = 0: the lower LLT factor, rejected when a pivot
+ * is not > 0.  allow_semi_definite != 0: Eigen's LDLT with diagonal pivoting, sqrt = P^T L sqrt(D) P,
+ * rejected when a pivot is below -1e-12 * (1 + max |diagonal entry|); a pivot between that bound and 0 gives a zero column.
+ * A rejected matrix or a NULL pointer gives VGX_ERR_INVALID. */
+int vgx_sqrt_information(const double information[16], int allow_semi_definite, double sqrt_information[16]);
 /* One entry per registration residual block (reference -> reading). The caller adds the
  * mirrored block for isosurface points as PoseGraph::addRegistrationConstraint does
  * (pose_graph.cpp:63-71). Replaces the previous list (resetRegistrationConstraints). */

@@ -23,19 +23,28 @@ int main(int argc, char** argv) {
     ctx.check(vgx_submap_info(ctx.get(), 777u, &vs, &vps, &nb, &finished));
     if (nb != n_blocks || !finished) { std::printf("projected submap inconsistent\n"); return 1; }
     ctx.check(vgx_submap_free(ctx.get(), 777u));
+    // the submap set is unchanged after every combined-mesh call: the inputs are there, and neither the
+    // projection nor the scratch submap (the fixture holds id 2^32 - 1, so the first free id is 2^32 - 2) is
+    const auto unchanged = [&] {
+      for (SubmapID id : ids)
+        if (vgx_submap_info(ctx.get(), id, nullptr, nullptr, nullptr, nullptr) != VGX_OK) return false;
+      for (SubmapID id : {777u, 0xFFFFFFFEu})
+        if (vgx_submap_info(ctx.get(), id, nullptr, nullptr, nullptr, nullptr) != VGX_ERR_NOT_FOUND) return false;
+      return true;
+    };
     const SeparatedMesh m = GenerateCombinedMesh(ctx, ids, poses);
     if ((size_t)m.vertex_offsets.back() * 3 != m.xyz.size() || (size_t)m.triangle_offsets.back() * 3 != m.triangles.size()) {
       std::printf("inconsistent offsets\n");
       return 1;
     }
+    if (!unchanged()) { std::printf("submap set changed\n"); return 1; }
     bool threw = false;
     try { GenerateCombinedMesh(ctx, {ids[0], 12345u}, {poses[0], poses[0]}); }
     catch (const Error& e) { threw = e.code() == VGX_ERR_NOT_FOUND; }
     if (!threw) { std::printf("unknown id not refused\n"); return 1; }
-    // the fixture holds id 2^32 - 1, so the scratch submap is 2^32 - 2; it is gone after every call
-    if (ProjectionScratchId(ctx, {}) != 0xFFFFFFFEu) { std::printf("scratch submap left behind\n"); return 1; }
+    if (!unchanged()) { std::printf("submap set changed\n"); return 1; }
     SaveCombinedMesh(ctx, argv[2], ids, poses);
-    if (ProjectionScratchId(ctx, {}) != 0xFFFFFFFEu) { std::printf("scratch submap left behind\n"); return 1; }
+    if (!unchanged()) { std::printf("submap set changed\n"); return 1; }
     std::printf("COMBINED_OK submaps=%zu blocks=%d vertices=%zu triangles=%zu\n", ids.size(), n_blocks,
                 m.xyz.size() / 3, m.triangles.size() / 3);
     return 0;

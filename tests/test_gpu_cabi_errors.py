@@ -93,6 +93,7 @@ ROWS = [
     ("vgx_mesh_ply", lambda: (None, None, 0, None), INVALID),
     ("vgx_mesh_ply_ex", lambda: (None, 0, None, 0, None), INVALID),
     ("vgx_project_map", lambda: (1, _ids(U), _pose(), U + 1, None), NOT_FOUND),
+    ("vgx_mesh_build_combined", lambda: (1, _ids(U), _pose(), None), NOT_FOUND),
     ("vgx_layer_load", lambda: (U, None, 5, None), INVALID),
     ("vgx_submap_transform", lambda: (U, _pose()), NOT_FOUND),
     ("vgx_evaluate_layers_rmse", lambda: (U, 0, U + 1, 0, C.byref(_lib.VoxelEvaluationDetails())), NOT_FOUND),
@@ -105,7 +106,7 @@ ROWS = [
 ]
 
 CONTEXT_FREE = {"vgx_device_count", "vgx_ctx_create", "vgx_ctx_destroy", "vgx_collection_scan",
-                "vgx_shard_constraints", "vgx_comm_unique_id"}
+                "vgx_shard_constraints", "vgx_sqrt_information", "vgx_comm_unique_id"}
 ACCESSORS = {"vgx_last_error", "vgx_ctx_stream", "vgx_launch_count"}
 
 

@@ -160,14 +160,15 @@ def test_errors_release_and_ply_paths(ctx):
     vo, to = ctx.mesh_build([a, b], None, cfg)
     xyz, tri = ctx.mesh_download()
     assert len(tri) > 0 and vo[-1] == len(xyz) and to[-1] == len(tri)
-    # PLY: the default palette equals submap_colour, and the file parses back to the mesh
+    # PLY: the default palette is rainbowColorMap((id mod 20) / 20), and the file parses back to the mesh
     data = ctx.mesh_ply()
-    assert bytes(data) == bytes(ctx.mesh_ply(np.stack([api.submap_colour(a), api.submap_colour(b)])))
+    assert bytes(data) == bytes(ctx.mesh_ply(np.array([me.rainbow((a % 20) / 20.0), me.rainbow((b % 20) / 20.0)],
+                                                      np.uint8)))
     px, prgba, ptri = me.read_ply(data)
     same_bits(xyz, px, "ply vertices")
     assert np.array_equal(ptri, tri.astype(np.int64))
     for k, sid in enumerate((a, b)):
-        assert (prgba[vo[k]:vo[k + 1]] == api.submap_colour(sid)).all()
+        assert (prgba[vo[k]:vo[k + 1]] == me.rainbow((sid % 20) / 20.0)).all()
     # size query, capacity error, exact capacity
     L, h = ctx._L, ctx._h
     size = C.c_uint64(0)
@@ -196,6 +197,21 @@ def test_errors_release_and_ply_paths(ctx):
     px, _, ptri = me.read_ply(ctx.mesh_ply())
     assert len(px) == 0 and len(ptri) == 0
     ctx.submap_free(a); ctx.submap_free(b)
+
+
+def test_default_palette_is_rainbow_of_id_mod_20(ctx):
+    """vgx_mesh_ply without colours gives submap id k rainbowColorMap((k mod 20) / 20): one full cycle, its wrap
+    and the largest id."""
+    lay = fx.layer((0.1, 8), "box", "sphere")
+    ids = list(range(21)) + [2 ** 32 - 1]
+    for sid in ids:
+        ctx.submap_upload(sid, *lay)
+    vo, _ = ctx.mesh_build(ids, None, ctx.mesh_config(min_weight=1.0))
+    _, rgba, _ = me.read_ply(ctx.mesh_ply())
+    for k, sid in enumerate(ids):
+        assert vo[k + 1] > vo[k] and (rgba[vo[k]:vo[k + 1]] == me.rainbow((sid % 20) / 20.0)).all(), sid
+    for sid in ids:
+        ctx.submap_free(sid)
 
 
 def test_non_interference_and_repeatability(ctx, pair_scene):

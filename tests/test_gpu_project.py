@@ -21,6 +21,7 @@ pytestmark = pytest.mark.gpu
 _ids = itertools.count(20000)
 F32 = np.float32
 LAUNCHES = 15    # candidates, sort, flags, 2 scans (3 each), scatter, occupancy, scan (3), fold
+SCRATCH_ID = 0xFFFFFFFE   # vgx_mesh_build_combined's scratch submap while the context holds no id above 20000
 
 
 def _oracle(oracle, layers, poses, ids):
@@ -193,12 +194,14 @@ def test_combined_mesh_equals_restatement(ctx, oracle):
         same_bits(ex, xyz, "combined vertices")
         same_bits(et.astype(np.uint32), tri, "combined triangles")
         assert len(tri) > 0
-        assert not exists(ctx, api.PROJECTION_SCRATCH_ID)
-    # projected_map returns the same layer and frees its scratch submap
-    got = api.projected_map(ctx, ids, T)
+        assert not exists(ctx, SCRATCH_ID)   # the projection's scratch submap is freed again
+    # the projected map it meshes is the restatement's layer
+    out = next(_ids)
+    ctx.project_map(ids, T, out)
+    got = ctx.submap_download(out)
+    ctx.submap_free(out)
     for x, y in zip((idx, d, w), got):
         assert np.asarray(x).tobytes() == y.tobytes()
-    assert not exists(ctx, api.PROJECTION_SCRATCH_ID)
     for sid in ids:
         ctx.submap_free(sid)
 

@@ -25,7 +25,8 @@ NESTED = {"vgx_ctx_destroy": {"vgx_comm_destroy"},
           "vgx_collection_load": {"vgx_collection_load_ex"},
           "vgx_mesh_ply": {"vgx_mesh_ply_ex"},
           "vgx_submap_finish_ex": {"vgx_submap_finish", "vgx_submap_extract_points"},
-          "vgx_map_evaluate": {"vgx_project_map", "vgx_submap_transform", "vgx_evaluate_layers_rmse"}}
+          "vgx_map_evaluate": {"vgx_project_map", "vgx_submap_transform", "vgx_evaluate_layers_rmse"},
+          "vgx_mesh_build_combined": {"vgx_project_map", "vgx_mesh_build"}}
 
 
 def _close(text, i, o, c):

@@ -194,9 +194,9 @@ def test_separated_offsets_and_transform():
 
 
 def test_palette():
-    from voxgraph_b200 import api
-    assert api.submap_colour(0).tolist() == [255, 0, 0, 255]
-    for i in range(45):
-        assert api.submap_colour(i).tolist() == me.rainbow((i % 20) / 20.0)
-    assert api.submap_colour(2 ** 32 - 1).tolist() == me.rainbow(((2 ** 32 - 1) % 20) / 20.0)
-    assert len({tuple(api.submap_colour(i)) for i in range(20)}) == 20
+    """The default submap colour, rainbowColorMap((id mod 20) / 20): id 0 is red, the 20 colours of a cycle
+    differ, and the largest id wraps like any other."""
+    colour = lambda i: me.rainbow((i % 20) / 20.0)   # noqa: E731
+    assert colour(0) == [255, 0, 0, 255]
+    assert colour(20) == colour(0) and colour(2 ** 32 - 1) == colour(15)
+    assert len({tuple(colour(i)) for i in range(20)}) == 20

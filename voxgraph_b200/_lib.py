@@ -199,6 +199,7 @@ SIGNATURES = {
     "vgx_mesh_ply_ex": (_i32, [_vp, _pu8, _i32, _vp, _u64, _pu64]),
     # projected global map, registration points
     "vgx_project_map": (_i32, [_vp, _i32, _pu32, _pf, _u32, _pi32]),
+    "vgx_mesh_build_combined": (_i32, [_vp, _i32, _pu32, _pf, _P(MeshConfig)]),
     "vgx_submap_upload_points": (_i32, [_vp, _u32, _i32, _i32, _pf, _pf, _pf]),
     # b3: TSDF integration, point-cloud messages
     "vgx_tsdf_config_default": (None, [_P(TsdfConfig)]),
@@ -217,6 +218,7 @@ SIGNATURES = {
     "vgx_graph_set_poses": (_i32, [_vp, _pd]),
     "vgx_graph_get_poses": (_i32, [_vp, _pd]),
     "vgx_graph_set_relative_edges": (_i32, [_vp, _i32, _pu32, _pu32, _pd, _pd]),
+    "vgx_sqrt_information": (_i32, [_pd, _i32, _pd]),
     "vgx_graph_set_registration_constraints": (_i32, [_vp, _i32, _pu32, _pu32, _P(RegConfig)]),
     "vgx_graph_set_registration_constraints_v": (_i32, [_vp, _i32, _pu32, _pu32, _P(RegConfig)]),
     "vgx_graph_get_sample_indices": (_i32, [_vp, _i32, _i32, _pi32, _pi32]),

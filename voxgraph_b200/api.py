@@ -348,6 +348,13 @@ class Context:
                                             int(out_id), C.byref(n)))
         return n.value
 
+    def mesh_build_combined(self, submap_ids, poses_T, cfg=None):
+        """cblox SubmapMesher::generateCombinedMesh: the mesh of the submaps' projected map (T_M_S (n, 7)) into the
+        context's mesh buffer, through a scratch submap that is freed again."""
+        ids, T = _ids_poses(submap_ids, poses_T, "mesh_build_combined")
+        self._check(self._L.vgx_mesh_build_combined(self._h, len(ids), _p(ids, C.c_uint32), _p(T, C.c_float),
+                                                    _ref(cfg)))
+
     # ---- map evaluation (voxgraph MapEvaluation)
     def layer_load(self, submap_id, data):
         """voxblox::io::LoadLayer<TsdfVoxel> of a layer file's bytes into a new finished submap -> block count."""
@@ -723,20 +730,6 @@ def save_submap_collection(ctx, path, submap_ids, poses_T):
     return len(data)
 
 
-def submap_colour(submap_id):
-    """voxblox rainbowColorMap((id mod 20) / 20), the colour voxgraph gives a submap -> uint8 [r, g, b, a]."""
-    h = (int(submap_id) % 20) / 20.0
-    h -= np.floor(h)
-    h *= 6
-    i = int(np.floor(h))
-    f = h - i
-    if not (i & 1):
-        f = 1 - f
-    n = 1 - f
-    r, g, b = [(1, n, 0), (n, 1, 0), (0, 1, n), (0, n, 1), (n, 0, 1), (1, 0, n)][i % 6]
-    return np.array([int(255 * r), int(255 * g), int(255 * b), 255], np.uint8)
-
-
 def separated_mesh(ctx, submap_ids, poses_T=None, min_weight=2.0):
     """cblox SubmapMesher::generateSeparatedMesh on the device -> (xyz (V, 3) float32 in the mission
     frame, triangles (T, 3) uint32, vertex_offsets (n + 1,), triangle_offsets (n + 1,))."""
@@ -747,59 +740,19 @@ def separated_mesh(ctx, submap_ids, poses_T=None, min_weight=2.0):
 
 def save_separated_mesh(ctx, path, submap_ids, poses_T, colours=None, min_weight=2.0):
     """SubmapVisuals::saveSeparatedMesh: the submaps at poses T_M_S (n, 7) as a binary PLY, one colour
-    per submap (default: submap_colour(id)).  Returns the file size in bytes."""
+    per submap (rgba (n, 4); default: the library's palette, voxblox rainbowColorMap((id mod 20) / 20)).
+    Returns the file size in bytes."""
     ctx.mesh_build(submap_ids, poses_T, ctx.mesh_config(min_weight=min_weight))
-    if colours is None:
-        colours = np.array([submap_colour(i) for i in np.asarray(submap_ids).reshape(-1)], np.uint8).reshape(-1, 4)
     data = ctx.mesh_ply(colours)
     with open(path, "wb") as f:
         f.write(data)
     return len(data)
 
 
-PROJECTION_SCRATCH_ID = 0xFFFFFFFF   # where the helpers below start looking for a free scratch submap id
-
-
-def projection_scratch_id(ctx, submap_ids):
-    """The submap id the projection helpers use and free again: the first id counting down from
-    PROJECTION_SCRATCH_ID that is neither an input nor present in ctx (2^32 - 1 is a valid cblox id)."""
-    taken = set(int(i) for i in np.asarray(submap_ids).reshape(-1))
-    sid = PROJECTION_SCRATCH_ID
-    while True:
-        if sid not in taken:
-            try:
-                ctx.submap_info(sid)
-            except VgxError as e:
-                if e.code != _lib.VGX_ERR_NOT_FOUND:
-                    raise
-                return sid
-        sid -= 1
-
-
-def projected_map(ctx, submap_ids, poses_T):
-    """cblox SubmapCollection::getProjectedMap on the device -> (block_idx (B, 3) int32, distance (B, vps^3),
-    weight (B, vps^3)), blocks in ascending packed key order.  Projects into projection_scratch_id and frees it."""
-    sid = projection_scratch_id(ctx, submap_ids)
-    ctx.project_map(submap_ids, poses_T, sid)
-    try:
-        return ctx.submap_download(sid)
-    finally:
-        ctx.submap_free(sid)
-
-
-def _combined_mesh_build(ctx, submap_ids, poses_T, min_weight):
-    sid = projection_scratch_id(ctx, submap_ids)
-    ctx.project_map(submap_ids, poses_T, sid)
-    try:
-        ctx.mesh_build([sid], None, ctx.mesh_config(min_weight=min_weight))
-    finally:
-        ctx.submap_free(sid)
-
-
 def combined_mesh(ctx, submap_ids, poses_T, min_weight=2.0):
     """cblox SubmapMesher::generateCombinedMesh on the device: the mesh of the projected global map (one
     surface where submaps overlap) -> (xyz (V, 3) float32 in the mission frame, triangles (T, 3) uint32)."""
-    _combined_mesh_build(ctx, submap_ids, poses_T, min_weight)
+    ctx.mesh_build_combined(submap_ids, poses_T, ctx.mesh_config(min_weight=min_weight))
     return ctx.mesh_download()
 
 
@@ -807,7 +760,7 @@ def save_combined_mesh(ctx, path, submap_ids, poses_T, colour=None, min_weight=2
     """voxgraph's save_combined_mesh service: the combined mesh as a binary PLY, as SubmapVisuals::saveCombinedMesh
     writes it: the voxel colours of the projected map where a submap had a colour channel, else the one colour
     given (rgba, default opaque white).  Returns the file size in bytes."""
-    _combined_mesh_build(ctx, submap_ids, poses_T, min_weight)
+    ctx.mesh_build_combined(submap_ids, poses_T, ctx.mesh_config(min_weight=min_weight))
     rgba = np.array([255, 255, 255, 255] if colour is None else colour, np.uint8).reshape(1, 4)
     data = ctx.mesh_ply(rgba, voxel_colours=True)
     with open(path, "wb") as f:
@@ -884,35 +837,14 @@ class AbsolutePoseConstraintConfig:   # absolute_pose_constraint.h:13-18
 
 def sqrt_information_matrix(information_matrix, allow_semi_definite=False):
     """Constraint ctor (constraint.cpp:4-38): the LLT lower factor, or for semi-definite matrices
-    Eigen's pivoted LDLT, sqrt = P^T L sqrt(D) P. Raises like the reference CHECKs."""
-    info = np.asarray(information_matrix, np.float64).reshape(4, 4)
-    if not allow_semi_definite:
-        try:
-            return np.linalg.cholesky(info)
-        except np.linalg.LinAlgError:
-            raise ValueError("The square root of the information matrix could not be computed, "
-                             "make sure it is symmetric and positive definite")
-    A = info.copy()
-    perm = np.arange(4)
-    for k in range(4):
-        piv = k + int(np.argmax(np.abs(np.diag(A)[k:])))
-        if piv != k:
-            A[[k, piv], :] = A[[piv, k], :]
-            A[:, [k, piv]] = A[:, [piv, k]]
-            perm[[k, piv]] = perm[[piv, k]]
-        d = A[k, k]
-        if d < -1e-12 * (1.0 + np.abs(np.diag(info)).max()):
-            raise ValueError("The information matrix must be positive semi-definite")
-        if abs(d) > 0:
-            A[k + 1:, k] /= d
-            A[k + 1:, k + 1:] -= np.outer(A[k + 1:, k], A[k + 1:, k]) * d
-        else:
-            A[k + 1:, k] = 0
-        A[k, k + 1:] = 0
-    Lm = np.tril(A, -1) + np.eye(4)
-    M = Lm * np.sqrt(np.maximum(np.diag(A), 0.0))[None, :]
+    Eigen's pivoted LDLT, sqrt = P^T L sqrt(D) P (vgx_sqrt_information). Raises like the reference CHECKs."""
+    info = _f64(information_matrix).reshape(4, 4)
     S = np.zeros((4, 4))
-    S[np.ix_(perm, perm)] = M
+    rc = _lib.load().vgx_sqrt_information(_p(info, C.c_double), int(bool(allow_semi_definite)), _p(S, C.c_double))
+    if rc != _lib.VGX_OK:
+        raise ValueError("The information matrix must be positive semi-definite" if allow_semi_definite else
+                         "The square root of the information matrix could not be computed, "
+                         "make sure it is symmetric and positive definite")
     return S
 
 

@@ -295,13 +295,22 @@ assemble_exchange_kernel(const double* __restrict__ csum, const VgxRelEdge* __re
                 (size_t)gridDim.x * blockDim.x, block_mask, N);
 }
 
-// ------------------------------------------------------------------ sharding (host only)
+// ------------------------------------------------------------------ host only: sharding, square-root information
 extern "C" int vgx_shard_constraints(int nranks, int n, const int32_t* num_residuals,
                                      const uint32_t* locality_keys, int32_t* owner) {
   return vgx_entry_noctx([&] {
     if (nranks < 1 || n < 0 || (n > 0 && (!num_residuals || !owner))) return VGX_ERR_INVALID;
     vgx_partition_constraints(nranks, n, num_residuals, locality_keys, owner);
     return VGX_OK;
+  });
+}
+
+extern "C" int vgx_sqrt_information(const double information[16], int allow_semi_definite,
+                                    double sqrt_information[16]) {
+  return vgx_entry_noctx([&] {
+    if (!information || !sqrt_information) return VGX_ERR_INVALID;
+    return vgx_sqrt_information_factor(information, allow_semi_definite != 0, sqrt_information) ? VGX_OK
+                                                                                                : VGX_ERR_INVALID;
   });
 }
 

@@ -1,7 +1,9 @@
-// Layout of the pose-graph tables (see graph_plan.h).  Plain C++: every decision here can be checked without a GPU.
+// Layout of the pose-graph tables and the square-root information factor (see graph_plan.h).  Plain C++: every
+// decision here can be checked without a GPU.
 #include "graph_plan.h"
 
 #include <algorithm>
+#include <cmath>
 #include <map>
 #include <numeric>
 #include <utility>
@@ -22,6 +24,53 @@ void vgx_partition_constraints(int nranks, int n, const int32_t* num_residuals, 
     owner[i] = std::min(std::max(r, 0), nranks - 1);
     before += cnt;
   }
+}
+
+bool vgx_sqrt_information_factor(const double info[16], bool allow_semi_definite, double S[16]) {
+  std::fill(S, S + 16, 0.0);
+  if (!allow_semi_definite) {
+    for (int j = 0; j < 4; ++j) {
+      double d = info[5 * j];
+      for (int k = 0; k < j; ++k) d -= S[4 * j + k] * S[4 * j + k];
+      if (!(d > 0)) return false;
+      S[5 * j] = std::sqrt(d);
+      for (int i = j + 1; i < 4; ++i) {
+        double v = info[4 * i + j];
+        for (int k = 0; k < j; ++k) v -= S[4 * i + k] * S[4 * j + k];
+        S[4 * i + j] = v / S[5 * j];
+      }
+    }
+    return true;
+  }
+  double A[4][4];
+  int perm[4] = {0, 1, 2, 3};
+  double scale = 0;
+  for (int i = 0; i < 4; ++i) {
+    scale = std::max(scale, std::fabs(info[5 * i]));
+    for (int j = 0; j < 4; ++j) A[i][j] = info[4 * i + j];
+  }
+  for (int k = 0; k < 4; ++k) {
+    int piv = k;
+    for (int i = k + 1; i < 4; ++i)
+      if (std::fabs(A[i][i]) > std::fabs(A[piv][piv])) piv = i;
+    if (piv != k) {
+      for (int j = 0; j < 4; ++j) std::swap(A[k][j], A[piv][j]);
+      for (int i = 0; i < 4; ++i) std::swap(A[i][k], A[i][piv]);
+      std::swap(perm[k], perm[piv]);
+    }
+    const double d = A[k][k];
+    if (d < -1e-12 * (1.0 + scale)) return false;
+    for (int i = k + 1; i < 4; ++i) A[i][k] = std::fabs(d) > 0 ? A[i][k] / d : 0.0;
+    for (int i = k + 1; i < 4; ++i)
+      for (int j = k + 1; j < 4; ++j) A[i][j] -= A[i][k] * d * A[j][k];
+    for (int j = k + 1; j < 4; ++j) A[k][j] = 0;
+  }
+  for (int i = 0; i < 4; ++i)
+    for (int j = 0; j <= i; ++j) {
+      const double l = (i == j) ? 1.0 : A[i][j];
+      S[4 * perm[i] + perm[j]] = l * (A[j][j] > 0 ? std::sqrt(A[j][j]) : 0.0);
+    }
+  return true;
 }
 
 VgxGraphPlan vgx_graph_plan(const std::vector<VgxPlanConstraint>& cons, const std::vector<int32_t>& owner,

@@ -1,6 +1,7 @@
 // Layout of the pose-graph tables (graph_plan.cpp): which registration constraints this rank owns, how their
-// points are cut into reduce tiles, how the output blocks are numbered and which items each block sums.  Host
-// only, no CUDA runtime: graph.cu collects the inputs, calls vgx_graph_plan and uploads what it returns.
+// points are cut into reduce tiles, how the output blocks are numbered and which items each block sums; and the
+// square-root information factor of a relative-pose edge.  Host only, no CUDA runtime: graph.cu collects the
+// inputs, calls vgx_graph_plan and uploads what it returns.
 #pragma once
 
 #include <stddef.h>
@@ -63,6 +64,10 @@ struct VgxGraphPlan {
 // keys, stable) and each goes to the rank whose equal share of the total residual count holds its midpoint.
 void vgx_partition_constraints(int nranks, int n, const int32_t* num_residuals, const uint32_t* locality_keys,
                                int32_t* owner);
+
+// The square-root information factor of a relative-pose edge (see vgx_sqrt_information); false when the matrix
+// is rejected.
+bool vgx_sqrt_information_factor(const double info[16], bool allow_semi_definite, double S[16]);
 
 // The tables of rank `rank` for the constraints `cons` partitioned by `owner` (identical on every rank), the
 // relative edges' node pairs `rel`, and N nodes of which constant[i] != 0 are held fixed.  sms: the device's SM

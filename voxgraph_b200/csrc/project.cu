@@ -483,6 +483,17 @@ extern "C" int vgx_project_map(vgx_ctx* c, int n, const uint32_t* ids, const flo
   });
 }
 
+extern "C" int vgx_mesh_build_combined(vgx_ctx* c, int n, const uint32_t* ids, const float* T_M_S,
+                                       const vgx_mesh_config* cfg) {
+  return vgx_entry(c, __func__, [&] {
+    const uint32_t pid = vgx_scratch_id(c);
+    VGX_TRY(vgx_project_map(c, n, ids, T_M_S, pid, nullptr));
+    const int rc = vgx_mesh_build(c, 1, &pid, nullptr, cfg, nullptr, nullptr);
+    vgx_submap_drop(c, pid);
+    return rc;
+  });
+}
+
 extern "C" int vgx_submap_transform(vgx_ctx* c, uint32_t id, const float* T_new_old) {
   return vgx_entry(c, __func__, [&] {
     if (!T_new_old) VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");

@@ -12,7 +12,6 @@
 
 #include <algorithm>
 #include <array>
-#include <cmath>
 #include <cstdint>
 #include <fstream>
 #include <iterator>
@@ -134,53 +133,13 @@ struct AbsolutePoseConstraintConfig {  // AbsolutePoseConstraint::Config
 constexpr uint32_t kFrameNodeIdBase = 0x80000000u;
 
 // Constraint ctor (constraint.cpp:4-38): LLT lower factor, or Eigen's pivoted LDLT
-// (sqrt = P^T L sqrt(D) P) when semi-definite matrices are allowed. Throws like the CHECKs.
+// (sqrt = P^T L sqrt(D) P) when semi-definite matrices are allowed (vgx_sqrt_information). Throws like the CHECKs.
 inline std::array<double, 16> SqrtInformation(const InformationMatrix& info, bool allow_semi_definite) {
   std::array<double, 16> S{};
-  if (!allow_semi_definite) {
-    for (int j = 0; j < 4; ++j) {
-      double d = info[5 * j];
-      for (int k = 0; k < j; ++k) d -= S[4 * j + k] * S[4 * j + k];
-      if (!(d > 0))
-        throw std::invalid_argument("The square root of the information matrix could not be computed, "
-                                    "make sure it is symmetric and positive definite");
-      S[5 * j] = std::sqrt(d);
-      for (int i = j + 1; i < 4; ++i) {
-        double v = info[4 * i + j];
-        for (int k = 0; k < j; ++k) v -= S[4 * i + k] * S[4 * j + k];
-        S[4 * i + j] = v / S[5 * j];
-      }
-    }
-    return S;
-  }
-  double A[4][4];
-  int perm[4] = {0, 1, 2, 3};
-  double scale = 0;
-  for (int i = 0; i < 4; ++i) {
-    scale = std::max(scale, std::fabs(info[5 * i]));
-    for (int j = 0; j < 4; ++j) A[i][j] = info[4 * i + j];
-  }
-  for (int k = 0; k < 4; ++k) {
-    int piv = k;
-    for (int i = k + 1; i < 4; ++i)
-      if (std::fabs(A[i][i]) > std::fabs(A[piv][piv])) piv = i;
-    if (piv != k) {
-      for (int j = 0; j < 4; ++j) std::swap(A[k][j], A[piv][j]);
-      for (int i = 0; i < 4; ++i) std::swap(A[i][k], A[i][piv]);
-      std::swap(perm[k], perm[piv]);
-    }
-    const double d = A[k][k];
-    if (d < -1e-12 * (1.0 + scale)) throw std::invalid_argument("The information matrix must be positive semi-definite");
-    for (int i = k + 1; i < 4; ++i) A[i][k] = std::fabs(d) > 0 ? A[i][k] / d : 0.0;
-    for (int i = k + 1; i < 4; ++i)
-      for (int j = k + 1; j < 4; ++j) A[i][j] -= A[i][k] * d * A[j][k];
-    for (int j = k + 1; j < 4; ++j) A[k][j] = 0;
-  }
-  for (int i = 0; i < 4; ++i)
-    for (int j = 0; j <= i; ++j) {
-      const double l = (i == j) ? 1.0 : A[i][j];
-      S[4 * perm[i] + perm[j]] = l * (A[j][j] > 0 ? std::sqrt(A[j][j]) : 0.0);
-    }
+  if (vgx_sqrt_information(info.data(), allow_semi_definite ? 1 : 0, S.data()) != VGX_OK)
+    throw std::invalid_argument(allow_semi_definite ? "The information matrix must be positive semi-definite"
+                                                    : "The square root of the information matrix could not be "
+                                                      "computed, make sure it is symmetric and positive definite");
   return S;
 }
 
@@ -498,28 +457,14 @@ inline int ProjectMap(Context& ctx, const std::vector<SubmapID>& ids, const std:
   return n_blocks;
 }
 
-// The submap id GenerateCombinedMesh / SaveCombinedMesh project into and free again: the first id counting down
-// from 2^32 - 1 that is neither an input nor present in the context (2^32 - 1 is a valid cblox id).
-inline SubmapID ProjectionScratchId(Context& ctx, const std::vector<SubmapID>& ids) {
-  for (SubmapID sid = 0xFFFFFFFFu;; --sid) {
-    if (std::find(ids.begin(), ids.end(), sid) != ids.end()) continue;
-    const int rc = vgx_submap_info(ctx.get(), sid, nullptr, nullptr, nullptr, nullptr);
-    if (rc == VGX_ERR_NOT_FOUND) return sid;
-    ctx.check(rc);
-  }
-}
-
 // cblox SubmapMesher::generateCombinedMesh on the device: the mesh of the projected global map.  The mesh is
 // left in the context's mesh buffer (vgx_mesh_download / vgx_mesh_ply read it).
 inline void BuildCombinedMesh(Context& ctx, const std::vector<SubmapID>& ids,
                               const std::vector<std::array<float, 7>>& poses, const MeshIntegratorConfig& config) {
-  const SubmapID sid = ProjectionScratchId(ctx, ids);
-  ProjectMap(ctx, ids, poses, sid);
+  if (ids.size() != poses.size()) throw std::invalid_argument("BuildCombinedMesh: one pose per submap");
   const vgx_mesh_config cfg = config.c();
-  const int rc = vgx_mesh_build(ctx.get(), 1, &sid, nullptr, &cfg, nullptr, nullptr);
-  const std::string msg = rc == VGX_OK ? std::string() : std::string(vgx_last_error(ctx.get()));
-  ctx.check(vgx_submap_free(ctx.get(), sid));
-  if (rc != VGX_OK) throw Error(rc, "BuildCombinedMesh: " + msg);
+  ctx.check(vgx_mesh_build_combined(ctx.get(), (int)ids.size(), ids.data(), ids.empty() ? nullptr : poses[0].data(),
+                                    &cfg));
 }
 
 // The combined mesh on the host: vertices in the mission frame and triangles indexing them.
