@@ -131,6 +131,79 @@ class TsdfTrace(C.Structure):
                 ("sdf", C.POINTER(C.c_float)), ("uw", C.POINTER(C.c_float))]
 
 
+class Sampler(C.Structure):
+    _fields_ = [("mt", C.c_uint32 * 624), ("idx", C.c_int)]
+
+
+_P = C.POINTER
+_vp, _i32, _u32, _f32, _f64 = C.c_void_p, C.c_int, C.c_uint32, C.c_float, C.c_double
+_pi32, _pi64, _pf, _pd = _P(C.c_int32), _P(C.c_int64), _P(C.c_float), _P(C.c_double)
+
+# (restype, argtypes) of every function vg_oracle.h declares, in the header's order.  c_void_p stands only for
+# the opaque vgo_layer* and vgo_graph*; tests/test_host_binding_signatures.py compares every entry with the header.
+SIGNATURES = {
+    # layer, index math, interpolation
+    "vgo_layer_create": (_vp, [_f32, _i32]),
+    "vgo_layer_destroy": (None, [_vp]),
+    "vgo_layer_add_block": (_i32, [_vp, _pi32, _pf, _pf]),
+    "vgo_layer_num_blocks": (_i32, [_vp]),
+    "vgo_layer_find_block": (_i32, [_vp, _pi32]),
+    "vgo_layer_export": (None, [_vp, _pi32, _pf, _pf]),
+    "vgo_layer_voxel_size_inv": (_f32, [_vp]),
+    "vgo_layer_block_size_inv": (_f32, [_vp]),
+    "vgo_grid_index_from_point": (None, [_pf, _f32, _pi32]),
+    "vgo_block_and_local_from_global": (None, [_pi64, _i32, _pi32, _pi32]),
+    "vgo_interp_voxels_and_q": (_i32, [_vp, _pf, _pi32, _pi32, _pi32, _pi32, _pf, _pf]),
+    # transforms
+    "vgo_T_exp": (None, [_pf, _pf]),
+    "vgo_T_inverse": (None, [_pf, _pf]),
+    "vgo_T_compose": (None, [_pf, _pf, _pf]),
+    "vgo_T_transform": (None, [_pf, _pf, _pf]),
+    # cost functions
+    "vgo_reg_evaluate": (_i32, [_vp, _i32, _pf, _pf, _pf, _f64, _pd, _pd, _pd, _pd, _pd]),
+    "vgo_reg_pose_setup": (None, [_pd, _pd, _pf, _pf]),
+    "vgo_relpose_evaluate": (None, [_pd, _pd, _pd, _f64, _pd, _pd, _pd, _pd]),
+    "vgo_sqrt_information": (_i32, [_pd, _pd]),
+    "vgo_sqrt_information_ldlt": (_i32, [_pd, _pd]),
+    "vgo_normalize_angle": (_f64, [_f64]),
+    # pose graph
+    "vgo_solver_options_default": (None, [_P(SolverOptions)]),
+    "vgo_graph_create": (_vp, []),
+    "vgo_graph_destroy": (None, [_vp]),
+    "vgo_graph_add_node": (_i32, [_vp, _u32, _pd, _i32]),
+    "vgo_graph_add_relative": (_i32, [_vp, _u32, _u32, _pd, _f64, _pd]),
+    "vgo_graph_add_registration": (_i32, [_vp, _u32, _u32, _vp, _i32, _pf, _pf, _pf, _f64]),
+    "vgo_graph_reset_registration": (None, [_vp]),
+    "vgo_graph_num_nodes": (_i32, [_vp]),
+    "vgo_graph_num_registration_residuals": (_i32, [_vp]),
+    "vgo_graph_get_poses": (None, [_vp, _pd]),
+    "vgo_graph_set_poses": (None, [_vp, _pd]),
+    "vgo_graph_eval": (_i32, [_vp, _i32, _i32, _pd, _pd, _pd]),
+    "vgo_graph_registration_costs": (None, [_vp, _pd]),
+    "vgo_graph_solve": (_i32, [_vp, _P(SolverOptions), _P(SolverSummary)]),
+    # submap finishing, bounding boxes, overlap
+    "vgo_find_relevant_voxels": (_i32, [_vp, _f64, _f64, _pf, _pf, _pf, _i32]),
+    "vgo_find_isosurface_vertices": (_i32, [_vp, _f64, _pf, _pf, _pf, _i32, _pi32, _i32, _pi32]),
+    "vgo_interp_voxel": (_i32, [_vp, _pf, _pf, _pf]),
+    "vgo_esdf_config_default": (None, [_P(EsdfConfig)]),
+    "vgo_generate_esdf": (_i32, [_vp, _P(EsdfConfig), _pf, _pf]),
+    "vgo_surface_obb": (_i32, [_vp, _f64, _f64, _pf, _pf]),
+    "vgo_aabb_from_obb_and_pose": (None, [_pf, _pf, _pf, _pf, _pf]),
+    "vgo_submaps_overlap": (_i32, [_pf, _pf, _pf, _pf, _pf, _pf, _pi32, _i32, _f32, _vp]),
+    # weighted sampler
+    "vgo_sampler_init": (None, [_P(Sampler)]),
+    "vgo_sampler_next_u32": (_u32, [_P(Sampler)]),
+    "vgo_sampler_canonical": (_f64, [_P(Sampler)]),
+    "vgo_sampler_draw": (None, [_P(Sampler), _pd, _i32, _i32, _pi32]),
+    # TSDF integration
+    "vgo_tsdf_config_default": (None, [_P(TsdfConfig)]),
+    "vgo_tsdf_integrate": (None, [_vp, _P(TsdfConfig), _pf, _i32, _pf, _P(TsdfStats)]),
+    "vgo_tsdf_integrate_trace": (None, [_vp, _P(TsdfConfig), _pf, _i32, _pf, _P(TsdfStats), _P(TsdfTrace)]),
+    "vgo_tsdf_trace_free": (None, [_P(TsdfTrace)]),
+    "vgo_tsdf_integrate_mt": (None, [_vp, _P(TsdfConfig), _pf, _i32, _pf, _i32, _P(TsdfStats)]),
+    "vgo_raycast": (_i32, [_pf, _pf, _i32, _i32, _f32, _f32, _f32, _i32, _pi64, _i32]),
+}
+
 _lib = None
 
 
@@ -144,74 +217,9 @@ def lib():
         return _lib
     build()
     L = C.CDLL(_LIB_PATH)
-    vp, i32p, f32p, f64p, i64p = (C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_float),
-                                  C.POINTER(C.c_double), C.POINTER(C.c_int64))
-    L.vgo_layer_create.restype = vp
-    L.vgo_layer_create.argtypes = [C.c_float, C.c_int]
-    L.vgo_layer_destroy.argtypes = [vp]
-    L.vgo_layer_add_block.argtypes = [vp, i32p, f32p, f32p]
-    L.vgo_layer_num_blocks.argtypes = [vp]
-    L.vgo_layer_find_block.argtypes = [vp, i32p]
-    L.vgo_layer_export.argtypes = [vp, i32p, f32p, f32p]
-    L.vgo_layer_voxel_size_inv.restype = C.c_float
-    L.vgo_layer_voxel_size_inv.argtypes = [vp]
-    L.vgo_layer_block_size_inv.restype = C.c_float
-    L.vgo_layer_block_size_inv.argtypes = [vp]
-    L.vgo_grid_index_from_point.argtypes = [f32p, C.c_float, i32p]
-    L.vgo_block_and_local_from_global.argtypes = [i64p, C.c_int, i32p, i32p]
-    L.vgo_interp_voxels_and_q.argtypes = [vp, f32p, i32p, i32p, i32p, i32p, f32p, f32p]
-    L.vgo_T_exp.argtypes = [f32p, f32p]
-    L.vgo_T_inverse.argtypes = [f32p, f32p]
-    L.vgo_T_compose.argtypes = [f32p, f32p, f32p]
-    L.vgo_T_transform.argtypes = [f32p, f32p, f32p]
-    L.vgo_reg_evaluate.argtypes = [vp, C.c_int, f32p, f32p, f32p, C.c_double, f64p, f64p, f64p,
-                                   f64p, f64p]
-    L.vgo_reg_pose_setup.argtypes = [f64p, f64p, f32p, f32p]
-    L.vgo_relpose_evaluate.argtypes = [f64p, f64p, f64p, C.c_double, f64p, f64p, f64p, f64p]
-    L.vgo_sqrt_information.argtypes = [f64p, f64p]
-    L.vgo_sqrt_information_ldlt.argtypes = [f64p, f64p]
-    L.vgo_normalize_angle.restype = C.c_double
-    L.vgo_normalize_angle.argtypes = [C.c_double]
-    L.vgo_solver_options_default.argtypes = [C.POINTER(SolverOptions)]
-    L.vgo_graph_create.restype = vp
-    L.vgo_graph_destroy.argtypes = [vp]
-    L.vgo_graph_add_node.argtypes = [vp, C.c_uint32, f64p, C.c_int]
-    L.vgo_graph_add_relative.argtypes = [vp, C.c_uint32, C.c_uint32, f64p, C.c_double, f64p]
-    L.vgo_graph_add_registration.argtypes = [vp, C.c_uint32, C.c_uint32, vp, C.c_int, f32p, f32p,
-                                             f32p, C.c_double]
-    L.vgo_graph_reset_registration.argtypes = [vp]
-    L.vgo_graph_num_nodes.argtypes = [vp]
-    L.vgo_graph_num_registration_residuals.argtypes = [vp]
-    L.vgo_graph_get_poses.argtypes = [vp, f64p]
-    L.vgo_graph_set_poses.argtypes = [vp, f64p]
-    L.vgo_graph_eval.argtypes = [vp, C.c_int, C.c_int, f64p, f64p, f64p]
-    L.vgo_graph_registration_costs.argtypes = [vp, f64p]
-    L.vgo_graph_solve.argtypes = [vp, C.POINTER(SolverOptions), C.POINTER(SolverSummary)]
-    L.vgo_find_relevant_voxels.argtypes = [vp, C.c_double, C.c_double, f32p, f32p, f32p, C.c_int]
-    L.vgo_find_isosurface_vertices.argtypes = [vp, C.c_double, f32p, f32p, f32p, C.c_int, i32p, C.c_int,
-                                               C.POINTER(C.c_int)]
-    L.vgo_interp_voxel.argtypes = [vp, f32p, f32p, f32p]
-    L.vgo_esdf_config_default.argtypes = [C.POINTER(EsdfConfig)]
-    L.vgo_generate_esdf.argtypes = [vp, C.POINTER(EsdfConfig), f32p, f32p]
-    L.vgo_surface_obb.argtypes = [vp, C.c_double, C.c_double, f32p, f32p]
-    L.vgo_aabb_from_obb_and_pose.argtypes = [f32p, f32p, f32p, f32p, f32p]
-    L.vgo_submaps_overlap.argtypes = [f32p, f32p, f32p, f32p, f32p, f32p, i32p, C.c_int, C.c_float, vp]
-    L.vgo_sampler_init.argtypes = [vp]
-    L.vgo_sampler_next_u32.argtypes = [vp]
-    L.vgo_sampler_next_u32.restype = C.c_uint32
-    L.vgo_sampler_canonical.argtypes = [vp]
-    L.vgo_sampler_canonical.restype = C.c_double
-    L.vgo_sampler_draw.argtypes = [vp, f64p, C.c_int, C.c_int, i32p]
-    L.vgo_tsdf_config_default.argtypes = [C.POINTER(TsdfConfig)]
-    L.vgo_tsdf_integrate.argtypes = [vp, C.POINTER(TsdfConfig), f32p, C.c_int, f32p,
-                                     C.POINTER(TsdfStats)]
-    L.vgo_tsdf_integrate_trace.argtypes = [vp, C.POINTER(TsdfConfig), f32p, C.c_int, f32p,
-                                           C.POINTER(TsdfStats), C.POINTER(TsdfTrace)]
-    L.vgo_tsdf_trace_free.argtypes = [C.POINTER(TsdfTrace)]
-    L.vgo_tsdf_integrate_mt.argtypes = [vp, C.POINTER(TsdfConfig), f32p, C.c_int, f32p, C.c_int,
-                                        C.POINTER(TsdfStats)]
-    L.vgo_raycast.argtypes = [f32p, f32p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float,
-                              C.c_int, i64p, C.c_int]
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = L
     return L
 
@@ -241,6 +249,15 @@ class Layer:
     def from_blocks(cls, voxel_size, vps, block_idx, distance, weight):
         l = cls(voxel_size, vps)
         l.add_blocks(block_idx, distance, weight)
+        return l
+
+    @classmethod
+    def adopt(cls, h, voxel_size, vps):
+        """A Layer that owns the vgo_layer* h made elsewhere (a C harness): it is destroyed with the Layer."""
+        l = cls.__new__(cls)
+        l.voxel_size = float(np.float32(voxel_size))
+        l.vps = int(vps)
+        l._h = h
         return l
 
     def add_blocks(self, block_idx, distance, weight):
@@ -479,20 +496,20 @@ class WeightedSampler:
     def __init__(self, weights):
         w = np.asarray(weights, np.float32)
         self.cumulative = np.cumsum(w.astype(np.float64))   # addItem: sequential double sums
-        self._state = (C.c_uint32 * 625)()
-        lib().vgo_sampler_init(C.cast(self._state, C.c_void_p))
+        self._state = Sampler()
+        lib().vgo_sampler_init(C.byref(self._state))
 
     def next_u32(self):
-        return int(lib().vgo_sampler_next_u32(C.cast(self._state, C.c_void_p)))
+        return int(lib().vgo_sampler_next_u32(C.byref(self._state)))
 
     def canonical(self):
-        return float(lib().vgo_sampler_canonical(C.cast(self._state, C.c_void_p)))
+        return float(lib().vgo_sampler_canonical(C.byref(self._state)))
 
     def draw(self, count):
         idx = np.zeros(count, np.int32)
         cum = np.ascontiguousarray(self.cumulative)
-        lib().vgo_sampler_draw(C.cast(self._state, C.c_void_p), _p(cum, C.c_double), len(cum),
-                               int(count), _p(idx, C.c_int32))
+        lib().vgo_sampler_draw(C.byref(self._state), _p(cum, C.c_double), len(cum), int(count),
+                               _p(idx, C.c_int32))
         return idx
 
 

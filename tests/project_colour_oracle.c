@@ -20,7 +20,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
-#include "vg_oracle.h"
+#include "oracle_harness.h"
 
 static uint32_t to_u8(float v) {
   if (!(v == v)) return 0;

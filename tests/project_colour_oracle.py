@@ -9,18 +9,17 @@ import project_oracle as po
 from oracle import oracle as o
 from support import build_oracle_harness
 
+# its prototype is in tests/oracle_harness.h
+SIGNATURES = {"vgpc_project_colour": (None, [C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_float, C.c_int,
+                                             C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_uint8),
+                                             C.POINTER(C.c_uint32), C.POINTER(C.c_float)])}
 _lib = None
 
 
 def lib():
     global _lib
     if _lib is None:
-        L = build_oracle_harness("project_colour_oracle.c", "libvg_project_colour_oracle.so")
-        L.vgpc_project_colour.restype = None
-        L.vgpc_project_colour.argtypes = [C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_float, C.c_int,
-                                          C.POINTER(C.c_float), C.c_int, C.POINTER(C.c_int32),
-                                          C.POINTER(C.c_uint8), C.POINTER(C.c_uint32), C.POINTER(C.c_float)]
-        _lib = L
+        _lib = build_oracle_harness("project_colour_oracle.c", "libvg_project_colour_oracle.so", SIGNATURES)
     return _lib
 
 

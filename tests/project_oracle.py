@@ -8,19 +8,17 @@ import numpy as np
 from oracle import oracle as o
 from support import build_oracle_harness
 
+# its prototype is in tests/oracle_harness.h
+SIGNATURES = {"vgp_project_layers": (C.c_void_p, [C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_float),
+                                                  C.POINTER(C.c_int), C.POINTER(C.c_float), C.POINTER(C.c_uint32)])}
 _lib = None
 
 
 def lib():
     global _lib
-    if _lib is not None:
-        return _lib
-    L = build_oracle_harness("project_oracle.c", "libvg_project_oracle.so")
-    L.vgp_project_layers.restype = C.c_void_p
-    L.vgp_project_layers.argtypes = [C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_float), C.POINTER(C.c_int),
-                                     C.POINTER(C.c_float), C.POINTER(C.c_uint32)]
-    _lib = L
-    return L
+    if _lib is None:
+        _lib = build_oracle_harness("project_oracle.c", "libvg_project_oracle.so", SIGNATURES)
+    return _lib
 
 
 def project_layers(layers, poses_T, ids):
@@ -40,8 +38,4 @@ def project_layers(layers, poses_T, ids):
                                  ids.ctypes.data_as(C.POINTER(C.c_uint32)))
     if not h:
         raise ValueError("vgp_project_layers refused the input")
-    out = o.Layer.__new__(o.Layer)   # owns the layer: oracle.Layer.__del__ destroys it
-    out.voxel_size = layers[0].voxel_size
-    out.vps = layers[0].vps
-    out._h = h
-    return out
+    return o.Layer.adopt(h, layers[0].voxel_size, layers[0].vps)

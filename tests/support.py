@@ -110,9 +110,10 @@ def compile_cpp_mirror(tmp_path, source):
     return exe
 
 
-def build_oracle_harness(c_file, so_name):
+def build_oracle_harness(c_file, so_name, signatures):
     """Compile the C harness tests/<c_file> into a temporary directory (never into the tree; removed at
-    exit), linked against oracle/libvg_oracle.so, whose layers it reads -> the loaded library."""
+    exit), linked against oracle/libvg_oracle.so, whose layers it reads -> the loaded library, with the
+    harness's {name: (restype, argtypes)} applied."""
     from oracle import oracle as o
     o.lib()   # builds and loads oracle/libvg_oracle.so first
     odir = os.path.join(ROOT, "oracle")
@@ -127,20 +128,31 @@ def build_oracle_harness(c_file, so_name):
     p = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, env=env)
     if p.returncode != 0:
         raise RuntimeError("building tests/%s failed:\n%s" % (c_file, p.stdout))
-    return C.CDLL(so)
+    L = C.CDLL(so)
+    for name, (restype, argtypes) in signatures.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
+    return L
 
 
-def header_functions():
-    """The names of the functions include/voxgraph_b200.h declares."""
-    hdr = open(os.path.join(ROOT, "include", "voxgraph_b200.h")).read()
-    hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
-    return set(re.findall(r"\b(vgx_[a-z0-9_]+)\s*\(", hdr))
+# The C headers that a ctypes table binds: the library's, the oracle's and the oracle harnesses' (which
+# includes the oracle's).
+LIBRARY_HEADER = os.path.join(ROOT, "include", "voxgraph_b200.h")
+ORACLE_HEADER = os.path.join(ROOT, "oracle", "vg_oracle.h")
+HARNESS_HEADER = os.path.join(ROOT, "tests", "oracle_harness.h")
 
 
-def c_layout(tmp_path, structs, constants=()):
-    """The C compiler's view of include/voxgraph_b200.h, from one gcc program: structs {typedef: [field
-    names]} and constant names -> {typedef: sizeof, "typedef.field": offsetof, constant: value}."""
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "voxgraph_b200.h"', 'int main(void) {']
+def header_functions(header=LIBRARY_HEADER, prefix="vgx_"):
+    """The names of the functions the header declares whose names start with prefix (a regular expression)."""
+    hdr = re.sub(r"/\*.*?\*/", "", open(header).read(), flags=re.S)
+    return set(re.findall(r"\b(%s\w+)\s*\(" % prefix, hdr))
+
+
+def c_layout(tmp_path, structs, constants=(), header=LIBRARY_HEADER):
+    """The C compiler's view of the header, from one gcc program: structs {typedef: [field names]} and
+    constant names -> {typedef: sizeof, "typedef.field": offsetof, constant: value}."""
+    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "%s"' % os.path.basename(header),
+             'int main(void) {']
     for cname, fields in structs.items():
         lines.append('printf("%s %%zu\\n", sizeof(%s));' % (cname, cname))
         for fname in fields:
@@ -151,6 +163,23 @@ def c_layout(tmp_path, structs, constants=()):
     src = tmp_path / "layout.c"
     src.write_text("\n".join(lines))
     exe = tmp_path / "layout"
-    subprocess.run(["gcc", "-I" + os.path.join(ROOT, "include"), str(src), "-o", str(exe)], check=True)
+    subprocess.run(["gcc", "-I" + os.path.dirname(header), str(src), "-o", str(exe)], check=True)
     out = subprocess.run([str(exe)], check=True, stdout=subprocess.PIPE, text=True).stdout
     return {k: int(v) for k, v in (line.split() for line in out.splitlines())}
+
+
+def check_struct_layouts(tmp_path, module, typedefs, header=LIBRARY_HEADER, constants=()):
+    """Every ctypes.Structure the module defines has the size and field offsets of its typedef in the header
+    (typedefs: {mirror name: typedef}, one entry per mirror), and every constant {name: value} the header's
+    value."""
+    mirrors = {n: v for n, v in vars(module).items()
+               if isinstance(v, type) and issubclass(v, C.Structure) and v.__module__ == module.__name__}
+    assert set(mirrors) == set(typedefs), "a ctypes struct without its header typedef, or a stale entry"
+    structs = {typedefs[n]: ct for n, ct in mirrors.items()}
+    out = c_layout(tmp_path, {c: [f for f, _ in ct._fields_] for c, ct in structs.items()}, constants, header)
+    for cname, ct in structs.items():
+        assert out[cname] == C.sizeof(ct), cname
+        for fname, _ in ct._fields_:
+            assert out["%s.%s" % (cname, fname)] == getattr(ct, fname).offset, (cname, fname)
+    for name, value in dict(constants).items():
+        assert out[name] == value, name

@@ -40,19 +40,9 @@ def test_struct_layouts_match_header(tmp_path):
     every field offset), and every VGX_ constant of _lib.py (status codes, layer selectors, profiling
     slots) against its value in the header."""
     from voxgraph_b200 import _lib
-    mirrors = {n: v for n, v in vars(_lib).items()
-               if isinstance(v, type) and issubclass(v, C.Structure) and v.__module__ == _lib.__name__}
-    assert set(mirrors) == set(HEADER_STRUCTS), "a ctypes struct without its header typedef, or a stale entry"
-    structs = {HEADER_STRUCTS[n]: ct for n, ct in mirrors.items()}
     constants = {n: v for n, v in vars(_lib).items() if n.startswith("VGX_") and isinstance(v, int)}
     assert "VGX_SLOT_EVAL" in constants and "VGX_PROFILE_SLOTS" in constants
-    out = support.c_layout(tmp_path, {c: [f for f, _ in ct._fields_] for c, ct in structs.items()}, constants)
-    for cname, ct in structs.items():
-        assert out[cname] == C.sizeof(ct), cname
-        for fname, _ in ct._fields_:
-            assert out["%s.%s" % (cname, fname)] == getattr(ct, fname).offset, (cname, fname)
-    for name, value in constants.items():
-        assert out[name] == value, name
+    support.check_struct_layouts(tmp_path, _lib, HEADER_STRUCTS, constants=constants)
     assert C.sizeof(_lib.TsdfConfig) == 14 * 4 and C.sizeof(_lib.TsdfStats) == 5 * 8
     assert C.sizeof(_lib.CollectionEntry) == 44
     assert C.sizeof(_lib.VoxelEvaluationDetails) == 48

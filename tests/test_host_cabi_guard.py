@@ -97,14 +97,14 @@ def minimal_collection(n_blocks):
 # Runs in a child: the address-space limit must not reach the test process.
 CHILD = textwrap.dedent("""
     import ctypes as C, os, resource, sys
-    lib = C.CDLL(sys.argv[1])
+    sys.path.insert(0, sys.argv[1])
+    from voxgraph_b200 import _lib
+    lib = _lib.load()
     stream = open(sys.argv[2], "rb").read()
     n_scan = C.c_int(-1)
-    out = (C.c_uint8 * 64)()
+    out = (_lib.CollectionEntry * 1)()
     n = 4 << 20
     residuals, owner = (C.c_int32 * n)(), (C.c_int32 * n)()
-    lib.vgx_collection_scan.argtypes = [C.c_char_p, C.c_uint64, C.c_int, C.c_void_p, C.POINTER(C.c_int)]
-    lib.vgx_shard_constraints.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     size = int(open("/proc/self/statm").read().split()[0]) * os.sysconf("SC_PAGE_SIZE")
     resource.setrlimit(resource.RLIMIT_AS, (size + (8 << 20), resource.getrlimit(resource.RLIMIT_AS)[1]))
     print(lib.vgx_collection_scan(stream, len(stream), 1, out, C.byref(n_scan)),
@@ -123,7 +123,7 @@ def test_host_allocation_failure_is_nomem(lib, tmp_path):
     from voxgraph_b200 import _lib
     path = tmp_path / "stream.bin"
     path.write_bytes(minimal_collection(1 << 20))
-    r = subprocess.run([sys.executable, "-c", CHILD, _lib.LIB_PATH, str(path)], capture_output=True, text=True,
+    r = subprocess.run([sys.executable, "-c", CHILD, ROOT, str(path)], capture_output=True, text=True,
                        timeout=300)
     assert r.returncode == 0, r.stderr
     assert r.stdout.split() == [str(_lib.VGX_ERR_NOMEM)] * 2

@@ -19,7 +19,7 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include "vg_oracle.h"
+#include "oracle_harness.h"
 
 #define VGT_BLOCK_INDEX_MIN (-(1 << 20) + 1)
 #define VGT_BLOCK_INDEX_MAX ((1 << 20) - 2)

@@ -8,18 +8,16 @@ import numpy as np
 from oracle import oracle as o
 from support import build_oracle_harness
 
+# its prototype is in tests/oracle_harness.h
+SIGNATURES = {"vgt_transform_layer": (C.c_void_p, [C.c_void_p, C.c_float, C.c_int, C.POINTER(C.c_float)])}
 _lib = None
 
 
 def lib():
     global _lib
-    if _lib is not None:
-        return _lib
-    L = build_oracle_harness("transform_oracle.c", "libvg_transform_oracle.so")
-    L.vgt_transform_layer.restype = C.c_void_p
-    L.vgt_transform_layer.argtypes = [C.c_void_p, C.c_float, C.c_int, C.POINTER(C.c_float)]
-    _lib = L
-    return L
+    if _lib is None:
+        _lib = build_oracle_harness("transform_oracle.c", "libvg_transform_oracle.so", SIGNATURES)
+    return _lib
 
 
 def transform_layer(layer, T_new_old):
@@ -29,8 +27,4 @@ def transform_layer(layer, T_new_old):
     h = lib().vgt_transform_layer(layer._h, layer.voxel_size, layer.vps, T.ctypes.data_as(C.POINTER(C.c_float)))
     if not h:
         raise ValueError("vgt_transform_layer refused the input")
-    out = o.Layer.__new__(o.Layer)   # owns the layer: oracle.Layer.__del__ destroys it
-    out.voxel_size = layer.voxel_size
-    out.vps = layer.vps
-    out._h = h
-    return out
+    return o.Layer.adopt(h, layer.voxel_size, layer.vps)
