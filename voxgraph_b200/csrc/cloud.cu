@@ -129,7 +129,7 @@ static int cloud_check(vgx_ctx* c, const vgx_cloud_layout* L, const uint8_t* dat
   return VGX_OK;
 }
 
-// Uploads the message (height * row_step bytes, one cudaMemcpyAsync from the caller's pageable buffer, the way
+// Uploads the message (height * row_step bytes, one asynchronous copy from the caller's pageable buffer, the way
 // vgx_tsdf_integrate sends its points) into d_raw and decodes it into the slot arrays.
 static int cloud_decode_launch(vgx_ctx* c, const vgx_cloud_layout& L, const uint8_t* data, float colour_max,
                                uint8_t* d_raw, float* d_pts, uint32_t* d_rgba, unsigned* d_flags,
@@ -140,7 +140,7 @@ static int cloud_decode_launch(vgx_ctx* c, const vgx_cloud_layout& L, const uint
   P.n_warps = L.height * P.warps_per_row;      // <= records <= INT_MAX
   P.stage_bytes = L.point_step <= CLOUD_STAGE_STEP ? 32 * L.point_step + 32 : 0;
   P.colour_max = colour_max;
-  VGX_CUDA(c, cudaMemcpyAsync(d_raw, data, (size_t)L.height * L.row_step, cudaMemcpyHostToDevice, c->stream));
+  VGX_TRY(vgx_upload(c, d_raw, data, (size_t)L.height * L.row_step));
   VgxProfileScope scope(c, VGX_SLOT_CLOUD_DECODE);
   return vgx_launch(c, cloud_decode_kernel, (P.n_warps + CLOUD_WARPS - 1) / CLOUD_WARPS, CLOUD_WARPS * 32,
                     CLOUD_WARPS * (size_t)P.stage_bytes, VgxLaunch::plain, P, d_raw, d_pts, d_rgba, d_flags, d_kept);
@@ -164,8 +164,7 @@ extern "C" int vgx_cloud_decode(vgx_ctx* c, const vgx_cloud_layout* L, const uin
                       vgx_part(d_kept, 1)));
     VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_flags, (size_t)n + 2), vgx_part(d_offsets, (size_t)n + 2),
                       vgx_part(d_scan_tmp, vgx_scan_tmp_count((size_t)n))));
-    cudaStream_t stream = c->stream;
-    VGX_CUDA(c, cudaMemsetAsync(d_kept, 0, sizeof(*d_kept), stream));
+    VGX_TRY(vgx_fill(c, d_kept, 1));
     VGX_TRY(cloud_decode_launch(c, *L, data, colour_max, d_raw, d_pts, d_rgba, d_flags, d_kept));
     {
       VgxProfileScope scope(c, VGX_SLOT_CLOUD_DECODE);
@@ -174,15 +173,14 @@ extern "C" int vgx_cloud_decode(vgx_ctx* c, const vgx_cloud_layout* L, const uin
                          d_flags, d_offsets, d_out_pts, d_out_rgba));
     }
     unsigned kept = 0;
-    VGX_CUDA(c, cudaMemcpyAsync(&kept, d_offsets + n, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
-    VGX_CUDA(c, cudaStreamSynchronize(stream));
+    VGX_TRY(vgx_read(c, &kept, d_offsets + n));
     if (n_points) *n_points = (int)kept;
     if ((points_C || rgba) && kept > (unsigned)max_points)
       VGX_FAIL(c, VGX_ERR_CAPACITY, "more kept points than max_points");
-    if (points_C) VGX_CUDA(c, cudaMemcpyAsync(points_C, d_out_pts, sizeof(float) * 3 * (size_t)kept, cudaMemcpyDeviceToHost, stream));
-    if (rgba) VGX_CUDA(c, cudaMemcpyAsync(rgba, d_out_rgba, 4 * (size_t)kept, cudaMemcpyDeviceToHost, stream));
-    VGX_CUDA(c, cudaStreamSynchronize(stream));
-    return VGX_OK;
+    if (points_C) VGX_TRY(vgx_download(c, points_C, d_out_pts, 3 * (size_t)kept));
+    // the caller's r, g, b, a bytes against the device's colour words: written in bytes
+    if (rgba) VGX_TRY(vgx_download(c, rgba, reinterpret_cast<const uint8_t*>(d_out_rgba), 4 * (size_t)kept));
+    return vgx_sync(c);
   });
 }
 
@@ -208,7 +206,7 @@ extern "C" int vgx_tsdf_integrate_cloud(vgx_ctx* c, uint32_t id, const float T_G
     VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_raw, (size_t)L->height * L->row_step), vgx_part(d_pts, 3 * (size_t)n),
                       vgx_part(d_stats, VGX_TSDF_STAT_WORDS), vgx_part(d_sets, vgx_tsdf_set_words(rcfg)),
                       vgx_part(d_rgba, colours ? (size_t)n : 0)));
-    VGX_CUDA(c, cudaMemsetAsync(d_stats, 0, sizeof(unsigned long long) * VGX_TSDF_STAT_WORDS, c->stream));
+    VGX_TRY(vgx_fill(c, d_stats, VGX_TSDF_STAT_WORDS));
     VGX_TRY(cloud_decode_launch(c, *L, data, colour_max, d_raw, d_pts, colours ? d_rgba : nullptr, nullptr,
                                 d_stats + VGX_TSDF_STAT_CALLER));
     return vgx_tsdf_integrate_resident(c, s, T_G_C, rcfg, n, d_pts, colours ? d_rgba : nullptr, d_stats, d_sets, stats,

@@ -734,12 +734,11 @@ int copy_h2d_chunked(vgx_ctx* c, uint8_t* d, const uint8_t* h, uint64_t n) {
     uint8_t* half = stage + (k & 1) * kChunk;
     if (k >= 2) VGX_CUDA(c, cudaEventSynchronize(ev.e[k & 1]));
     memcpy(half, h + off, len);
-    VGX_CUDA(c, cudaMemcpyAsync(d + off, half, len, cudaMemcpyHostToDevice, c->stream));
+    VGX_TRY(vgx_upload(c, d + off, half, len));
     VGX_CUDA(c, cudaEventRecord(ev.e[k & 1], c->stream));
     off += len;
   }
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // the staging buffer is reused by the next call
-  return VGX_OK;
+  return vgx_sync(c);   // the staging buffer is reused by the next call
 }
 
 int copy_d2h_chunked(vgx_ctx* c, uint8_t* h, const uint8_t* d, uint64_t n) {
@@ -752,7 +751,7 @@ int copy_d2h_chunked(vgx_ctx* c, uint8_t* h, const uint8_t* d, uint64_t n) {
   for (uint64_t k = 0; k <= chunks; ++k) {
     if (k < chunks) {   // enqueue chunk k, then drain chunk k - 1 while it runs
       const size_t len = (size_t)std::min<uint64_t>(kChunk, n - k * kChunk);
-      VGX_CUDA(c, cudaMemcpyAsync(stage + (k & 1) * kChunk, d + k * kChunk, len, cudaMemcpyDeviceToHost, c->stream));
+      VGX_TRY(vgx_download(c, stage + (k & 1) * kChunk, d + k * kChunk, len));
       VGX_CUDA(c, cudaEventRecord(ev.e[k & 1], c->stream));
     }
     if (k >= 1) {
@@ -804,13 +803,12 @@ static int decode_layout(vgx_ctx* c, const CollLayout& L, const uint8_t* bytes, 
   VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_regions, L.blocks.size()), vgx_part(d_err, 1),
                     vgx_part(d_any, keep_colour ? L.submaps.size() : 0), vgx_part(d_bytes, (size_t)n)));
   if (keep_colour && !L.submaps.empty())
-    VGX_CUDA(c, cudaMemsetAsync(d_any, 0, sizeof(int) * L.submaps.size(), c->stream));
+    VGX_TRY(vgx_fill(c, d_any, L.submaps.size()));
   {
     VgxProfileScope copies(c, VGX_SLOT_COLL_COPY);
     if (!L.blocks.empty())
-      VGX_CUDA(c, cudaMemcpyAsync(d_regions, L.blocks.data(), L.blocks.size() * sizeof(CollBlockRef),
-                                  cudaMemcpyHostToDevice, c->stream));
-    VGX_CUDA(c, cudaMemsetAsync(d_err, 0, sizeof(int), c->stream));
+      VGX_TRY(vgx_upload(c, d_regions, L.blocks.data(), L.blocks.size()));
+    VGX_TRY(vgx_fill(c, d_err, 1));
     VGX_TRY(copy_h2d_chunked(c, d_bytes, bytes, n));
   }
   for (size_t k = 0; k < L.submaps.size(); ++k) {
@@ -823,8 +821,7 @@ static int decode_layout(vgx_ctx* c, const CollLayout& L, const uint8_t* bytes, 
     if (keep_colour) VGX_TRY(vgx_submap_ensure_colour(c, sm));
     {
       VgxProfileScope copies(c, VGX_SLOT_COLL_COPY);
-      VGX_CUDA(c, cudaMemcpyAsync(sm->d_block_idx.get(), L.block_idx.data() + 3 * s.first_block,
-                                  sizeof(int32_t) * 3 * s.n_blocks, cudaMemcpyHostToDevice, c->stream));
+      VGX_TRY(vgx_upload(c, sm->d_block_idx.get(), L.block_idx.data() + 3 * s.first_block, 3 * (size_t)s.n_blocks));
     }
     VgxProfileScope scope(c, VGX_SLOT_COLL_CODEC);
     VGX_TRY(vgx_launch(c, collection_decode_kernel, s.n_blocks, COLL_THREADS, 0, VgxLaunch::plain, d_bytes,
@@ -833,10 +830,9 @@ static int decode_layout(vgx_ctx* c, const CollLayout& L, const uint8_t* bytes, 
   }
   int h_err = 0;
   std::vector<int> h_any(keep_colour ? L.submaps.size() : 0);
-  VGX_CUDA(c, cudaMemcpyAsync(&h_err, d_err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  if (!h_any.empty())
-    VGX_CUDA(c, cudaMemcpyAsync(h_any.data(), d_any, sizeof(int) * h_any.size(), cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+  VGX_TRY(vgx_download(c, &h_err, d_err, 1));
+  if (!h_any.empty()) VGX_TRY(vgx_download(c, h_any.data(), d_any, h_any.size()));
+  VGX_TRY(vgx_sync(c));
   if (h_err) {
     c->set_error(std::string("voxel_data: ") +
                  ((h_err & COLL_ERR_TAG) ? "unexpected tag; " : "") +
@@ -900,7 +896,7 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
         VGX_FAIL(c, VGX_ERR_INVALID, "a collection has one voxel size and voxels_per_side");
       subs.push_back(s);
     }
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // n_blocks of an active submap is final after its integration
+    VGX_TRY(vgx_sync(c));   // n_blocks of an active submap is final after its integration
     const double voxel_size = subs.empty() ? 0.0 : (double)subs[0]->voxel_size;
     const int vps = subs.empty() ? 16 : subs[0]->vps;
     const uint32_t hdr = block_header_bytes(vps);
@@ -928,10 +924,8 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
       first += (size_t)s->n_blocks;
     }
     std::vector<uint32_t> sizes(total_blocks);
-    if (total_blocks)
-      VGX_CUDA(c, cudaMemcpyAsync(sizes.data(), d_sizes, total_blocks * sizeof(uint32_t), cudaMemcpyDeviceToHost,
-                                  c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (total_blocks) VGX_TRY(vgx_download(c, sizes.data(), d_sizes, total_blocks));
+    VGX_TRY(vgx_sync(c));
     // layout: header, then per submap its SubmapProto and its blocks; block messages are contiguous per
     // submap in the device buffer
     std::vector<std::vector<uint8_t>> framing((size_t)n + 1);
@@ -960,10 +954,8 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
                       vgx_part(d_msgs, (size_t)dev_bytes)));
     if (total_blocks) {
       VgxProfileScope copies(c, VGX_SLOT_COLL_COPY);
-      VGX_CUDA(c, cudaMemcpyAsync(d_sizes, sizes.data(), total_blocks * sizeof(uint32_t), cudaMemcpyHostToDevice,
-                                  c->stream));
-      VGX_CUDA(c, cudaMemcpyAsync(d_offs, offsets.data(), total_blocks * sizeof(uint64_t), cudaMemcpyHostToDevice,
-                                  c->stream));
+      VGX_TRY(vgx_upload(c, d_sizes, sizes.data(), total_blocks));
+      VGX_TRY(vgx_upload(c, d_offs, offsets.data(), total_blocks));
     }
     a.dst = d_msgs;
     first = 0;
@@ -994,8 +986,7 @@ extern "C" int vgx_collection_save(vgx_ctx* c, int n, const uint32_t* ids, const
       o += span[k];
       dev_off += span[k];
     }
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    return VGX_OK;
+    return vgx_sync(c);
   });
 }
 

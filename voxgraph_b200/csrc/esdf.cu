@@ -130,7 +130,6 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
     P.vps = s->vps;
     P.sh = s->sh;
     P.n_blocks = s->n_blocks;
-    cudaStream_t st = c->stream;
     VGX_TRY(s->d_esdf.alloc(c, sizeof(float2) * nvox, "ESDF bricks"));
     unsigned char* d_fixed;
     int *d_nb, *d_changed;
@@ -144,15 +143,14 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
     int sweeps = 0;
     const int max_sweeps = 4 * (int)ceilf(dc.max_distance_m / s->voxel_size) + 16;
     for (;;) {
-      VGX_CUDA(c, cudaMemsetAsync(d_changed, 0, sizeof(int), st));
+      VGX_TRY(vgx_fill(c, d_changed, 1));
       for (int k = 0; k < 2; ++k) {
         VGX_TRY(vgx_launch(c, esdf_sweep_kernel, grid, 256, 0, VgxLaunch::plain, P, s->d_esdf.get(), d_fixed, d_nb,
                            d_changed));
         ++sweeps;
       }
       int changed = 0;
-      VGX_CUDA(c, cudaMemcpyAsync(&changed, d_changed, sizeof(int), cudaMemcpyDeviceToHost, st));
-      VGX_CUDA(c, cudaStreamSynchronize(st));
+      VGX_TRY(vgx_read(c, &changed, d_changed));
       if (!changed) break;
       if (sweeps > max_sweeps) VGX_FAIL(c, VGX_ERR_INVALID, "relaxation did not converge");
     }
@@ -160,8 +158,7 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
     // registration view of the ESDF layer (observed <=> weight 1), same octet layout as the TSDF view
     VGX_TRY(s->d_view_esdf.alloc(c, sizeof(float) * 8 * nvox, "ESDF registration view"));
     VGX_TRY(vgx_submap_build_view(c, s, s->d_esdf.get(), s->d_view_esdf.get()));
-    VGX_CUDA(c, cudaStreamSynchronize(st));
-    return VGX_OK;
+    return vgx_sync(c);
   });
 }
 
@@ -177,8 +174,7 @@ extern "C" int vgx_submap_download_esdf(vgx_ctx* c, uint32_t id, int max_blocks,
     if (n == 0) return VGX_OK;
     const size_t nvox = (size_t)n * s->vox_per_block;
     std::vector<float2> h(nvox);
-    VGX_CUDA(c, cudaMemcpyAsync(h.data(), s->d_esdf.get(), sizeof(float2) * nvox, cudaMemcpyDeviceToHost, c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    VGX_TRY(vgx_read(c, h.data(), s->d_esdf.get(), nvox));
     for (size_t i = 0; i < nvox; ++i) {
       if (distance) distance[i] = h[i].x;
       if (observed) observed[i] = h[i].y;

@@ -164,7 +164,6 @@ extern "C" int vgx_evaluate_layers_rmse(vgx_ctx* c, uint32_t gt_id, int gt_layer
     if (n_part > 0) {
       RmsePartial* d_part;
       VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_part, n_part + 1)));
-      cudaStream_t st = c->stream;
       const int threads = std::min(RMSE_THREADS, g->vox_per_block);
       {
         VgxProfileScope scope(c, VGX_SLOT_EVAL);
@@ -176,8 +175,7 @@ extern "C" int vgx_evaluate_layers_rmse(vgx_ctx* c, uint32_t gt_id, int gt_layer
         VGX_TRY(vgx_launch(c, rmse_total_kernel, 1, RMSE_THREADS, 0, VgxLaunch::plain, d_part, (int)n_part,
                            d_part + n_part));
       }
-      VGX_CUDA(c, cudaMemcpyAsync(&total, d_part + n_part, sizeof(RmsePartial), cudaMemcpyDeviceToHost, st));
-      VGX_CUDA(c, cudaStreamSynchronize(st));
+      VGX_TRY(vgx_read(c, &total, d_part + n_part));
     }
     out->rmse = (float)sqrt(total.sum / (double)total.n_eval);
     out->max_error = total.max_error;

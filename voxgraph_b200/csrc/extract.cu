@@ -119,10 +119,7 @@ scan_add_kernel(unsigned* __restrict__ out, const unsigned* __restrict__ tile_su
 
 // d_tmp: (tiles + 1) unsigned of scratch.  3 launches.
 int vgx_exclusive_scan_u32(vgx_ctx* c, const unsigned* d_in, unsigned* d_out, size_t n, unsigned* d_tmp) {
-  if (n == 0) {
-    VGX_CUDA(c, cudaMemsetAsync(d_out, 0, sizeof(unsigned), c->stream));
-    return VGX_OK;
-  }
+  if (n == 0) return vgx_fill(c, d_out, 1);
   const size_t tiles = (n + SCAN_TILE - 1) / SCAN_TILE;
   VGX_TRY(vgx_launch(c, scan_tile_kernel, (unsigned)tiles, SCAN_THREADS, 0, VgxLaunch::plain, d_in, d_out, d_tmp, n));
   VGX_TRY(vgx_launch(c, scan_sums_kernel, 1, 1024, 0, VgxLaunch::plain, d_tmp, tiles, d_tmp + tiles));
@@ -334,8 +331,7 @@ static int install_points(vgx_ctx* c, VgxSubmap* s, int type, VgxBuffer<float>&&
   float* d_w;
   VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_w, (size_t)n)));
   VGX_TRY(vgx_launch(c, gather_weights_kernel, (n + 255) / 256, 256, 0, VgxLaunch::plain, d_pts.get(), n, d_w));
-  VGX_CUDA(c, cudaMemcpyAsync(w.data(), d_w, sizeof(float) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+  VGX_TRY(vgx_read(c, w.data(), d_w, (size_t)n));
   p.cumulative_w.resize((size_t)n);
   double sum = 0;
   for (int i = 0; i < n; ++i) { sum += (double)w[i]; p.cumulative_w[i] = sum; }
@@ -348,8 +344,7 @@ static int install_points(vgx_ctx* c, VgxSubmap* s, int type, VgxBuffer<float>&&
 static int alloc_points(vgx_ctx* c, int n, VgxBuffer<float>& out) {
   const size_t units = ((size_t)std::max(n, 1) + VGX_PT_UNIT - 1) / VGX_PT_UNIT;
   VGX_TRY(out.alloc(c, units * VGX_PT_UNIT_FLOATS * sizeof(float), "registration points"));
-  VGX_CUDA(c, cudaMemsetAsync(out.get(), 0, units * VGX_PT_UNIT_FLOATS * sizeof(float), c->stream));
-  return VGX_OK;
+  return vgx_fill(c, out.get(), units * VGX_PT_UNIT_FLOATS);
 }
 
 extern "C" void vgx_registration_filter_default(vgx_registration_filter* f) {
@@ -382,7 +377,6 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
       return install_points(c, s, VGX_POINTS_ISOSURFACE, VgxBuffer<float>(), 0);
     }
     if (nvox >= 0xFFFFFFFFull / 12) VGX_FAIL(c, VGX_ERR_CAPACITY, "submap too large for 32-bit candidate indices");
-    cudaStream_t st = c->stream;
     unsigned *d_counts, *d_offsets, *d_tmp, *d_flags;
     float* d_obb;
     VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_counts, nvox + 1), vgx_part(d_offsets, nvox + 1),
@@ -394,20 +388,18 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
     {
       const float inf = INFINITY;
       const float init[6] = {inf, inf, inf, -inf, -inf, -inf};
-      VGX_CUDA(c, cudaMemcpyAsync(d_obb, init, sizeof(init), cudaMemcpyHostToDevice, st));
+      VGX_TRY(vgx_upload(c, d_obb, init, std::size(init)));
       VGX_TRY(vgx_launch(c, relevant_count_kernel, grid256, 256, 0, VgxLaunch::plain, L, f.min_voxel_weight,
                          f.max_voxel_distance, d_counts));
       VGX_TRY(vgx_exclusive_scan_u32(c, d_counts, d_offsets, nvox, d_tmp));
       unsigned total = 0;
-      VGX_CUDA(c, cudaMemcpyAsync(&total, d_offsets + nvox, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-      VGX_CUDA(c, cudaStreamSynchronize(st));
+      VGX_TRY(vgx_read(c, &total, d_offsets + nvox));
       VgxBuffer<float> d_pts;
       VGX_TRY(alloc_points(c, (int)total, d_pts));
       VGX_TRY(vgx_launch(c, relevant_emit_kernel, grid256, 256, 0, VgxLaunch::plain, L, d_counts, d_offsets,
                          f.use_esdf_distance ? s->d_esdf.get() : nullptr, d_pts.get(), d_obb));
       float obb[6];
-      VGX_CUDA(c, cudaMemcpyAsync(obb, d_obb, sizeof(obb), cudaMemcpyDeviceToHost, st));
-      VGX_CUDA(c, cudaStreamSynchronize(st));
+      VGX_TRY(vgx_read(c, obb, d_obb, std::size(obb)));
       for (int a = 0; a < 3; ++a) { s->surface_obb_min[a] = obb[a]; s->surface_obb_max[a] = obb[3 + a]; }
       s->surface_obb_valid = total > 0;
       VGX_TRY(install_points(c, s, VGX_POINTS_VOXELS, std::move(d_pts), (int)total));
@@ -420,8 +412,7 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
       VGX_TRY(vgx_launch(c, iso_count_kernel, grid128, 128, 0, VgxLaunch::plain, L, min_weight, d_counts));
       VGX_TRY(vgx_exclusive_scan_u32(c, d_counts, d_offsets, nvox, d_tmp));
       unsigned M = 0;
-      VGX_CUDA(c, cudaMemcpyAsync(&M, d_offsets + nvox, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-      VGX_CUDA(c, cudaStreamSynchronize(st));
+      VGX_TRY(vgx_read(c, &M, d_offsets + nvox));
       unsigned kept = 0;
       VgxBuffer<float> d_pts;
       if (M > 0) {
@@ -442,30 +433,24 @@ extern "C" int vgx_submap_extract_points(vgx_ctx* c, uint32_t id, const vgx_regi
         VGX_TRY(vgx_launch(c, iso_select_kernel, (M + 127) / 128, 128, 0, VgxLaunch::plain, L, d_cand, d_key, d_table,
                            tsize - 1, M, d_keep, d_cdw));
         VGX_TRY(vgx_exclusive_scan_u32(c, d_keep, d_koff, M, d_tmp2));
-        VGX_CUDA(c, cudaMemcpyAsync(&kept, d_koff + M, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-        VGX_CUDA(c, cudaStreamSynchronize(st));
+        VGX_TRY(vgx_read(c, &kept, d_koff + M));
         VGX_TRY(alloc_points(c, (int)kept, d_pts));
-        VGX_CUDA(c, cudaMemsetAsync(d_flags, 0, sizeof(unsigned) * (size_t)s->n_blocks, st));
+        VGX_TRY(vgx_fill(c, d_flags, (size_t)s->n_blocks));
         VGX_TRY(vgx_launch(c, iso_compact_kernel, (M + 127) / 128, 128, 0, VgxLaunch::plain, L, d_cand, d_cdw, d_keep,
                            d_koff, M, d_pts.get(), d_flags));
         // isosurface block list (slots, ascending) for overlapsWith
         std::vector<unsigned> flags((size_t)s->n_blocks);
-        VGX_CUDA(c, cudaMemcpyAsync(flags.data(), d_flags, sizeof(unsigned) * (size_t)s->n_blocks,
-                                    cudaMemcpyDeviceToHost, st));
-        VGX_CUDA(c, cudaStreamSynchronize(st));
+        VGX_TRY(vgx_read(c, flags.data(), d_flags, flags.size()));
         for (int b = 0; b < s->n_blocks; ++b)
           if (flags[b]) s->iso_blocks.push_back(b);
         if (!s->iso_blocks.empty()) {
           std::vector<int32_t> bidx(3 * (size_t)s->n_blocks), iso(3 * s->iso_blocks.size());
-          VGX_CUDA(c, cudaMemcpyAsync(bidx.data(), s->d_block_idx.get(), sizeof(int32_t) * bidx.size(),
-                                      cudaMemcpyDeviceToHost, st));
-          VGX_CUDA(c, cudaStreamSynchronize(st));
+          VGX_TRY(vgx_read(c, bidx.data(), s->d_block_idx.get(), bidx.size()));
           for (size_t k = 0; k < s->iso_blocks.size(); ++k)
             for (int a = 0; a < 3; ++a) iso[3 * k + a] = bidx[3 * (size_t)s->iso_blocks[k] + a];
           VGX_TRY(s->d_iso_idx.alloc(c, sizeof(int32_t) * iso.size(), "isosurface block list"));
-          VGX_CUDA(c, cudaMemcpyAsync(s->d_iso_idx.get(), iso.data(), sizeof(int32_t) * iso.size(),
-                                      cudaMemcpyHostToDevice, st));
-          VGX_CUDA(c, cudaStreamSynchronize(st));
+          VGX_TRY(vgx_upload(c, s->d_iso_idx.get(), iso.data(), iso.size()));
+          VGX_TRY(vgx_sync(c));
           s->n_iso = (int)s->iso_blocks.size();
         }
       } else {
@@ -509,11 +494,10 @@ extern "C" int vgx_submap_download_points(vgx_ctx* c, uint32_t id, int type, int
     VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_xyz, 3 * n), vgx_part(d_d, n), vgx_part(d_w, n)));
     VGX_TRY(vgx_launch(c, unpack_points_kernel, (unsigned)((n + 255) / 256), 256, 0, VgxLaunch::plain, p.data.get(), p.n,
                        d_xyz, d_d, d_w));
-    if (xyz) VGX_CUDA(c, cudaMemcpyAsync(xyz, d_xyz, 3 * n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    if (distance) VGX_CUDA(c, cudaMemcpyAsync(distance, d_d, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    if (weight) VGX_CUDA(c, cudaMemcpyAsync(weight, d_w, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    return VGX_OK;
+    if (xyz) VGX_TRY(vgx_download(c, xyz, d_xyz, 3 * n));
+    if (distance) VGX_TRY(vgx_download(c, distance, d_d, n));
+    if (weight) VGX_TRY(vgx_download(c, weight, d_w, n));
+    return vgx_sync(c);
   });
 }
 

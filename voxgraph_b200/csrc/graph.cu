@@ -20,7 +20,7 @@
 
 void vgx_graph_free(vgx_ctx* c) {
   if (!c->graph) return;
-  cudaStreamSynchronize(c->stream);
+  vgx_drain(c);
   if (c->graph->copy_stream) {
     cudaStreamDestroy(c->graph->copy_stream);
     for (int k = 0; k < 2; ++k) { cudaEventDestroy(c->graph->ev_iter[k]); cudaEventDestroy(c->graph->ev_copy[k]); }
@@ -327,16 +327,13 @@ static int table_alloc(vgx_ctx* c, VgxBuffer<T>& d, size_t n) {
 template <class T>
 static int table_upload(vgx_ctx* c, VgxBuffer<T>& d, const std::vector<T>& v) {
   VGX_TRY(table_alloc(c, d, std::max<size_t>(v.size(), 1)));
-  if (!v.empty())
-    VGX_CUDA(c, cudaMemcpyAsync(d.get(), v.data(), sizeof(T) * v.size(), cudaMemcpyHostToDevice, c->stream));
-  return VGX_OK;
+  return v.empty() ? VGX_OK : vgx_upload(c, d.get(), v.data(), v.size());
 }
 
 // The device tables of `plan`; all[i] is the descriptor of constraint i, is_sampled[i] whether its points are the
 // draws in g->samples[i].  Every buffer is t's, so a failure leaves nothing behind.
 static int upload_tables(vgx_ctx* c, VgxGraph* g, const VgxGraphPlan& plan, const std::vector<RegConstraintDev>& all,
                          const std::vector<uint8_t>& is_sampled, int sms, VgxGraphTables& t) {
-  cudaStream_t st = c->stream;
   const int N = g->N, n_local = plan.n_local(), n_tiles = plan.n_tiles(), n = plan.n_free;
   std::vector<RegConstraintDev> cons(n_local);
   for (int k = 0; k < n_local; ++k) cons[k] = all[plan.local[k]];
@@ -352,15 +349,14 @@ static int upload_tables(vgx_ctx* c, VgxGraph* g, const VgxGraphPlan& plan, cons
       const int i = plan.local[k];
       if (!is_sampled[i]) continue;
       const VgxPoints& p = c->find(g->reg_ref[i])->points[g->reg_cfgs[i].registration_point_type];
-      VGX_CUDA(c, cudaMemcpyAsync(t.d_sample_idx.get() + io, g->samples[i].data(), sizeof(int32_t) * cons[k].n,
-                                  cudaMemcpyHostToDevice, st));
+      VGX_TRY(vgx_upload(c, t.d_sample_idx.get() + io, g->samples[i].data(), (size_t)cons[k].n));
       float* dst = t.d_sample_pts.get() + uo * VGX_PT_UNIT_FLOATS;
       VGX_TRY(vgx_launch_reg_gather_samples(c, p.data.get(), t.d_sample_idx.get() + io, cons[k].n, dst));
       cons[k].pts = dst;
       uo += ((size_t)cons[k].n + 31) / 32;
       io += (size_t)cons[k].n;
     }
-    VGX_CUDA(c, cudaStreamSynchronize(st));  // g->samples[] are pageable host vectors
+    VGX_TRY(vgx_sync(c));  // g->samples[] are pageable host vectors
   }
   // what the CTA of a tile needs to start its bulk copies without a dependent load
   std::vector<RegTile> tiles(n_tiles);
@@ -415,7 +411,7 @@ static int upload_tables(vgx_ctx* c, VgxGraph* g, const VgxGraphPlan& plan, cons
       VGX_CUDA(c, cudaEventCreateWithFlags(&g->ev_copy[k], cudaEventDisableTiming));
     }
   }
-  VGX_CUDA(c, cudaStreamSynchronize(st));
+  VGX_TRY(vgx_sync(c));
   // the fused assembly and exchange spins on its peers, so its grid must be co-resident as a whole
   int per_sm = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, assemble_exchange_kernel, 128, 0) != cudaSuccess)
@@ -425,7 +421,7 @@ static int upload_tables(vgx_ctx* c, VgxGraph* g, const VgxGraphPlan& plan, cons
 }
 
 static int build_tables(vgx_ctx* c, VgxGraph* g) {
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+  VGX_TRY(vgx_sync(c));
   g->dev = VgxGraphTables();   // before the new tables are allocated: a rebuild needs no more device memory
   // ---- collect: the descriptors, nodes and sampling draws of all constraints, and their partition over ranks
   const int P = (int)g->reg_ref.size();
@@ -601,9 +597,9 @@ extern "C" int vgx_graph_set_poses(vgx_ctx* c, const double* xyzyaw) {
       // stage through pinned memory so the copy is a true async H2D
       double* h;
       VGX_TRY(vgx_carve(c, c->h_pinned, vgx_part(h, 4 * (size_t)g->N)));
-      VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+      VGX_TRY(vgx_sync(c));
       memcpy(h, xyzyaw, sizeof(double) * 4 * g->N);
-      VGX_CUDA(c, cudaMemcpyAsync(g->dev.d_x.get(), h, sizeof(double) * 4 * g->N, cudaMemcpyHostToDevice, c->stream));
+      return vgx_upload(c, g->dev.d_x.get(), h, 4 * (size_t)g->N);
     }
     return VGX_OK;
   });
@@ -730,9 +726,7 @@ extern "C" int vgx_graph_eval(vgx_ctx* c, int exclude_registration, double* cost
     VGX_TRY(eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, exclude_registration != 0));
     double* h;
     VGX_TRY(vgx_carve(c, c->h_pinned, vgx_part(h, g->plan.packed_len)));
-    VGX_CUDA(c, cudaMemcpyAsync(h, g->dev.d_packed[0].get(), sizeof(double) * g->plan.packed_len,
-                                cudaMemcpyDeviceToHost, c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    VGX_TRY(vgx_read(c, h, g->dev.d_packed[0].get(), g->plan.packed_len));
     const int N = g->N, dim = 4 * N;
     if (cost) *cost = h[0];
     if (gradient) memcpy(gradient, h + PACK_HDR, sizeof(double) * dim);
@@ -770,10 +764,8 @@ extern "C" int vgx_graph_registration_costs(vgx_ctx* c, double* per_constraint) 
     VGX_TRY(eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[1].get(), false, false));
     const int P = (int)g->reg_ref.size(), n_local = g->plan.n_local();
     std::vector<double> cs((size_t)n_local * VGX_REG_NSTRIDE + 1);
-    if (n_local > 0)
-      VGX_CUDA(c, cudaMemcpyAsync(cs.data(), g->dev.d_csum.get(), sizeof(double) * VGX_REG_NSTRIDE * n_local,
-                                  cudaMemcpyDeviceToHost, c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (n_local > 0) VGX_TRY(vgx_download(c, cs.data(), g->dev.d_csum.get(), VGX_REG_NSTRIDE * (size_t)n_local));
+    VGX_TRY(vgx_sync(c));
     for (int i = 0; i < P; ++i) per_constraint[i] = 0.0;
     for (int k = 0; k < n_local; ++k) per_constraint[g->plan.local[k]] = cs[(size_t)k * VGX_REG_NSTRIDE + 20];
     return VGX_OK;

@@ -165,10 +165,14 @@ int ensure_table(vgx_ctx* c) {
     built = true;
   }
   if (!ok) VGX_FAIL(c, VGX_ERR_INVALID, "the face-walk rule failed to build its table");
-  VGX_CUDA(c, cudaMemcpyToSymbolAsync(c_mesh_ntri, table.ntri, sizeof(table.ntri), 0, cudaMemcpyHostToDevice, c->stream));
-  VGX_CUDA(c, cudaMemcpyToSymbolAsync(c_mesh_tri, table.tri, sizeof(table.tri), 0, cudaMemcpyHostToDevice, c->stream));
-  VGX_CUDA(c, cudaMemcpyToSymbolAsync(c_mesh_edge, table.edge, sizeof(table.edge), 0, cudaMemcpyHostToDevice, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // the host table outlives the copies anyway
+  uint8_t *ntri, (*tri)[15], *edge;
+  VGX_CUDA(c, cudaGetSymbolAddress(reinterpret_cast<void**>(&ntri), c_mesh_ntri));
+  VGX_CUDA(c, cudaGetSymbolAddress(reinterpret_cast<void**>(&tri), c_mesh_tri));
+  VGX_CUDA(c, cudaGetSymbolAddress(reinterpret_cast<void**>(&edge), c_mesh_edge));
+  VGX_TRY(vgx_upload(c, ntri, table.ntri, std::size(table.ntri)));
+  VGX_TRY(vgx_upload(c, tri, table.tri, std::size(table.tri)));
+  VGX_TRY(vgx_upload(c, edge, table.edge, std::size(table.edge)));
+  VGX_TRY(vgx_sync(c));   // the host table outlives the copies anyway
   c->mesh_table_ready = true;
   return VGX_OK;
 }
@@ -425,15 +429,14 @@ extern "C" void vgx_mesh_config_default(vgx_mesh_config* cfg) {
 static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, float min_weight, bool coloured,
                       std::vector<int64_t>& voff, std::vector<int64_t>& toff) {
   const int nj = (int)jobs.size();
-  cudaStream_t st = c->stream;
   unsigned *d_cnt, *d_toff, *d_flag, *d_voff, *d_tmp, *d_offs;
   MeshJob* d_jobs;
   VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_cnt, n_vox + 1), vgx_part(d_toff, n_vox + 1),
                     vgx_part(d_flag, n_vox + 1), vgx_part(d_voff, n_vox + 1),
                     vgx_part(d_tmp, vgx_scan_tmp_count(n_vox)), vgx_part(d_jobs, (size_t)nj),
                     vgx_part(d_offs, 2 * ((size_t)nj + 1))));
-  VGX_CUDA(c, cudaMemcpyAsync(d_jobs, jobs.data(), (size_t)nj * sizeof(MeshJob), cudaMemcpyHostToDevice, st));
-  VGX_CUDA(c, cudaMemsetAsync(d_flag, 0, n_vox * sizeof(unsigned), st));
+  VGX_TRY(vgx_upload(c, d_jobs, jobs.data(), (size_t)nj));
+  VGX_TRY(vgx_fill(c, d_flag, n_vox));
   const unsigned g128 = (unsigned)((n_vox + 127) / 128), g256 = (unsigned)((n_vox + 255) / 256);
   {
     VgxProfileScope scope(c, VGX_SLOT_MESH);
@@ -458,8 +461,7 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
                        d_voff, d_offs));
   }
   std::vector<unsigned> offs(2 * ((size_t)nj + 1));
-  VGX_CUDA(c, cudaMemcpyAsync(offs.data(), d_offs, offs.size() * sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-  VGX_CUDA(c, cudaStreamSynchronize(st));
+  VGX_TRY(vgx_read(c, offs.data(), d_offs, offs.size()));
   const size_t vbase = (size_t)c->mesh_nv, tbase = (size_t)c->mesh_nt;
   const size_t nv = vbase + offs[2 * (size_t)nj + 1], nt = tbase + offs[2 * (size_t)nj];
   if (nv > (size_t)INT32_MAX || nt > (size_t)INT32_MAX)
@@ -487,7 +489,7 @@ static int mesh_batch(vgx_ctx* c, std::vector<MeshJob>& jobs, size_t n_vox, floa
     VGX_TRY(vgx_launch(c, mesh_triangle_kernel, g128, 128, 0, VgxLaunch::plain, d_jobs, nj, n_vox, min_weight, d_toff,
                        d_flag, d_voff, vbase, tbase, c->d_mesh_tri.get()));
   }
-  VGX_CUDA(c, cudaStreamSynchronize(st));   // the scratch is reused by the next batch
+  VGX_TRY(vgx_sync(c));   // the scratch is reused by the next batch
   c->mesh_nv = (int64_t)nv;
   c->mesh_nt = (int64_t)nt;
   return VGX_OK;
@@ -497,7 +499,7 @@ static int mesh_build(vgx_ctx* c, int n, const uint32_t* ids, const float* T_M_S
                       std::vector<int64_t>& voff, std::vector<int64_t>& toff) {
   std::vector<VgxSubmap*> subs((size_t)n);
   for (int k = 0; k < n; ++k) VGX_TRY(vgx_submap_get(c, ids[k], &subs[k]));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // n_blocks of an active submap is final after its integration
+  VGX_TRY(vgx_sync(c));   // n_blocks of an active submap is final after its integration
   VGX_TRY(ensure_table(c));
   // the build carries vertex colours iff one of its submaps has a colour channel
   bool coloured = false;
@@ -569,14 +571,9 @@ extern "C" int vgx_mesh_download(vgx_ctx* c, int64_t max_vertices, float* xyz, i
     if (n_triangles) *n_triangles = c->mesh_nt;
     if ((xyz && c->mesh_nv > max_vertices) || (triangles && c->mesh_nt > max_triangles))
       VGX_FAIL(c, VGX_ERR_CAPACITY, "output too small");
-    if (xyz && c->mesh_nv)
-      VGX_CUDA(c, cudaMemcpyAsync(xyz, c->d_mesh_xyz.get(), 3 * sizeof(float) * (size_t)c->mesh_nv, cudaMemcpyDeviceToHost,
-                                  c->stream));
-    if (triangles && c->mesh_nt)
-      VGX_CUDA(c, cudaMemcpyAsync(triangles, c->d_mesh_tri.get(), 3 * sizeof(uint32_t) * (size_t)c->mesh_nt,
-                                  cudaMemcpyDeviceToHost, c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    return VGX_OK;
+    if (xyz && c->mesh_nv) VGX_TRY(vgx_download(c, xyz, c->d_mesh_xyz.get(), 3 * (size_t)c->mesh_nv));
+    if (triangles && c->mesh_nt) VGX_TRY(vgx_download(c, triangles, c->d_mesh_tri.get(), 3 * (size_t)c->mesh_nt));
+    return vgx_sync(c);
   });
 }
 
@@ -589,10 +586,7 @@ extern "C" int vgx_mesh_download_colours(vgx_ctx* c, int64_t max_vertices, uint3
       memset(rgba, 0, sizeof(uint32_t) * (size_t)c->mesh_nv);
       return VGX_OK;
     }
-    VGX_CUDA(c, cudaMemcpyAsync(rgba, c->d_mesh_rgba.get(), sizeof(uint32_t) * (size_t)c->mesh_nv, cudaMemcpyDeviceToHost,
-                                c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    return VGX_OK;
+    return vgx_read(c, rgba, c->d_mesh_rgba.get(), (size_t)c->mesh_nv);
   });
 }
 
@@ -632,11 +626,9 @@ extern "C" int vgx_mesh_ply_ex(vgx_ctx* c, const uint8_t* rgba, int voxel_colour
     uint32_t *d_col, *d_use;
     VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_body, (size_t)body), vgx_part(d_voff, c->mesh_voff.size()),
                       vgx_part(d_col, col.size()), vgx_part(d_use, voxel ? use.size() : 0)));
-    if (voxel)
-      VGX_CUDA(c, cudaMemcpyAsync(d_use, use.data(), use.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
-    VGX_CUDA(c, cudaMemcpyAsync(d_voff, c->mesh_voff.data(), c->mesh_voff.size() * sizeof(int64_t),
-                                cudaMemcpyHostToDevice, c->stream));
-    VGX_CUDA(c, cudaMemcpyAsync(d_col, col.data(), col.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, c->stream));
+    if (voxel) VGX_TRY(vgx_upload(c, d_use, use.data(), use.size()));
+    VGX_TRY(vgx_upload(c, d_voff, c->mesh_voff.data(), c->mesh_voff.size()));
+    VGX_TRY(vgx_upload(c, d_col, col.data(), col.size()));
     const int64_t recs = c->mesh_nv + c->mesh_nt;
     {
       VgxProfileScope scope(c, VGX_SLOT_MESH);
@@ -644,8 +636,6 @@ extern "C" int vgx_mesh_ply_ex(vgx_ctx* c, const uint8_t* rgba, int voxel_colour
                          c->d_mesh_tri.get(), c->mesh_nv, c->mesh_nt, d_voff, ns, d_col,
                          voxel ? c->d_mesh_rgba.get() : nullptr, d_use, d_body));
     }
-    VGX_CUDA(c, cudaMemcpyAsync(out + hn, d_body, (size_t)body, cudaMemcpyDeviceToHost, c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    return VGX_OK;
+    return vgx_read(c, out + hn, d_body, (size_t)body);
   });
 }

@@ -83,7 +83,7 @@ extern "C" int vgx_comm_init(vgx_ctx* c, int nranks, int rank, const uint8_t id[
 extern "C" int vgx_comm_destroy(vgx_ctx* c) {
   return vgx_entry(c, __func__, [&] {
     if (c->nccl_comm && g_nccl.handle) {
-      cudaStreamSynchronize(c->stream);
+      vgx_drain(c);
       g_nccl.CommDestroy((ncclComm_t)c->nccl_comm);
     }
     c->nccl_comm = nullptr;

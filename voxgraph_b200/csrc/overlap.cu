@@ -125,11 +125,10 @@ extern "C" int vgx_find_overlapping_pairs(vgx_ctx* c, int n, const uint32_t* ids
     OverlapJob* d_jobs;
     int* d_flags;
     VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_jobs, jobs.size()), vgx_part(d_flags, jobs.size())));
-    VGX_CUDA(c, cudaMemcpyAsync(d_jobs, jobs.data(), jobs.size() * sizeof(OverlapJob), cudaMemcpyHostToDevice, c->stream));
+    VGX_TRY(vgx_upload(c, d_jobs, jobs.data(), jobs.size()));
     VGX_TRY(vgx_launch(c, overlap_pairs_kernel, (unsigned)jobs.size(), 128, 0, VgxLaunch::plain, d_jobs, d_flags));
     std::vector<int> flags(jobs.size());
-    VGX_CUDA(c, cudaMemcpyAsync(flags.data(), d_flags, jobs.size() * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    VGX_TRY(vgx_read(c, flags.data(), d_flags, flags.size()));
     int np = 0;
     for (size_t k = 0; k < jobs.size(); ++k) {
       if (!flags[k]) continue;

@@ -24,7 +24,7 @@ p2p_gather_kernel(VgxP2PGather G, double* __restrict__ out, size_t count,
 
 void vgx_p2p_free(vgx_ctx* c) {
   if (!c->p2p_base) return;
-  cudaStreamSynchronize(c->stream);
+  vgx_drain(c);
   for (int r = 0; r < 8; ++r)
     if (c->p2p_peer[r] && c->p2p_peer[r] != c->p2p_base) cudaIpcCloseMemHandle(c->p2p_peer[r]);
   cudaFree(c->p2p_base);
@@ -43,7 +43,9 @@ extern "C" int vgx_comm_p2p_export(vgx_ctx* c, uint64_t capacity_doubles, uint8_
     // the rank count is not known yet: room for the 8 source ranks of one node, two parities
     const size_t bytes = P2P_FLAG_BYTES + 2 * (size_t)P2P_MAX_RANKS * cap * P2P_ELEM_BYTES;
     VGX_CUDA(c, cudaMalloc(&c->p2p_base, bytes));
-    VGX_CUDA(c, cudaMemset(c->p2p_base, 0, bytes));
+    // zero before the handle leaves: the exchange protocol relies on a region that starts zeroed
+    VGX_TRY(vgx_fill(c, static_cast<uint8_t*>(c->p2p_base), bytes));
+    VGX_TRY(vgx_sync(c));
     cudaIpcMemHandle_t h;
     VGX_CUDA(c, cudaIpcGetMemHandle(&h, c->p2p_base));
     memcpy(handle, &h, 64);
@@ -92,10 +94,9 @@ int vgx_p2p_check(vgx_ctx* c) {
   if (!c->p2p_ready) return VGX_OK;
   int t = 0;
   int* d_t = (int*)((char*)c->p2p_base + 128);
-  VGX_CUDA(c, cudaMemcpyAsync(&t, d_t, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+  VGX_TRY(vgx_read(c, &t, d_t));
   if (t) {
-    VGX_CUDA(c, cudaMemsetAsync(d_t, 0, sizeof(int), c->stream));   // not sticky: the next call starts clean
+    VGX_TRY(vgx_fill(c, d_t, 1));   // not sticky: the next call starts clean
     VGX_FAIL(c, VGX_ERR_NCCL, "peer exchange timed out waiting for a rank (NVLink all-gather-reduce); "
                               "the result of that evaluation is NaN");
   }

@@ -373,8 +373,8 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
                     vgx_part(scan_tmp, vgx_scan_tmp_count(P + 1)), vgx_part(d_src, (size_t)ns), vgx_part(d_ctl, 1),
                     vgx_part(d_sort_tmp, sort_tmp)));
   if (P > 0) {
-    VGX_CUDA(c, cudaMemcpyAsync(d_src, h.data(), sizeof(ProjSrc) * (size_t)ns, cudaMemcpyHostToDevice, st));
-    VGX_CUDA(c, cudaMemsetAsync(d_ctl, 0, sizeof(int), st));
+    VGX_TRY(vgx_upload(c, d_src, h.data(), (size_t)ns));
+    VGX_TRY(vgx_fill(c, d_ctl, 1));
     {
       VgxProfileScope scope(c, VGX_SLOT_PROJECT);
       VGX_TRY(vgx_launch(c, project_candidate_kernel, (unsigned)((n_in + 127) / 128), 128, 0, VgxLaunch::plain, d_src, ns,
@@ -402,15 +402,14 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
       VGX_TRY(vgx_launch(c, project_scatter_kernel, gp, 256, 0, VgxLaunch::plain, keys_b, ranks_b, P, pair_head, key_head,
                          pair_pos, key_pos, keys_a, ranks_a, useg));
     }
-    int ctl[2] = {0, 0};
-    VGX_CUDA(c, cudaMemcpyAsync(&ctl[0], d_ctl, sizeof(int), cudaMemcpyDeviceToHost, st));
-    VGX_CUDA(c, cudaMemcpyAsync(&ctl[1], key_pos + P, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-    VGX_CUDA(c, cudaStreamSynchronize(st));
-    if (ctl[0] & 2)
+    int ctl = 0;
+    VGX_TRY(vgx_download(c, &ctl, d_ctl, 1));
+    VGX_TRY(vgx_download(c, &n_keys, key_pos + P, 1));
+    VGX_TRY(vgx_sync(c));
+    if (ctl & 2)
       VGX_FAIL(c, VGX_ERR_INVALID, "a projected block index lies outside the accepted range");
-    if (ctl[0] & 4)
+    if (ctl & 4)
       VGX_FAIL(c, VGX_ERR_INVALID, "more than two candidate samples on an axis");
-    n_keys = (unsigned)ctl[1];
   }
   unsigned* keep = pair_head;
   unsigned* slot = pair_pos;
@@ -424,8 +423,7 @@ static int project(vgx_ctx* c, const std::vector<VgxSubmap*>& subs, const std::v
       VgxProfileScope scope(c, VGX_SLOT_PROJECT);
       VGX_TRY(vgx_exclusive_scan_u32(c, keep, slot, n_keys, scan_tmp));
     }
-    VGX_CUDA(c, cudaMemcpyAsync(&n_out, slot + n_keys, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
-    VGX_CUDA(c, cudaStreamSynchronize(st));
+    VGX_TRY(vgx_read(c, &n_out, slot + n_keys));
   }
   VgxSubmap* s = nullptr;
   VGX_TRY(vgx_submap_alloc(c, out_id, g0.voxel_size, g0.vps, (int)n_out, true, &s));
@@ -471,7 +469,7 @@ extern "C" int vgx_project_map(vgx_ctx* c, int n, const uint32_t* ids, const flo
     for (int r = 1; r < n; ++r)
       if (subs[r]->voxel_size != subs[0]->voxel_size || subs[r]->vps != subs[0]->vps)
         VGX_FAIL(c, VGX_ERR_INVALID, "the submaps differ in voxel size or voxels_per_side");
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // n_blocks of an active submap is final after its integration
+    VGX_TRY(vgx_sync(c));   // n_blocks of an active submap is final after its integration
     int nb = 0;
     const int rc = project(c, subs, poses, out_id, &nb);
     if (rc != VGX_OK) {
@@ -499,7 +497,7 @@ extern "C" int vgx_submap_transform(vgx_ctx* c, uint32_t id, const float* T_new_
     if (!T_new_old) VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
     VgxSubmap* s;
     VGX_TRY(vgx_submap_get(c, id, &s));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // n_blocks of an active submap is final after its integration
+    VGX_TRY(vgx_sync(c));   // n_blocks of an active submap is final after its integration
     // the result is built in a scratch submap next to the old copy, then takes the submap's id
     const uint32_t tmp = vgx_scratch_id(c);
     int nb = 0;

@@ -662,9 +662,9 @@ extern "C" int vgx_reg_eval_emit(vgx_ctx* c, uint32_t ref_id, uint32_t read_id,
       VgxPoints& p = c->submaps.at(ref_id)->points[cfg->registration_point_type];
       int32_t* h_idx;
       VGX_TRY(vgx_carve(c, c->h_pinned, vgx_part(h_idx, Kp)));
-      VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+      VGX_TRY(vgx_sync(c));
       vgx_points_draw(p, (int)K, h_idx);
-      VGX_CUDA(c, cudaMemcpyAsync(d_idx, h_idx, K * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+      VGX_TRY(vgx_upload(c, d_idx, h_idx, K));
       VGX_TRY(vgx_launch_reg_gather_samples(c, p.data.get(), d_idx, (int)K, d_pts));
       C.pts = d_pts;
     }
@@ -677,12 +677,9 @@ extern "C" int vgx_reg_eval_emit(vgx_ctx* c, uint32_t ref_id, uint32_t read_id,
       VGX_TRY(vgx_launch(c, reg_emit_kernel, (unsigned)((K + 255) / 256), 256, 0, VgxLaunch::plain, C, P, d_r, d_jr,
                          d_je));
     }
-    VGX_CUDA(c, cudaMemcpyAsync(residuals, d_r, K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    if (jac_ref)
-      VGX_CUDA(c, cudaMemcpyAsync(jac_ref, d_jr, 4 * K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    if (jac_read)
-      VGX_CUDA(c, cudaMemcpyAsync(jac_read, d_je, 4 * K * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    return VGX_OK;
+    VGX_TRY(vgx_download(c, residuals, d_r, K));
+    if (jac_ref) VGX_TRY(vgx_download(c, jac_ref, d_jr, 4 * K));
+    if (jac_read) VGX_TRY(vgx_download(c, jac_read, d_je, 4 * K));
+    return vgx_sync(c);
   });
 }

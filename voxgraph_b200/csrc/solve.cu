@@ -758,7 +758,6 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
     }
     for (int k = 0; k < 16 * m; ++k) cov[k] = 0.0;   // constant blocks: zero covariance
     if (n == 0 || cols.empty()) return VGX_OK;
-    cudaStream_t st = c->stream;
     VGX_TRY(eval_enqueue(c, g, g->dev.d_x.get(), g->dev.d_packed[0].get(), true, false));
     const size_t M = (size_t)n + 1;
     // scratch: requested column indices | X (ncols x n)
@@ -781,8 +780,8 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
     memset(init, 0, sizeof(*init));
     init->radius = INFINITY;
     init->step_valid = 1;
-    VGX_CUDA(c, cudaMemsetAsync(g->dev.d_A.get(), 0, sizeof(double) * M * M, st));
-    VGX_CUDA(c, cudaMemcpyAsync(g->dev.d_state.get(), init, sizeof(*init), cudaMemcpyHostToDevice, st));
+    VGX_TRY(vgx_fill(c, g->dev.d_A.get(), M * M));
+    VGX_TRY(vgx_upload(c, g->dev.d_state.get(), init, 1));
     {
       VgxProfileScope s(c, VGX_SLOT_SOLVE);
       VGX_TRY(enqueue_lm_build(c, g, n, lo));
@@ -790,7 +789,7 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
                          g->dev.d_state.get(), g->dev.d_diag.get(), VGX_COV_RANK_TOL));
     }
     // inverse columns
-    VGX_CUDA(c, cudaMemcpyAsync(d_cols, cols.data(), sizeof(int) * ncols, cudaMemcpyHostToDevice, st));
+    VGX_TRY(vgx_upload(c, d_cols, cols.data(), ncols));
     if (sizeof(double) * (size_t)n > 48 * 1024)
       VGX_CUDA(c, cudaFuncSetAttribute(cov_column_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                        (int)(sizeof(double) * (size_t)n)));
@@ -801,9 +800,9 @@ extern "C" int vgx_graph_edge_covariances(vgx_ctx* c, int m, const uint32_t* ids
     }
     std::vector<double> X(ncols * (size_t)n);
     LmState hs;
-    VGX_CUDA(c, cudaMemcpyAsync(X.data(), d_X, sizeof(double) * X.size(), cudaMemcpyDeviceToHost, st));
-    VGX_CUDA(c, cudaMemcpyAsync(&hs, g->dev.d_state.get(), sizeof(hs), cudaMemcpyDeviceToHost, st));
-    VGX_CUDA(c, cudaStreamSynchronize(st));
+    VGX_TRY(vgx_download(c, X.data(), d_X, X.size()));
+    VGX_TRY(vgx_download(c, &hs, g->dev.d_state.get(), 1));
+    VGX_TRY(vgx_sync(c));
     if (!hs.step_valid)   // a pivot failed the rank rule above (ceres::Covariance::Compute returns false)
       VGX_FAIL(c, VGX_ERR_INVALID, "J^T J is not positive definite (rank deficient)");
     for (int k = 0; k < m; ++k) {
@@ -893,8 +892,7 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
       VGX_TRY(vgx_launch(c, lm_init_kernel, 1, 256, 0, VgxLaunch::plain, g->dev.d_packed[0].get(),
                          g->dev.d_red_offset.get(), N, g->dev.d_state.get(), o->initial_trust_region_radius, lo));
     }
-    VGX_CUDA(c, cudaMemcpyAsync(g->h_state.get(), g->dev.d_state.get(), sizeof(LmState), cudaMemcpyDeviceToHost, st));
-    VGX_CUDA(c, cudaStreamSynchronize(st));
+    VGX_TRY(vgx_read(c, g->h_state.get(), g->dev.d_state.get()));
     S.initial_cost = g->h_state.get()->cost;
     // Ceres checks the time budget before every iteration, the first included, and before the other
     // tests (iterations, gradient, radius): a budget spent by now ends the solve with x untouched.
@@ -912,7 +910,7 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
       {
         VgxProfileScope s(c, VGX_SLOT_SOLVE);
         if (!use_smem_chol)   // the shared-memory solver reads the written blocks only
-          VGX_CUDA(c, cudaMemsetAsync(g->dev.d_A.get(), 0, sizeof(double) * (size_t)(n + 1) * (n + 1), st));
+          VGX_TRY(vgx_fill(c, g->dev.d_A.get(), (size_t)(n + 1) * (n + 1)));
         VGX_TRY(enqueue_lm_build(c, g, n, lo));
         if (use_smem_chol) {
           VGX_TRY(vgx_launch(c, chol_solve_smem_kernel, 1, 512, smem_chol_bytes, VgxLaunch::plain, g->dev.d_A.get(), n,
@@ -943,8 +941,7 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
       // outcome of iteration k -> host, on the copy stream (the main stream keeps running ahead)
       VGX_CUDA(c, cudaEventRecord(g->ev_iter[k & 1], st));
       VGX_CUDA(c, cudaStreamWaitEvent(g->copy_stream, g->ev_iter[k & 1], 0));
-      VGX_CUDA(c, cudaMemcpyAsync(g->h_snap.get() + (k & 1), g->dev.d_snap.get() + (k & 1), sizeof(LmState),
-                                  cudaMemcpyDeviceToHost, g->copy_stream));
+      VGX_TRY(vgx_download(c, g->h_snap.get() + (k & 1), g->dev.d_snap.get() + (k & 1), 1, g->copy_stream));
       VGX_CUDA(c, cudaEventRecord(g->ev_copy[k & 1], g->copy_stream));
       return VGX_OK;
     };
@@ -964,26 +961,21 @@ extern "C" int vgx_graph_solve(vgx_ctx* c, const vgx_solver_options* opts, doubl
         if (c->nranks == 1 && wall_s() - t0 >= o->max_solver_time_s) { timed_out = true; break; }
         ++k;
       }
-      if (timed_out) VGX_CUDA(c, cudaStreamSynchronize(st));   // iterations in flight still move x
+      if (timed_out) VGX_TRY(vgx_sync(c));   // iterations in flight still move x
       // final poses: the main stream may still be draining the empty launches of the speculative
       // iteration; the copy stream is ordered after the deciding iteration only
-      VGX_CUDA(c, cudaMemcpyAsync(g->h_x.get(), g->dev.d_x.get(), sizeof(double) * 4 * N, cudaMemcpyDeviceToHost,
-                                  timed_out ? st : g->copy_stream));
-      VGX_CUDA(c, cudaStreamSynchronize(timed_out ? st : g->copy_stream));
-      if (timed_out) {
-        VGX_CUDA(c, cudaMemcpyAsync(g->h_state.get(), g->dev.d_state.get(), sizeof(LmState), cudaMemcpyDeviceToHost, st));
-        VGX_CUDA(c, cudaStreamSynchronize(st));
-      }
+      const cudaStream_t fin = timed_out ? st : g->copy_stream;
+      VGX_TRY(vgx_download(c, g->h_x.get(), g->dev.d_x.get(), 4 * (size_t)N, fin));
+      VGX_TRY(vgx_sync(c, fin));
+      if (timed_out) VGX_TRY(vgx_read(c, g->h_state.get(), g->dev.d_state.get()));
       memcpy(g->x.data(), g->h_x.get(), sizeof(double) * 4 * N);
     } else {
-      VGX_CUDA(c, cudaMemcpyAsync(g->x.data(), g->dev.d_x.get(), sizeof(double) * 4 * N, cudaMemcpyDeviceToHost, st));
-      VGX_CUDA(c, cudaStreamSynchronize(st));
+      VGX_TRY(vgx_read(c, g->x.data(), g->dev.d_x.get(), 4 * (size_t)N));
     }
     if (n == 0) { g->h_state.get()->termination = 2; }
     if (d_chol_dbg) {
       long long h[5] = {0, 0, 0, 0, 0};
-      cudaStreamSynchronize(st);
-      cudaMemcpy(h, d_chol_dbg, sizeof(h), cudaMemcpyDeviceToHost);
+      VGX_TRY(vgx_read(c, h, d_chol_dbg, std::size(h)));
       fprintf(stderr, "[vgx] chol n=%d cycles: load %lld update %lld factor+solve %lld back %lld total %lld\n", n, h[0],
               h[1], h[2], h[3], h[4]);
     }

@@ -45,7 +45,7 @@ extern "C" void vgx_ctx_destroy(vgx_ctx* c) {
   vgx_entry_noctx([&] {
     if (!c) return VGX_OK;
     vgx_comm_destroy(c);   // as an entry point, it selects the context's device
-    cudaStreamSynchronize(c->stream);
+    vgx_drain(c);
     vgx_p2p_free(c);
     vgx_graph_free(c);
     for (auto& kv : c->submaps) delete kv.second;
@@ -60,10 +60,7 @@ extern "C" void vgx_ctx_destroy(vgx_ctx* c) {
 extern "C" const char* vgx_last_error(const vgx_ctx* c) { return c ? c->error.c_str() : "null context"; }
 extern "C" void* vgx_ctx_stream(vgx_ctx* c) { return c ? (void*)c->stream : nullptr; }
 extern "C" int vgx_ctx_synchronize(vgx_ctx* c) {
-  return vgx_entry(c, __func__, [&] {
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    return VGX_OK;
-  });
+  return vgx_entry(c, __func__, [&] { return vgx_sync(c); });
 }
 
 extern "C" int vgx_profile_enable(vgx_ctx* c, int on) {
@@ -166,8 +163,7 @@ __global__ void hash_insert_kernel(VgxHash h, const int32_t* block_idx, int n, i
 // new submap is dropped and the upload fails.
 static int check_uploaded_blocks(vgx_ctx* c, VgxSubmap* s) {
   int bad = 0;
-  VGX_CUDA(c, cudaMemcpyAsync(&bad, s->d_counters.get() + 2, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+  VGX_TRY(vgx_read(c, &bad, s->d_counters.get() + 2));
   if (!bad) return VGX_OK;
   vgx_submap_drop(c, s->id);
   VGX_FAIL(c, VGX_ERR_INVALID, (bad & 2) ? "block index outside the accepted range" : "repeated block index");
@@ -239,9 +235,7 @@ int vgx_submap_build_grid(vgx_ctx* c, VgxSubmap* s) {
   const int n = s->n_blocks;
   if (n <= 0) return VGX_OK;
   std::vector<int32_t> idx(3 * (size_t)n);
-  VGX_CUDA(c, cudaMemcpyAsync(idx.data(), s->d_block_idx.get(), sizeof(int32_t) * 3 * n, cudaMemcpyDeviceToHost,
-                              c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+  VGX_TRY(vgx_read(c, idx.data(), s->d_block_idx.get(), idx.size()));
   int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
   for (int i = 0; i < n; ++i)
     for (int a = 0; a < 3; ++a) {
@@ -257,13 +251,13 @@ int vgx_submap_build_grid(vgx_ctx* c, VgxSubmap* s) {
     grid[(size_t)(idx[3 * i + 2] - lo[2]) * dy * dx + (size_t)(idx[3 * i + 1] - lo[1]) * dx +
          (idx[3 * i] - lo[0])] = i;
   VGX_TRY(s->d_grid.alloc(c, sizeof(int32_t) * cells, "dense block grid"));
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_grid.get(), grid.data(), sizeof(int32_t) * cells, cudaMemcpyHostToDevice, c->stream));
+  VGX_TRY(vgx_upload(c, s->d_grid.get(), grid.data(), grid.size()));
   // 16-bit copy for the registration kernel's shared-memory grid (one bulk copy per tile)
   std::vector<uint16_t> g16(((size_t)cells + 7) & ~(size_t)7, 0xFFFF);
   for (long long k = 0; k < cells; ++k) g16[(size_t)k] = grid[(size_t)k] < 0 ? 0xFFFF : (uint16_t)grid[(size_t)k];
   VGX_TRY(s->d_grid16.alloc(c, sizeof(uint16_t) * g16.size(), "dense block grid"));
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_grid16.get(), g16.data(), sizeof(uint16_t) * g16.size(), cudaMemcpyHostToDevice, c->stream));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+  VGX_TRY(vgx_upload(c, s->d_grid16.get(), g16.data(), g16.size()));
+  VGX_TRY(vgx_sync(c));
   for (int a = 0; a < 3; ++a) { s->grid_min[a] = lo[a]; s->grid_dim[a] = hi[a] - lo[a] + 1; }
   return VGX_OK;
 }
@@ -296,7 +290,7 @@ int vgx_submap_alloc(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int cap
     VGX_FAIL(c, VGX_ERR_INVALID, "invalid voxel_size / voxels_per_side / capacity");
   VgxSubmap* old = c->find(id);
   if (old) {
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    VGX_TRY(vgx_sync(c));
     delete old;
     c->submaps.erase(id);
     vgx_graph_invalidate_registration(c);
@@ -328,7 +322,7 @@ int vgx_submap_alloc(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int cap
     delete s;
     return rc;
   }
-  VGX_CUDA(c, cudaMemsetAsync(s->d_counters.get(), 0, sizeof(int) * 4, c->stream));
+  VGX_TRY(vgx_fill(c, s->d_counters.get(), 4));
   c->submaps[id] = s;
   *out = s;
   return VGX_OK;
@@ -348,10 +342,9 @@ extern "C" int vgx_submap_upload(vgx_ctx* c, uint32_t id, float voxel_size, int 
     const size_t nvox = (size_t)n_blocks * s->vox_per_block;
     float *tmp_d, *tmp_w;
     VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(tmp_d, nvox), vgx_part(tmp_w, nvox)));
-    VGX_CUDA(c, cudaMemcpyAsync(tmp_d, distance, nvox * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    VGX_CUDA(c, cudaMemcpyAsync(tmp_w, weight, nvox * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx.get(), block_idx, sizeof(int32_t) * 3 * n_blocks,
-                                cudaMemcpyHostToDevice, c->stream));
+    VGX_TRY(vgx_upload(c, tmp_d, distance, nvox));
+    VGX_TRY(vgx_upload(c, tmp_w, weight, nvox));
+    VGX_TRY(vgx_upload(c, s->d_block_idx.get(), block_idx, 3 * (size_t)n_blocks));
     VGX_TRY(vgx_launch(c, interleave_kernel, (unsigned)((nvox + 255) / 256), 256, 0, VgxLaunch::plain, tmp_d, tmp_w,
                        s->d_dw.get(), nvox));
     // synchronises: the host buffers are the caller's
@@ -364,7 +357,7 @@ extern "C" int vgx_submap_peek_device(vgx_ctx* c, uint32_t id, const int32_t** d
   return vgx_entry(c, __func__, [&] {
     VgxSubmap* s;
     VGX_TRY(vgx_submap_get(c, id, &s));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // the caller reads the bricks on its own stream
+    VGX_TRY(vgx_sync(c));   // the caller reads the bricks on its own stream
     if (d_block_idx) *d_block_idx = s->d_block_idx.get();
     if (d_dw) *d_dw = reinterpret_cast<const float*>(s->d_dw.get());
     if (n_blocks) *n_blocks = s->n_blocks;
@@ -382,9 +375,8 @@ extern "C" int vgx_submap_upload_device(vgx_ctx* c, uint32_t id, float voxel_siz
     s->finished = true;
     if (n_blocks == 0) return VGX_OK;
     const size_t nvox = (size_t)n_blocks * s->vox_per_block;
-    VGX_CUDA(c, cudaMemcpyAsync(s->d_block_idx.get(), d_block_idx, sizeof(int32_t) * 3 * n_blocks,
-                                cudaMemcpyDeviceToDevice, c->stream));
-    VGX_CUDA(c, cudaMemcpyAsync(s->d_dw.get(), d_dw, sizeof(float2) * nvox, cudaMemcpyDeviceToDevice, c->stream));
+    VGX_TRY(vgx_copy(c, s->d_block_idx.get(), d_block_idx, 3 * (size_t)n_blocks));
+    VGX_TRY(vgx_copy(c, s->d_dw.get(), reinterpret_cast<const float2*>(d_dw), nvox));   // (distance, weight) pairs
     // synchronises: the source buffers are the caller's
     return vgx_submap_upload_finish(c, s);
   });
@@ -393,10 +385,10 @@ extern "C" int vgx_submap_upload_device(vgx_ctx* c, uint32_t id, float voxel_siz
 // ------------------------------------------------------------------ colour channel
 int vgx_submap_ensure_colour(vgx_ctx* c, VgxSubmap* s) {
   if (s->d_rgba.get()) return VGX_OK;
-  const size_t bytes = sizeof(uint32_t) * (size_t)s->cap_blocks * s->vox_per_block;
+  const size_t words = (size_t)s->cap_blocks * s->vox_per_block;
   VgxBuffer<uint32_t> q;
-  VGX_TRY(q.alloc(c, bytes, "submap colour channel", VGX_ERR_NOMEM));
-  VGX_CUDA(c, cudaMemsetAsync(q.get(), 0, bytes, c->stream));
+  VGX_TRY(q.alloc(c, sizeof(uint32_t) * words, "submap colour channel", VGX_ERR_NOMEM));
+  VGX_TRY(vgx_fill(c, q.get(), words));
   s->d_rgba = std::move(q);
   return VGX_OK;
 }
@@ -419,38 +411,36 @@ extern "C" int vgx_submap_download_colour(vgx_ctx* c, uint32_t id, int max_block
     if (n_out) *n_out = n;
     if (n > max_blocks) VGX_FAIL(c, VGX_ERR_CAPACITY, "max_blocks too small");
     if (n == 0 || !rgba) return VGX_OK;
-    const size_t bytes = sizeof(uint32_t) * (size_t)n * s->vox_per_block;
+    const size_t words = (size_t)n * s->vox_per_block;
     if (!s->d_rgba.get()) {
-      memset(rgba, 0, bytes);
+      memset(rgba, 0, sizeof(uint32_t) * words);
       return VGX_OK;
     }
-    VGX_CUDA(c, cudaMemcpyAsync(rgba, s->d_rgba.get(), bytes, cudaMemcpyDeviceToHost, c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    return VGX_OK;
+    return vgx_read(c, rgba, s->d_rgba.get(), words);
   });
 }
 
 // the channel of submap id from n_blocks x vps^3 words in host or device memory; the submap keeps its
 // previous channel (or none) when anything fails
-static int upload_colour(vgx_ctx* c, uint32_t id, int n_blocks, const uint32_t* rgba, cudaMemcpyKind kind) {
+static int upload_colour(vgx_ctx* c, uint32_t id, int n_blocks, const uint32_t* rgba, bool on_device) {
   VgxSubmap* s;
   VGX_TRY(vgx_submap_get(c, id, &s));
   if (n_blocks != s->n_blocks) VGX_FAIL(c, VGX_ERR_INVALID, "n_blocks differs from the submap's");
   if (n_blocks > 0 && !rgba) VGX_FAIL(c, VGX_ERR_INVALID, "null input");
-  const size_t cap_bytes = sizeof(uint32_t) * (size_t)s->cap_blocks * s->vox_per_block;
-  const size_t bytes = sizeof(uint32_t) * (size_t)n_blocks * s->vox_per_block;
+  const size_t cap_words = (size_t)s->cap_blocks * s->vox_per_block;
+  const size_t words = (size_t)n_blocks * s->vox_per_block;
   VgxBuffer<uint32_t> q;
-  VGX_TRY(q.alloc(c, cap_bytes, "colour channel", VGX_ERR_NOMEM));
-  VGX_CUDA(c, cudaMemsetAsync(q.get(), 0, cap_bytes, c->stream));
-  if (bytes) VGX_CUDA(c, cudaMemcpyAsync(q.get(), rgba, bytes, kind, c->stream));
+  VGX_TRY(q.alloc(c, sizeof(uint32_t) * cap_words, "colour channel", VGX_ERR_NOMEM));
+  VGX_TRY(vgx_fill(c, q.get(), cap_words));
+  if (words) VGX_TRY(on_device ? vgx_copy(c, q.get(), rgba, words) : vgx_upload(c, q.get(), rgba, words));
   // synchronises: the source is the caller's, and the stream may still read the old channel
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+  VGX_TRY(vgx_sync(c));
   s->d_rgba = std::move(q);
   return VGX_OK;
 }
 
 extern "C" int vgx_submap_upload_colour(vgx_ctx* c, uint32_t id, int n_blocks, const uint32_t* rgba) {
-  return vgx_entry(c, __func__, [&] { return upload_colour(c, id, n_blocks, rgba, cudaMemcpyHostToDevice); });
+  return vgx_entry(c, __func__, [&] { return upload_colour(c, id, n_blocks, rgba, false); });
 }
 
 extern "C" int vgx_submap_peek_device_colour(vgx_ctx* c, uint32_t id, const uint32_t** d_rgba) {
@@ -458,19 +448,19 @@ extern "C" int vgx_submap_peek_device_colour(vgx_ctx* c, uint32_t id, const uint
     if (!d_rgba) return VGX_ERR_INVALID;
     VgxSubmap* s;
     VGX_TRY(vgx_submap_get(c, id, &s));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));   // the caller reads the channel on its own stream
+    VGX_TRY(vgx_sync(c));   // the caller reads the channel on its own stream
     *d_rgba = s->d_rgba.get();
     return VGX_OK;
   });
 }
 
 extern "C" int vgx_submap_upload_device_colour(vgx_ctx* c, uint32_t id, int n_blocks, const uint32_t* d_rgba) {
-  return vgx_entry(c, __func__, [&] { return upload_colour(c, id, n_blocks, d_rgba, cudaMemcpyDeviceToDevice); });
+  return vgx_entry(c, __func__, [&] { return upload_colour(c, id, n_blocks, d_rgba, true); });
 }
 
 int vgx_submap_upload_finish(vgx_ctx* c, VgxSubmap* s) {
   if (s->n_blocks == 0) return VGX_OK;
-  VGX_CUDA(c, cudaMemcpyAsync(s->d_counters.get(), &s->n_blocks, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  VGX_TRY(vgx_upload(c, s->d_counters.get(), &s->n_blocks, 1));
   VGX_TRY(vgx_launch(c, hash_insert_kernel, (s->n_blocks + 127) / 128, 128, 0, VgxLaunch::plain, s->hash(),
                      s->d_block_idx.get(), s->n_blocks, s->d_counters.get() + 2));
   VGX_TRY(vgx_submap_build_view(c, s, s->d_dw.get(), s->d_view.get()));
@@ -484,8 +474,7 @@ extern "C" int vgx_submap_create(vgx_ctx* c, uint32_t id, float voxel_size, int 
     VgxSubmap* s = nullptr;
     VGX_TRY(vgx_submap_alloc(c, id, voxel_size, vps, capacity, false, &s));
     // new voxblox blocks are zero-initialised (distance 0, weight 0)
-    VGX_CUDA(c, cudaMemsetAsync(s->d_dw.get(), 0, sizeof(float2) * (size_t)capacity * s->vox_per_block,
-                                c->stream));
+    VGX_TRY(vgx_fill(c, s->d_dw.get(), (size_t)capacity * s->vox_per_block));
     s->finished = false;
     return VGX_OK;
   });
@@ -512,7 +501,7 @@ extern "C" int vgx_submap_free(vgx_ctx* c, uint32_t id) {
   return vgx_entry(c, __func__, [&] {
     VgxSubmap* s;
     VGX_TRY(vgx_submap_get(c, id, &s));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    VGX_TRY(vgx_sync(c));
     delete s;
     c->submaps.erase(id);
     vgx_graph_invalidate_registration(c);
@@ -527,7 +516,7 @@ void vgx_submap_drop(vgx_ctx* c, uint32_t id) {
 int vgx_submap_move(vgx_ctx* c, uint32_t from_id, uint32_t id) {
   VgxSubmap* s;
   VGX_TRY(vgx_submap_get(c, from_id, &s));
-  VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+  VGX_TRY(vgx_sync(c));
   VgxSubmap* old = c->find(id);
   delete old;
   c->submaps.erase(from_id);
@@ -576,21 +565,16 @@ extern "C" int vgx_submap_download(vgx_ctx* c, uint32_t id, int max_blocks, int3
     if (n > max_blocks) VGX_FAIL(c, VGX_ERR_CAPACITY, "max_blocks too small");
     if (n == 0) return VGX_OK;
     const size_t nvox = (size_t)n * s->vox_per_block;
-    if (block_idx)
-      VGX_CUDA(c, cudaMemcpyAsync(block_idx, s->d_block_idx.get(), sizeof(int32_t) * 3 * n,
-                                  cudaMemcpyDeviceToHost, c->stream));
+    if (block_idx) VGX_TRY(vgx_download(c, block_idx, s->d_block_idx.get(), 3 * (size_t)n));
     if (distance || weight) {
       float *tmp_d, *tmp_w;
       VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(tmp_d, nvox), vgx_part(tmp_w, nvox)));
       VGX_TRY(vgx_launch(c, deinterleave_kernel, (unsigned)((nvox + 255) / 256), 256, 0, VgxLaunch::plain,
                          s->d_dw.get(), tmp_d, tmp_w, nvox));
-      if (distance)
-        VGX_CUDA(c, cudaMemcpyAsync(distance, tmp_d, nvox * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-      if (weight)
-        VGX_CUDA(c, cudaMemcpyAsync(weight, tmp_w, nvox * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+      if (distance) VGX_TRY(vgx_download(c, distance, tmp_d, nvox));
+      if (weight) VGX_TRY(vgx_download(c, weight, tmp_w, nvox));
     }
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-    return VGX_OK;
+    return vgx_sync(c);
   });
 }
 
@@ -601,7 +585,7 @@ extern "C" int vgx_submap_upload_points(vgx_ctx* c, uint32_t id, int type, int n
       VGX_FAIL(c, VGX_ERR_INVALID, "invalid argument");
     VgxSubmap* s;
     VGX_TRY(vgx_submap_get(c, id, &s));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    VGX_TRY(vgx_sync(c));
     VgxPoints& p = s->points[type];
     p = VgxPoints();
     vgx_graph_invalidate_registration(c);
@@ -626,8 +610,8 @@ extern "C" int vgx_submap_upload_points(vgx_ctx* c, uint32_t id, int type, int n
     }
     VgxBuffer<float> d;
     VGX_TRY(d.alloc(c, floats * sizeof(float), "points upload"));
-    VGX_CUDA(c, cudaMemcpyAsync(d.get(), h, floats * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
+    VGX_TRY(vgx_upload(c, d.get(), h, floats));
+    VGX_TRY(vgx_sync(c));
     p.n = n;
     p.data = std::move(d);
     p.sum_w = sum_w;

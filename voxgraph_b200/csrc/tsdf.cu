@@ -691,7 +691,7 @@ static int tsdf_sort_and_apply(vgx_ctx* c, VgxSubmap* s, const TsdfParams& P, co
                     vgx_part(d_heads, (size_t)total / VGX_TSDF_LONG_SEGMENT + 2), vgx_part(d_sort_tmp, sort_tmp)));
   uint32_t* d_rgba = kColour ? s->d_rgba.get() : nullptr;
   VgxProfileScope scope(c, VGX_SLOT_TSDF_INTEGRATE);
-  VGX_CUDA(c, cudaMemsetAsync(d_nlong, 0, 256, stream));
+  VGX_TRY(vgx_fill(c, d_nlong, 64));
   VGX_TRY(vgx_launch(c, tsdf_emit_kernel<kColour>, grid, 128, 0, VgxLaunch::plain, P, d_pts, d_ray_rgba, s->hash(),
                      d_offsets, sentinel, k_in, v_in, d_stats));
   VGX_CUDA(c, cub::DeviceRadixSort::SortPairs(d_sort_tmp, sort_tmp, k_in, k_out, (SortValue*)v_in, (SortValue*)v_out,
@@ -737,10 +737,8 @@ int vgx_tsdf_integrate_resident(vgx_ctx* c, VgxSubmap* s, const float T_G_C[7], 
   // the first coloured scan gives the submap its colour channel, once its scratch is in place; a call that
   // fails later (block capacity) or whose points are all rejected still leaves the channel, all zero
   if (rgba) VGX_TRY(vgx_submap_ensure_colour(c, s));
-  const size_t set_bytes = sizeof(unsigned long long) << 20;
   unsigned long long* d_obs = d_start + (1u << 20);
-  cudaStream_t stream = c->stream;
-  if (P.cfg.mode == 1) VGX_CUDA(c, cudaMemsetAsync(d_start, 0xff, 2 * set_bytes, stream));
+  if (P.cfg.mode == 1) VGX_TRY(vgx_fill(c, d_start, vgx_tsdf_set_words(P.cfg), 0xff));
   const int blocks_before = s->n_blocks;
   const unsigned grid = (unsigned)((n + 127) / 128);
   if (P.cfg.mode == 0) {
@@ -759,8 +757,7 @@ int vgx_tsdf_integrate_resident(vgx_ctx* c, VgxSubmap* s, const float T_G_C[7], 
       VGX_TRY(vgx_launch(c, tsdf_count_kernel, grid, 128, 0, VgxLaunch::plain, P, d_pts, d_counts));
       VGX_TRY(vgx_exclusive_scan_u32(c, d_counts, d_offsets, (size_t)n, d_scan_tmp));   // hand-written, 3 launches
     }
-    VGX_CUDA(c, cudaMemcpyAsync(&total, d_offsets + n, sizeof(unsigned), cudaMemcpyDeviceToHost, stream));
-    VGX_CUDA(c, cudaStreamSynchronize(stream));
+    VGX_TRY(vgx_read(c, &total, d_offsets + n));
     if (total > 0) {
       VGX_TRY(rgba ? tsdf_sort_and_apply<true>(c, s, P, d_pts, d_ray_rgba, d_offsets, total, d_stats)
                                                : tsdf_sort_and_apply<false>(c, s, P, d_pts, nullptr, d_offsets, total, d_stats));
@@ -774,9 +771,9 @@ int vgx_tsdf_integrate_resident(vgx_ctx* c, VgxSubmap* s, const float T_G_C[7], 
   }
   unsigned long long h_stats[VGX_TSDF_STAT_CALLER + 1];
   int h_counters[2];
-  VGX_CUDA(c, cudaMemcpyAsync(h_stats, d_stats, sizeof(h_stats), cudaMemcpyDeviceToHost, stream));
-  VGX_CUDA(c, cudaMemcpyAsync(h_counters, s->d_counters.get(), sizeof(h_counters), cudaMemcpyDeviceToHost, stream));
-  VGX_CUDA(c, cudaStreamSynchronize(stream));
+  VGX_TRY(vgx_download(c, h_stats, d_stats, std::size(h_stats)));
+  VGX_TRY(vgx_download(c, h_counters, s->d_counters.get(), std::size(h_counters)));
+  VGX_TRY(vgx_sync(c));
   const bool overflow = h_counters[1] != 0 || h_counters[0] > s->cap_blocks;
   s->n_blocks = h_counters[0] < s->cap_blocks ? h_counters[0] : s->cap_blocks;
   st.rays_valid = (int64_t)h_stats[0];
@@ -787,11 +784,12 @@ int vgx_tsdf_integrate_resident(vgx_ctx* c, VgxSubmap* s, const float T_G_C[7], 
   if (stats) *stats = st;
   if (n_points) *n_points = (int)h_stats[VGX_TSDF_STAT_CALLER];
   if (overflow) {
-    // keys without a brick must not stay in the table: rebuild it from the blocks that exist
-    int fixed[2] = {s->n_blocks, 0};
-    cudaMemcpyAsync(s->d_counters.get(), fixed, sizeof(fixed), cudaMemcpyHostToDevice, stream);
-    vgx_submap_rebuild_hash(c, s);
-    cudaStreamSynchronize(stream);
+    // keys without a brick must not stay in the table: rebuild it from the blocks that exist.  A repair that
+    // fails leaves the hash in an unknown state, so its status and message are the call's.
+    const int fixed[2] = {s->n_blocks, 0};
+    VGX_TRY(vgx_upload(c, s->d_counters.get(), fixed, std::size(fixed)));
+    VGX_TRY(vgx_submap_rebuild_hash(c, s));
+    VGX_TRY(vgx_sync(c));
     VGX_FAIL(c, VGX_ERR_CAPACITY, "submap block capacity exhausted");
   }
   return VGX_OK;
@@ -815,10 +813,10 @@ extern "C" int vgx_tsdf_integrate(vgx_ctx* c, uint32_t id, const float T_G_C[7],
     uint32_t* d_ray_rgba;   // r, g, b, a bytes per point, as the caller has them
     VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_pts, 3 * (size_t)n), vgx_part(d_stats, VGX_TSDF_STAT_WORDS),
                       vgx_part(d_start, vgx_tsdf_set_words(rcfg)), vgx_part(d_ray_rgba, rgba ? (size_t)n : 0)));
-    cudaStream_t stream = c->stream;
-    VGX_CUDA(c, cudaMemcpyAsync(d_pts, points_C, sizeof(float) * 3 * (size_t)n, cudaMemcpyHostToDevice, stream));
-    if (rgba) VGX_CUDA(c, cudaMemcpyAsync(d_ray_rgba, rgba, 4 * (size_t)n, cudaMemcpyHostToDevice, stream));
-    VGX_CUDA(c, cudaMemsetAsync(d_stats, 0, sizeof(unsigned long long) * VGX_TSDF_STAT_WORDS, stream));
+    VGX_TRY(vgx_upload(c, d_pts, points_C, 3 * (size_t)n));
+    // the caller's r, g, b, a bytes into the device's colour words: written in bytes
+    if (rgba) VGX_TRY(vgx_upload(c, reinterpret_cast<uint8_t*>(d_ray_rgba), rgba, 4 * (size_t)n));
+    VGX_TRY(vgx_fill(c, d_stats, VGX_TSDF_STAT_WORDS));
     return vgx_tsdf_integrate_resident(c, s, T_G_C, rcfg, n, d_pts, rgba ? d_ray_rgba : nullptr, d_stats, d_start, stats,
                                        nullptr);
   });
@@ -847,7 +845,7 @@ extern "C" int vgx_tsdf_integrate_device(vgx_ctx* c, uint32_t id, const float T_
     }
     unsigned long long *d_stats, *d_start;
     VGX_TRY(vgx_carve(c, c->d_scratch, vgx_part(d_stats, VGX_TSDF_STAT_WORDS), vgx_part(d_start, vgx_tsdf_set_words(rcfg))));
-    VGX_CUDA(c, cudaMemsetAsync(d_stats, 0, sizeof(unsigned long long) * VGX_TSDF_STAT_WORDS, c->stream));
+    VGX_TRY(vgx_fill(c, d_stats, VGX_TSDF_STAT_WORDS));
     return vgx_tsdf_integrate_resident(c, s, T_G_C, rcfg, n, d_points_C, d_rgba, d_stats, d_start, stats, nullptr);
   });
 }

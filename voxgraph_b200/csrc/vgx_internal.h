@@ -333,19 +333,6 @@ int VgxBuffer<T>::alloc(vgx_ctx* c, size_t bytes, const char* what, int nomem) {
   return VGX_OK;
 }
 
-template <class T>
-int VgxBuffer<T>::grow_keep(vgx_ctx* c, size_t need, size_t used, const char* what) {
-  if (need <= bytes_) return VGX_OK;
-  VgxBuffer q(kind_);
-  VGX_TRY(q.alloc(c, need + need / 4, what));
-  if (used) {
-    VGX_CUDA(c, cudaMemcpyAsync(q.p_, p_, used, cudaMemcpyDefault, c->stream));
-    VGX_CUDA(c, cudaStreamSynchronize(c->stream));
-  }
-  *this = std::move(q);
-  return VGX_OK;
-}
-
 // ------------------------------------------------------------------ scratch layout
 // one part of a vgx_carve layout: n elements of T at *at
 template <class T>
@@ -436,6 +423,64 @@ int vgx_launch(vgx_ctx* c, void (*kernel)(P...), dim3 grid, dim3 block, size_t s
     c->set_error(std::string("kernel launch: ") + cudaGetErrorString(e));
     return VGX_ERR_CUDA;
   }
+  return VGX_OK;
+}
+
+// ------------------------------------------------------------------ host-device copies
+// The one place that calls the runtime's copies, memsets and stream synchronises.  A transfer states its element
+// count once and takes the element type from its pointers (two sides of different types are written in uint8_t
+// bytes at the call site).  It runs on the context's stream unless one is passed, and a failure sets the message
+// as VGX_CUDA sets it and returns VGX_ERR_CUDA.  Copies are asynchronous; vgx_read is a download that ends in a
+// synchronise, the idiom of a count read back from the device.
+static inline int vgx_cuda_status(vgx_ctx* c, cudaError_t e, const char* call) {
+  if (e == cudaSuccess) return VGX_OK;
+  c->set_error(std::string(call) + ": " + cudaGetErrorString(e));
+  return VGX_ERR_CUDA;
+}
+template <class T>
+int vgx_upload(vgx_ctx* c, T* d, const T* h, size_t n) {
+  return vgx_cuda_status(c, cudaMemcpyAsync(d, h, sizeof(T) * n, cudaMemcpyHostToDevice, c->stream),
+                         "cudaMemcpyAsync host to device");
+}
+template <class T>
+int vgx_download(vgx_ctx* c, T* h, const T* d, size_t n, cudaStream_t st) {
+  return vgx_cuda_status(c, cudaMemcpyAsync(h, d, sizeof(T) * n, cudaMemcpyDeviceToHost, st),
+                         "cudaMemcpyAsync device to host");
+}
+template <class T>
+int vgx_download(vgx_ctx* c, T* h, const T* d, size_t n) { return vgx_download(c, h, d, n, c->stream); }
+// device to device, or pinned to pinned
+template <class T>
+int vgx_copy(vgx_ctx* c, T* dst, const T* src, size_t n) {
+  return vgx_cuda_status(c, cudaMemcpyAsync(dst, src, sizeof(T) * n, cudaMemcpyDefault, c->stream), "cudaMemcpyAsync");
+}
+// every byte of the n elements at d set to `byte`
+template <class T>
+int vgx_fill(vgx_ctx* c, T* d, size_t n, int byte = 0) {
+  return vgx_cuda_status(c, cudaMemsetAsync(d, byte, sizeof(T) * n, c->stream), "cudaMemsetAsync");
+}
+static inline int vgx_sync(vgx_ctx* c, cudaStream_t st) {
+  return vgx_cuda_status(c, cudaStreamSynchronize(st), "cudaStreamSynchronize");
+}
+static inline int vgx_sync(vgx_ctx* c) { return vgx_sync(c, c->stream); }
+template <class T>
+int vgx_read(vgx_ctx* c, T* h, const T* d, size_t n = 1) {
+  VGX_TRY(vgx_download(c, h, d, n));
+  return vgx_sync(c);
+}
+// unchecked synchronise for the void teardown paths: it leaves the context's message alone
+static inline void vgx_drain(vgx_ctx* c) { cudaStreamSynchronize(c->stream); }
+
+template <class T>
+int VgxBuffer<T>::grow_keep(vgx_ctx* c, size_t need, size_t used, const char* what) {
+  if (need <= bytes_) return VGX_OK;
+  VgxBuffer q(kind_);
+  VGX_TRY(q.alloc(c, need + need / 4, what));
+  if (used) {   // bytes
+    VGX_TRY(vgx_copy(c, reinterpret_cast<uint8_t*>(q.p_), reinterpret_cast<const uint8_t*>(p_), used));
+    VGX_TRY(vgx_sync(c));
+  }
+  *this = std::move(q);
   return VGX_OK;
 }
 
