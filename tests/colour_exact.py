@@ -1,14 +1,17 @@
 """Exact numpy-float32 models of the voxel colour rules (csrc/colour.cuh, csrc/tsdf.cu), for
-tests/test_oracle_colour.py and tests/test_gpu_colour.py.  The rules are restated from the published
-voxblox sources; like the kernels they have not been checked against a compiled voxblox.
+tests/test_oracle_colour.py, tests/test_gpu_tsdf_exact.py and tests/test_gpu_colour*.py.  The rules are
+restated from the published voxblox sources; like the kernels they have not been checked against a compiled
+voxblox.
 
 * `pack`: r, g, b, a bytes -> the stored word  a | b << 8 | g << 16 | r << 24  (the third word of a voxel
-  in a collection file).
+  in a collection file).  `colours`: test colours whose four channels differ.
 * `blend`: Color::blendTwoColors.
-* `trace_rays`: the oracle's update trace with the ray each tuple belongs to (one oracle call per point:
-  in mode 0, and in mode 1 with every ray cast, the rays do not interact except through the voxels).
+* `trace_rays`: the oracle's statistics and update trace with the ray each tuple belongs to (one oracle
+  call per point: in mode 0, and in mode 1 with every ray cast, the rays do not interact except through
+  the voxels).
 * `replay`: updateTsdfVoxel's colour rule applied voxel by voxel in ray order next to tsdf_exact's
-  (distance, weight) update: the sequential coloured integrator.
+  (distance, weight) update: the sequential coloured integrator.  `expected_words` lays its result out
+  as a downloaded layer's colour words.
 * `merge`: mergeVoxelAIntoVoxelB's colour and weight.  `interp_channels`: Interpolator::interpVoxel's colour from
   the 8 neighbour words and the offset of the point in the cell.  `containing_voxel` / `vertex_colours`:
   MeshIntegrator::updateMeshColor's rule, the colour of the voxel that contains a vertex.
@@ -31,6 +34,11 @@ def unpack(words):
     """(n,) uint32 stored words -> (n, 4) uint8 [r g b a]."""
     w = np.asarray(words, np.uint32).reshape(-1)
     return np.stack([w >> 24, (w >> 16) & 255, (w >> 8) & 255, w & 255], -1).astype(np.uint8)
+
+
+def colours(rs, n):
+    """n colours [r g b a] from the RandomState rs, the four channels of each one distinct."""
+    return np.argsort(rs.rand(n, 256), 1)[:, :4].astype(np.uint8)
 
 
 def blend(c1, w1, c2, w2):
@@ -59,16 +67,16 @@ def colour_step(trunc, sdf, uw, vw, ray, colour):
 
 
 def trace_rays(oracle, layer, cfg, T, pts):
-    """oracle.tsdf_integrate_trace point by point -> (g (m, 3), sdf (m,), uw (m,), ray (m,) point index)."""
+    """oracle.tsdf_integrate_trace point by point (it integrates into `layer`) -> ((rays_valid, rays_cast,
+    voxel_updates, blocks_allocated) summed over the points, g (m, 3), sdf (m,), uw (m,), ray (m,) point index)."""
     pts = np.asarray(pts, F32).reshape(-1, 3)
-    G, S, U, R = [], [], [], []
+    st = np.zeros(4, np.int64)
+    G, S, U, R = [np.zeros((0, 3), np.int64)], [np.zeros(0, F32)], [np.zeros(0, F32)], [np.zeros(0, np.int64)]
     for i in range(len(pts)):
-        _, g, s, u = oracle.tsdf_integrate_trace(layer, cfg, T, pts[i:i + 1])
-        if len(s):
-            G.append(g); S.append(s); U.append(u); R.append(np.full(len(s), i, np.int64))
-    if not G:
-        return np.zeros((0, 3), np.int64), np.zeros(0, F32), np.zeros(0, F32), np.zeros(0, np.int64)
-    return np.concatenate(G), np.concatenate(S), np.concatenate(U), np.concatenate(R)
+        o, g, s, u = oracle.tsdf_integrate_trace(layer, cfg, T, pts[i:i + 1])
+        st += (o.rays_valid, o.rays_cast, o.voxel_updates, o.blocks_allocated)
+        G.append(g); S.append(s); U.append(u); R.append(np.full(len(s), i, np.int64))
+    return tuple(int(v) for v in st), np.concatenate(G), np.concatenate(S), np.concatenate(U), np.concatenate(R)
 
 
 class State(tx.State):
@@ -112,7 +120,9 @@ def replay(keys, sdf, uw, ray_words, trunc, max_weight, state):
     for r in range(int(cnt_s[0]) if len(cnt_s) else 0):
         n = int(np.searchsorted(neg, -r, side="left"))   # voxels with more than r updates
         j = start_s[:n] + r
-        cc[:n] = colour_step(trunc, s[j], u[j], ww[:n], rw[j], cc[:n])
+        b = np.nonzero(np.abs(s[j]) < trunc)[0]     # colour_step changes nothing outside the band
+        if b.size:
+            cc[b] = colour_step(trunc, s[j[b]], u[j[b]], ww[b], rw[j[b]], cc[b])
         dd[:n], ww[:n] = tx.apply_update(s[j], u[j], dd[:n], ww[:n], trunc, M)
     inv = np.empty_like(by); inv[by] = np.arange(len(by))
     d_out, w_out, c_out = dd[inv], ww[inv], cc[inv]
@@ -128,6 +138,17 @@ def layer_colours(idx, words, vps):
     k = tx.voxel_keys((idx[:, None, :] * vps + loc[None]).reshape(-1, 3))
     o = np.argsort(k, kind="stable")
     return k[o], np.asarray(words, np.uint32).reshape(-1)[o]
+
+
+def expected_words(idx, vps, state):
+    """The colours of `state` (a State) laid out as the voxels of the downloaded blocks `idx` sorted by key (as
+    layer_colours); 0 where never touched.  Every voxel of `state` must lie in those blocks."""
+    keys = layer_colours(idx, np.zeros((len(idx), vps ** 3), np.uint32), vps)[0]
+    exp = np.zeros(len(keys), np.uint32)
+    pos = np.searchsorted(keys, state.keys)
+    assert np.array_equal(keys[pos], state.keys)
+    exp[pos] = state.c
+    return exp
 
 
 def merge(cA, wA, cB, wB):

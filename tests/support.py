@@ -2,7 +2,8 @@
 test_*.py only); a helper that one module uses stays in that module.
 
 A GPU module takes the context fixture with `from support import ctx  # noqa: F401`: the fixture is
-module-scoped, so each module that imports it gets a context of its own."""
+module-scoped, so each module that imports it gets a context of its own.  The synthetic room `world` is
+imported the same way."""
 import atexit
 import ctypes as C
 import os
@@ -28,6 +29,13 @@ def ctx():
     c = api.Context(0)
     yield c
     c.close()
+
+
+@pytest.fixture(scope="module")
+def world():
+    """The 30 m x 30 m synthetic room the integration tests scan."""
+    from voxgraph_b200 import synth
+    return synth.make_world(3, size_xy=(30.0, 30.0), n_clutter=40, n_walls=4)
 
 
 def same_bits(exp, got, what):

@@ -11,7 +11,7 @@ import pytest
 import cloud_exact as ce
 import colour_exact as cx
 import tsdf_exact as tx
-from support import IDENTITY, ctx  # noqa: F401
+from support import IDENTITY, ctx, world  # noqa: F401
 from voxgraph_b200 import _lib, api, mapper as vm, synth
 
 pytestmark = pytest.mark.gpu
@@ -19,14 +19,7 @@ pytestmark = pytest.mark.gpu
 F32 = np.float32
 F = api.POINTFIELD_FLOAT32
 _ids = itertools.count(9000)
-FAST_ALL = dict(mode=1, start_voxel_subsampling_factor=1e3, max_consecutive_ray_collisions=1 << 30,
-                use_weight_dropoff=0)
 LAYOUTS = ["xyz16", "xyzi32", "xyzi16", "xyzrgb32", "odd19", "organised"]
-
-
-@pytest.fixture(scope="module")
-def world():
-    return synth.make_world(3, size_xy=(30.0, 30.0), n_clutter=40, n_walls=4)
 
 
 def _records(n, step, parts):
@@ -153,7 +146,7 @@ def test_integrate_cloud_mode1_contract(ctx, world, layout):
     """What two Fast runs of one scan share: statistics, the block set, the (integer, order-free) weights, and the
     distance of every voxel with a single update (the others depend on the order of the updates)."""
     scans = _message_scans(world, layout)[:1]
-    (la, ca, ha), (lb, cb, hb) = _feed_pair(ctx, scans, ctx.tsdf_config(**FAST_ALL), True)
+    (la, ca, ha), (lb, cb, hb) = _feed_pair(ctx, scans, ctx.tsdf_config(**tx.FAST_ALL), True)
     ka, da, wa = tx.layer_voxels(*la, 16)
     kb, db, wb = tx.layer_voxels(*lb, 16)
     assert np.array_equal(ka, kb) and np.array_equal(wa.view(np.uint32), wb.view(np.uint32))

@@ -1,10 +1,9 @@
 """Voxel colour on the device, against the exact models of tests/colour_exact.py.
 
-Mode 0: the colour words equal the sequential coloured replay bit for bit, and distance, weight, statistics and
-launch counts equal those of the same scans without colours.  Mode 1: the stated contract (exact where a voxel
-has one update in the call, channel-wise range elsewhere, exact for a one-colour scene; weights, statistics and
-the block set independent of colours), one run each.  Collection files carry the channel; submaps that never saw
-a colour have no channel and save as before."""
+Mode 1: the stated contract (exact where a voxel has one update in the call, channel-wise range elsewhere, exact
+for a one-colour scene; weights, statistics and the block set independent of colours), one run each.  Host and
+device colour uploads and downloads.  Collection files carry the channel; submaps that never saw a colour have no
+channel and save as before.  Ray-ordered (mode 0) colour is pinned in test_gpu_tsdf_exact.py."""
 import itertools
 
 import numpy as np
@@ -13,109 +12,19 @@ import pytest
 import collection_stream as cs
 import colour_exact as cx
 import tsdf_exact as tx
-from support import ctx  # noqa: F401
+from support import ctx, world  # noqa: F401
 from voxgraph_b200 import _lib, api, synth
 
 pytestmark = pytest.mark.gpu
 
 F32 = np.float32
 _ids = itertools.count(7000)
-FAST_ALL = dict(mode=1, start_voxel_subsampling_factor=1e3, max_consecutive_ray_collisions=1 << 30,
-                use_weight_dropoff=0)
-
-
-@pytest.fixture(scope="module")
-def world():
-    return synth.make_world(3, size_xy=(30.0, 30.0), n_clutter=40, n_walls=4)
-
-
-def _ring(n, z, ranges, az0=0.1):
-    a = az0 + 2 * np.pi * np.arange(n) / n
-    r = np.resize(np.asarray(ranges, np.float64), n)
-    zz = np.resize(np.asarray(z, np.float64), n)
-    return np.stack([r * np.cos(a), r * np.sin(a), zz], -1).astype(F32)
-
-
-def _scans(world, n_beams, n_azimuth, seed=0):
-    """Three overlapping scans from different poses (two with clearing rays), then a 200-ray ring twice from one
-    pose (its sensor voxel takes the long-segment path, and the closed-form batches the second time), every
-    point with a colour of its own whose four channels differ."""
-    rs = np.random.RandomState(seed)
-    out = []
-    for k, (px, py, yaw) in enumerate([(15.0, 15.0, 0.4), (16.5, 14.0, 1.9), (13.0, 16.0, -2.6)]):
-        pts = synth.lidar_scan(world, np.array([px, py, 1.2, yaw]), n_beams=n_beams, n_azimuth=n_azimuth, seed=k,
-                               miss_range=40.0 if k != 1 else None)
-        out.append((synth.pose_to_T([px - 15.0, py - 15.0, 0.1 * k, yaw]), pts))
-    ring = _ring(200, 0.125, [3.0, 4.2, 5.5])
-    T = synth.pose_to_T([0.1, 0.1, 0.1, 0.0])
-    out += [(T, ring), (T, ring)]
-    return [(T, p, rs.randint(0, 256, (len(p), 4)).astype(np.uint8)) for (T, p) in out]
-
-
-def _expected_words(idx, vps, st):
-    """The model's colours laid out as the downloaded layer's voxels sorted by key; 0 where never touched."""
-    keys = cx.layer_colours(idx, np.zeros((len(idx), vps ** 3), np.uint32), vps)[0]
-    exp = np.zeros(len(keys), np.uint32)
-    pos = np.searchsorted(keys, st.keys)
-    assert np.array_equal(keys[pos], st.keys)
-    exp[pos] = st.c
-    return exp
-
-
-@pytest.mark.parametrize("vs,vps,max_ray", [(0.2, 16, 16.0), (0.05, 8, 5.0)])
-def test_mode0_colour_bit_exact(ctx, oracle, world, vs, vps, max_ray):
-    scans = _scans(world, 16, 256) if vps == 16 else _scans(world, 8, 128)
-    kw = dict(max_ray_length_m=max_ray)
-    layer = oracle.Layer(vs, vps)
-    st = cx.State()
-    ocfg = oracle.tsdf_config(**kw)
-    n_band = 0
-    for (T, pts, rgba) in scans:
-        g, s, u, r = cx.trace_rays(oracle, layer, ocfg, T, pts)
-        n_band += int(np.count_nonzero(np.abs(s) < F32(ocfg.default_truncation_distance)))
-        cx.replay(tx.voxel_keys(g), s, u, cx.pack(rgba)[r], ocfg.default_truncation_distance, ocfg.max_weight, st)
-    assert n_band > 1000
-    plain, col = next(_ids), next(_ids)
-    cfg = ctx.tsdf_config(**kw)
-    try:
-        for sid in (plain, col):
-            ctx.submap_create(sid, vs, vps, layer.num_blocks)
-        stats, launches = {plain: [], col: []}, {plain: [], col: []}
-        for (T, pts, rgba) in scans:
-            for sid in (plain, col):
-                before = ctx.launch_count
-                sg = ctx.tsdf_integrate(sid, T, pts, cfg, rgba=rgba if sid == col else None)
-                launches[sid].append(ctx.launch_count - before)
-                stats[sid].append((sg.rays_valid, sg.rays_cast, sg.voxel_updates, sg.blocks_allocated,
-                                   sg.saturated_batches))
-        assert stats[col] == stats[plain] and launches[col] == launches[plain]
-        assert stats[col][-1][4] > 0                       # the closed-form batches are still taken with colours
-        assert ctx.submap_has_colour(col) and not ctx.submap_has_colour(plain)
-        got = ctx.submap_download(col)
-        tx.assert_layers_bit_equal(layer.export(), got)                      # the oracle's distance and weight
-        tx.assert_layers_bit_equal(ctx.submap_download(plain), got)          # ... and the colourless run's
-        words = ctx.submap_download_colour(col)
-        gk, gc = cx.layer_colours(got[0], words, vps)
-        exp = _expected_words(got[0], vps, st)
-        bad = np.nonzero(gc != exp)[0]
-        assert bad.size == 0, (len(bad), gk[bad[0]], hex(int(gc[bad[0]])), hex(int(exp[bad[0]])))
-        assert np.count_nonzero(exp) > 1000
-        assert not ctx.submap_download_colour(plain).any()
-        # a later colourless scan leaves the channel untouched
-        ctx.tsdf_integrate(col, scans[0][0], scans[0][1], cfg)
-        assert np.array_equal(ctx.submap_download_colour(col), words)
-        # finishing keeps the channel
-        ctx.submap_finish_ex(col)
-        assert ctx.submap_has_colour(col) and np.array_equal(ctx.submap_download_colour(col), words)
-    finally:
-        for sid in (plain, col):
-            ctx.submap_free(sid)
 
 
 def _fast_pair(ctx, vs, vps, cap, calls):
     """The calls [(T, pts, rgba)] in mode 1 into one coloured and one colourless submap -> per call the coloured
     submap's (idx, d, w, colour words) after it; checks contract (c) along the way."""
-    cfg = ctx.tsdf_config(**FAST_ALL)
+    cfg = ctx.tsdf_config(**tx.FAST_ALL)
     plain, col = next(_ids), next(_ids)
     out = []
     try:
@@ -150,12 +59,12 @@ def test_mode1_contract(ctx, oracle):
     rs = np.random.RandomState(3)
     calls = []
     for k, (t, n) in enumerate([((0.1, 0.1, 0.1), 150), ((1.3, -0.8, 0.2), 140)]):
-        pts = _ring(n, np.linspace(-0.8, 0.9, 7), [3.0, 4.2, 5.5, 2.4], az0=0.1 + 0.37 * k)
+        pts = tx.ring(n, np.linspace(-0.8, 0.9, 7), [3.0, 4.2, 5.5, 2.4], az0=0.1 + 0.37 * k)
         palette = rs.randint(0, 256, (2, 4)).astype(np.uint8)          # two colours per call
         calls.append((synth.pose_to_T([*t, 0.3 * k]), pts, palette[rs.randint(0, 2, n)]))
-    ocfg = oracle.tsdf_config(**FAST_ALL)
+    ocfg = oracle.tsdf_config(**tx.FAST_ALL)
     layer = oracle.Layer(vs, vps)
-    traces = [cx.trace_rays(oracle, layer, ocfg, T, pts) for (T, pts, _) in calls]
+    traces = [cx.trace_rays(oracle, layer, ocfg, T, pts)[1:] for (T, pts, _) in calls]
     res = _fast_pair(ctx, vs, vps, layer.num_blocks, calls)
     trunc = F32(ocfg.default_truncation_distance)
     n_single = n_multi = 0
@@ -211,9 +120,9 @@ def test_mode1_one_colour_is_exact(ctx, oracle, world):
     pts = synth.lidar_scan(world, np.array([15.0, 15.0, 1.2, 0.4]), n_beams=8, n_azimuth=64, seed=1, miss_range=40.0)
     T = synth.pose_to_T([0.3, -0.2, 0.1, 0.4])
     c = np.array([201, 17, 96, 254], np.uint8)
-    ocfg = oracle.tsdf_config(**FAST_ALL)
+    ocfg = oracle.tsdf_config(**tx.FAST_ALL)
     layer = oracle.Layer(vs, vps)
-    g, s, u, r = cx.trace_rays(oracle, layer, ocfg, T, pts)
+    _, g, s, u, r = cx.trace_rays(oracle, layer, ocfg, T, pts)
     (idx, d, w, words, _), = _fast_pair(ctx, vs, vps, layer.num_blocks, [(T, pts, np.tile(c, (len(pts), 1)))])
     k_all, c_all = cx.layer_colours(idx, words, vps)
     keys = tx.voxel_keys(g)

@@ -1,14 +1,11 @@
-"""Voxel colour pinned across the matrices the colourless kernels are pinned on (tests/test_gpu_tsdf_exact.py,
-tests/test_gpu_fast_schedule.py, tests/test_gpu_colour_map.py), against the exact models of tests/colour_exact.py.
+"""Voxel colour pinned across the matrices the colourless kernels are pinned on (tests/test_gpu_fast_schedule.py,
+tests/test_gpu_colour_map.py), against the exact models of tests/colour_exact.py.  Ray-ordered (mode 0) colour is
+pinned with distance and weight in tests/test_gpu_tsdf_exact.py.
 
 Every ray carries a colour of its own whose four channels differ, so an update applied out of order, with the
 wrong weight or with another ray's colour changes the bytes.
 
-* Ray-ordered integration (mode 0): each case runs into a coloured submap and a colourless twin.  Statistics,
-  saturated batches and launch counts are equal; distance and weight equal the oracle and the twin bit for bit;
-  every colour word equals the sequential coloured replay.  Cases: the configuration matrix, the weight cap
-  crossed inside closed-form batches with band updates after it, segment lengths around the 32-tuple batches,
-  five resolutions, the crafted ray edges, and clearing rays whose last voxels lie inside the band.
+* Clearing rays whose last voxels lie inside the band, in mode 1 with every ray cast.
 * Fast scheduling (mode 1) at voxgraph's schedule (start-cell factor 2, two collisions): the race-aware model of
   tests/fast_schedule.py decodes which rays updated each voxel, and the colour contract of csrc/tsdf.cu is
   checked on that decoding; a one-colour scan at the default configuration.
@@ -27,220 +24,26 @@ import mesh_exact as me
 import project_colour_oracle as pco
 import project_oracle as po
 import tsdf_exact as tx
-from support import ctx, yaw_T  # noqa: F401
+from support import ctx, world, yaw_T  # noqa: F401
 from voxgraph_b200 import synth
 
 pytestmark = pytest.mark.gpu
 
 F32 = np.float32
 _ids = itertools.count(11000)
-FAST_ALL = dict(mode=1, start_voxel_subsampling_factor=1e3, max_consecutive_ray_collisions=1 << 30,
-                use_weight_dropoff=0)
 VOXGRAPH = dict(start_voxel_subsampling_factor=2.0, max_consecutive_ray_collisions=2)
 
 
-@pytest.fixture(scope="module")
-def world():
-    return synth.make_world(3, size_xy=(30.0, 30.0), n_clutter=40, n_walls=4)
-
-
-def _colours(rs, n):
-    """n colours [r g b a], the four channels of each one distinct."""
-    return np.argsort(rs.rand(n, 256), 1)[:, :4].astype(np.uint8)
-
-
-def _trace(oracle, layer, ocfg, T, pts):
-    """The oracle point by point (it integrates into `layer`) -> (stats without saturated batches, g, sdf, uw,
-    ray index of every tuple)."""
-    st = np.zeros(4, np.int64)
-    G, S, U, R = [np.zeros((0, 3), np.int64)], [np.zeros(0, F32)], [np.zeros(0, F32)], [np.zeros(0, np.int64)]
-    for i in range(len(pts)):
-        o, g, s, u = oracle.tsdf_integrate_trace(layer, ocfg, T, pts[i:i + 1])
-        st += (o.rays_valid, o.rays_cast, o.voxel_updates, o.blocks_allocated)
-        G.append(g); S.append(s); U.append(u); R.append(np.full(len(s), i, np.int64))
-    return tuple(int(v) for v in st), np.concatenate(G), np.concatenate(S), np.concatenate(U), np.concatenate(R)
-
-
-def _expected_words(idx, vps, st):
-    """The model's colours laid out as the downloaded layer's voxels sorted by key; 0 where never touched."""
-    keys = cx.layer_colours(idx, np.zeros((len(idx), vps ** 3), np.uint32), vps)[0]
-    exp = np.zeros(len(keys), np.uint32)
-    pos = np.searchsorted(keys, st.keys)
-    assert np.array_equal(keys[pos], st.keys)
-    exp[pos] = st.c
-    return exp
-
-
-def _mode0(ctx, oracle, vs, vps, scans, seed=0, **kw):
-    """Integrate scans [(T, points[, cfg overrides])] ray ordered, every point with a colour of its own, into a
-    coloured submap and a colourless twin, and check both against the models.  -> (per-scan model stats with
-    saturated batches, [(ray index, sdf, uw) per tuple] per scan, number of non-zero expected colour words)."""
-    rs = np.random.RandomState(seed)
-    layer = oracle.Layer(vs, vps)
-    st_c, st_t = cx.State(), tx.State()
-    exp, calls, traces = [], [], []
-    for sc in scans:
-        T, pts = sc[0], np.asarray(sc[1], F32)
-        kwc = {**kw, **(sc[2] if len(sc) > 2 else {})}
-        ocfg = oracle.tsdf_config(**kwc)
-        trunc, M = ocfg.default_truncation_distance, ocfg.max_weight
-        rgba = _colours(rs, len(pts))
-        stats, g, s, u, r = _trace(oracle, layer, ocfg, T, pts)
-        keys = tx.voxel_keys(g)
-        sat = tx.replay(keys, s, u, trunc, M, st_t)[3]
-        cx.replay(keys, s, u, cx.pack(rgba)[r], trunc, M, st_c)
-        exp.append(stats + (sat,))
-        calls.append((T, pts, rgba, kwc))
-        traces.append((keys, r, s, u))
-    plain, col = next(_ids), next(_ids)
-    try:
-        for sid in (plain, col):
-            ctx.submap_create(sid, vs, vps, layer.num_blocks)
-        got = {plain: [], col: []}
-        for (T, pts, rgba, kwc) in calls:
-            cfg = ctx.tsdf_config(**kwc)
-            for sid in (plain, col):
-                before = ctx.launch_count
-                sg = ctx.tsdf_integrate(sid, T, pts, cfg, rgba=rgba if sid == col else None)
-                got[sid].append((sg.rays_valid, sg.rays_cast, sg.voxel_updates, sg.blocks_allocated,
-                                 sg.saturated_batches, ctx.launch_count - before))
-        assert [g[:5] for g in got[col]] == exp, (got[col], exp)
-        assert got[col] == got[plain]
-        assert ctx.submap_has_colour(col) and not ctx.submap_has_colour(plain)
-        lay = ctx.submap_download(col)
-        tx.assert_layers_bit_equal(layer.export(), lay)
-        tx.assert_layers_bit_equal(ctx.submap_download(plain), lay)
-        gk, gc = cx.layer_colours(lay[0], ctx.submap_download_colour(col), vps)
-        want = _expected_words(lay[0], vps, st_c)
-        bad = np.nonzero(gc != want)[0]
-        assert bad.size == 0, (len(bad), gk[bad[0]], hex(int(gc[bad[0]])), hex(int(want[bad[0]])))
-    finally:
-        for sid in (plain, col):
-            ctx.submap_free(sid)
-    return exp, traces, int(np.count_nonzero(want))
-
-
-# ---------------------------------------------------------------------- mode 0
-@pytest.mark.parametrize("kw", tx.CONFIGS, ids=tx.config_id)
-def test_mode0_config_matrix(ctx, oracle, world, kw):
-    exp, _, n_col = _mode0(ctx, oracle, 0.2, 16, tx.scans(world), **kw)
-    assert n_col > 1000
-    if kw.get("use_const_weight", 1) and kw.get("max_weight", 1e4) <= 2.0 ** 20 and kw.get("voxel_carving_enabled", 1):
-        assert sum(e[4] for e in exp) > 0     # the closed-form batches are taken with colours too
-
-
-def _band_at_cap(keys, s, u, trunc, M):
-    """Band updates of the most-updated voxel that find it at the weight cap (sequential replay)."""
-    k, c = np.unique(keys, return_counts=True)
-    sel = keys == k[np.argmax(c)]
-    d, w, n = F32(0), F32(0), 0
-    for ss, uu in zip(s[sel], u[sel]):
-        n += bool(w == F32(M) and abs(ss) < F32(trunc))
-        d, w = tx.apply_update(ss, uu, d, w, F32(trunc), F32(M))
-    return n
-
-
-@pytest.mark.parametrize("mw", [3.0, 40.0, 100.5, 1e4, tx.MW24 - 8, tx.MW24])
-def test_mode0_capped_weight_reaches_the_blend(ctx, oracle, mw):
-    """Integer update weights of 2^14 drive the sensor voxel to the cap inside closed-form batches (as in
-    test_gpu_tsdf_exact); points 0.3-0.45 m from the sensor then give that voxel band updates (sdf ~ range <
-    trunc), some between the far rays and the rest after them, so the colour step runs at the capped weight in
-    full and partial batches."""
-    far = tx.ring(1100, [2.0 ** -7, -2.0 ** -7], [3.0, 4.5, 6.0])
-    near = tx.ring(80, [2.0 ** -7, -2.0 ** -7], [0.3, 0.45], az0=0.2)
-    pts = np.concatenate([far[:600], near[:13], far[600:], near[13:]])
-    T = synth.pose_to_T([0.1, 0.1, 0.1, 0.3])
-    exp, traces, _ = _mode0(ctx, oracle, 0.2, 16, [(T, pts)], use_const_weight=0, max_weight=mw)
-    assert exp[0][4] > 0
-    keys, _, s, u = traces[0]
-    assert _band_at_cap(keys, s, u, 0.6, mw) >= 60
-
-
-def _segment_streams(n):
-    """Saturated (integer 2^6 weights far behind the sensor), mixed (sdf below 2 trunc at the sensor voxel,
-    fractional weights) and band (points 1, 3 and 4 of every 5 lie 0.35-0.5 m away: band updates at the sensor
-    voxel, in every batch and in the one-tuple tails at 65, 97 and 129)."""
-    return {"saturated": tx.ring(n, 0.125, [3.0, 4.2, 5.5]),
-            "mixed": tx.ring(n, [0.125, 0.3, 0.125, -0.2, 0.125, 0.125, 0.125], [3.0, 1.0, 4.2, 5.5, 1.1]),
-            "band": tx.ring(n, [0.125, 0.3, -0.2], [3.0, 0.35, 4.2, 0.5, 0.42])}
-
-
-@pytest.mark.parametrize("n", [1, 31, 32, 33, 63, 64, 65, 95, 96, 97, 128, 129])
-def test_mode0_segment_lengths(ctx, oracle, n):
-    """The sensor voxel's segment has exactly n tuples per call (short path up to 64, warp path with 32-tuple
-    batches and a tail beyond), each stream integrated twice."""
-    T = synth.pose_to_T([0.1, 0.1, 0.1, 0.0])
-    sensor = tx.voxel_keys([[0, 0, 0]])[0]
-    for name, pts in _segment_streams(n).items():
-        exp, traces, _ = _mode0(ctx, oracle, 0.2, 16, [(T, pts), (T, pts)], seed=n, use_const_weight=0)
-        keys, _, s, _ = traces[0]
-        at = keys == sensor
-        assert np.count_nonzero(at) == n
-        if name == "band":
-            assert np.count_nonzero(np.abs(s[at]) < F32(0.6)) == sum(i % 5 in (1, 3, 4) for i in range(n))
-        if name == "saturated" and n >= 65:
-            assert exp[1][4] > 0
-        if n <= 64:
-            assert exp[0][4] == exp[1][4] == 0
-
-
-@pytest.mark.parametrize("vs,vps", [(0.05, 8), (0.1, 16), (0.15, 8), (0.05, 32), (0.2, 16)])
-def test_mode0_resolutions(ctx, oracle, world, vs, vps):
-    """A sensor at negative coordinates, one 2 km from the origin, and a quaternion that is not exactly unit."""
-    scans = tx.scans(world, n_beams=8, n_azimuth=128)
-    T_neg = scans[0][0].copy(); T_neg[4:] = [-7.3, -11.9, -2.05]
-    T_far = scans[1][0].copy(); T_far[4:] += np.array([2000.0, -1312.5, 3.0], F32)
-    q = np.array([0.71, 0.12, -0.2, 0.67], F32)
-    T_q = np.concatenate([q, F32([0.4, -0.3, 0.2])]).astype(F32)
-    cfg = dict(max_ray_length_m=6.0)
-    assert _mode0(ctx, oracle, vs, vps, [(T_neg, scans[0][1]), (T_q, scans[2][1])], **cfg)[2] > 100
-    assert _mode0(ctx, oracle, vs, vps, [(T_far, scans[1][1]), (T_far, scans[0][1])], seed=1, **cfg)[2] > 100
-
-
-def test_mode0_ray_edges(ctx, oracle):
-    """The crafted points under the four edge configurations from two sensors, accumulated in one submap; from
-    the second sensor in an order that interleaves the valid points with the NaN, inf and huge ones, so a ray
-    colour taken from the wrong point index shows."""
-    pts = tx.edge_points()
-    mixed = pts[np.random.RandomState(4).permutation(len(pts))]
-    scans = []
-    for t, p in (([0.0, 0.0, 0.0], pts), ([0.3, -0.45, 0.1], mixed)):
-        T = np.array([1, 0, 0, 0, *t], F32)
-        scans += [(T, p, c) for c in tx.EDGE_CFGS]
-    exp, _, n_col = _mode0(ctx, oracle, 0.25, 8, scans)
-    assert all(e[0] == e[1] for e in exp) and exp[0][0] == 32 and n_col > 20
-
-
 # ---------------------------------------------------------------------- clearing rays
-def _clearing_scene(vs, n=400, seed=0):
-    """n points max_ray_length_m + U(0.001, trunc + one voxel) away in random directions: every one is a
-    clearing ray, cut at norm - trunc, and its last voxels can have their centres inside the band."""
-    rs = np.random.RandomState(seed)
-    d = rs.normal(size=(n, 3))
-    d /= np.linalg.norm(d, axis=1)[:, None]
-    return (d * (8.0 + rs.uniform(0.001, 0.6 + vs, n))[:, None]).astype(F32)
-
-
-@pytest.mark.parametrize("vs,vps", [(0.2, 16), (0.05, 8)])
-def test_mode0_clearing_rays_in_the_band(ctx, oracle, vs, vps):
-    pts = _clearing_scene(vs)
-    T = synth.pose_to_T([0.1, 0.1, 0.1, 0.3])
-    exp, traces, n_col = _mode0(ctx, oracle, vs, vps, [(T, pts), (T, pts)], max_ray_length_m=8.0)
-    assert exp[0][:2] == (400, 400)
-    _, r, s, _ = traces[0]
-    band = np.abs(s) < F32(0.6)
-    assert len(np.unique(r[band])) > 100 and n_col > 100
-
-
 def _contract(ctx, oracle, vs, vps, T, pts, rgba, **kw):
     """One mode-1 call with every ray cast into an empty coloured submap and its colourless twin: statistics,
     block set and the order-free integer weights equal; a voxel with one update holds the exact rule, one with
     more lies channel-wise within black and its band rays' colours, one without a band update stays 0.
     -> (ray index, sdf) of every tuple."""
-    ocfg = oracle.tsdf_config(**{**FAST_ALL, **kw})
+    ocfg = oracle.tsdf_config(**{**tx.FAST_ALL, **kw})
     layer = oracle.Layer(vs, vps)
-    g, s, u, r = cx.trace_rays(oracle, layer, ocfg, T, pts)
-    cfg = ctx.tsdf_config(**{**FAST_ALL, **kw})
+    _, g, s, u, r = cx.trace_rays(oracle, layer, ocfg, T, pts)
+    cfg = ctx.tsdf_config(**{**tx.FAST_ALL, **kw})
     plain, col = next(_ids), next(_ids)
     try:
         res = {}
@@ -284,8 +87,8 @@ def _contract(ctx, oracle, vs, vps, T, pts, rgba, **kw):
 
 @pytest.mark.parametrize("vs,vps", [(0.2, 16), (0.05, 8)])
 def test_mode1_clearing_rays_in_the_band(ctx, oracle, vs, vps):
-    pts = _clearing_scene(vs, seed=1)
-    rgba = _colours(np.random.RandomState(2), len(pts))
+    pts = tx.clearing_points(vs, seed=1)
+    rgba = cx.colours(np.random.RandomState(2), len(pts))
     r, s = _contract(ctx, oracle, vs, vps, synth.pose_to_T([0.1, 0.1, 0.1, 0.3]), pts, rgba, max_ray_length_m=8.0)
     assert len(np.unique(r[np.abs(s) < F32(0.6)])) > 100
 
@@ -304,7 +107,7 @@ def _fast_colour(ctx, sc, positions, slot_rgba, reach=None):
     every channel at most the largest of the band rays' channels, no band update -> 0.  -> checker info."""
     pts = np.full((N_PAD, 3), np.nan, F32)
     pts[positions] = sc.pts
-    rgba = _colours(np.random.RandomState(len(positions)), N_PAD)
+    rgba = cx.colours(np.random.RandomState(len(positions)), N_PAD)
     for i in sc.valid:
         rgba[positions[i]] = slot_rgba[sc.rays[i].slot]
     cap = len({sc.block(g) for i in sc.valid for g in sc.rays[i].seq}) + 1
@@ -367,7 +170,7 @@ def test_mode1_voxgraph_schedule_micro_scenes(ctx, oracle, vs, vps, sensor):
         reach = {sc.canonical(o) for o in sc.reachable()}
         layout = list(LAYOUTS)[n % 3]
         try:
-            info = _fast_colour(ctx, sc, LAYOUTS[layout](len(pts)), _colours(rs, len(sc.slots)), reach)
+            info = _fast_colour(ctx, sc, LAYOUTS[layout](len(pts)), cx.colours(rs, len(sc.slots)), reach)
         except AssertionError as e:
             raise AssertionError((name, layout, str(e)))
         for k in tot:
@@ -386,7 +189,7 @@ def test_mode1_voxgraph_schedule_random_scenes(ctx, oracle):
         assert sc.decodable()
         positions = np.sort(rs.choice(N_PAD, len(sc.pts), replace=False))
         try:
-            info = _fast_colour(ctx, sc, positions, _colours(rs, len(sc.slots)))
+            info = _fast_colour(ctx, sc, positions, cx.colours(rs, len(sc.slots)))
         except AssertionError as e:
             raise AssertionError((k, sc.kw, str(e)))
         for key in tot:
@@ -405,7 +208,7 @@ def test_mode1_one_colour_default_config(ctx, oracle, world):
     T = synth.pose_to_T([0.3, -0.2, 0.1, 0.4])
     c = np.array([201, 17, 96, 254], np.uint8)
     ocfg = oracle.tsdf_config(mode=1, start_voxel_subsampling_factor=1e3, max_consecutive_ray_collisions=1 << 30)
-    g, s, _, _ = cx.trace_rays(oracle, oracle.Layer(vs, vps), ocfg, T, pts)
+    _, g, s, _, _ = cx.trace_rays(oracle, oracle.Layer(vs, vps), ocfg, T, pts)
     sid = next(_ids)
     ctx.submap_create(sid, vs, vps, 4096)
     try:

@@ -12,7 +12,7 @@ import mesh_exact as me
 import project_colour_oracle as pco
 import project_oracle as po
 import tsdf_exact as tx
-from support import ctx, yaw_T  # noqa: F401
+from support import ctx, world, yaw_T  # noqa: F401
 from voxgraph_b200 import api, synth
 
 pytestmark = pytest.mark.gpu
@@ -20,11 +20,6 @@ pytestmark = pytest.mark.gpu
 F32 = np.float32
 _ids = itertools.count(9000)
 VS, VPS = 0.2, 8
-
-
-@pytest.fixture(scope="module")
-def world():
-    return synth.make_world(3, size_xy=(30.0, 30.0), n_clutter=40, n_walls=4)
 
 
 @pytest.fixture(scope="module")

@@ -207,8 +207,6 @@ def test_fused_far_translation_aliases_nothing(ctx, oracle, nc):
 # --------------------------------------------------------------------------- 3. TSDF far field
 TVS, TVPS, TBS = 0.125, 16, 2.0
 FAR_CFG = dict(voxel_carving_enabled=0, max_ray_length_m=1.0e11)
-FAST_ALL = dict(mode=1, start_voxel_subsampling_factor=1e3, max_consecutive_ray_collisions=1 << 30,
-                use_weight_dropoff=0)
 T_ID = np.array([1, 0, 0, 0, 0, 0, 0], np.float32)
 
 
@@ -291,7 +289,7 @@ def test_tsdf_far_field_simple(ctx, oracle):
 def test_tsdf_far_field_fast(ctx, oracle):
     near, far, p32 = _far_scan()
     pts = np.concatenate([near, far])
-    ocfg = oracle.tsdf_config(**{**FAR_CFG, **FAST_ALL})
+    ocfg = oracle.tsdf_config(**{**FAR_CFG, **tx.FAST_ALL})
     layer = oracle.Layer(TVS, TVPS)
     st, g, s, u = oracle.tsdf_integrate_trace(layer, ocfg, T_ID, pts)
     assert st.rays_cast == st.rays_valid
@@ -300,7 +298,7 @@ def test_tsdf_far_field_fast(ctx, oracle):
     sid = next(_ids)
     ctx.submap_create(sid, TVS, TVPS, len(oi))
     try:
-        sg = ctx.tsdf_integrate(sid, T_ID, np.concatenate([pts, p32]), ctx.tsdf_config(**{**FAR_CFG, **FAST_ALL}))
+        sg = ctx.tsdf_integrate(sid, T_ID, np.concatenate([pts, p32]), ctx.tsdf_config(**{**FAR_CFG, **tx.FAST_ALL}))
         assert (sg.rays_valid, sg.rays_cast, sg.voxel_updates, sg.blocks_allocated) == \
             (st.rays_valid + 1, st.rays_cast + 1, len(gi_), len(oi))
         gi, gd, gw = ctx.submap_download(sid)

@@ -79,7 +79,7 @@ def test_replay_matches_oracle_distance_and_weight(oracle):
     layer = oracle.Layer(0.2, 16)
     st = cx.State()
     for _ in range(2):
-        g, s, u, r = cx.trace_rays(oracle, layer, cfg, T, pts)
+        _, g, s, u, r = cx.trace_rays(oracle, layer, cfg, T, pts)
         k, d, w, c = cx.replay(tx.voxel_keys(g), s, u, cx.pack(rgba)[r], cfg.default_truncation_distance,
                                cfg.max_weight, st)
     oracle.tsdf_integrate(ref, cfg, T, pts)
@@ -109,7 +109,7 @@ def test_clearing_rays_reach_the_band(oracle):
         d /= np.linalg.norm(d, axis=1)[:, None]
         pts = (d * (8.0 + rs.uniform(0.001, float(trunc) + vs, 400))[:, None]).astype(F32)
         assert (np.linalg.norm(pts.astype(np.float64), axis=1) > 8.0).all()
-        g, s, u, r = cx.trace_rays(oracle, oracle.Layer(vs, 8), cfg, T, pts)
+        _, g, s, u, r = cx.trace_rays(oracle, oracle.Layer(vs, 8), cfg, T, pts)
         band = np.abs(s) < trunc
         assert len(np.unique(r[band])) > 100, vs
         assert (s[band] > 0).all() and (u[band] > 0).all()

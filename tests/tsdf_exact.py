@@ -1,4 +1,6 @@
-"""Exact models of the TSDF integrator for the GPU parity tests (tests/test_gpu_tsdf_exact.py).
+"""Exact models of the TSDF integrator for the GPU parity tests (tests/test_gpu_tsdf_exact.py, with
+tests/colour_exact.py for the colour of the same updates), and the scans, configurations and crafted
+points they run.
 
 * `replay` applies a list of ray-ordered (voxel, sdf, update weight) tuples, as the oracle's
   `tsdf_integrate_trace` records them, with the integrator's float32 update (updateTsdfVoxel's
@@ -150,9 +152,13 @@ def replay(keys, sdf, uw, trunc, max_weight, state=None, order=None):
 
 
 # ---------------------------------------------------------------------- the parity matrix
-# Scans, configurations and crafted points that tests/test_gpu_tsdf_exact.py runs colourless and
-# tests/test_gpu_colour_exact.py runs with ray colours.
+# Scans, configurations and crafted points that tests/test_gpu_tsdf_exact.py runs into a coloured
+# submap and a colourless twin.
 MW24 = 2.0 ** 24
+# Mode 1 with every ray cast (start keys all distinct, unlimited ray collisions) and integer update
+# weights (no drop-off): the set of updates is fixed, as check_fast needs.
+FAST_ALL = dict(mode=1, start_voxel_subsampling_factor=1e3, max_consecutive_ray_collisions=1 << 30,
+                use_weight_dropoff=0)
 CONFIGS = [
     dict(),
     dict(use_const_weight=0),
@@ -223,6 +229,16 @@ EDGE_CFGS = [dict(min_ray_length_m=0.5, max_ray_length_m=8.0),
              dict(min_ray_length_m=0.0, max_ray_length_m=8.0, voxel_carving_enabled=0),
              dict(min_ray_length_m=0.0, max_ray_length_m=8.0, allow_clear=0),
              dict(min_ray_length_m=0.0, max_ray_length_m=8.0, use_weight_dropoff=0)]
+
+
+def clearing_points(vs, n=400, seed=0):
+    """n points 8 m + U(0.001, 0.6 m + one voxel) away in random directions: with max_ray_length_m = 8
+    and the default trunc of 0.6 m every one is a clearing ray, cut at norm - trunc, and its last voxels
+    can have their centres inside the band."""
+    rs = np.random.RandomState(seed)
+    d = rs.normal(size=(n, 3))
+    d /= np.linalg.norm(d, axis=1)[:, None]
+    return (d * (8.0 + rs.uniform(0.001, 0.6 + vs, n))[:, None]).astype(F32)
 
 
 def check_fast(cand, keys, sdf, uw, trunc, max_weight, exact=None):

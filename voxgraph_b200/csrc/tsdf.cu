@@ -491,7 +491,7 @@ tsdf_apply_kernel(const unsigned* __restrict__ keys, const typename TsdfTuple<kC
 // is crossed, pinned at the cap from then on (a voxel already at the cap simply stays there).
 // Everything else (first updates, dropped-off weights, fractional weights) takes the sequential replay, so
 // the result stays bit-identical to the single-threaded reference
-// (tests/test_gpu_tsdf.py::test_deterministic_mode_bit_exact_dense_scans).
+// (tests/test_gpu_tsdf_exact.py::test_dense_scans_bit_exact).
 // With colours the shortcut stays valid and is still taken: it needs sdf >= 2 trunc on every lane, and
 // the colour rule acts only where |sdf| < trunc, so a saturated batch changes no colour.
 template <bool kColour>
