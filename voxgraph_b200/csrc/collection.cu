@@ -33,7 +33,7 @@
 #include <string>
 #include <vector>
 
-#include "vgx_internal.h"
+#include "layer_access.cuh"
 
 // ------------------------------------------------------------------ format table
 namespace {
@@ -458,7 +458,7 @@ struct Parser {
 
   // the layer geometry of the header, as the upload path accepts it
   bool geometry(const CollLayout& L) {
-    if (L.vps < 2 || L.vps > 32 || (L.vps & (L.vps - 1)) != 0)
+    if (!vgx_vps_ok(L.vps))
       return fail("voxels_per_side must be a power of two in [2, 32]");
     if (!(L.voxel_size > 0) || !((float)L.voxel_size > 0) || !isfinite((float)L.voxel_size))
       return fail("voxel_size must be positive and finite");

@@ -17,21 +17,18 @@
 
 #include <vector>
 
-#include "vgx_internal.h"
+#include "layer_access.cuh"
 
 struct EsdfParams {
-  float voxel_size, max_distance, default_distance, min_distance, min_weight;
-  int vps, sh, n_blocks;
+  float max_distance, default_distance, min_distance, min_weight;
 };
 
 // (distance, observed) from the TSDF brick + "fixed" mask
 __global__ void __launch_bounds__(256)
-esdf_init_kernel(EsdfParams P, const float2* __restrict__ tsdf, float2* __restrict__ esdf,
-                 unsigned char* __restrict__ fixed) {
+esdf_init_kernel(EsdfParams P, LayerDev L, float2* __restrict__ esdf, unsigned char* __restrict__ fixed) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t nvox = (size_t)P.n_blocks << (3 * P.sh);
-  if (i >= nvox) return;
-  const float2 t = tsdf[i];
+  if (i >= vgx_voxel_count(L.n_blocks, L.sh)) return;
+  const float2 t = L.dw[i];
   float2 e = make_float2(0.f, 0.f);
   unsigned char f = 0;
   if (!(t.y < P.min_weight)) {
@@ -44,28 +41,25 @@ esdf_init_kernel(EsdfParams P, const float2* __restrict__ tsdf, float2* __restri
 }
 
 // 27 neighbour slots per block (centre included), -1 where the block does not exist
-__global__ void esdf_neighbours_kernel(VgxHash hash, const int32_t* __restrict__ block_idx, int n_blocks,
-                                       int* __restrict__ nb) {
+__global__ void esdf_neighbours_kernel(LayerDev L, int* __restrict__ nb) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= 27 * n_blocks) return;
+  if (t >= 27 * L.n_blocks) return;
   const int b = t / 27, k = t % 27;
-  nb[t] = vgx_hash_find(hash, block_idx[3 * b] + (k % 3) - 1, block_idx[3 * b + 1] + ((k / 3) % 3) - 1,
-                        block_idx[3 * b + 2] + (k / 9) - 1);
+  nb[t] = vgx_hash_find(L.hash, L.block_idx[3 * b] + (k % 3) - 1, L.block_idx[3 * b + 1] + ((k / 3) % 3) - 1,
+                        L.block_idx[3 * b + 2] + (k / 9) - 1);
 }
 
 __global__ void __launch_bounds__(256)
-esdf_sweep_kernel(EsdfParams P, float2* esdf, const unsigned char* __restrict__ fixed,
+esdf_sweep_kernel(EsdfParams P, LayerDev L, float2* esdf, const unsigned char* __restrict__ fixed,
                   const int* __restrict__ nb, int* __restrict__ changed) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t nvox = (size_t)P.n_blocks << (3 * P.sh);
-  if (i >= nvox) return;
+  if (i >= vgx_voxel_count(L.n_blocks, L.sh)) return;
   volatile float2* ev = esdf;
   const float2 me = make_float2(ev[i].x, ev[i].y);
   if (me.y == 0.f || fixed[i]) return;
-  const int b = (int)(i >> (3 * P.sh));
-  const int lin = (int)(i & (((size_t)1 << (3 * P.sh)) - 1));
-  const int v0 = lin & (P.vps - 1), v1 = (lin >> P.sh) & (P.vps - 1), v2 = lin >> (2 * P.sh);
-  const float s1 = 1.0f * P.voxel_size, s2 = sqrtf(2.0f) * P.voxel_size, s3 = sqrtf(3.0f) * P.voxel_size;
+  int v[3];
+  const int b = vgx_voxel_of(i, L.sh, v);
+  const float s1 = 1.0f * L.voxel_size, s2 = sqrtf(2.0f) * L.voxel_size, s3 = sqrtf(3.0f) * L.voxel_size;
   float d = me.x;
 #pragma unroll 1
   for (int dz = -1; dz <= 1; ++dz)
@@ -74,13 +68,13 @@ esdf_sweep_kernel(EsdfParams P, float2* esdf, const unsigned char* __restrict__ 
 #pragma unroll
       for (int dx = -1; dx <= 1; ++dx) {
         if (!dx && !dy && !dz) continue;
-        int q0 = v0 + dx, q1 = v1 + dy, q2 = v2 + dz, bo0 = 1, bo1 = 1, bo2 = 1;
-        if (q0 < 0) { q0 += P.vps; bo0 = 0; } else if (q0 >= P.vps) { q0 -= P.vps; bo0 = 2; }
-        if (q1 < 0) { q1 += P.vps; bo1 = 0; } else if (q1 >= P.vps) { q1 -= P.vps; bo1 = 2; }
-        if (q2 < 0) { q2 += P.vps; bo2 = 0; } else if (q2 >= P.vps) { q2 -= P.vps; bo2 = 2; }
+        int q0 = v[0] + dx, q1 = v[1] + dy, q2 = v[2] + dz, bo0 = 1, bo1 = 1, bo2 = 1;
+        if (q0 < 0) { q0 += L.vps; bo0 = 0; } else if (q0 >= L.vps) { q0 -= L.vps; bo0 = 2; }
+        if (q1 < 0) { q1 += L.vps; bo1 = 0; } else if (q1 >= L.vps) { q1 -= L.vps; bo1 = 2; }
+        if (q2 < 0) { q2 += L.vps; bo2 = 0; } else if (q2 >= L.vps) { q2 -= L.vps; bo2 = 2; }
         const int s = nb[27 * b + bo0 + 3 * bo1 + 9 * bo2];
         if (s < 0) continue;
-        const size_t j = ((size_t)s << (3 * P.sh)) + q0 + (q1 << P.sh) + (q2 << (2 * P.sh));
+        const size_t j = vgx_voxel_index(s, q0, q1, q2, L.sh);
         const float ny = ev[j].y;
         if (ny == 0.f) continue;
         const float dn = ev[j].x;
@@ -124,28 +118,24 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
     if (sweeps_out) *sweeps_out = 0;
     if (nvox == 0) return s->d_view_esdf.alloc(c, 32, "ESDF registration view");
     EsdfParams P;
-    P.voxel_size = s->voxel_size;
     P.max_distance = dc.max_distance_m; P.default_distance = dc.default_distance_m;
     P.min_distance = dc.min_distance_m; P.min_weight = dc.min_weight;
-    P.vps = s->vps;
-    P.sh = s->sh;
-    P.n_blocks = s->n_blocks;
+    const LayerDev L = layer_of(s);
     VGX_TRY(s->d_esdf.alloc(c, sizeof(float2) * nvox, "ESDF bricks"));
     unsigned char* d_fixed;
     int *d_nb, *d_changed;
     VGX_TRY(vgx_carve(c, c->d_work, vgx_part(d_fixed, nvox), vgx_part(d_nb, (size_t)27 * s->n_blocks),
                       vgx_part(d_changed, 1)));
     const unsigned grid = (unsigned)((nvox + 255) / 256);
-    VGX_TRY(vgx_launch(c, esdf_init_kernel, grid, 256, 0, VgxLaunch::plain, P, s->d_dw.get(), s->d_esdf.get(), d_fixed));
-    VGX_TRY(vgx_launch(c, esdf_neighbours_kernel, (27 * s->n_blocks + 127) / 128, 128, 0, VgxLaunch::plain, s->hash(),
-                       s->d_block_idx.get(), s->n_blocks, d_nb));
+    VGX_TRY(vgx_launch(c, esdf_init_kernel, grid, 256, 0, VgxLaunch::plain, P, L, s->d_esdf.get(), d_fixed));
+    VGX_TRY(vgx_launch(c, esdf_neighbours_kernel, (27 * s->n_blocks + 127) / 128, 128, 0, VgxLaunch::plain, L, d_nb));
     // relax to convergence: the flag is read back every other sweep
     int sweeps = 0;
     const int max_sweeps = 4 * (int)ceilf(dc.max_distance_m / s->voxel_size) + 16;
     for (;;) {
       VGX_TRY(vgx_fill(c, d_changed, 1));
       for (int k = 0; k < 2; ++k) {
-        VGX_TRY(vgx_launch(c, esdf_sweep_kernel, grid, 256, 0, VgxLaunch::plain, P, s->d_esdf.get(), d_fixed, d_nb,
+        VGX_TRY(vgx_launch(c, esdf_sweep_kernel, grid, 256, 0, VgxLaunch::plain, P, L, s->d_esdf.get(), d_fixed, d_nb,
                            d_changed));
         ++sweeps;
       }
@@ -157,7 +147,7 @@ extern "C" int vgx_submap_generate_esdf(vgx_ctx* c, uint32_t id, const vgx_esdf_
     if (sweeps_out) *sweeps_out = sweeps;
     // registration view of the ESDF layer (observed <=> weight 1), same octet layout as the TSDF view
     VGX_TRY(s->d_view_esdf.alloc(c, sizeof(float) * 8 * nvox, "ESDF registration view"));
-    VGX_TRY(vgx_submap_build_view(c, s, s->d_esdf.get(), s->d_view_esdf.get()));
+    VGX_TRY(vgx_submap_build_view(c, s, VGX_LAYER_ESDF));
     return vgx_sync(c);
   });
 }

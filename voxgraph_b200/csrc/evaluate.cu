@@ -34,11 +34,8 @@ struct RmsePartial {
 };
 
 struct RmseLayer {
-  VgxHash hash;
-  const float2* dw;       // (distance, weight) or (distance, observed 1 / 0)
-  const int32_t* block_idx;
-  int n_blocks;
-  int esdf;               // observed: esdf ? flag != 0 : weight > 1e-6
+  LayerDev L;   // L.dw: (distance, weight) or, esdf, (distance, observed 1 / 0)
+  int esdf;     // observed: esdf ? flag != 0 : weight > 1e-6
 };
 
 __device__ __forceinline__ bool rmse_observed(int esdf, float2 q) {
@@ -72,25 +69,26 @@ __device__ void rmse_cta_reduce(RmsePartial& p) {
 }
 
 __global__ void __launch_bounds__(RMSE_THREADS)
-rmse_block_kernel(RmseLayer gt, RmseLayer test, int vpb, RmsePartial* __restrict__ out) {
-  const bool test_side = blockIdx.x < (unsigned)test.n_blocks;
+rmse_block_kernel(RmseLayer gt, RmseLayer test, RmsePartial* __restrict__ out) {
+  const bool test_side = blockIdx.x < (unsigned)test.L.n_blocks;
   // the layer whose block this CTA owns (a_*) and the other one (field by field: no local copy)
-  const int32_t* a_idx = test_side ? test.block_idx : gt.block_idx;
-  const float2* a_dw = test_side ? test.dw : gt.dw;
+  const int32_t* a_idx = test_side ? test.L.block_idx : gt.L.block_idx;
+  const float2* a_dw = test_side ? test.L.dw : gt.L.dw;
   const int a_esdf = test_side ? test.esdf : gt.esdf;
-  const VgxHash b_hash = test_side ? gt.hash : test.hash;
-  const int slot = test_side ? (int)blockIdx.x : (int)blockIdx.x - test.n_blocks;
+  const VgxHash b_hash = test_side ? gt.L.hash : test.L.hash;
+  const int slot = test_side ? (int)blockIdx.x : (int)blockIdx.x - test.L.n_blocks;
   const int other = vgx_hash_find(b_hash, a_idx[3 * slot], a_idx[3 * slot + 1], a_idx[3 * slot + 2]);
   RmsePartial p;
   p.sum = 0.0;
   p.max_error = 0.0f;
   p.pad = 0;
   p.n_eval = p.n_ign = p.n_ovl = p.n_non = 0;
+  const int vpb = vgx_voxels_per_block(test.L.sh);   // the two layers share vps
   const float2* a = a_dw + (size_t)slot * vpb;
   if (other < 0) {   // a block of one layer only: its observed voxels are non-overlapping
     for (int v = threadIdx.x; v < vpb; v += blockDim.x) p.n_non += rmse_observed(a_esdf, a[v]) ? 1 : 0;
   } else if (test_side) {   // shared block (counted once, from the test side)
-    const float2* g = gt.dw + (size_t)other * vpb;
+    const float2* g = gt.L.dw + (size_t)other * vpb;
     for (int v = threadIdx.x; v < vpb; v += blockDim.x) {
       const float2 qt = a[v], qg = g[v];
       if (!rmse_observed(test.esdf, qt) || !rmse_observed(gt.esdf, qg)) {
@@ -136,10 +134,7 @@ static int rmse_layer(vgx_ctx* c, VgxSubmap* s, int which, const char* name, Rms
   if (!s->finished) VGX_FAIL(c, VGX_ERR_INVALID, std::string("the ") + name + " is not finished");
   if (which == VGX_LAYER_ESDF && !s->d_view_esdf.get())
     VGX_FAIL(c, VGX_ERR_INVALID, std::string("the ") + name + " has no ESDF");
-  L->hash = s->hash();
-  L->dw = which == VGX_LAYER_ESDF ? s->d_esdf.get() : s->d_dw.get();
-  L->block_idx = s->d_block_idx.get();
-  L->n_blocks = s->n_blocks;
+  L->L = layer_of(s, which);
   L->esdf = which == VGX_LAYER_ESDF;
   return VGX_OK;
 }
@@ -157,7 +152,7 @@ extern "C" int vgx_evaluate_layers_rmse(vgx_ctx* c, uint32_t gt_id, int gt_layer
     RmseLayer G, T;
     VGX_TRY(rmse_layer(c, g, gt_layer, "ground truth", &G));
     VGX_TRY(rmse_layer(c, t, test_layer, "test layer", &T));
-    const size_t n_part = (size_t)G.n_blocks + (size_t)T.n_blocks;
+    const size_t n_part = (size_t)G.L.n_blocks + (size_t)T.L.n_blocks;
     if (n_part > (size_t)INT32_MAX) VGX_FAIL(c, VGX_ERR_CAPACITY, "too many blocks");
     RmsePartial total;
     memset(&total, 0, sizeof(total));
@@ -167,8 +162,7 @@ extern "C" int vgx_evaluate_layers_rmse(vgx_ctx* c, uint32_t gt_id, int gt_layer
       const int threads = std::min(RMSE_THREADS, g->vox_per_block);
       {
         VgxProfileScope scope(c, VGX_SLOT_EVAL);
-        VGX_TRY(vgx_launch(c, rmse_block_kernel, (unsigned)n_part, threads, 0, VgxLaunch::plain, G, T, g->vox_per_block,
-                           d_part));
+        VGX_TRY(vgx_launch(c, rmse_block_kernel, (unsigned)n_part, threads, 0, VgxLaunch::plain, G, T, d_part));
       }
       {
         VgxProfileScope scope(c, VGX_SLOT_EVAL);

@@ -136,8 +136,7 @@ size_t vgx_scan_tmp_count(size_t n) { return (n + SCAN_TILE - 1) / SCAN_TILE + 2
 __global__ void __launch_bounds__(256)
 relevant_count_kernel(LayerDev L, double min_w, double max_d, unsigned* __restrict__ counts) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t nvox = (size_t)L.n_blocks << (3 * L.sh);
-  if (i >= nvox) return;
+  if (i >= vgx_voxel_count(L.n_blocks, L.sh)) return;
   const float2 x = L.dw[i];
   counts[i] = ((double)x.y > min_w && fabs((double)x.x) < max_d) ? 1u : 0u;  // cpp:177-178
 }
@@ -157,19 +156,15 @@ relevant_emit_kernel(LayerDev L, const unsigned* __restrict__ counts, const unsi
                      const float2* __restrict__ esdf /* null: TSDF distance */, float* __restrict__ pts,
                      float* __restrict__ obb /* min[3], max[3] */) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t nvox = (size_t)L.n_blocks << (3 * L.sh);
-  if (i >= nvox || counts[i] == 0) return;
-  const int slot = (int)(i >> (3 * L.sh));
-  const int lin = (int)(i & (((size_t)1 << (3 * L.sh)) - 1));
-  const int v[3] = {lin & (L.vps - 1), (lin >> L.sh) & (L.vps - 1), lin >> (2 * L.sh)};
+  if (i >= vgx_voxel_count(L.n_blocks, L.sh) || counts[i] == 0) return;
+  int v[3];
+  const int slot = vgx_voxel_of(i, L.sh, v);
   const float2 x = L.dw[i];
   float cpos[3];
   const float half = 0.5f * L.voxel_size;
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
-    // Block::computeCoordinatesFromLinearIndex: origin + (voxel_index + 0.5) * voxel_size
-    const float origin = (float)L.block_idx[3 * slot + a] * L.block_size;
-    cpos[a] = origin + ((float)v[a] + 0.5f) * L.voxel_size;
+    cpos[a] = vgx_voxel_centre(L.block_idx[3 * slot + a], v[a], L.block_size, L.voxel_size);
     atomicMinFloat(obb + a, cpos[a] - half);
     atomicMaxFloat(obb + 3 + a, cpos[a] + half);
   }
@@ -182,8 +177,7 @@ relevant_emit_kernel(LayerDev L, const unsigned* __restrict__ counts, const unsi
 __global__ void __launch_bounds__(128)
 iso_count_kernel(LayerDev L, float min_weight, unsigned* __restrict__ counts) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t nvox = (size_t)L.n_blocks << (3 * L.sh);
-  if (i >= nvox) return;
+  if (i >= vgx_voxel_count(L.n_blocks, L.sh)) return;
   float sdf[8], coords[3];
   unsigned n = 0;
   if (ex_cube(L, i, min_weight, sdf, coords)) {
@@ -227,8 +221,7 @@ iso_emit_kernel(LayerDev L, float min_weight, double threshold_inv, const unsign
                 const unsigned* __restrict__ offsets, float* __restrict__ cand /* M x 3 */,
                 unsigned long long* __restrict__ cand_key, IsoBucket* __restrict__ table, size_t mask) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const size_t nvox = (size_t)L.n_blocks << (3 * L.sh);
-  if (i >= nvox || counts[i] == 0) return;
+  if (i >= vgx_voxel_count(L.n_blocks, L.sh) || counts[i] == 0) return;
   float sdf[8], coords[3];
   if (!ex_cube(L, i, min_weight, sdf, coords)) return;
   unsigned o = offsets[i];

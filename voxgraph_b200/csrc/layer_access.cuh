@@ -1,11 +1,91 @@
-// Device access to a resident block layer shared by the kernels that sweep marching cubes over it
-// (extract.cu: isosurface vertices, mesh.cu: submap meshes), the trilinear interpolator shared by
-// extract.cu and project.cu, and the minkindr float transform and its inverse shared by overlap.cu,
-// mesh.cu, project.cu and evaluate.cu.  Compiled with -fmad=false by every includer.
+// Device access to a resident block layer.  Brick addressing: how a voxel is found in a layer's bricks, for every
+// kernel that reads or writes them (the registration path keeps its own, see registration.cuh).  LayerDev: the one
+// kernel-facing view of a resident layer.  The cube gather shared by the kernels that sweep marching cubes over a
+// layer (extract.cu: isosurface vertices, mesh.cu: submap meshes), the trilinear interpolator shared by extract.cu
+// and project.cu, and the minkindr float transform and its inverse shared by overlap.cu, mesh.cu, project.cu,
+// evaluate.cu and tsdf.cu.  Every kernel that uses the float helpers is compiled with -fmad=false.
 #pragma once
 
 #include "vgx_internal.h"
 
+// ------------------------------------------------------------------ brick addressing
+// A brick holds vps^3 voxels, vps = 2^sh, voxel (x, y, z) at the linear index x + vps (y + vps z).  The layer-wide
+// index of a voxel is slot vps^3 + linear index, slot being its brick's.  A global voxel index (per axis, in voxels
+// from the origin) lies in block g >> sh at voxel g mod vps.
+
+// the voxels_per_side a layer accepts
+__host__ __device__ __forceinline__ bool vgx_vps_ok(long long vps) {
+  return vps >= 2 && vps <= 32 && (vps & (vps - 1)) == 0;
+}
+// voxels in one brick, and in n_blocks bricks
+__host__ __device__ __forceinline__ int vgx_voxels_per_block(int sh) { return 1 << (3 * sh); }
+__host__ __device__ __forceinline__ size_t vgx_voxel_count(int n_blocks, int sh) { return (size_t)n_blocks << (3 * sh); }
+// linear index in its brick of voxel (x, y, z), and back
+__host__ __device__ __forceinline__ int vgx_voxel_linear(int x, int y, int z, int sh) {
+  return x + (y << sh) + (z << (2 * sh));
+}
+__host__ __device__ __forceinline__ void vgx_voxel_xyz(int lin, int sh, int v[3]) {
+  const int m = (1 << sh) - 1;
+  v[0] = lin & m;
+  v[1] = (lin >> sh) & m;
+  v[2] = lin >> (2 * sh);
+}
+// layer-wide index of the voxel with linear index lin, or (x, y, z), in the brick at slot
+__host__ __device__ __forceinline__ size_t vgx_voxel_index(int slot, int lin, int sh) {
+  return ((size_t)slot << (3 * sh)) + lin;
+}
+__host__ __device__ __forceinline__ size_t vgx_voxel_index(int slot, int x, int y, int z, int sh) {
+  return ((size_t)slot << (3 * sh)) + x + (y << sh) + (z << (2 * sh));
+}
+// layer-wide voxel index i -> its brick's slot (returned) and the voxel (x, y, z) in the brick
+__host__ __device__ __forceinline__ int vgx_voxel_of(size_t i, int sh, int v[3]) {
+  vgx_voxel_xyz((int)(i & (((size_t)1 << (3 * sh)) - 1)), sh, v);
+  return (int)(i >> (3 * sh));
+}
+// one axis of the centre of voxel v of block b (voxblox Block::computeCoordinatesFromLinearIndex)
+__host__ __device__ __forceinline__ float vgx_voxel_centre(int b, int v, float block_size, float voxel_size) {
+  return (float)b * block_size + ((float)v + 0.5f) * voxel_size;
+}
+// one axis of a global voxel index (int or 64-bit) -> the voxel's index in its block; also the index in its own
+// block of a neighbour one voxel past the brick's face
+template <class I>
+__host__ __device__ __forceinline__ int vgx_voxel_in_block(I g, int sh) {
+  return (int)(g & (((I)1 << sh) - 1));
+}
+// global voxel index g -> the linear index of the voxel in its block
+template <class I>
+__host__ __device__ __forceinline__ int vgx_global_voxel(const I g[3], int sh) {
+  return vgx_voxel_linear(vgx_voxel_in_block(g[0], sh), vgx_voxel_in_block(g[1], sh), vgx_voxel_in_block(g[2], sh), sh);
+}
+// global voxel index g -> its block b.  False when a component lies outside [VGX_BLOCK_INDEX_MIN, VGX_BLOCK_INDEX_MAX]:
+// no such block exists (vgx_block_in_range).  The test is made on the index as given, before the cast to int could
+// wrap a 64-bit one.
+template <class I>
+__host__ __device__ __forceinline__ bool vgx_global_block(const I g[3], int sh, int b[3]) {
+  const I c0 = g[0] >> sh, c1 = g[1] >> sh, c2 = g[2] >> sh;
+  b[0] = (int)c0; b[1] = (int)c1; b[2] = (int)c2;
+  return c0 >= VGX_BLOCK_INDEX_MIN && c0 <= VGX_BLOCK_INDEX_MAX && c1 >= VGX_BLOCK_INDEX_MIN &&
+         c1 <= VGX_BLOCK_INDEX_MAX && c2 >= VGX_BLOCK_INDEX_MIN && c2 <= VGX_BLOCK_INDEX_MAX;
+}
+// Slots of the bricks that hold the 2x2x2 forward neighbourhood of voxel v of block b (in brick `slot`): nslot[m]
+// for the offset m (bit 0 = +x, bit 1 = +y, bit 2 = +z), -1 where the brick does not exist.  An offset leaves the
+// brick only on an axis where v is the brick's last voxel, so there is one hash lookup per distinct brick.
+__device__ __forceinline__ void vgx_forward_slots(const VgxHash& hash, const int b[3], const int v[3], int slot, int sh,
+                                                  int nslot[8]) {
+  const int last = (1 << sh) - 1;
+  const bool lx = v[0] == last, ly = v[1] == last, lz = v[2] == last;   // an offset along the axis leaves the brick
+  nslot[0] = slot;
+#pragma unroll
+  for (int m = 1; m < 8; ++m) {   // offset m is in the brick of m without an axis that stays, or in a new one
+    if ((m & 1) && !lx) nslot[m] = nslot[m ^ 1];
+    else if ((m & 2) && !ly) nslot[m] = nslot[m ^ 2];
+    else if ((m & 4) && !lz) nslot[m] = nslot[m ^ 4];
+    else nslot[m] = vgx_hash_find(hash, b[0] + (m & 1), b[1] + ((m >> 1) & 1), b[2] + (m >> 2));
+  }
+}
+
+// ------------------------------------------------------------------ layer view
+// dw: the (distance, weight) bricks, or the ESDF bricks (distance, observed 1 / 0) of a view of the ESDF layer
 struct LayerDev {
   VgxHash hash;
   const float2* dw;
@@ -15,10 +95,11 @@ struct LayerDev {
   int vps, sh, n_blocks;
 };
 
-static inline LayerDev layer_of(const VgxSubmap* s) {
+// which: VGX_LAYER_TSDF or VGX_LAYER_ESDF (the bricks dw points at)
+static inline LayerDev layer_of(const VgxSubmap* s, int which = VGX_LAYER_TSDF) {
   LayerDev L;
   L.hash = s->hash();
-  L.dw = s->d_dw.get();
+  L.dw = which == VGX_LAYER_ESDF ? s->d_esdf.get() : s->d_dw.get();
   L.block_idx = s->d_block_idx.get();
   L.rgba = s->d_rgba.get();
   L.voxel_size = s->voxel_size; L.voxel_size_inv = s->voxel_size_inv;
@@ -29,6 +110,7 @@ static inline LayerDev layer_of(const VgxSubmap* s) {
   return L;
 }
 
+// ------------------------------------------------------------------ cube gather and interpolation
 // Cube corner offsets and edges (voxblox MarchingCubes order); host copies use the same initialisers.
 #define VGX_CUBE_OFF {{0, 0, 0}, {1, 0, 0}, {1, 1, 0}, {0, 1, 0}, {0, 0, 1}, {1, 0, 1}, {1, 1, 1}, {0, 1, 1}}
 #define VGX_CUBE_EDGE {{0, 1}, {1, 2}, {2, 3}, {3, 0}, {4, 5}, {5, 6}, {6, 7}, {7, 4}, {0, 4}, {1, 5}, {2, 6}, {3, 7}}
@@ -41,29 +123,20 @@ __device__ __forceinline__ int ex_floor(float v) { return __float2int_rd(v); }
 // corner (may be null): the layer-wide voxel index (slot << 3 sh | linear index) of every corner.
 __device__ __forceinline__ bool ex_cube(const LayerDev& L, size_t i, float min_weight, float sdf[8],
                                         float coords[3], size_t* corner = nullptr) {
-  const int slot = (int)(i >> (3 * L.sh));
-  const int lin = (int)(i & (((size_t)1 << (3 * L.sh)) - 1));
-  const int v[3] = {lin & (L.vps - 1), (lin >> L.sh) & (L.vps - 1), lin >> (2 * L.sh)};
+  int v[3];
+  const int slot = vgx_voxel_of(i, L.sh, v);
   const int b[3] = {L.block_idx[3 * slot], L.block_idx[3 * slot + 1], L.block_idx[3 * slot + 2]};
 #pragma unroll
-  for (int a = 0; a < 3; ++a) coords[a] = (float)b[a] * L.block_size + ((float)v[a] + 0.5f) * L.voxel_size;
+  for (int a = 0; a < 3; ++a) coords[a] = vgx_voxel_centre(b[a], v[a], L.block_size, L.voxel_size);
   int nslot[8];
-  nslot[0] = slot;
-#pragma unroll
-  for (int k = 1; k < 8; ++k) {  // k bit0 = x overflow, bit1 = y, bit2 = z
-    const bool ux = (k & 1) && v[0] == L.vps - 1, uy = (k & 2) && v[1] == L.vps - 1,
-               uz = (k & 4) && v[2] == L.vps - 1;
-    const int j = (ux ? 1 : 0) | (uy ? 2 : 0) | (uz ? 4 : 0);
-    nslot[k] = (j == k) ? vgx_hash_find(L.hash, b[0] + (ux ? 1 : 0), b[1] + (uy ? 1 : 0), b[2] + (uz ? 1 : 0))
-                        : nslot[j];
-  }
+  vgx_forward_slots(L.hash, b, v, slot, L.sh, nslot);
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
     const int ox = c_cube_off[c][0], oy = c_cube_off[c][1], oz = c_cube_off[c][2];
     const int s = nslot[ox | (oy << 1) | (oz << 2)];
     if (s < 0) return false;
-    const int x = (v[0] + ox) & (L.vps - 1), y = (v[1] + oy) & (L.vps - 1), z = (v[2] + oz) & (L.vps - 1);
-    const size_t at = ((size_t)s << (3 * L.sh)) + x + (y << L.sh) + (z << (2 * L.sh));
+    const size_t at = vgx_voxel_index(s, vgx_voxel_in_block(v[0] + ox, L.sh), vgx_voxel_in_block(v[1] + oy, L.sh),
+                                      vgx_voxel_in_block(v[2] + oz, L.sh), L.sh);
     const float2 q = L.dw[at];
     if (q.y <= min_weight) return false;  // utils::getSdfIfValid
     sdf[c] = q.x;
@@ -98,7 +171,7 @@ __device__ inline bool ex_interp_voxel_impl(const LayerDev& L, float p0, float p
     const float origin = (float)b[a] * L.block_size;
     int vi = ex_floor((p[a] - origin) * L.voxel_size_inv + 1e-6f);
     vi = max(min(vi, vps - 1), 0);
-    const float centre = origin + ((float)vi + 0.5f) * L.voxel_size;
+    const float centre = vgx_voxel_centre(b[a], vi, L.block_size, L.voxel_size);
     if (p[a] - centre < 0) {
       if (--vi < 0) { --b[a]; vi += vps; }
     }
@@ -120,14 +193,14 @@ __device__ inline bool ex_interp_voxel_impl(const LayerDev& L, float p0, float p
       float off[3];
 #pragma unroll
       for (int a = 0; a < 3; ++a) {
-        const float centre = (float)b[a] * L.block_size + ((float)cv[a] + 0.5f) * L.voxel_size;
+        const float centre = vgx_voxel_centre(b[a], cv[a], L.block_size, L.voxel_size);
         off[a] = (p[a] - centre) * L.voxel_size_inv;
       }
       q[0] = 1.0f; q[1] = off[0]; q[2] = off[1]; q[3] = off[2];
       q[4] = off[0] * off[1]; q[5] = off[1] * off[2]; q[6] = off[2] * off[0];
       q[7] = off[0] * off[1] * off[2];
     }
-    const size_t at = ((size_t)slot << (3 * L.sh)) + cv[0] + (cv[1] << L.sh) + (cv[2] << (2 * L.sh));
+    const size_t at = vgx_voxel_index(slot, cv[0], cv[1], cv[2], L.sh);
     const float2 x = L.dw[at];
     if (kColour) col[i] = L.rgba[at];
     d[i] = x.x;
@@ -171,6 +244,7 @@ __device__ inline bool ex_interp_voxel(const LayerDev& L, float p0, float p1, fl
   return ex_interp_voxel_impl<false>(L, p0, p1, p2, out_d, out_w, unused);
 }
 
+// ------------------------------------------------------------------ minkindr float transform
 // Eigen Quaternion::_transformVector (minkindr RotationQuaternion::rotate), float
 __host__ __device__ inline void ov_rotate(const float q[4], const float v[3], float o[3]) {
   const float w = q[0], x = q[1], y = q[2], z = q[3];

@@ -299,14 +299,13 @@ mesh_vertex_kernel(const MeshJob* __restrict__ jobs, int n_jobs, size_t n_vox, c
   const MeshJob& J = mesh_job_of(jobs, n_jobs, i);
   const LayerDev& L = J.L;
   const size_t local = i - J.vox_base;
-  const int slot = (int)(local >> (3 * L.sh));
-  const int lin = (int)(local & (((size_t)1 << (3 * L.sh)) - 1));
-  const int v[3] = {lin & (L.vps - 1), (lin >> L.sh) & (L.vps - 1), lin >> (2 * L.sh)};
+  int v[3];
+  const int slot = vgx_voxel_of(local, L.sh, v);
   const int b[3] = {L.block_idx[3 * slot], L.block_idx[3 * slot + 1], L.block_idx[3 * slot + 2]};
   const float s_lo = L.dw[local].x;
   float c_lo[3];
 #pragma unroll
-  for (int a = 0; a < 3; ++a) c_lo[a] = (float)b[a] * L.block_size + ((float)v[a] + 0.5f) * L.voxel_size;
+  for (int a = 0; a < 3; ++a) c_lo[a] = vgx_voxel_centre(b[a], v[a], L.block_size, L.voxel_size);
   size_t o = vbase + vert_off[i];
 #pragma unroll
   for (int ax = 0; ax < 3; ++ax) {
@@ -319,7 +318,7 @@ mesh_vertex_kernel(const MeshJob* __restrict__ jobs, int n_jobs, size_t n_vox, c
       ++nb[ax];
       s = vgx_hash_find(L.hash, nb[0], nb[1], nb[2]);
     }
-    const float s_hi = L.dw[((size_t)s << (3 * L.sh)) + nv[0] + (nv[1] << L.sh) + (nv[2] << (2 * L.sh))].x;
+    const float s_hi = L.dw[vgx_voxel_index(s, nv[0], nv[1], nv[2], L.sh)].x;
     float c_hi[3] = {c_lo[0], c_lo[1], c_lo[2]};
     c_hi[ax] = c_lo[ax] + L.voxel_size;
     const float d = s_lo - s_hi;
@@ -340,10 +339,9 @@ mesh_vertex_kernel(const MeshJob* __restrict__ jobs, int n_jobs, size_t n_vox, c
       if (L.rgba) {
         const int g[3] = {ex_floor(p[0] * L.voxel_size_inv + 1e-6f), ex_floor(p[1] * L.voxel_size_inv + 1e-6f),
                           ex_floor(p[2] * L.voxel_size_inv + 1e-6f)};
-        const int cs = vgx_hash_find(L.hash, g[0] >> L.sh, g[1] >> L.sh, g[2] >> L.sh);
-        if (cs >= 0)
-          col = L.rgba[((size_t)cs << (3 * L.sh)) + (g[0] & (L.vps - 1)) + ((g[1] & (L.vps - 1)) << L.sh) +
-                       ((g[2] & (L.vps - 1)) << (2 * L.sh))];
+        int gb[3];
+        const int cs = vgx_global_block(g, L.sh, gb) ? vgx_hash_find(L.hash, gb[0], gb[1], gb[2]) : -1;
+        if (cs >= 0) col = L.rgba[vgx_voxel_index(cs, vgx_global_voxel(g, L.sh), L.sh)];
       }
       vcol[o] = col;
     }

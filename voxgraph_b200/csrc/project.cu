@@ -67,26 +67,21 @@ struct ProjSrc {
   int first_block;   // this submap's first block in the rank-ordered list of all input blocks
 };
 
-__device__ __forceinline__ void proj_unpack(uint64_t key, int b[3]) {
-  b[0] = (int)(key & 0x1FFFFFu) - (1 << 20);
-  b[1] = (int)((key >> 21) & 0x1FFFFFu) - (1 << 20);
-  b[2] = (int)((key >> 42) & 0x1FFFFFu) - (1 << 20);
-}
-
 // voxel v of output block b (geometry of S), moved into S's frame
 __device__ __forceinline__ void proj_voxel_in_submap(const ProjSrc& S, const int b[3], int v, float p[3]) {
   const LayerDev& L = S.L;
-  const int x[3] = {v & (L.vps - 1), (v >> L.sh) & (L.vps - 1), v >> (2 * L.sh)};
+  int x[3];
+  vgx_voxel_xyz(v, L.sh, x);
   float c[3];
 #pragma unroll
-  for (int a = 0; a < 3; ++a) c[a] = (float)b[a] * L.block_size + ((float)x[a] + 0.5f) * L.voxel_size;
+  for (int a = 0; a < 3; ++a) c[a] = vgx_voxel_centre(b[a], x[a], L.block_size, L.voxel_size);
   ov_transform(S.T_inv, c, p);
 }
 
 // does output block b exist in S's transformed layer: any of its voxels interpolates.  Called by every
 // thread of the CTA; stops at the first chunk of voxels with a success.
 __device__ __forceinline__ bool proj_block_exists(const ProjSrc& S, const int b[3]) {
-  const int vpb = 1 << (3 * S.L.sh);
+  const int vpb = vgx_voxels_per_block(S.L.sh);
   for (int base = 0; base < vpb; base += blockDim.x) {
     const int v = base + (int)threadIdx.x;
     bool ok = false;
@@ -198,7 +193,7 @@ project_occupancy_kernel(const ProjSrc* __restrict__ src, const uint64_t* __rest
                          unsigned* __restrict__ keep) {
   const int k = blockIdx.x;
   int b[3];
-  proj_unpack(ukey[k], b);
+  vgx_unpack_key(ukey[k], b);
   unsigned any = keep_own && vgx_hash_find(src[0].L.hash, b[0], b[1], b[2]) >= 0 ? 1u : 0u;
   for (uint32_t j = useg[k]; !any && j < useg[k + 1]; ++j)
     if (proj_block_exists(src[urank[j]], b)) { any = 1; break; }
@@ -226,7 +221,7 @@ project_fold_kernel(const ProjSrc* __restrict__ src, const uint64_t* __restrict_
   const unsigned s = out_slot[k];
   if (out_slot[k + 1] == s) return;
   int b[3];
-  proj_unpack(ukey[k], b);
+  vgx_unpack_key(ukey[k], b);
   if (threadIdx.x == 0) {
     out_idx[3 * (size_t)s] = b[0];
     out_idx[3 * (size_t)s + 1] = b[1];
@@ -289,7 +284,7 @@ transform_fold_kernel(const ProjSrc* __restrict__ src, const uint64_t* __restric
   const unsigned s = out_slot[k];
   if (out_slot[k + 1] == s) return;
   int b[3];
-  proj_unpack(ukey[k], b);
+  vgx_unpack_key(ukey[k], b);
   if (threadIdx.x == 0) {
     out_idx[3 * (size_t)s] = b[0];
     out_idx[3 * (size_t)s + 1] = b[1];
@@ -297,14 +292,14 @@ transform_fold_kernel(const ProjSrc* __restrict__ src, const uint64_t* __restric
   }
   const ProjSrc& S = src[0];
   const int old = vgx_hash_find(S.L.hash, b[0], b[1], b[2]);
-  const int vpb = 1 << (3 * S.L.sh);
+  const int vpb = vgx_voxels_per_block(S.L.sh);
   float2* brick = out_dw + (size_t)s * vpb;
   for (int v = threadIdx.x; v < vpb; v += blockDim.x) {
     float p[3], d = 0.0f, w = 0.0f;
     proj_voxel_in_submap(S, b, v, p);
     float2 q;
     if (ex_interp_voxel(S.L, p[0], p[1], p[2], d, w)) q = make_float2(d, w);
-    else q = old >= 0 ? S.L.dw[((size_t)old << (3 * S.L.sh)) + v] : make_float2(0.0f, 0.0f);
+    else q = old >= 0 ? S.L.dw[vgx_voxel_index(old, v, S.L.sh)] : make_float2(0.0f, 0.0f);
     brick[v] = q;
   }
 }

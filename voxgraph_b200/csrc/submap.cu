@@ -12,7 +12,7 @@
 #include <string>
 #include <vector>
 
-#include "vgx_internal.h"
+#include "layer_access.cuh"
 
 // ------------------------------------------------------------------ context
 extern "C" int vgx_device_count(void) {
@@ -181,36 +181,25 @@ __global__ void interleave_kernel(const float* __restrict__ d, const float* __re
 // brick faces through the hash) and stores the 8 distances, NaN where
 // utils::isObservedVoxel (weight > 1e-6) fails or the neighbour block does not exist.
 __global__ void __launch_bounds__(256)
-build_view_kernel(const float2* __restrict__ dw, const int32_t* __restrict__ block_idx, VgxHash hash,
-                  float* __restrict__ view, int n_blocks, int vps, int sh) {
-  const size_t vpb = (size_t)1 << (3 * sh);
+build_view_kernel(LayerDev L, float* __restrict__ view) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (size_t)n_blocks * vpb) return;
-  const int slot = (int)(i >> (3 * sh));
-  const int lin = (int)(i & (vpb - 1));
-  const int vx = lin & (vps - 1), vy = (lin >> sh) & (vps - 1), vz = lin >> (2 * sh);
-  const int bx = block_idx[3 * slot], by = block_idx[3 * slot + 1], bz = block_idx[3 * slot + 2];
-  const bool cx = vx == vps - 1, cy = vy == vps - 1, cz = vz == vps - 1;
+  if (i >= vgx_voxel_count(L.n_blocks, L.sh)) return;
+  int v[3];
+  const int slot = vgx_voxel_of(i, L.sh, v);
+  const int b[3] = {L.block_idx[3 * slot], L.block_idx[3 * slot + 1], L.block_idx[3 * slot + 2]};
   int s[8];
-  s[0] = slot;
-#pragma unroll
-  for (int c = 1; c < 8; ++c) {
-    const bool ux = (c & 4) && cx, uy = (c & 2) && cy, uz = (c & 1) && cz;
-    const int j = (ux ? 4 : 0) | (uy ? 2 : 0) | (uz ? 1 : 0);
-    if (j == c) s[c] = vgx_hash_find(hash, bx + (ux ? 1 : 0), by + (uy ? 1 : 0), bz + (uz ? 1 : 0));
-    else s[c] = s[j];
-  }
+  vgx_forward_slots(L.hash, b, v, slot, L.sh, s);
   float o[8];
 #pragma unroll
-  for (int c = 0; c < 8; ++c) {
-    const int x = (vx + ((c >> 2) & 1)) & (vps - 1), y = (vy + ((c >> 1) & 1)) & (vps - 1),
-              z = (vz + (c & 1)) & (vps - 1);
-    float v = __int_as_float(0x7fc00000);
-    if (s[c] >= 0) {
-      const float2 q = dw[(size_t)s[c] * vpb + x + (y << sh) + (z << (2 * sh))];
-      if (q.y > 1e-6f) v = q.x;
+  for (int m = 0; m < 8; ++m) {   // offset m = (x, y, z) bits (0, 1, 2) is corner x = bit 2, y = bit 1, z = bit 0
+    float d = __int_as_float(0x7fc00000);
+    if (s[m] >= 0) {
+      const float2 q = L.dw[vgx_voxel_index(s[m], vgx_voxel_in_block(v[0] + (m & 1), L.sh),
+                                            vgx_voxel_in_block(v[1] + ((m >> 1) & 1), L.sh),
+                                            vgx_voxel_in_block(v[2] + (m >> 2), L.sh), L.sh)];
+      if (q.y > 1e-6f) d = q.x;
     }
-    o[c] = v;
+    o[((m & 1) << 2) | (m & 2) | (m >> 2)] = d;
   }
   float4* dst = reinterpret_cast<float4*>(view + i * 8);
   dst[0] = make_float4(o[0], o[1], o[2], o[3]);
@@ -262,11 +251,11 @@ int vgx_submap_build_grid(vgx_ctx* c, VgxSubmap* s) {
   return VGX_OK;
 }
 
-int vgx_submap_build_view(vgx_ctx* c, VgxSubmap* s, const float2* bricks, float* view) {
+int vgx_submap_build_view(vgx_ctx* c, VgxSubmap* s, int which) {
   const size_t used = (size_t)s->n_blocks * s->vox_per_block;
   if (used == 0) return VGX_OK;
-  return vgx_launch(c, build_view_kernel, (unsigned)((used + 255) / 256), 256, 0, VgxLaunch::plain, bricks,
-                    s->d_block_idx.get(), s->hash(), view, s->n_blocks, s->vps, s->sh);
+  return vgx_launch(c, build_view_kernel, (unsigned)((used + 255) / 256), 256, 0, VgxLaunch::plain, layer_of(s, which),
+                    which == VGX_LAYER_ESDF ? s->d_view_esdf.get() : s->d_view.get());
 }
 
 int vgx_submap_rebuild_hash(vgx_ctx* c, VgxSubmap* s) {
@@ -286,7 +275,7 @@ static uint32_t table_size_for(int cap) {
 
 int vgx_submap_alloc(vgx_ctx* c, uint32_t id, float voxel_size, int vps, int cap, bool with_view,
                         VgxSubmap** out) {
-  if (!(voxel_size > 0) || vps < 2 || vps > 32 || (vps & (vps - 1)) != 0 || cap < 0)
+  if (!(voxel_size > 0) || !vgx_vps_ok(vps) || cap < 0)
     VGX_FAIL(c, VGX_ERR_INVALID, "invalid voxel_size / voxels_per_side / capacity");
   VgxSubmap* old = c->find(id);
   if (old) {
@@ -463,7 +452,7 @@ int vgx_submap_upload_finish(vgx_ctx* c, VgxSubmap* s) {
   VGX_TRY(vgx_upload(c, s->d_counters.get(), &s->n_blocks, 1));
   VGX_TRY(vgx_launch(c, hash_insert_kernel, (s->n_blocks + 127) / 128, 128, 0, VgxLaunch::plain, s->hash(),
                      s->d_block_idx.get(), s->n_blocks, s->d_counters.get() + 2));
-  VGX_TRY(vgx_submap_build_view(c, s, s->d_dw.get(), s->d_view.get()));
+  VGX_TRY(vgx_submap_build_view(c, s, VGX_LAYER_TSDF));
   VGX_TRY(check_uploaded_blocks(c, s));
   return vgx_submap_build_grid(c, s);
 }
@@ -490,7 +479,7 @@ extern "C" int vgx_submap_finish(vgx_ctx* c, uint32_t id) {
     if (!s->d_view.get()) {
       VGX_TRY(s->d_view.alloc(c, sizeof(float) * 8 * (used > 0 ? used : 1), "registration view"));
     }
-    VGX_TRY(vgx_submap_build_view(c, s, s->d_dw.get(), s->d_view.get()));
+    VGX_TRY(vgx_submap_build_view(c, s, VGX_LAYER_TSDF));
     s->finished = true;
     vgx_graph_invalidate_registration(c);
     return vgx_submap_build_grid(c, s);

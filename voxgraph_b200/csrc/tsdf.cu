@@ -52,14 +52,14 @@
 #include <cub/cub.cuh>
 
 #include "colour.cuh"
-#include "vgx_internal.h"
+#include "layer_access.cuh"
 
 #define VGX_EPS 1e-6f
 
 struct TsdfParams {
   float q[4], t[3];  // T_G_C
   float voxel_size, voxel_size_inv;
-  int vps, vps_shift;
+  int sh;            // log2(voxels_per_side)
   vgx_tsdf_config cfg;
   int n;
 };
@@ -70,17 +70,6 @@ struct DevRay {
   float t_next[3], t_step[3];
   long long steps, step;
 };
-
-// Eigen Quaternion::_transformVector (general q)
-__device__ __forceinline__ void quat_rotate(const float q[4], const float v[3], float o[3]) {
-  const float w = q[0], x = q[1], y = q[2], z = q[3];
-  float uv0 = y * v[2] - z * v[1], uv1 = z * v[0] - x * v[2], uv2 = x * v[1] - y * v[0];
-  uv0 += uv0; uv1 += uv1; uv2 += uv2;
-  const float c0 = y * uv2 - z * uv1, c1 = z * uv0 - x * uv2, c2 = x * uv1 - y * uv0;
-  o[0] = (v[0] + w * uv0) + c0;
-  o[1] = (v[1] + w * uv1) + c1;
-  o[2] = (v[2] + w * uv2) + c2;
-}
 
 __device__ __forceinline__ void ray_setup(DevRay& rc, const float s[3], const float e[3]) {
   rc.step = 0;
@@ -141,7 +130,7 @@ __device__ __forceinline__ bool point_to_ray(const TsdfParams& P, const float* _
   }
   origin[0] = P.t[0]; origin[1] = P.t[1]; origin[2] = P.t[2];
   float r[3];
-  quat_rotate(P.q, pC, r);
+  ov_rotate(P.q, pC, r);
   pG[0] = r[0] + P.t[0]; pG[1] = r[1] + P.t[1]; pG[2] = r[2] + P.t[2];
   // getVoxelWeight
   if (P.cfg.use_const_weight) weight = 1.0f;
@@ -246,16 +235,6 @@ __device__ __forceinline__ int tsdf_get_or_alloc(const VgxHash& hash, int32_t* _
   return -1;
 }
 
-// Block of the global voxel index g.  False when a component lies outside [VGX_BLOCK_INDEX_MIN,
-// VGX_BLOCK_INDEX_MAX]: such a block is never allocated and its voxels are skipped (its key would alias
-// a block 2^21 away).  The test is made on the 64-bit index, before the cast to int could wrap it.
-__device__ __forceinline__ bool tsdf_block_of(const long long g[3], int sh, int& b0, int& b1, int& b2) {
-  const long long c0 = g[0] >> sh, c1 = g[1] >> sh, c2 = g[2] >> sh;
-  b0 = (int)c0; b1 = (int)c1; b2 = (int)c2;
-  return c0 >= VGX_BLOCK_INDEX_MIN && c0 <= VGX_BLOCK_INDEX_MAX && c1 >= VGX_BLOCK_INDEX_MIN &&
-         c1 <= VGX_BLOCK_INDEX_MAX && c2 >= VGX_BLOCK_INDEX_MIN && c2 <= VGX_BLOCK_INDEX_MAX;
-}
-
 // ------------------------------------------------------------------ pass 1: allocate
 __global__ void __launch_bounds__(128)
 tsdf_allocate_kernel(TsdfParams P, const float* __restrict__ pts, VgxHash hash,
@@ -268,11 +247,13 @@ tsdf_allocate_kernel(TsdfParams P, const float* __restrict__ pts, VgxHash hash,
   long long g[3];
   int lb0 = INT_MIN, lb1 = 0, lb2 = 0;   // INT_MIN: no block (outside the range)
   while (ray_next(rc, g)) {
-    int b0, b1, b2;
-    if (!tsdf_block_of(g, P.vps_shift, b0, b1, b2)) { lb0 = INT_MIN; continue; }
-    if (b0 == lb0 && b1 == lb1 && b2 == lb2) continue;
-    lb0 = b0; lb1 = b1; lb2 = b2;
-    tsdf_get_or_alloc<false>(hash, block_idx, counters, capacity, b0, b1, b2);
+    int b[3];
+    // a block outside the range is never allocated and its voxels are skipped (its key would alias a block
+    // 2^21 away)
+    if (!vgx_global_block(g, P.sh, b)) { lb0 = INT_MIN; continue; }
+    if (b[0] == lb0 && b[1] == lb1 && b[2] == lb2) continue;
+    lb0 = b[0]; lb1 = b[1]; lb2 = b[2];
+    tsdf_get_or_alloc<false>(hash, block_idx, counters, capacity, b[0], b[1], b[2]);
   }
 }
 
@@ -411,20 +392,18 @@ tsdf_emit_kernel(TsdfParams P, const float* __restrict__ pts, const uint32_t* __
       const uint32_t ray = kColour ? vgx_colour_pack(ray_rgba[i]) : 0u;
       long long g[3];
       int lb0 = INT_MIN, lb1 = 0, lb2 = 0, slot = -1;
-      const int vmask = P.vps - 1, sh = P.vps_shift;
       while (ray_next(rc, g)) {
-        int b0, b1, b2;
-        if (!tsdf_block_of(g, sh, b0, b1, b2)) {
+        int b[3];
+        if (!vgx_global_block(g, P.sh, b)) {
           lb0 = INT_MIN; slot = -1;            // outside the range: the voxel is skipped
-        } else if (!(b0 == lb0 && b1 == lb1 && b2 == lb2)) {
-          lb0 = b0; lb1 = b1; lb2 = b2;
-          slot = vgx_hash_find(hash, b0, b1, b2);
+        } else if (!(b[0] == lb0 && b[1] == lb1 && b[2] == lb2)) {
+          lb0 = b[0]; lb1 = b[1]; lb2 = b[2];
+          slot = vgx_hash_find(hash, b[0], b[1], b[2]);
         }
         unsigned key = sentinel;
         float sdf = 0.f, uw = 0.f;
         if (slot >= 0) {
-          const int lin = (int)(g[0] & vmask) + (((int)(g[1] & vmask)) << sh) + (((int)(g[2] & vmask)) << (2 * sh));
-          key = ((unsigned)slot << (3 * sh)) + (unsigned)lin;
+          key = (unsigned)vgx_voxel_index(slot, vgx_global_voxel(g, P.sh), P.sh);
           tsdf_update_terms(P, origin, pG, g, weight, sdf, uw);
           ++n_upd;
         }
@@ -602,8 +581,6 @@ tsdf_integrate_kernel(TsdfParams P, const float* __restrict__ pts, const uint32_
         long long g[3];
         int lb0 = INT_MIN, lb1 = 0, lb2 = 0, slot = -1;
         long long collisions = 0;
-        const int vmask = P.vps - 1, sh = P.vps_shift;
-        const size_t vpb = (size_t)1 << (3 * sh);
         while (ray_next(rc, g)) {
           if (P.cfg.mode == 1) {
             const unsigned long long h = any_index_hash64(g[0], g[1], g[2]);
@@ -611,17 +588,16 @@ tsdf_integrate_kernel(TsdfParams P, const float* __restrict__ pts, const uint32_
             if (old == h) ++collisions; else collisions = 0;
             if (collisions > P.cfg.max_consecutive_ray_collisions) break;
           }
-          int b0, b1, b2;
-          if (!tsdf_block_of(g, sh, b0, b1, b2)) {
+          int b[3];
+          if (!vgx_global_block(g, P.sh, b)) {
             lb0 = INT_MIN; slot = -1;          // outside the range: the voxel is skipped
-          } else if (!(b0 == lb0 && b1 == lb1 && b2 == lb2)) {
-            lb0 = b0; lb1 = b1; lb2 = b2;
-            slot = tsdf_get_or_alloc<true>(hash, block_idx, counters, capacity, b0, b1, b2);
+          } else if (!(b[0] == lb0 && b[1] == lb1 && b[2] == lb2)) {
+            lb0 = b[0]; lb1 = b[1]; lb2 = b[2];
+            slot = tsdf_get_or_alloc<true>(hash, block_idx, counters, capacity, b[0], b[1], b[2]);
           }
           if (slot < 0) continue;  // outside the range, or capacity exhausted (reported by the host)
-          const int lin = (int)(g[0] & vmask) + (((int)(g[1] & vmask)) << sh) + (((int)(g[2] & vmask)) << (2 * sh));
-          update_tsdf_voxel<kColour>(P, origin, pG, g, weight, dw + (size_t)slot * vpb + lin,
-                                     kColour ? rgba + (size_t)slot * vpb + lin : nullptr, ray);
+          const size_t at = vgx_voxel_index(slot, vgx_global_voxel(g, P.sh), P.sh);
+          update_tsdf_voxel<kColour>(P, origin, pG, g, weight, dw + at, kColour ? rgba + at : nullptr, ray);
           ++n_upd;
         }
       }
@@ -675,7 +651,7 @@ static int tsdf_sort_and_apply(vgx_ctx* c, VgxSubmap* s, const TsdfParams& P, co
   const int n = P.n;
   const unsigned grid = (unsigned)((n + 127) / 128);
   // keys = slot * 4096 + voxel; the sentinel (unmapped block) is one past the largest key
-  const unsigned long long sent64 = (unsigned long long)s->cap_blocks << (3 * P.vps_shift);
+  const unsigned long long sent64 = vgx_voxel_count(s->cap_blocks, P.sh);
   if (sent64 >= 0xFFFFFFFFull) VGX_FAIL(c, VGX_ERR_CAPACITY, "submap too large for 32-bit voxel keys");
   const unsigned sentinel = (unsigned)sent64;
   int end_bit = 1;
@@ -727,8 +703,7 @@ int vgx_tsdf_integrate_resident(vgx_ctx* c, VgxSubmap* s, const float T_G_C[7], 
   for (int k = 0; k < 3; ++k) P.t[k] = T_G_C[4 + k];
   P.voxel_size = s->voxel_size;
   P.voxel_size_inv = s->voxel_size_inv;
-  P.vps = s->vps;
-  P.vps_shift = s->sh;
+  P.sh = s->sh;
   P.n = n;
   vgx_tsdf_stats st;
   memset(&st, 0, sizeof(st));

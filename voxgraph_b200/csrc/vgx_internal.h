@@ -98,6 +98,12 @@ __host__ __device__ __forceinline__ uint64_t vgx_pack_key(int bx, int by, int bz
          ((uint64_t)((uint32_t)(by + (1 << 20)) & 0x1FFFFFu) << 21) |
          ((uint64_t)((uint32_t)(bz + (1 << 20)) & 0x1FFFFFu) << 42);
 }
+// the block index a key packs (the inverse of vgx_pack_key inside the range)
+__host__ __device__ __forceinline__ void vgx_unpack_key(uint64_t key, int b[3]) {
+  b[0] = (int)(key & 0x1FFFFFu) - (1 << 20);
+  b[1] = (int)((key >> 21) & 0x1FFFFFu) - (1 << 20);
+  b[2] = (int)((key >> 42) & 0x1FFFFFu) - (1 << 20);
+}
 // an uploaded block index component whose +-1 neighbours pack to keys of their own
 __host__ __device__ __forceinline__ bool vgx_block_index_ok(int b) {
   return b >= VGX_BLOCK_INDEX_MIN && b <= VGX_BLOCK_INDEX_MAX;
@@ -501,8 +507,9 @@ void vgx_submap_drop(vgx_ctx* ctx, uint32_t submap_id);
 int vgx_submap_move(vgx_ctx* ctx, uint32_t from_id, uint32_t id);
 // an id for a scratch submap: the first unused one counting down from 2^32 - 2 (2^32 - 1 is a valid cblox id)
 uint32_t vgx_scratch_id(vgx_ctx* ctx);
-// registration view (octets) of `bricks` (n_blocks x vps^3 (distance, weight/observed)) into `view`
-int vgx_submap_build_view(vgx_ctx* ctx, VgxSubmap* s, const float2* bricks, float* view);
+// registration view (octets) of the layer `which` (VGX_LAYER_TSDF: d_dw into d_view, VGX_LAYER_ESDF: d_esdf into
+// d_view_esdf)
+int vgx_submap_build_view(vgx_ctx* ctx, VgxSubmap* s, int which);
 // clears the block hash and re-inserts the first s->n_blocks blocks (after a capacity overflow
 // left keys without a brick behind)
 int vgx_submap_rebuild_hash(vgx_ctx* ctx, VgxSubmap* s);
